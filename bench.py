@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — boosting-iteration throughput of the B200-native hot path (BASELINE.json metric).
+"""bench.py — boosting-iteration throughput of the H100-native hot path (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 Workload (config.workload): one GBMRegressor boosting iteration, squared loss, on N_rows x 128 fp32
 synthetic rows per GPU (default 100 M x 128, the configuration the metric is quoted on):
@@ -13,7 +13,9 @@ i.e. regression/GBMRegressor.scala:398-442 + :368-385 of the reference, per roun
 `e2e`    = the same round through the host-side mirror with HOST (pinned) buffers: the direction h is
            copied host->device and the pseudo-residuals device->host inside the timed region.
 `roofline` is for the dominant kernel K1 (fused update+residual+loss), timed with CUDA events on the
-library's own stream, against MEASURED_PEAKS.json's HBM copy bandwidth.
+library's own stream, against MEASURED_PEAKS.json's HBM copy bandwidth (else the H100 SXM data sheet's 3.35 TB/s).
+`--dump-outputs DIR`: after the timed steps, what the last timed round returned — alpha, the loss sum, and a fixed
+seeded sample of the updated F and of the next pseudo-residuals r (with the sampled row indices) — as DIR/<name>.npy.
 `extras.strong_scaling`: the SAME round on a fixed GLOBAL dataset (--strong-rows, default 100 M rows) split over
 the ranks (12.5 M rows per GPU at N=8), measured in the same run after the weak-scaling figure; `extras.strong_c3`:
 BASELINE config 3 (bernoulli, 50 M rows global, Brent line search + update per round) split the same way.
@@ -46,20 +48,6 @@ BYTES_K2 = 8   # squared-loss statistics read the current residual r = y - F and
 BYTES_ROUND = BYTES_K1 + BYTES_K2  # the one-launch round runs both passes inside one kernel
 
 
-def _ncu_traffic(rows: int, bytes_per_row: int):
-    """DRAM bytes per launch of the roofline kernel from the committed `ncu --set full` capture (profiles/), if it
-    was taken at this row count for this kernel."""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        d = json.load(open(p))
-        key = "fused_round" if bytes_per_row == BYTES_ROUND else "k1"
-        if int(d[key]["rows"]) == int(rows):
-            return float(d[key]["dram_bytes_per_launch"])
-    except Exception:
-        pass
-    return None
-
-
 def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -67,11 +55,11 @@ def _peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s, not measured)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -250,6 +238,24 @@ def parity_check(ctx, n, lr, tol, max_iter, world, rank, dist, label):
             "r_max_rel_err": r_err, "tolerance": 1e-5, "seconds": time.perf_counter() - t_start}
 
 
+# ------------------------------------------------------------------ outputs of the timed path
+DUMP_SAMPLE_ROWS = 2_000_000  # F and r sampled at these many rows: 8 MB each in fp32, 16 MB of fp64 indices
+
+
+def dump_outputs(out_dir, ctx, n, last, suffix=""):
+    """What a caller of the timed round receives after its last step: alpha and the loss sum, and the updated F and
+    next pseudo-residuals r on a fixed seeded sample of the rows (all rows when the shard is small)."""
+    from spark_ensemble_b200 import _native as N
+    os.makedirs(out_dir, exist_ok=True)
+    rows = np.arange(n) if n <= DUMP_SAMPLE_ROWS else np.sort(
+        np.random.default_rng(0).choice(n, DUMP_SAMPLE_ROWS, replace=False))
+    alpha, loss_sum = last if last is not None else (float("nan"), float("nan"))
+    arrays = {"alpha": np.array([alpha], dtype=np.float64), "loss_sum": np.array([loss_sum], dtype=np.float64),
+              "rows": rows.astype(np.float64), "F": ctx.download(N.SLOT_F)[:n][rows], "r": ctx.download(N.SLOT_R)[:n][rows]}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}{suffix}.npy"), a)
+
+
 # ------------------------------------------------------------------ main
 def main():
     ap = argparse.ArgumentParser()
@@ -266,6 +272,8 @@ def main():
                     help="GLOBAL rows of the strong-scaling measurement (split over the ranks); 0 disables")
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle self-check after the timed regions")
     ap.add_argument("--no-extras", action="store_true", help="skip the tree / async / config-3 extras")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed round computed (alpha, loss sum, sampled F and r) as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
 
@@ -364,8 +372,9 @@ def main():
     barrier()
     ctx.timer_start()
     t0 = time.perf_counter()
+    last = None
     for _ in range(args.steps):
-        step()
+        last = step()
     ms_dev = ctx.timer_stop()
     ctx.sync()
     ms_wall = 1e3 * (time.perf_counter() - t0)
@@ -374,6 +383,8 @@ def main():
     ktimes = ctx.kernel_times()
     ctx.kernel_timing(False)
     ms = max(ms_dev, ms_wall)  # device events and host clock bracket the same region; host syncs are inside
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ctx, n, last, f"_rank{rank}" if world > 1 else "")
     if dist is not None:
         import torch
         t = torch.tensor([ms], dtype=torch.float64, device="cuda")
@@ -387,7 +398,7 @@ def main():
     for _ in range(2):
         eng.boost_round(h_host, lr, tol, max_iter, r_host)
     barrier()
-    e2e_steps = max(3, min(args.steps, 10))
+    e2e_steps = args.steps
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
         eng.boost_round(h_host, lr, tol, max_iter, r_host)
@@ -493,7 +504,7 @@ def main():
     strong = strong_c3 = None
     if args.strong_rows > 0:
         ns = min(n, (args.strong_rows // world) // 4 * 4)
-        ms_s, ne_s = timed_rounds(ns, max(args.steps, 20))
+        ms_s, ne_s = timed_rounds(ns, args.steps)
         strong = {"rows_global": ns * world, "rows_per_gpu": ns, "ms_per_step": ms_s, "value": ns * world / (ms_s * 1e-3),
                   "unit": "rows/s", "one_launch_round": int(ctx.get_option("last_round_fused")),
                   "brent_evals_per_round": ne_s, "scaling": "strong",
@@ -561,7 +572,7 @@ def main():
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload, "rows_per_gpu": n, "features": d, "loss": "squared",
-                   "l2": "inputs (1.2 GB of y/F/h per GPU) are larger than L2 (126 MB); no flush needed",
+                   "l2": "inputs (1.2 GB of y/F/h per GPU) are larger than L2 (50 MB); no flush needed",
                    "features_resident": have_x,
                    "parallelism": (f"rows sharded x{world}; the <=3 fp64 sums of every reduction are exchanged over NVLink peer "
                                    f"memory by the reducing kernel's last CTA (fused all-reduce, p2p_active={p2p_active}; NCCL only "
@@ -575,7 +586,7 @@ def main():
         "parity_ok": (all(p["ok"] for p in parity) if parity else None), "parity": parity, "p2p_active": p2p_active,
         "roofline": {"kernel": roof_kernel,
                      "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": _ncu_traffic(n, roof_bytes), "peak_source": peak_src, "bytes_per_row": roof_bytes, "ms_per_launch": k1_ms,
+                     "peak_source": peak_src, "bytes_per_row": roof_bytes, "ms_per_launch": k1_ms,
                      "launches_timed": k1["launches"]},
         "cpu_baseline": cpu,
         "extras": extras,

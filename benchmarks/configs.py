@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """The five BASELINE.json configurations, device-resident.
 
-    python benchmarks/configs.py [--out profiles/r02_configs_n1.json]                       # one GPU
+    python benchmarks/configs.py [--out /tmp/configs_n1.json]                       # one GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \\
-        --master-port 29541 benchmarks/configs.py --out profiles/r02_configs_n8.json         # one rank per GPU
+        --master-port 29541 benchmarks/configs.py --out /tmp/configs_n8.json         # one rank per GPU
 
 C1 GBMRegressor cpusmall 20 rounds (host base learner: the reference's plumbing case, timed end to end; rank 0 only)
 C2 GBMRegressor 10 M x 64 squared, 100 rounds, 1 GPU     (one cooperative launch per round)

@@ -2,7 +2,7 @@
 """GBMRegressionModel.transform for tree members: se_forest_predict (one pass) vs one se_tree_predict per member into
 an [M][n] array + the aggregation kernel.
 
-    python benchmarks/forest_time.py [--rows 50000000] [--out profiles/r02_forest.json]
+    python benchmarks/forest_time.py [--rows 50000000] [--out /tmp/forest.json]
 """
 import argparse
 import json

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Persistent line search: cp.async ring depth x CTAs per SM (experiment driver behind profiles/r02_ls_ring.json).
+"""Persistent line search: cp.async ring depth x CTAs per SM (experiment driver).
 
-    python benchmarks/ls_ring.py [--rows 50000000 6250000] [--loss bernoulli huber] [--out profiles/r02_ls_ring.json]
+    python benchmarks/ls_ring.py [--rows 50000000 6250000] [--loss bernoulli huber] [--out /tmp/ls_ring.json]
 """
 import argparse
 import json

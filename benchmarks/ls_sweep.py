@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Line-search / fused-round variants on one GPU (experiment driver behind profiles/r02_*; not a bench line).
+"""Line-search / fused-round variants on one GPU (experiment driver; not a bench line).
 
     python benchmarks/ls_sweep.py [--rows 50000000] [--loss bernoulli]
 """

@@ -12,7 +12,7 @@ from spark_ensemble_b200.context import Context  # noqa: E402
 
 ctx = Context(0)
 M, K, n = 64, 26, 10_000_000
-peak = 6580.9
+peak = 3350.0  # H100 SXM data sheet, GB/s
 for kind, name, w in ((N.AGG_BAGGING_HARD, "hard votes", None), (N.AGG_BOOSTING_DISCRETE, "weighted votes", np.linspace(0.5, 1.5, M))):
     ctx.agg_configure(kind, M, K, 1, 0, n)
     ctx.fill_synthetic(N.SLOT_P, "randint", 5, 0, K)

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Weighted median (BoostingRegressor.predict) over 25 M rows: fast path vs exact kernel, by weight pattern.
 
-    python benchmarks/wmedian_time.py [--out profiles/r02_wmedian.json]
+    python benchmarks/wmedian_time.py [--out /tmp/wmedian.json]
 """
 import argparse
 import json

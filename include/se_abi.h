@@ -1,11 +1,11 @@
 /*
- * se_abi.h — C ABI of libse_b200.so: the B200-native (sm_100a) row-parallel boosting hot path of
+ * se_abi.h — C ABI of libse_b200.so: the H100-native (sm_90a) row-parallel boosting hot path of
  * pierrenodet/spark-ensemble.  This is the drop-in boundary: the entry points below are what the
  * reference's Scala train()/predict() bodies bind through JNI (jni/se_jni.cpp) once their per-row
  * RDD closures are replaced by native calls; the same symbols are driven through ctypes by
  * spark_ensemble_b200/ (host-side mirror of the Spark ML surface) and by tests/.
  *
- * Reference citations are relative to /root/reference/core/src/main/scala/org/apache/spark/ml/.
+ * Reference citations are relative to core/src/main/scala/org/apache/spark/ml/ of the reference repository.
  *
  * Conventions
  *  - plain C: opaque handle, int status (0 = SE_OK, negative = error; text via se_last_error()),

@@ -403,7 +403,7 @@ def generate():
     scala = ['''/*
  * SeNative.scala — GENERATED by jni/gen_jni.py (edit the table there, not this file).
  * JVM side of the drop-in boundary: @native bindings of jni/se_jni.cpp, which forwards 1:1 to the C ABI of
- * include/se_abi.h (libse_b200.so, sm_100a kernels).  Not compiled in this repository's image (no JDK/scalac/sbt);
+ * include/se_abi.h (libse_b200.so, sm_90a kernels).  Not compiled in this repository's image (no JDK/scalac/sbt);
  * INTEGRATION.md shows how the reference's train()/predict() bodies call these in place of their per-row RDD closures
  * and scala/org/apache/spark/ml/regression/GBMRegressorNative.scala is the rewired GBMRegressor.train().
  */

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY.  Exists so the C oracle is cross-checked by a second, separately written
 restatement (different language, vectorised instead of per-row).  PARITY UNPINNED like the C oracle.
-Citations relative to /root/reference/core/src/main/scala/org/apache/spark/ml/.
+Citations relative to core/src/main/scala/org/apache/spark/ml/ of the reference repository.
 """
 from __future__ import annotations
 

@@ -3,7 +3,7 @@
  * TEST INFRASTRUCTURE ONLY (see se_oracle.h).  PARITY UNPINNED (no JVM here, no golden vectors
  * in the reference's tests); pinned against portable properties + an independent numpy restatement.
  *
- * Citations: paths relative to /root/reference/core/src/main/scala/org/apache/spark/ml/.
+ * Citations: paths relative to core/src/main/scala/org/apache/spark/ml/ of the reference repository.
  * Spark-internal helpers (softmax, log1pExp, EPSILON: org.apache.spark.ml.impl.Utils, Spark 3.3.1,
  * not vendored) are restated from their published definitions.
  */

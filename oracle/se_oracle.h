@@ -11,7 +11,7 @@
  * reference's tests assert (finite-difference gradient check, zero-sum raw predictions, ...),
  * against an independent numpy restatement (oracle/np_oracle.py) and against closed forms.
  *
- * All citations are relative to /root/reference/core/src/main/scala/org/apache/spark/ml/.
+ * All citations are relative to core/src/main/scala/org/apache/spark/ml/ of the reference repository.
  * Layout convention shared with the product: per-row arrays are [dim][n] ("class-major",
  * rows contiguous); model-output matrices are [M][n] or [M][K][n].
  */

@@ -1,6 +1,6 @@
 /*
  * BoostingClassifierNative.scala — the reference's BoostingClassifier (SAMME / SAMME.R) with its train() body rewired
- * onto the B200 hot path.
+ * onto the H100 hot path.
  *
  * Unchanged from the reference (classification/BoostingClassifier.scala:135-282): Params, label validation, the base
  * learner fit on the normalised weights (third party), the estimator-weight bookkeeping (SAMME.R: 1.0; SAMME: log(1/beta),

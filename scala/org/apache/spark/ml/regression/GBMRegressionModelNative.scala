@@ -1,6 +1,6 @@
 /*
  * GBMRegressionModelNative.scala — the reference's GBMRegressionModel with transform() evaluated per PARTITION on the
- * B200 instead of per row on the JVM (regression/GBMRegressor.scala:531-539:
+ * H100 instead of per row on the JVM (regression/GBMRegressor.scala:531-539:
  *     sum = init.predict(x); for (i <- models) sum += models(i).predict(slice(subspaces(i))(x)) * weights(i)).
  *
  * Two routes, both through org.apache.spark.ml.se.SeNative (include/se_abi.h):

@@ -1,5 +1,5 @@
 /*
- * GBMRegressorNative.scala — the reference's GBMRegressor with its train() body rewired onto the B200 hot path.
+ * GBMRegressorNative.scala — the reference's GBMRegressor with its train() body rewired onto the H100 hot path.
  *
  * What stays exactly as in the reference (regression/GBMRegressor.scala:237-476): Params, instrumentation, the
  * train/validation split, the init model (DummyRegressor / base learner), sub-spaces (HasSubBag.subspace), the base

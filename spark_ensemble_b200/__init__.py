@@ -1,4 +1,4 @@
-"""spark_ensemble_b200 — B200-native (sm_100a) implementation of the row-parallel boosting hot path of
+"""spark_ensemble_b200 — H100-native (sm_90a) implementation of the row-parallel boosting hot path of
 pierrenodet/spark-ensemble behind the reference's Estimator/Model surface.
 
     csrc/            hand-written CUDA kernels + the C ABI of include/se_abi.h (libse_b200.so)

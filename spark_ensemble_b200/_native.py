@@ -142,7 +142,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -m spark_ensemble_b200.build` "
-            "(nvcc, sm_100a). The boosting hot path has no CPU fallback.")
+            "(nvcc, sm_90a). The boosting hot path has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, argtypes in PROTOTYPES.items():
         fn = getattr(lib, name)  # AttributeError here == ABI mismatch: fail loudly

@@ -1,8 +1,8 @@
-"""Builds libse_b200.so (the C-ABI of include/se_abi.h) for sm_100a with nvcc, in-tree.
+"""Builds libse_b200.so (the C-ABI of include/se_abi.h) for sm_90a (H100) with nvcc, in-tree.
 
     python -m spark_ensemble_b200.build [--force]
 
-The shared library lands in spark_ensemble_b200/lib/ (git-ignored, travels to the GPU box).
+The shared library lands in spark_ensemble_b200/lib/ (git-ignored).
 """
 from __future__ import annotations
 
@@ -21,8 +21,9 @@ SOURCES = ["se_api.cu", "se_gbm.cu", "se_gbm_tiled.cu", "se_gbm_fused.cu", "se_g
 # the device Brent must round every multiply and add separately to reproduce the host line search bit for bit
 EXTRA_FLAGS = {"se_brent.cu": ["-fmad=false"], "se_gbm_fused.cu": ["-fmad=false"]}
 HEADERS = ["se_common.cuh", "se_kernels.h", "se_loss.cuh", "se_tma.cuh", "se_brent.h", "se_sortnet.h", os.path.join("..", "..", "include", "se_abi.h")]
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
+    "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
 
@@ -44,7 +45,8 @@ def _stale(target: str, deps: list[str]) -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJDIR, exist_ok=True)
     nvcc = _nvcc()
-    hdrs = [os.path.join(CSRC, h) for h in HEADERS]
+    # this file holds the flags: editing it rebuilds every object
+    hdrs = [os.path.join(CSRC, h) for h in HEADERS] + [os.path.abspath(__file__)]
     jobs = []
     for src in SOURCES:
         s = os.path.join(CSRC, src)
@@ -64,8 +66,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             list(ex.map(compile_one, jobs))
     objs = [os.path.join(OBJDIR, s.replace(".cu", ".o")) for s in SOURCES]
     if jobs or force or _stale(LIB, objs):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-                                                    "-Xcompiler", "-fPIC", "-ldl"]
+        cmd = [nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-Xcompiler", "-fPIC", "-ldl"]
         if verbose:
             print(" ".join(cmd), flush=True)
         subprocess.check_call(cmd)

@@ -1,4 +1,4 @@
-// se_agg.cu — ensemble Model.predict / predictRaw aggregation kernels (sm_100a).
+// se_agg.cu — ensemble Model.predict / predictRaw aggregation kernels (sm_90a).
 //
 // Reference per-row bodies (one JVM call per row through a UDF, SURVEY.md §3.4):
 //   regression/GBMRegressor.scala:531-539        init + Σ_m a_m·P[m]
@@ -246,7 +246,7 @@ __global__ void __launch_bounds__(kBlock) agg_votes_kernel(const float* __restri
 }
 
 // Unweighted (hard) votes, the packed form: ncu on the histogram kernel above (M = 64, K = 26, 10 M rows): 2660
-// instructions per row — 41 per vote — at 60 % issue utilisation and 47 % of the DRAM peak: issue-bound, not
+// instructions per row — 41 per vote — at 60 % issue utilisation and about half of the DRAM peak: issue-bound, not
 // memory-bound.  Here a thread owns FOUR consecutive rows (one 128-bit load per model), counts are 8-bit fields packed
 // four to a 32-bit word (class c -> word c >> 2, byte c & 3: M <= 255 never overflows a field), the words live in the
 // thread's own shared-memory column (conflict-free, 4x less shared memory than one float per class), and the four
@@ -318,8 +318,8 @@ __global__ void __launch_bounds__(kBlock) agg_hard_votes_packed_kernel(const flo
   if (bad_vote && f.bad_label != nullptr) *reinterpret_cast<volatile int*>(f.bad_label) = 1;
 }
 
-// (A four-rows-per-thread fp64 form of the WEIGHTED vote histogram was measured too: [K][4][128] doubles leave two
-// 128-thread CTAs per SM and ran 2.81 ms vs 1.56 ms for agg_votes_kernel<double> at M = 64, K = 26, 10 M rows — the
+// (A four-rows-per-thread fp64 form of the WEIGHTED vote histogram was tried too: [K][4][128] doubles leave two
+// 128-thread CTAs per SM and it was slower than agg_votes_kernel<double> — the
 // fp64 read-modify-write chains need the resident warps more than they need wider loads.  Not kept.)
 
 // ------------------------------------------------------------------ class-wide sums through TMA tiles
@@ -538,8 +538,8 @@ __global__ void __launch_bounds__(kBlock) agg_finalize_kernel(const FinArgs f) {
 // One thread per row.  The row's M values become 64-bit words (order-preserving key << 32 | model index: all words
 // distinct, ties keep model order = stable sort) in the thread's own column of shared memory [Mp][T] (conflict-free),
 // padded to a power of two Mp with +inf words, and are sorted by a bitonic network — uniform control flow for the
-// whole warp, O(M log² M) compare-exchanges instead of the O(M²) threshold scan it replaces (which was 0.07 of the
-// HBM roofline at M = 32 because per-lane pruning diverges).  Total and running sums are then accumulated in fp64 in
+// whole warp, O(M log² M) compare-exchanges instead of the O(M²) threshold scan it replaces (far from the HBM
+// roofline because per-lane pruning diverges).  Total and running sums are then accumulated in fp64 in
 // sorted order, exactly like the reference.
 __device__ __forceinline__ uint32_t wm_key(float x) {
   const uint32_t u = __float_as_uint(x + 0.0f);  // -0 -> +0: equal values stay ties
@@ -691,7 +691,7 @@ __device__ __forceinline__ unsigned long long wm_exact_pick(unsigned long long (
 
 // Same algorithm with the row's words in REGISTERS (Mp <= 64): the network is fully unrolled, so every
 // compare-exchange is ~6 ALU instructions and no memory traffic — the shared-memory form above moves 32 B per
-// compare-exchange and thread and is bound by shared-memory bandwidth (measured 8.0 ms for 25 M rows at M = 32).
+// compare-exchange and thread and is bound by shared-memory bandwidth.
 template <int MP>
 __global__ void __launch_bounds__(128) agg_wmedian_reg_kernel(const __grid_constant__ CUtensorMap mapP, int64_t n,
                                                               int M, const double* __restrict__ a,
@@ -740,7 +740,7 @@ __global__ void __launch_bounds__(128) agg_wmedian_reg_kernel(const __grid_const
 // ---- weighted median, fast path (M <= 64, all weights finite and >= 0) -------------------------------------------
 // The exact kernels above carry (key, model) words through the sort because the reference accumulates the weights in
 // SORTED order (ensemble/Utils.scala:31-38) — 6 ALU-pipe instructions per compare-exchange, and the ALU pipe issues at
-// half rate: 4.07 ms for 25 M rows x 32 models.  With weights >= 0 the answer is `the smallest value v whose group-end
+// half rate.  With weights >= 0 the answer is `the smallest value v whose group-end
 // cumulative weight C(v) reaches h = total / 2` (cumulative sums are monotone in fp64 too).  C(v) and h are recursive
 // fp64 sums of the same addends as Ĉ(v) = Σ_{x_j <= v} a_j and ĥ = T̂ / 2 taken in MODEL order, so
 //     |(C(v) - h) - (Ĉ(v) - ĥ)| <= 3 (M - 1) 2^-53 T (1 + eps)
@@ -889,8 +889,7 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   static const int enabled = [] { const char* e = getenv("SE_AGG_TILE"); return e ? atoi(e) : 1; }();
   if (!enabled || a.M < 1 || a.n < 1 || a.n >= (int64_t)0x7fffff00) return cudaSuccess;
   // one warp per CTA (128-row tiles), one stage: shared memory bounds occupancy and what counts is the number of
-  // boxes in flight per SM (measured, boosting-real M=10 K=26: 1 warp x 1 stage 2.75 ms, 2 warps x 1 stage 2.78,
-  // 2 warps x 2 stages 4.32, 2 warps x 4 stages 8.59; streaming path 3.01)
+  // boxes in flight per SM (more warps or stages per CTA leave fewer CTAs resident)
   constexpr int warps = 1;
   const int kAT = 32 * warps, kAR = 128 * warps;
   ClassTileArgs ta{};

@@ -91,7 +91,6 @@ thread_local std::string g_last_error;
 constexpr int kScal = 1024;         // doubles in the device/host scalar blocks ([0, 160): generic reductions)
 constexpr int kScalHist = 704;      // 256-bin radix-select histogram
 constexpr int kScalRound = 160;     // offset of the squared-round results (statistics, alpha, loss)
-constexpr int64_t kL2HintRows = 16000000;  // 16 B/row of y, F, h, r: up to ~2x the 126 MB L2
 constexpr int kScalHost = 192;      // offset used by se_comm_allreduce_host (up to kScalHist - kScalHost values)
 constexpr int kSmallBytes = 1 << 20;  // small device scratch: weights, init, tree arrays, factors
 
@@ -125,7 +124,7 @@ struct se_ctx {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   bool timing = false;
   double last_ms = 0.0;
-  int sms = 148;
+  int sms = 132;
   int ctas_per_sm = 8;  // upper bound; launchers scale the grid down for small shards (se_gbm.cu grid_for)
   int64_t launches = 0;
   SlotBuf slot[SE_NUM_SLOTS];
@@ -197,13 +196,14 @@ struct se_ctx {
   unsigned pass_parity = 0;           // alternates the tile direction of consecutive GBM passes (L2 reuse)
   bool alternate = true;
   int l2_hints = -1;                  // evict_first hints on the GBM streams: -1 by shard size, 0 off, 1 on (SE_L2_HINTS)
+  int64_t l2_hint_rows = 0;           // shard size up to which l2_hints = -1 turns them on: 16 B/row of y, F, h, r up to ~2x the L2
   // ---- cooperative whole-round / whole-line-search kernels (se_gbm_fused.cu)
   FusedSync* d_fsync = nullptr;
   unsigned long long fused_epoch = 0;
   int fused_round = -1;               // squared-loss round in one launch: -1 by shard size, 0 off, 1 on
-  int64_t fused_round_max_rows = (int64_t)1 << 40;  // measured faster than two launches from 6 M to 100 M rows
+  int64_t fused_round_max_rows = (int64_t)1 << 40;  // no size limit by default
   int fused_ctas_per_sm = 3;
-  double fused_prefetch_mb = 0.0;     // (measured: no gain at 6-12 M rows, -2 % at 25-50 M rows: off)
+  double fused_prefetch_mb = 0.0;     // off by default
   int fused_loss_reduce = 0;          // 1: reduce the train loss over the rows even when the closed form applies
   int fused_l2_mode = 0;              // experiment: 1 = evict_last on r/h, 2 = persisting window over r
   int fused_timing = 0;               // diagnostic: in-kernel %globaltimer stamps of the fused round
@@ -213,11 +213,9 @@ struct se_ctx {
                                       // the persistent kernel (bit-identity check of mode 1)
   int ls_resident = 1;                // workers keep their first tiles in shared memory
   int ls_ctas_per_sm = 4;
-  int ls_ring = 0;                    // cp.async ring stages for the streamed tiles (0 off = register prefetch, 2..4; measured: no gain)
-  int l2_persist = 0;                 // mark the packed line-search view as L2-persisting.  OFF by default: measured on
-                                      // B200 the 83 MB carve-out buys the search nothing (2.86 vs 2.75 ms of evaluations per
-                                      // round at 50 M rows) and, while it is configured, every STREAMING kernel runs 2x slower
-                                      // (K1 0.36 vs 0.17 ms at 50 M rows) — profiles/r02_ls_sweep.json
+  int ls_ring = 0;                    // cp.async ring stages for the streamed tiles (0 off = register prefetch, 2..4)
+  int l2_persist = 0;                 // mark the packed line-search view as L2-persisting.  OFF by default: while a
+                                      // carve-out is configured, every STREAMING kernel works with a smaller L2
   size_t l2_persist_max = 0;          // cudaDevAttrMaxPersistingL2CacheSize
   size_t l2_window_max = 0;           // cudaDevAttrMaxAccessPolicyWindowSize
   size_t l2_persist_set = 0;          // current cudaLimitPersistingL2CacheSize
@@ -626,7 +624,7 @@ GbmArgs gbm_args(se_ctx* ctx, bool validation) {
   a.param = (float)g.param;
   a.reverse = (ctx->alternate && !validation) ? (int)(ctx->pass_parity++ & 1u) : 0;
   // shards whose four per-row arrays (y, F, h, r) are of the order of the L2: evict_first hints (se_common.cuh)
-  a.l2_hints = ctx->l2_hints >= 0 ? ctx->l2_hints : ((validation ? ctx->gbm.nv : ctx->gbm.n) <= kL2HintRows ? 1 : 0);
+  a.l2_hints = ctx->l2_hints >= 0 ? ctx->l2_hints : ((validation ? ctx->gbm.nv : ctx->gbm.n) <= ctx->l2_hint_rows ? 1 : 0);
   a.ws = red_ws(ctx, 0, /*exchange=*/false);  // armed (sequence number taken) only at reducing launches
   return a;
 }
@@ -687,6 +685,7 @@ int se_ctx_create(int device, se_ctx** out) {
   cudaDeviceProp prop;
   SE_CREATE_CUDA(cudaGetDeviceProperties(&prop, device));
   ctx->sms = prop.multiProcessorCount;
+  ctx->l2_hint_rows = 2 * (int64_t)prop.l2CacheSize / 16;
   if (const char* s = getenv("SE_ALTERNATE_PASSES")) ctx->alternate = atoi(s) != 0;
   if (const char* s = getenv("SE_L2_HINTS")) ctx->l2_hints = atoi(s) != 0 ? 1 : 0;
   if (const char* s = getenv("SE_CTAS_PER_SM")) {
@@ -1609,7 +1608,7 @@ static int newton_finish(se_ctx* ctx, double* sum_hess) {
   // S_j (all-reduced) -> the base-learner weights are WOUT_j * 1/S_j  (GBMRegressor.scala:373,379;
   // GBMClassifier.scala:344-355,364).  The kernel left the unnormalised 1/2 hc w in SE_SLOT_WOUT; the per-dimension
   // factor 1/S_j is applied where the weights LEAVE the device (se_download / se_download_scaled on SE_SLOT_WOUT) —
-  // round 1 ran a separate 8 B/row pass over WOUT for it (newton K1 0.76-0.87 of the HBM roofline because of that pass).
+  // no separate 8 B/row pass over WOUT for it.
   const int dim = ctx->gbm.dim;
   std::vector<double> s((size_t)dim + 1);
   SE_TRY(gbm_fetch(ctx, 1 + dim, s.data()));
@@ -1794,8 +1793,7 @@ int linesearch_persist(se_ctx* ctx, double lo, double hi, double start, double r
   const unsigned long long seq0 = ctx->red_seq;
   LsLaunch cfg;
   // small shards (what strong scaling leaves per GPU) live entirely in shared memory + L2: fewer, fatter CTAs keep more
-  // tiles resident and shorten the per-evaluation rendezvous (measured at 6.25 M rows: 0.355 ms/round with 3 CTAs/SM vs
-  // 0.384 with 4; at 50 M rows 4 CTAs/SM are 12 % faster than 3)
+  // tiles resident and shorten the per-evaluation rendezvous; large shards want more CTAs in flight
   cfg.max_ctas_per_sm = (ctx->ls_ctas_per_sm == 4 && ctx->gbm.n <= 8000000) ? 3 : ctx->ls_ctas_per_sm;
   cfg.resident = ctx->ls_resident;
   cfg.ring = ctx->ls_ring;
@@ -1962,7 +1960,7 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   a.bag = g.use_bag ? ctx->slot[SE_SLOT_BAG].d : nullptr;
   a.n = g.n;
   a.stats_from_r = g.r_current ? 1 : 0;
-  a.l2_hints = ctx->l2_hints >= 0 ? ctx->l2_hints : (g.n <= kL2HintRows ? 1 : 0);
+  a.l2_hints = ctx->l2_hints >= 0 ? ctx->l2_hints : (g.n <= ctx->l2_hint_rows ? 1 : 0);
   a.lr = learning_rate;
   a.wsum = g.wsum;
   a.lo = 0.0; a.hi = 100.0; a.start = 1.0; a.rel = tol; a.abs_tol = tol; a.max_eval = max_iter;
@@ -2058,7 +2056,7 @@ int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, i
   if (sq_search) {
     // commons-math3 BrentOptimizer constructor checks (the host path performs them in brent_impl's caller)
     SE_REQUIRE(ctx, tol >= 2.0 * 2.220446049250313e-16 && tol > 0.0, SE_ERR_ARG, "tolerance %g too small for Brent", tol);
-    // One cooperative launch per round (measured on B200: 52 vs 74 us at 12.5 M rows, 440 vs 454 us at 100 M rows).
+    // One cooperative launch per round: no host round trip between the line search and the update.
     // With a communicator it needs the fused peer exchange (an NCCL all-reduce cannot run inside the kernel).
     const bool can = (ctx->nranks <= 1 || ctx->p2p);
     const bool want = ctx->fused_round > 0 || (ctx->fused_round < 0 && ctx->gbm.n <= ctx->fused_round_max_rows);

@@ -1,4 +1,4 @@
-// se_boost.cu — BoostingClassifier sample-weight update kernels (sm_100a).
+// se_boost.cu — BoostingClassifier sample-weight update kernels (sm_90a).
 //
 // Reference: classification/BoostingClassifier.scala:168-187 (normalise), :198-230 (SAMME.R: error,
 // weight update), :231-260 (SAMME), :269 (Σw').  The reference makes two (real) or three (discrete)
@@ -19,13 +19,12 @@ constexpr float kSparkEps = 2.220446049250313e-16f;  // Spark ml.impl.Utils.EPSI
 constexpr int KU = 8;                                // classes loaded per batch (8 x 16 B in flight)
 
 // Persistent grid: a multiple of the SM count, up to `ctas_per_sm` CTAs per SM, but never so many that a CTA
-// gets fewer than ~8 work units (tiles).  Measured on B200 (squared loss): at 100 M rows 8 CTAs/SM beats 2
-// (K1 0.97 vs 0.93 of the HBM peak: later waves rebalance the tail), at 10 M rows 2 beats 8 (0.82 vs 0.77:
-// fewer, longer-lived CTAs amortise ramp-up and the per-CTA reduction epilogue).
+// gets fewer than ~8 work units (tiles): on large inputs later waves rebalance the tail, on small ones fewer,
+// longer-lived CTAs amortise ramp-up and the per-CTA reduction epilogue.
 inline int grid_for(int64_t work_items, int64_t per_cta, int ctas_per_sm, int sms) {
   int64_t units = (work_items + per_cta - 1) / per_cta;
   if (units < 1) units = 1;
-  if (ctas_per_sm > 4) ctas_per_sm = 4;  // light grid-stride kernels (all CTAs resident): 4/SM measured best
+  if (ctas_per_sm > 4) ctas_per_sm = 4;  // light grid-stride kernels (all CTAs resident)
   int64_t cap = (int64_t)ctas_per_sm * sms;
   if (cap > kMaxGridPartials) cap = (kMaxGridPartials / sms) * sms;
   int64_t want = (units / 8 / sms) * sms;  // >= 8 units per CTA, whole multiples of the SM count
@@ -111,8 +110,8 @@ __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
 }
 
 // SAMME.R through TMA tiles (K >= 5): the register-streaming kernel above keeps 8 x 16 B of P per thread in
-// registers (99 registers, 2 CTAs/SM, ~64 KB of loads in flight per SM; ncu: long-scoreboard bound at 0.82 of the
-// HBM roofline, K = 26).  Here a 2-warp CTA owns a 256-row x K tile of P that arrives as one 2-D tensor-map box
+// registers (99 registers, 2 CTAs/SM, ~64 KB of loads in flight per SM; long-scoreboard bound below the
+// HBM roofline at large K).  Here a 2-warp CTA owns a 256-row x K tile of P that arrives as one 2-D tensor-map box
 // (`cp.async.bulk.tensor.2d`, rows past n zero-filled), up to 8 CTAs per SM keep ~200 KB in flight, and a thread
 // walks the classes of its four rows with 128-bit shared-memory reads: first-maximum argmax, Σ_k lg2 max(p, ε);
 // log p_y is picked from the tile afterwards.  Same arithmetic as boost_real_kernel (BoostingClassifier.scala:198-230).

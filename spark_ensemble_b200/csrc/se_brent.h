@@ -105,8 +105,7 @@ SE_HD inline int brent_core(F f, double lo, double hi, double start, double rel,
 
 // squared-loss line-search objective from the sufficient statistics: Σ (y-F-αh)²/2 / Σw.  The division by 2Σw is a
 // multiplication by its reciprocal, formed once: an fp64 division is a ~30-instruction dependent chain on the GPU and
-// the objective is evaluated ~10-35 times per search by ONE thread while the whole grid waits for the step (the
-// in-kernel search of the fused round measured 0.29 us per evaluation with the division).  Host and device use this
+// the objective is evaluated ~10-35 times per search by ONE thread while the whole grid waits for the step.  Host and device use this
 // same struct, so their iterates stay bit-identical to each other.
 struct BrentParabola {
   double s0, s1, s2, inv2ws;

@@ -1,4 +1,4 @@
-// se_common.cuh — shared device helpers for the sm_100a streaming kernels.
+// se_common.cuh — shared device helpers for the sm_90a streaming kernels.
 //
 // Every kernel on this path is elementwise + reduction and HBM-bound (no tensor cores): the
 // helpers here are the 128-bit streaming loads/stores (read-once data bypasses L1 allocation),
@@ -52,13 +52,11 @@ __device__ __forceinline__ void st_stream1(float* p, float v) {
 }
 
 // ---- the same accesses with an explicit L2 eviction policy (createpolicy + .L2::cache_hint) -----------------
-// Measured on B200 (100 M-row squared-loss round, same box, profiles/README.md):
-//  * kernels that WRITE per-row results (K1: read y,F,h, write F,r) run 3 % faster when every access carries an
-//    explicit evict_normal policy than with the plain instructions (0.312 vs 0.322 ms, 0.97 vs 0.945 of the copy
-//    peak), while read-only passes lose 4 % with it (K2 0.142 vs 0.137 ms) — so POL is a template flag set per mode;
-//  * on shards whose four arrays are of the order of the 126 MB L2 (10 M rows: 160 MB) marking what the next pass
-//    does not re-read as evict_first keeps r and h resident between the statistics pass and the update: +8 % per
-//    round; on 100 M-row shards the same hints cost 3 %, so they are enabled by size (se_api.cu gbm_args).
+//  * kernels that WRITE per-row results (K1: read y,F,h, write F,r) may carry an explicit evict_normal policy on
+//    every access while read-only passes use the plain instructions — so POL is a template flag set per mode;
+//  * on shards whose four arrays are of the order of the L2, marking what the next pass does not re-read as
+//    evict_first keeps r and h resident between the statistics pass and the update; on shards much larger than the
+//    L2 the hints buy nothing, so they are enabled by size (se_api.cu gbm_args, l2_hint_rows from the device's L2).
 __device__ __forceinline__ uint64_t l2_policy(bool evict_first) {
   uint64_t p;
   if (evict_first) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

@@ -1,4 +1,4 @@
-// se_gbm.cu — GBM inner-loop kernels (sm_100a): pseudo-residuals, line-search evaluation,
+// se_gbm.cu — GBM inner-loop kernels (sm_90a): pseudo-residuals, line-search evaluation,
 // fused prediction update + next-round residual + loss, validation loss.
 //
 // Reference (fp64, Spark RDD closures): regression/GBMRegressor.scala:368-385 (residuals),
@@ -22,8 +22,8 @@ namespace {
 constexpr int U_SCALAR = 4;  // float4 groups per thread per tile (cheap losses: pure streaming)
 
 // Transcendental-heavy losses spend ~30 instructions per row: with U = 4 (76-80 registers, 3 CTAs/SM) the
-// warps of an SM bunch up in the same load-then-compute phase (ncu: 0.66 eligible warps/cycle, 47 % issue
-// utilisation, 61 % DRAM).  They use U = 2 and a 4-CTA/SM register budget (64 regs, no spills) instead: 32 warps per SM in
+// warps of an SM bunch up in the same load-then-compute phase (few eligible warps per cycle, low issue
+// utilisation and DRAM throughput).  They use U = 2 and a 4-CTA/SM register budget (64 regs, no spills) instead: 32 warps per SM in
 // different phases overlap one warp's math with another's loads.
 template <int LOSS>
 struct LossTune {
@@ -98,8 +98,7 @@ __global__ void __launch_bounds__(kBlock, LossTune<LOSS>::kMinCtas) gbm_scalar_k
   };
 
   // tiles are interleaved across CTAs: at any moment the grid works inside one compact moving window of
-  // each array (measured ~4 % faster at 100 M rows than one contiguous region per CTA, which keeps
-  // thousands of distinct 2 MB pages live at once)
+  // each array (one contiguous region per CTA instead keeps thousands of distinct 2 MB pages live at once)
   for (int64_t t0 = blockIdx.x; t0 < ntiles; t0 += gridDim.x) {
     const int64_t t = a.reverse ? (ntiles - 1 - t0) : t0;
     const int64_t base = t * tile + threadIdx.x;
@@ -290,8 +289,8 @@ __global__ void __launch_bounds__(kBlock) gbm_logloss_kernel(const GbmArgs a) {
     // ---- per-row math
     float outR[KMAX][VEC], outW[KMAX][VEC];
     // the VEC rows of a group are summed in fp32 and converted to fp64 once per group: the float->double
-    // conversions share the SFU pipe with ex2/lg2/rcp (ncu, K = 2 eval: 46 % XU utilisation, 101 instructions per row
-    // with one conversion per row and class)
+    // conversions share the SFU pipe with ex2/lg2/rcp (one conversion per row and class made the SFU pipe
+    // the busiest)
     float g_loss = 0.f, g_cls[KMAX];
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) g_cls[k] = 0.f;
@@ -408,9 +407,8 @@ __global__ void sq_alpha_kernel(const double* stats, double* out) {
 }
 
 // Persistent grid: a multiple of the SM count, up to `ctas_per_sm` CTAs per SM, but never so many that a CTA
-// gets fewer than ~8 work units (tiles).  Measured on B200 (squared loss): at 100 M rows 8 CTAs/SM beats 2
-// (K1 0.97 vs 0.93 of the HBM peak: later waves rebalance the tail), at 10 M rows 2 beats 8 (0.82 vs 0.77:
-// fewer, longer-lived CTAs amortise ramp-up and the per-CTA reduction epilogue).
+// gets fewer than ~8 work units (tiles): on large inputs later waves rebalance the tail, on small ones fewer,
+// longer-lived CTAs amortise ramp-up and the per-CTA reduction epilogue.
 inline int grid_for(int64_t work_items, int64_t per_cta, int ctas_per_sm, int sms) {
   int64_t units = (work_items + per_cta - 1) / per_cta;
   if (units < 1) units = 1;
@@ -505,7 +503,7 @@ cudaError_t launch_gbm(int loss, int mode, const GbmArgs& a, int ctas_per_sm, in
     return v < 2 ? 2 : (v > 9 ? 9 : v);  // the register kernels exist for K <= 8 only
   }();
   if (K >= staged_min_k) return launch_gbm_logloss_tiled(mode, a, sms, st);
-  if (ctas_per_sm > 4) ctas_per_sm = 4;  // register-resident K <= 4 kernels: 4 CTAs/SM measured best
+  if (ctas_per_sm > 4) ctas_per_sm = 4;  // register-resident K <= 4 kernels
   if (K <= 2) return launch_logloss_k<2, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
   if (K <= 4) return launch_logloss_k<4, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
   return launch_logloss_k<8, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);

@@ -1,20 +1,20 @@
-// se_gbm_fused.cu — whole-round and whole-line-search kernels (sm_100a): the per-round fixed costs (kernel
+// se_gbm_fused.cu — whole-round and whole-line-search kernels (sm_90a): the per-round fixed costs (kernel
 // launches, host round trips between the line search and the update, one cross-GPU exchange per launch) are what
-// bounds small row shards — exactly the shards STRONG scaling produces (100 M rows / 8 GPUs = 12.5 M rows = a 53 us
-// round at the HBM roofline).  Two cooperative (co-resident, persistent) kernels remove them:
+// bounds small row shards — exactly the shards STRONG scaling produces (100 M rows / 8 GPUs = 12.5 M rows per GPU,
+// tens of microseconds per round at the HBM roofline).  Two cooperative (co-resident, persistent) kernels remove them:
 //
 //  * gbm_round_sq_fused_kernel — a complete squared-loss boosting round (regression/GBMRegressor.scala:398-442 +
 //    :368-385 of the reference) in ONE launch: statistics pass (8 B/row) -> last CTA folds the partials, sums them
 //    across GPUs over peer memory and runs Brent (se_brent.h, the same template as the host line search) -> the step
 //    is published through an acquire/release flag while every other CTA already has the first update tile's loads in
 //    flight -> fused F update + next pseudo-residuals + loss (20 B/row), walking the tiles in the opposite direction
-//    so that the statistics pass's tail of h is still in the 126 MB L2 -> loss reduction + second exchange + host
+//    so that the statistics pass's tail of h is still in the L2 -> loss reduction + second exchange + host
 //    mirror.  1 launch, 0 host round trips inside the round, the Brent latency hidden behind the preloads.
 //
 //  * gbm_linesearch_persist_kernel — Brent's <= MaxEval evaluations of the line-search objective
 //    (boosting/GBMLoss.scala:50-74 through RDDLossFunction; GBMRegressor.scala:408-421) for the non-squared scalar
 //    losses in ONE launch: worker CTAs own a fixed set of tiles, keep the first of them in SHARED MEMORY for the whole
-//    search (148 SMs x ~190 KB = 28 MB that never touch HBM again) and stream the rest (the caller marks the packed
+//    search (132 SMs x ~190 KB = 25 MB on an H100 that never touch HBM again) and stream the rest (the caller marks the packed
 //    view as L2-persisting); a coordinator warp folds the per-CTA partials in a fixed order, performs the cross-GPU
 //    sum, advances Brent and publishes the next abscissa.  The first evaluation of the binary losses also BUILDS the
 //    signed view u = (2y-1)F, v = (2y-1)h (exact sign flips: later evaluations read 8 B/row and are bit-identical to
@@ -189,7 +189,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   int64_t i = cnt - 1;
   if (i >= 0) load_tile(i);  // in flight while the last CTA reduces, exchanges and runs Brent
   if (threadIdx.x == 0) {
-    // The wait (partials fold + cross-GPU exchange + ~30 dependent fp64 Brent iterations: 10-20 us) is turned into
+    // The wait (partials fold + cross-GPU exchange + ~30 dependent fp64 Brent iterations) is turned into
     // useful HBM time: every CTA pulls the y and F ranges of its next update tiles into the L2 with bulk prefetches
     // (one instruction per 16 KB), bounded so that the whole grid stays within a.prefetch_tiles tiles per CTA.
     int64_t pf = i - 1;
@@ -620,8 +620,7 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
   const int64_t per_cta = (ntiles + workers - 1) / workers;
   // ring stages for the tiles that do not stay resident: none when every tile of a worker fits in shared memory,
   // else cfg.ring as far as the budget allows; what is left of the budget holds resident tiles.  Off by default:
-  // measured (profiles/r02_ls_ring.json) the ring does not beat the register prefetch at 4 CTAs/SM (73.6 vs 75.3 us
-  // per 50 M-row pass) and costs resident tiles on small shards.
+  // the ring costs resident tiles on small shards.
   const int64_t tb = T::kTileBytes;
   int ring = 0;
   if (per_cta > (cfg.resident ? budget / tb : 0)) {

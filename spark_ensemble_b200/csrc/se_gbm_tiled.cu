@@ -14,8 +14,8 @@
 //       classes k ≡ w (mod 2), a lane sums eight rows of the tile per class and keeps one fp64 accumulator per
 //       class in registers, so there are no per-tile shuffles and no per-row class registers.
 // The one-hot term is folded in shared memory before pass B (e_y <- e_y - s, so that e_y / s = softmax_y - 1).
-// About 8 instructions per (row, class) instead of ~37 for the one-row-per-thread form (ncu: 1500 instr/row at
-// K = 26), which was issue-bound at 0.36 of the HBM roofline in eval mode.
+// About 8 instructions per (row, class) instead of ~37 for the one-row-per-thread form which was
+// issue-bound, far from the HBM roofline in eval mode.
 #include <stdlib.h>
 
 #include "se_kernels.h"
@@ -320,7 +320,7 @@ cudaError_t launch_tiled_k(int mode, const GbmArgs& a, int sms, cudaStream_t st)
   }
   const size_t stage_bytes = (size_t)(read_h ? 2 : 1) * K * kTR * sizeof(float);
   // one stage: with shared memory bounding occupancy, more resident CTAs beat double buffering at every K
-  // (measured: K = 8 eval 0.86 vs 0.80 of the roofline, K = 26 eval 0.79 vs 0.55); SE_LOGLOSS_STAGES=2 for experiments
+  // SE_LOGLOSS_STAGES=2 for experiments
   static const int forced_stages = [] { const char* s = getenv("SE_LOGLOSS_STAGES"); return s ? atoi(s) : 0; }();
   const int stages = forced_stages >= 2 ? 2 : 1;
   GbmArgs args = a;
@@ -361,7 +361,7 @@ cudaError_t launch_tiled_k(int mode, const GbmArgs& a, int sms, cudaStream_t st)
 cudaError_t launch_gbm_logloss_tiled(int mode, const GbmArgs& a, int sms, cudaStream_t st) {
   const int K = a.dim;
   if (K < 1 || K > kMaxDim) return cudaErrorInvalidValue;
-  // two warps per CTA (256-row tiles) measured best: one warp / 128 rows loses 2-15 % in the per-class modes
+  // two warps per CTA (256-row tiles)
   if (K <= 8) return launch_tiled_k<8, 2>(mode, a, sms, st);
   if (K <= 16) return launch_tiled_k<16, 2>(mode, a, sms, st);
   if (K <= 32) return launch_tiled_k<32, 2>(mode, a, sms, st);

@@ -1,4 +1,4 @@
-// se_kernels.h — host-callable launchers of the sm_100a kernels (internal to libse_b200.so).
+// se_kernels.h — host-callable launchers of the sm_90a kernels (internal to libse_b200.so).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -47,7 +47,7 @@ struct GbmArgs {
   int stats_from_r = 0;  // squared-loss statistics read the current residual slot r = y - F (8 B/row) instead of y, F (12 B/row)
   int l2_hints = 0; // L2-sized shard: evict_first for the arrays the next pass does not re-read (se_common.cuh)
   int reverse = 0; // walk the tiles from the end: consecutive passes alternate direction so the tail of one
-                   // pass (still in the 126 MB L2) is the head of the next
+                   // pass (still in the L2) is the head of the next
   RedWs ws{};
 };
 

@@ -91,7 +91,7 @@ __global__ void __launch_bounds__(kBlock) tree_predict_kernel(const TreeArgs a) 
 }
 
 // ------------------------------------------------------------------ binned feature matrix (uint8) and its tree walk
-// ncu on the fp32 walk above (round 1): 174 B/row of DRAM traffic for a depth-6 tree whose algorithmic need is 24 B/row
+// The fp32 walk above moves several times the DRAM traffic a depth-6 tree needs (24 B/row)
 // — once the rows of a warp diverge every 4-byte gather drags a whole 32-byte sector (8 rows) in.  Decision trees only
 // COMPARE features with thresholds, and Spark's trees draw every threshold of a feature from the <= maxBins - 1 split
 // candidates `findSplits` computes once per fit: so X can be replaced, for the walk, by the RANK of each value among the
@@ -132,9 +132,8 @@ __global__ void __launch_bounds__(kBlock) bin_columns_kernel(const BinArgs a) {
 
 // Packed node (16 bytes, one 128-bit shared-memory read per row and level): x,y = byte offset of the node's column
 // in X8 (column * ld8, 64 bit); z = bin threshold | leaf << 31; w = left | right << 16.
-// ncu on the first version (two 8-byte node reads per row and level, 64-bit multiply for the column offset): 39
-// instructions per row and level, 45 % issue utilisation at 49 % occupancy — the walk was issue-bound, not DRAM-bound
-// (52 % of peak).
+// The first version (two 8-byte node reads per row and level, 64-bit multiply for the column offset) was
+// issue-bound, not DRAM-bound.
 template <int W, int MINB>  // W words of 4 consecutive rows per thread (independent gather chains), MINB CTAs per SM
 __global__ void __launch_bounds__(kBlock, MINB) tree_predict_binned_kernel(const TreeArgs a, const uint8_t* __restrict__ X8,
                                                                            const uint4* __restrict__ nodes) {
@@ -207,11 +206,11 @@ __global__ void __launch_bounds__(kBlock, MINB) tree_predict_binned_kernel(const
 // ---- shallow trees (<= 64 internal nodes, e.g. depth <= 6): evaluate EVERY node's comparison, then walk in registers.
 // The walk above fetches, per 32 consecutive rows, one 32-byte sector per DISTINCT node its rows sit on at each level:
 // 1 + 2 + 4 + ... sectors, i.e. about one byte per row and internal node — exactly what reading the node's column for
-// every row costs (ncu: 62 B/row for 63 internal nodes).  Same bytes, but here they arrive as fully coalesced,
+// every row costs (one byte per row and internal node).  Same bytes, but here they arrive as fully coalesced,
 // INDEPENDENT vector loads (no level-to-level dependency, one wavefront per 128 rows instead of one per sector), four
 // byte-compares at a time in SWAR form, and the per-row walk reads its decision bits from shared memory.
 //   bit j of a row = rank(x[col_j]) <= t_j; internal node ordinals j are assigned in node order by warp 0.
-constexpr int kTreeMaskWords = 4;  // measured at 100 M x 128, depth 6: 1.51 / 1.22 / 1.15 ms for 1 / 2 / 4 words (walk: 1.47)
+constexpr int kTreeMaskWords = 4;
 template <int RW> struct MaskVec;
 template <> struct MaskVec<1> { using type = uint32_t; };
 template <> struct MaskVec<2> { using type = uint2; };
@@ -321,7 +320,7 @@ __global__ void __launch_bounds__(kBlock, 4) tree_predict_mask_kernel(const Tree
 
 // ---- a forest in one pass -----------------------------------------------------------------------------------------
 // transform() of a tree ensemble evaluated tree by tree reads each tree's columns of the rank matrix again (one byte per
-// row and internal node, 0.73 ms per depth-5 tree and 100 M rows) and needs an [M][n] prediction array for the
+// row and internal node) and needs an [M][n] prediction array for the
 // aggregation kernel.  Here a CTA stages a 256-row tile of the ranks of every column the forest uses in shared memory
 // (C x 256 bytes), keeps the packed trees next to it, and every thread walks ALL trees for its row out of shared
 // memory, two trees interleaved, accumulating w_t · leaf in fp64 in model order like the reference's loop: the rank

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's regression ensembles for the hot path:
 GBMRegressor / GBMRegressionModel (regression/GBMRegressor.scala) and BaggingRegressionModel.predict
 (regression/BaggingRegressor.scala:221-228) — same class names, UID prefixes, Params and defaults; the
-per-row RDD closures of train()/predict() are replaced by calls into libse_b200 (sm_100a kernels).
+per-row RDD closures of train()/predict() are replaced by calls into libse_b200 (sm_90a kernels).
 
 On a JVM host the same substitution is made in Scala (scala/ + jni/se_jni.cpp, see INTEGRATION.md).
 """

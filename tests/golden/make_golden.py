@@ -1,10 +1,10 @@
-"""Generates the committed fixtures under tests/golden/ (run in the build container only: reads the
-reference's LIBSVM data files, which do not exist on the GPU box).
+"""Generates the committed fixtures under tests/golden/ from the reference's LIBSVM data files (the tests
+read only the committed fixtures).
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <reference checkout>/data
 
 * cpusmall.npz / letter.npz / adult8k.npz — the reference's own test datasets
-  (/root/reference/data/*, loaded at e.g. test/regression/GBMRegressorSuite.scala:54) as compact arrays.
+  (data/* of the reference repository, loaded at e.g. test/regression/GBMRegressorSuite.scala:54) as compact arrays.
 * gbm_cpusmall_oracle.json — BASELINE config 1 (GBMRegressor, cpusmall, 20 rounds, squared loss,
   DecisionTree depth 5) run through the ORACLE-driven reference control flow (tests/ref_fit.py): per-round
   alpha, train loss and a prediction checksum.  These are oracle outputs, not outputs of the Scala
@@ -19,7 +19,7 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-REF = "/root/reference/data"
+REF = sys.argv[1] if len(sys.argv) > 1 else "data"
 
 
 def read_libsvm(path, d):

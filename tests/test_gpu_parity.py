@@ -1146,7 +1146,7 @@ def test_options_roundtrip(ctx):
 def test_bad_labels_fail_loudly(ctx, rng, K, bad):
     """A label that is not an integer class index in [0, K) makes the reference throw on the JVM
     (GBMLoss.scala:200-204 `res(label.toInt) = 1.0`; Classifier.validateLabel).  Here: SE_ERR_ARG from the call that
-    observes it, never an out-of-bounds access (run under compute-sanitizer in profiles/r02_sanitizer.md), and the
+    observes it, never an out-of-bounds access, and the
     context stays usable."""
     from spark_ensemble_b200 import _native as N
     n = 5003

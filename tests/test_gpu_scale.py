@@ -1,5 +1,5 @@
 """Parity at BASELINE.json's shard sizes (VERDICT r1 'What's weak' 2): the code paths that only exist at scale —
-multi-CTA-per-SM persistent grids, the >16 M-row L2 policy, element offsets beyond 2^31 in [K][n] arrays, 32-bit TMA
+multi-CTA-per-SM persistent grids, the L2 policy of shards larger than the L2, element offsets beyond 2^31 in [K][n] arrays, 32-bit TMA
 tile coordinates near their range, M = 512 fp64 batch folding — checked against the fp64 OpenMP oracle evaluated in
 row chunks on data generated on the device and downloaded chunk by chunk.
 
@@ -91,7 +91,7 @@ def test_c2_squared_round_10m(ctx, orc):
 
 @pytest.mark.parametrize("name,dim", [("bernoulli", 1), ("logloss", 2)])
 def test_c3_binary_50m(ctx, orc, name, dim):
-    """Config 3 shard: 50 M rows (8 CTAs/SM grids, no L2 hints above 16 M rows): line-search objective and
+    """Config 3 shard: 50 M rows (8 CTAs/SM grids, no L2 hints at this size): line-search objective and
     gradient, the device line search (bernoulli), fused update + residuals + loss."""
     from spark_ensemble_b200 import _native as N
     n = 50_000_000

@@ -2,7 +2,7 @@
 BrentOptimizer, Spark's ml.impl.Utils (log1pExp / softmax / EPSILON), MurmurHash3 + XORShiftRandom — from their
 PUBLISHED test suites / tables (tests/golden/thirdparty_*.json hold the citations; make_thirdparty_golden.py
 re-derives every expectation).  This is what moves the oracle from "pinned by properties" to "pinned by published
-vectors" for the pieces whose source is not under /root/reference."""
+vectors" for the pieces whose source is not part of the reference repository."""
 import ctypes
 import json
 import math
