@@ -303,7 +303,8 @@ SE_API int se_spark_bernoulli_sample(int64_t seed, double fraction, int64_t n, i
  * The arrays must describe a TREE rooted at node 0: a node reached twice (cycle / shared child) fails with
  * SE_ERR_ARG before anything is launched.  Thresholds: the device compares the fp32 feature with the fp32 threshold;
  * pass the LARGEST float <= the fp64 threshold (round toward -inf: learners.py / FlatTree do) — then `x <= thr`
- * decides exactly like the JVM for every feature value that is itself a float (which is what HBM holds).  A fp64
+ * decides exactly like the JVM for every feature value that is itself a float (which is what HBM holds), NaN, +-inf,
+ * +-0 and denormals included: NaN goes right at every node, on the fp32 walk and on the uint8 rank matrix alike.  A fp64
  * feature value strictly between that float and the fp64 threshold can still change sides: the resident feature
  * matrix is fp32 by contract (north_star), so transform with the model on the same fp32 features. */
 SE_API int se_tree_predict(se_ctx* ctx, int which, int n_nodes, const int32_t* feature,

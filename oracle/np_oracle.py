@@ -87,6 +87,34 @@ def logloss_parts(y_idx, P):
     return lo, s - onehot, s * (1.0 - s)
 
 
+def logloss_stable(y_idx, P):
+    """P [K][n]. The same (loss[n], grad[K][n], hess[K][n]) as logloss_parts, in a form that keeps full relative
+    precision on well-fitted rows, where the label class leads the others by a wide margin and the loss, the gradient
+    and 1 - softmax_argmax all shrink like exp(-margin):
+        S = Σ_{k != argmax} exp(p_k - m),  loss = log1p(S) + m - p_y,  1 - softmax_argmax = S / (1 + S).
+    The argmax is the first maximum; tied maxima beyond it count in S.  The unshifted form of the reference (and of
+    logloss_parts / se_oracle.c) loses the loss to the rounding of log Σ exp(p_k) once exp(-margin) nears the fp64
+    epsilon of the margin, i.e. from a margin of about 25-30."""
+    K, n = P.shape
+    cols = np.arange(n)
+    am = np.argmax(P, axis=0)
+    m = P[am, cols]
+    E = np.exp(P - m)
+    E[am, cols] = 0.0
+    S = E.sum(axis=0)
+    inv = 1.0 / (1.0 + S)
+    sm = E * inv
+    sm[am, cols] = inv
+    om = S * inv  # 1 - softmax_argmax
+    onehot = np.arange(K)[:, None] == y_idx[None, :]
+    g = sm - onehot
+    top_is_label = am == y_idx
+    g[am[top_is_label], cols[top_is_label]] = -om[top_is_label]
+    hs = sm * (1.0 - sm)
+    hs[am, cols] = sm[am, cols] * om
+    return np.log1p(S) + (m - P[y_idx, cols]), g, hs
+
+
 def linesearch_eval(name, param, y, w, F, h, alpha):
     """(lossSum/weightSum, gradSum/weightSum) with the dim-times loss quirk (GBMLoss.scala:50-74)."""
     alpha = np.atleast_1d(np.asarray(alpha, dtype=np.float64))

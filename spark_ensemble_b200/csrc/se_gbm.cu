@@ -308,7 +308,8 @@ __global__ void __launch_bounds__(kBlock) gbm_logloss_kernel(const GbmArgs a) {
         }
       }
       // log Σ exp(p_k) = m + log1p(Σ_{k != argmax} exp(p_k - m)): the max term is exactly 1 and is kept
-      // out of the sum so a well-fitted row (loss -> 0) keeps full relative precision
+      // out of the sum so a well-fitted row (loss -> 0) keeps full relative precision; so does 1 - softmax of the
+      // argmax class (= srest / (1 + srest)), which the label-class gradient and newton's hessian need
       float srest = 0.f, py = 0.f;
       float ex[KMAX];
 #pragma unroll
@@ -319,17 +320,18 @@ __global__ void __launch_bounds__(kBlock) gbm_logloss_kernel(const GbmArgs a) {
           if (yf == (float)k) py = p[k][e];
         }
       }
-      const float lse = m + log1p_pos(srest);
       const float inv_s = rcp_approx(1.0f + srest);
-      if (T::kSumLoss && in) g_loss += ((MODE == GBM_EVAL) ? cv[e] : 1.0f) * (lse - py);  // -Σ y_k (p_k - lse)  :206-221
+      const float om = srest * inv_s;  // 1 - softmax of the argmax class, without the cancellation of 1 - x
+      if (T::kSumLoss && in) g_loss += ((MODE == GBM_EVAL) ? cv[e] : 1.0f) * ((m - py) + log1p_pos(srest));  // -Σ y_k (p_k - lse)  :206-221
 #pragma unroll
       for (int k = 0; k < KMAX; ++k) {
         if (k < K) {
-          const float sm = ex[k] * inv_s;                    // exp(p_k - lse)
-          const float gk = sm - ((yf == (float)k) ? 1.0f : 0.0f);   // :223-238
+          const bool top = (k == am);
+          const float sm = top ? inv_s : ex[k] * inv_s;      // exp(p_k - lse)
+          const float gk = (yf == (float)k) ? (top ? -om : sm - 1.0f) : sm;  // :223-238
           if (MODE == GBM_EVAL && in) g_cls[k] = fmaf(cv[e] * hh[k][e], gk, g_cls[k]);  // :66-72
           if (T::kNewton) {
-            const float hc = fmaxf(sm * (1.0f - sm), 1e-2f);  // :240-256, GBMClassifier.scala:342
+            const float hc = fmaxf(sm * (top ? om : 1.0f - sm), 1e-2f);  // :240-256, GBMClassifier.scala:342
             outR[k][e] = -gk * rcp_approx(hc);                           // :362
             outW[k][e] = 0.5f * hc * wv[e];                   // :364 (× 1/S_k later)
             if (in) g_cls[k] = fmaf(cv[e], hc, g_cls[k]);

@@ -48,11 +48,12 @@ __global__ void __launch_bounds__(32) gbm_logloss_generic_kernel(const GbmArgs a
     const float w = (T::kNewton && has_w) ? a.w[ii] : 1.0f;
     // sweep 1: p_k = F_k + coef_k h_k (GBMLoss.scala:56-59), running max (first maximum), F update
     float m = -INFINITY, py = 0.f;
+    int am = 0;
     for (int k = 0; k < K; ++k) {
       float p = a.F[(int64_t)k * ld + ii];
       if (T::kReadH) p = fmaf(__ldg(ga.coef + k), a.h[(int64_t)k * ld + ii], p);
       if (T::kWriteF && in) a.F[(int64_t)k * ld + ii] = p;
-      m = fmaxf(m, p);
+      if (p > m) m = p, am = k;
       if (k == yi) py = p;
     }
     auto pk = [&](int k) -> float {  // p_k again: from the updated F, or recomputed (same fma, same value)
@@ -60,22 +61,27 @@ __global__ void __launch_bounds__(32) gbm_logloss_generic_kernel(const GbmArgs a
       if (T::kReadH && !(T::kWriteF && in)) p = fmaf(__ldg(ga.coef + k), a.h[(int64_t)k * ld + ii], p);
       return p;
     };
-    // sweep 2: Σ exp(p_k - m) — shifted log-sum-exp (identical wherever the reference's unshifted form is finite)
-    float s = 0.f;
-    for (int k = 0; k < K; ++k) s += ex2_approx((pk(k) - m) * kLog2e);
-    const float inv_s = rcp_approx(s);
+    // sweep 2: Σ_{k != argmax} exp(p_k - m) — shifted log-sum-exp (identical wherever the reference's unshifted form is
+    // finite) with the max term, exactly 1, kept out of the sum: a well-fitted row keeps full relative precision in its
+    // loss and in 1 - softmax_argmax
+    float srest = 0.f;
+    for (int k = 0; k < K; ++k)
+      if (k != am) srest += ex2_approx((pk(k) - m) * kLog2e);
+    const float inv_s = rcp_approx(1.0f + srest);
+    const float om = srest * inv_s;  // 1 - softmax of the argmax class
     if (T::kSumLoss && in) {
-      const float l = (m - py) + log_fast(s);  // -Σ y_k (p_k - lse)  (:206-221)
+      const float l = (m - py) + log1p_pos(srest);  // -Σ y_k (p_k - lse)  (:206-221)
       loss_acc += (double)(((MODE == GBM_EVAL) ? c : 1.0f) * l);
     }
     // sweep 3: gradients / outputs / per-class sums
     if (T::kWriteR || T::kPerClass) {
       for (int k = 0; k < K; ++k) {
-        const float sm = ex2_approx((pk(k) - m) * kLog2e) * inv_s;   // exp(p_k - lse)
-        const float gk = sm - ((k == yi) ? 1.0f : 0.0f);             // :223-238
+        const bool top = (k == am);
+        const float sm = top ? inv_s : ex2_approx((pk(k) - m) * kLog2e) * inv_s;   // exp(p_k - lse)
+        const float gk = (k == yi) ? (top ? -om : sm - 1.0f) : sm;                // :223-238
         float term = 0.f;
         if (T::kNewton) {
-          const float hc = fmaxf(sm * (1.0f - sm), 1e-2f);           // :240-256, GBMClassifier.scala:342
+          const float hc = fmaxf(sm * (top ? om : 1.0f - sm), 1e-2f);             // :240-256, GBMClassifier.scala:342
           if (in) {
             a.r[(int64_t)k * ld + ii] = -gk * rcp_approx(hc);        // :362
             a.wout[(int64_t)k * ld + ii] = 0.5f * hc * w;            // :364 (x 1/S_k when it leaves the device)

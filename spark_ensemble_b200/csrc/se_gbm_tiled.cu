@@ -7,13 +7,14 @@
 // over the class-major [K][ld] array, so a whole stage arrives with ONE `cp.async.bulk.tensor.2d` per array
 // (rows past n are zero-filled by the TMA unit), completion counted on an mbarrier.  A thread owns four
 // consecutive rows and walks the classes with 128-bit shared-memory accesses:
-//   A1  p = F + c_k h (written back into the F slot; F' stored to HBM when the mode updates F), running max
-//   A2  e = 2^((p - m) log2 e) written back over p, s = Σ e                       (one MUFU per row and class)
+//   A1  p = F + c_k h (written back into the F slot; F' stored to HBM when the mode updates F), running max / argmax
+//   A2  e = 2^((p - m) log2 e) written back over p, srest = Σ_{k != argmax} e      (one MUFU per row and class)
 //   B   row-wise outputs (residuals / newton weights) with 128-bit global stores, or — for the line-search
 //       gradient Σ_i h_ik (softmax_ik - [y_i = k]) and newton's Σ_i hc_ik — a CLASS-wise sweep: warp w owns the
 //       classes k ≡ w (mod 2), a lane sums eight rows of the tile per class and keeps one fp64 accumulator per
 //       class in registers, so there are no per-tile shuffles and no per-row class registers.
-// The one-hot term is folded in shared memory before pass B (e_y <- e_y - s, so that e_y / s = softmax_y - 1).
+// The one-hot term is folded in shared memory before pass B (e_y <- e_y - s, or -srest when y is the argmax, so that
+// e_y / s = softmax_y - 1 keeps full relative precision on well-fitted rows).
 // About 8 instructions per (row, class) instead of ~37 for the one-row-per-thread form which was
 // issue-bound, far from the HBM roofline in eval mode.
 #include <stdlib.h>
@@ -118,8 +119,9 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
     float* sF = stage_base + (size_t)stage * stage_floats + 4 * tid;
     const float* sH = sF + K * kTR;
 
-    // ---- A1: p = F + c_k h (GBMLoss.scala:56-59), running max; p replaces F in shared memory
+    // ---- A1: p = F + c_k h (GBMLoss.scala:56-59), running max and argmax (first maximum); p replaces F in shared memory
     float4 m4 = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+    int am[4] = {0, 0, 0, 0};
 #pragma unroll 2
     for (int k = 0; k < K; ++k) {
       float4 p = lds4(sF + k * kTR);
@@ -139,14 +141,18 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
             if (in[j]) g[j] = f4at(p, j);
         }
       }
-      m4.x = fmaxf(m4.x, p.x), m4.y = fmaxf(m4.y, p.y), m4.z = fmaxf(m4.z, p.z), m4.w = fmaxf(m4.w, p.w);
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (f4at(p, j) > f4at(m4, j)) f4at(m4, j) = f4at(p, j), am[j] = k;
     }
     float py[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) py[j] = sF[yi[j] * kTR + j];
 
-    // ---- A2: e = exp(p - m) (the max term is exactly 1), s = Σ e; e replaces p when pass B needs it
-    float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    // ---- A2: e = exp(p - m), srest = Σ_{k != argmax} e (the max term, exactly 1, is kept out of the sum so that a
+    // well-fitted row keeps full relative precision in its loss and in 1 - softmax_argmax); e replaces p when pass B
+    // needs it
+    float4 r4 = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll 2
     for (int k = 0; k < K; ++k) {
       const float4 p = lds4(sF + k * kTR);
@@ -154,20 +160,25 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
       e.x = ex2_approx((p.x - m4.x) * kLog2e), e.y = ex2_approx((p.y - m4.y) * kLog2e);
       e.z = ex2_approx((p.z - m4.z) * kLog2e), e.w = ex2_approx((p.w - m4.w) * kLog2e);
       if (T::kKeepE) sts4(sF + k * kTR, e);
-      s4.x += e.x, s4.y += e.y, s4.z += e.z, s4.w += e.w;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) f4at(r4, j) += (k == am[j]) ? 0.f : f4at(e, j);
     }
     float inv_s[4];
     {
       float lsum = 0.f;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const float s = f4at(s4, j);
-        inv_s[j] = rcp_approx(s);
-        // log Σ exp(p_k) - p_y = (m - p_y) + log1p(s - 1), s >= 1                     (GBMLoss.scala:206-221)
-        const float l = (f4at(m4, j) - py[j]) + log1p_pos(s - 1.0f);
+        const float srest = f4at(r4, j);
+        inv_s[j] = rcp_approx(1.0f + srest);
+        // log Σ exp(p_k) - p_y = (m - p_y) + log1p(srest)                                 (GBMLoss.scala:206-221)
+        const float l = (f4at(m4, j) - py[j]) + log1p_pos(srest);
         lsum += in[j] ? ((MODE == GBM_EVAL) ? f4at(c4, j) * l : l) : 0.f;
-        // one-hot folded into the exponentials: (e_y - s)/s = softmax_y - 1                       (:223-238)
-        if (T::kKeepE && !T::kNewton) sF[yi[j] * kTR + j] -= s;
+        // one-hot folded into the exponentials so that e_y / s = softmax_y - 1 (:223-238): -srest when y is the
+        // argmax, e_y - s otherwise (|e_y - s| >= 1: no cancellation)
+        if (T::kKeepE && !T::kNewton) {
+          float& ey = sF[yi[j] * kTR + j];
+          ey = (yi[j] == am[j]) ? -srest : ey - (1.0f + srest);
+        }
       }
       if (T::kSumLoss) acc_loss += (double)lsum;
     }
@@ -205,9 +216,11 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
         float4 rr, ww, hh;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          const float sm = f4at(e, j) * inv_s[j];
-          const float gk = sm - ((k == yi[j]) ? 1.0f : 0.0f);
-          const float hc = fmaxf(sm * (1.0f - sm), 1e-2f);
+          const bool top = (k == am[j]);
+          const float sm = top ? inv_s[j] : f4at(e, j) * inv_s[j];
+          const float om = f4at(r4, j) * inv_s[j];  // 1 - softmax of the argmax class
+          const float gk = (k == yi[j]) ? (top ? -om : sm - 1.0f) : sm;
+          const float hc = fmaxf(sm * (top ? om : 1.0f - sm), 1e-2f);
           f4at(rr, j) = -gk * rcp_approx(hc);
           f4at(ww, j) = 0.5f * hc * f4at(w4, j);
           f4at(hh, j) = f4at(c4, j) * hc;

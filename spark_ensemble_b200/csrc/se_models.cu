@@ -119,11 +119,13 @@ __global__ void __launch_bounds__(kBlock) bin_columns_kernel(const BinArgs a) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const float xv = f4at(v, e);
-      // rank = number of edges strictly below xv (NaN ranks 0... Spark sends NaN/missing nowhere: not supported)
+      // rank = number of edges strictly below xv.  NaN compares false with every edge: it ranks 255, above every node's
+      // bin threshold (<= 254), so it goes right at every node like `x <= t` does in the fp32 walk and on the JVM
       int lo = 0;
 #pragma unroll
       for (int step = 128; step > 0; step >>= 1)
         if (lo + step <= 256 && s_edge[lo + step - 1] < xv) lo += step;
+      if (isnan(xv)) lo = 255;
       word |= (uint32_t)(lo > 255 ? 255 : lo) << (8 * e);
     }
     *reinterpret_cast<uint32_t*>(out + 4 * g) = word;

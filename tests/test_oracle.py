@@ -83,6 +83,66 @@ def test_linesearch_eval_matches_numpy(oracle, rng, name, weighted):
     np.testing.assert_allclose(gc, gn, rtol=1e-11, atol=1e-14)
 
 
+def _fitted_logloss_rows(rng, K, n, margin):
+    """Label class at +margin over N(0, 0.5) classes: the late-round regime of a boosted classifier."""
+    y = rng.integers(0, K, n)
+    F = rng.normal(0.0, 0.5, (K, n))
+    F[y, np.arange(n)] += margin
+    return y, F
+
+
+@pytest.mark.parametrize("K", [2, 9, 100])
+def test_logloss_stable_form_and_where_the_unshifted_oracle_departs(oracle, rng, K):
+    """The stable fp64 LogLoss of np_oracle (max term kept out of the exp-sum) is the reference the GPU tests use on
+    well-fitted rows.  Up to a margin of 20 the C oracle's unshifted form (the reference's arithmetic) agrees with it
+    to 1e-6 on the mean loss and the line-search sums, and on every residual up to a margin of 16; from a margin of
+    about 30 the unshifted form itself loses the loss and the label-class gradient to the rounding of log Σ exp(p_k).
+    That is why the GPU tests stop at a margin of 20."""
+    n = 4000
+    for margin in (0, 4, 8, 12, 16, 20, 30, 40):
+        y, F = _fitted_logloss_rows(rng, K, n, margin)
+        yf = y.astype(np.float64)
+        ls, gs, hs = NP.logloss_stable(y, F)
+        lu, gu, hu = NP.logloss_parts(y, F)
+        lc = oracle.mean_loss(O.LOGLOSS, 0.0, K, yf, F)
+        rc, _, _ = oracle.pseudo_residuals(O.LOGLOSS, 0.0, K, yf, None, F, False)
+        rel_loss = abs(lc - ls.mean()) / ls.mean()
+        rel_res = float(np.max(np.abs(rc + gs) / np.abs(gs)))
+        if margin <= 20:
+            assert rel_loss <= 1e-6, (margin, rel_loss)
+            h = np.abs(gs) * rng.uniform(0.5, 1.5, (K, n))       # a direction along the residual: no cancellation
+            lsum, gsum = oracle.linesearch_eval(O.LOGLOSS, 0.0, yf, None, F, h, np.zeros(K))
+            assert lsum == pytest.approx(K * ls.mean(), rel=1e-6)
+            np.testing.assert_allclose(gsum, (h * gs).sum(axis=1) / n, rtol=1e-6)
+            assert lu.mean() == pytest.approx(lc, rel=1e-12)      # the numpy restatement of the unshifted form
+        if margin <= 16:
+            assert rel_res <= 1e-6, (margin, rel_res)
+            np.testing.assert_allclose(hu, hs, rtol=1e-6)
+        if margin == 30:
+            assert rel_res > 1e-4, rel_res                         # label-class gradient: 1 - softmax cancels in fp64
+        if margin == 40:
+            assert rel_loss > 0.5, rel_loss                        # log Σ exp(p_k) rounds to m: the loss is lost
+        # the stable form itself: loss = log1p(S) + m - p_y > 0, gradients of a row sum to 0 to its own precision
+        assert np.all(ls >= 0)
+        assert np.all(np.abs(gs.sum(axis=0)) <= 1e-15 * np.abs(gs).sum(axis=0) * K)
+
+
+def test_logloss_stable_ties_and_non_argmax_labels():
+    """Tied maxima count in S beyond the first; a label that is not the argmax keeps its O(margin) loss."""
+    P = np.array([[3.0, 0.0, 0.0], [3.0, 25.0, 0.0], [-1.0, 0.0, 25.0]])
+    y = np.array([1, 0, 2])
+    lo, g, hs = NP.logloss_stable(y, P)
+    lu, gu, hu = NP.logloss_parts(y, P)
+    np.testing.assert_allclose(lo[:2], lu[:2], rtol=1e-14)
+    np.testing.assert_allclose(g[:, 0], gu[:, 0], rtol=1e-14)
+    assert lo[0] == pytest.approx(np.log(2.0 + np.exp(-4.0)), rel=1e-15)
+    assert lo[1] == pytest.approx(25.0 + np.log1p(2.0 * np.exp(-25.0)), rel=1e-15)
+    assert lo[2] == pytest.approx(np.log1p(np.exp(-25.0) + np.exp(-25.0)), rel=1e-14)
+    s = 2.0 * np.exp(-25.0)
+    assert g[2, 2] == pytest.approx(-s / (1.0 + s), rel=1e-14)
+    assert hs[2, 2] == pytest.approx(s / (1.0 + s) ** 2, rel=1e-14)
+
+
 def test_logloss_loss_counted_dim_times(oracle, rng):
     """Reference quirk (GBMLoss.scala:60-64): lossSum accumulates loss `dim` times per row."""
     n, K = 100, 4
