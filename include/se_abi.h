@@ -65,7 +65,8 @@ enum se_loss {
 enum se_slot {
   SE_SLOT_Y = 0,      /* [n]        labels (Instance.label)                                   */
   SE_SLOT_W = 1,      /* [n]        instance weights (Instance.weight); absent => 1.0          */
-  SE_SLOT_F = 2,      /* [dim][n]   running predictions  (GBMRegressor.scala:313, GBMClassifier.scala:294) */
+  SE_SLOT_F = 2,      /* [dim][n]   running predictions  (GBMRegressor.scala:313, GBMClassifier.scala:294);
+                                    held as y - r after a one-launch squared round, see se_gbm_round */
   SE_SLOT_H = 3,      /* [dim][n]   directions = base model outputs this round (:405,:435)     */
   SE_SLOT_R = 4,      /* [dim][n]   pseudo-residuals = base-learner labels (:368-385)          */
   SE_SLOT_WOUT = 5,   /* [dim][n]   base-learner weights (newton: 1/2 h/S w, :379; the device holds 1/2 h w, se_download applies 1/S_dim) */
@@ -225,7 +226,12 @@ SE_API int se_gbm_linesearch_brent(se_ctx* ctx, double lo, double hi, double sta
                             double abs_tol, int max_eval, double* alpha, double* loss, int* n_eval);
 /* One boosting round for dim == 1 in a single call (GBMRegressor.scala:398-442): Brent line search
  * (optimized != 0; else alpha = 1), weight = learning_rate·alpha, then se_gbm_update(weight, flags).
- * Same results as se_gbm_linesearch_brent + se_gbm_update; saves the host round-trips between them. */
+ * Same results as se_gbm_linesearch_brent + se_gbm_update, up to rounding; saves the host round-trips between them.
+ * SE_SLOT_F after a squared-loss round in one launch (fused_round) with SE_UPD_RESIDUAL: the round writes only
+ * R = r - weight·H and F is held as Y - R.  It is rebuilt (F = y - r, then R = y - F) the first time a call reads
+ * SE_SLOT_F, writes SE_SLOT_Y, SE_SLOT_F or SE_SLOT_R, or hands out their device pointer (se_slot_info); reading R,
+ * Y or H does not rebuild it.  The values are what the update computes, up to rounding: r - c·h and y - r instead of
+ * F + c·h and y - F'.  A round that fails with SE_ERR_OPT (MaxEval) leaves F and R as they were. */
 SE_API int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, int max_iter, int flags,
                         double* alpha, double* loss_sum, int* n_eval);
 /* Opt-in fast line search for dim == 1 losses with a hessian (squared, bernoulli, exponential, logcosh): each

@@ -144,6 +144,8 @@ struct se_ctx {
     bool has_w = false;
     bool use_bag = false;
     bool r_current = false;  // SE_SLOT_R holds -g(y, F) of the CURRENT F (squared loss: y - F)
+    bool f_owed = false;     // SE_SLOT_F is stale: its value is y - r (residual-mode fused squared round); settle_f
+                             // rebuilds it.  Implies r_current.
     double wsum = 0.0;
     bool wsum_valid = false;
     double n_global = 0.0, nv_global = 0.0;
@@ -484,6 +486,19 @@ int fetch_scalars(se_ctx* ctx, int off, int count, double* out, int op = kNcclSu
   return check_p2p(ctx);
 }
 
+// The residual-mode fused squared round leaves F owed (gbm.f_owed): rebuild it as y - r before anything reads train F
+// or writes Y, F or R.  R is re-derived from the rebuilt F (y - F), as an eager update would have left it.
+int settle_f(se_ctx* ctx) {
+  if (!ctx->gbm.f_owed) return SE_OK;
+  SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  SE_LAUNCH_T(ctx, SE_KF_OTHER, launch_gbm_settle_f(ctx->slot[SE_SLOT_Y].d, ctx->slot[SE_SLOT_R].d, ctx->slot[SE_SLOT_F].d,
+                                                    ctx->gbm.n, ctx->sms, ctx->stream));
+  ctx->gbm.f_owed = false;
+  return SE_OK;
+}
+
+bool is_yfr(int slot) { return slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R; }
+
 // any write to a feature-matrix slot makes its rank matrix stale
 void touch_slot(se_ctx* ctx, int slot) {
   if (slot == SE_SLOT_Y) ctx->y_state[0] = 0;
@@ -504,6 +519,7 @@ void free_bins(BinState& B) {
 
 int slot_alloc2d(se_ctx* ctx, int slot, int64_t rows, int64_t cols) {
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   touch_slot(ctx, slot);
   SE_REQUIRE(ctx, rows >= 1 && cols >= 0, SE_ERR_ARG, "bad slot shape %lld x %lld", (long long)rows,
              (long long)cols);
@@ -1195,6 +1211,7 @@ int se_slot_free(se_ctx* ctx, int slot) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (ctx->slot[slot].d) SE_CUDA(ctx, cudaFree(ctx->slot[slot].d));
   ctx->slot[slot] = SlotBuf();
@@ -1207,10 +1224,15 @@ int se_slot_info(const se_ctx* ctx, int slot, void** device_ptr, int64_t* count)
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   if (slot < 0 || slot >= SE_NUM_SLOTS) return fail(nullptr, SE_ERR_ARG, "bad slot %d", slot);
   if (device_ptr) {
-    *device_ptr = ctx->slot[slot].d;
-    touch_slot(const_cast<se_ctx*>(ctx), slot);
-    // the caller may write through the raw pointer: drop everything cached about the slot's contents
     se_ctx* mctx = const_cast<se_ctx*>(ctx);
+    // the caller may read or write through the raw pointer: F must hold its value, and everything cached about the
+    // slot's contents is dropped
+    if (is_yfr(slot) && ctx->gbm.f_owed) {
+      SE_TRY(settle_f(mctx));
+      SE_CUDA(mctx, cudaStreamSynchronize(ctx->stream));  // the caller's own stream may touch the slot next
+    }
+    *device_ptr = ctx->slot[slot].d;
+    touch_slot(mctx, slot);
     if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) mctx->gbm.r_current = false;
     if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) mctx->gbm.wsum_valid = false;
   }
@@ -1233,6 +1255,7 @@ int se_upload(se_ctx* ctx, int slot, const float* host, int64_t count, int64_t o
   touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
   if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
   SE_TRY(for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_CUDA(ctx, cudaMemcpyAsync(d, host + done, sizeof(float) * len, cudaMemcpyHostToDevice, ctx->stream));
@@ -1249,6 +1272,7 @@ int se_upload_f64(se_ctx* ctx, int slot, const double* host, int64_t count, int6
   touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
   if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
   // narrow on the host (halves PCIe bytes) through pinned staging, in chunks
   const int64_t chunk = 1 << 22;
@@ -1276,6 +1300,7 @@ int se_upload_rowmajor(se_ctx* ctx, int slot, const float* host, int64_t n_rows,
              "rows [%lld,+%lld) outside the slot's %lld rows", (long long)row_offset, (long long)n_rows, (long long)X.cols);
   if (n_rows == 0) return SE_OK;
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   const int64_t ld = X.rows > 1 ? X.ld : X.cols;
   // ~32 MB chunks, whole rows, multiple of 32 rows
   int64_t chunk_rows = (int64_t)(32u << 20) / ((int64_t)d * (int64_t)sizeof(float));
@@ -1346,6 +1371,7 @@ int se_download(se_ctx* ctx, int slot, float* host, int64_t count, int64_t offse
   if (!ctx || !host) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
   SE_TRY(for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_CUDA(ctx, cudaMemcpyAsync(host + done, d, sizeof(float) * len, cudaMemcpyDeviceToHost, ctx->stream));
     return SE_OK;
@@ -1376,6 +1402,7 @@ int se_fill(se_ctx* ctx, int slot, float value, int64_t count, int64_t offset) {
   touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
   if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
   return for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t, int64_t len) {
     SE_LAUNCH(ctx, launch_fill(d, value, len, ctx->sms, ctx->stream));
@@ -1389,9 +1416,10 @@ int se_copy_slot(se_ctx* ctx, int dst_slot, int src_slot) {
              SE_ERR_ARG, "bad slot");
   const SlotBuf &d = ctx->slot[dst_slot], &s = ctx->slot[src_slot];
   SE_REQUIRE(ctx, d.d && s.d && d.rows == s.rows && d.cols == s.cols, SE_ERR_STATE, "slot shapes differ");
+  SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (is_yfr(dst_slot) || src_slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
   touch_slot(ctx, dst_slot);
   if (dst_slot == SE_SLOT_Y || dst_slot == SE_SLOT_F || dst_slot == SE_SLOT_R) ctx->gbm.r_current = false;
-  SE_CUDA(ctx, cudaSetDevice(ctx->device));
   SE_CUDA(ctx, cudaMemcpyAsync(d.d, s.d, sizeof(float) * (size_t)(s.rows * s.ld), cudaMemcpyDeviceToDevice, ctx->stream));
   return SE_OK;
 }
@@ -1404,6 +1432,7 @@ int se_fill_synthetic(se_ctx* ctx, int slot, int kind, uint64_t seed, double a, 
   SE_REQUIRE(ctx, kind >= 0 && kind <= 3, SE_ERR_ARG, "bad synthetic kind %d", kind);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
   if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
+  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
   if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
   return for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_LAUNCH(ctx, launch_fill_synthetic(d, kind, seed, a, b, len, offset + done, ctx->sms, ctx->stream));
@@ -1417,6 +1446,7 @@ int se_slot_sum(se_ctx* ctx, int slot, int64_t count, double* out) {
   const SlotBuf& s = ctx->slot[slot];
   SE_REQUIRE(ctx, s.d && s.rows == 1 && count <= s.cols, SE_ERR_STATE, "slot %d is not a [n] vector of >= %lld", slot, (long long)count);
   SE_TRY(begin(ctx));
+  if (slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
   SE_LAUNCH(ctx, launch_sum(s.d, count, red_ws(ctx), ctx->ctas_per_sm, ctx->sms, ctx->stream));
   return fetch_scalars(ctx, 0, 1, out);
 }
@@ -1438,6 +1468,7 @@ int se_quantile(se_ctx* ctx, int which, int slot, int64_t count, double q, doubl
     a = s.d;
   }
   SE_TRY(begin(ctx));
+  if (which == 1 || slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
   double total = (double)n;
   SE_TRY(se_comm_allreduce_host(ctx, &total, 1));
   SE_REQUIRE(ctx, total >= 1.0, SE_ERR_ARG, "quantile of an empty column");
@@ -1478,6 +1509,7 @@ int se_gbm_configure(se_ctx* ctx, int64_t n_train, int64_t n_valid, int dim, int
   SE_REQUIRE(ctx, dim >= 1 && dim <= kMaxDimGeneric, SE_ERR_ARG, "dim %d outside [1,%d]", dim, kMaxDimGeneric);
   SE_REQUIRE(ctx, (loss == SE_LOSS_LOGLOSS) || dim == 1, SE_ERR_ARG, "scalar losses have dim 1 (got %d)", dim);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  SE_TRY(settle_f(ctx));  // F is kept across a reconfiguration that does not reallocate it
   auto& g = ctx->gbm;
   g.on = true; g.n = n_train; g.nv = n_valid; g.dim = dim; g.loss = loss; g.param = param;
   g.has_w = has_weights != 0;
@@ -1502,6 +1534,7 @@ int se_gbm_configure(se_ctx* ctx, int64_t n_train, int64_t n_valid, int dim, int
 int se_gbm_set_loss_param(se_ctx* ctx, double param) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, ctx->gbm.on, SE_ERR_STATE, "se_gbm_configure first");
+  SE_TRY(settle_f(ctx));
   ctx->gbm.param = param;
   ctx->gbm.r_current = false;
   return SE_OK;
@@ -1627,6 +1660,7 @@ int se_gbm_pseudo_residuals(se_ctx* ctx, int newton, double* sum_hess) {
   SE_REQUIRE(ctx, ctx->gbm.on, SE_ERR_STATE, "se_gbm_configure first");
   SE_REQUIRE(ctx, !newton || loss_has_hessian(ctx->gbm.loss), SE_ERR_ARG, "loss %d has no hessian (updates=newton)", ctx->gbm.loss);
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   if (newton) SE_TRY(slot_alloc2d(ctx, SE_SLOT_WOUT, ctx->gbm.dim, ctx->gbm.n));
   GbmArgs a = gbm_args(ctx, false);
   ctx->wout_scaled = false;
@@ -1642,6 +1676,7 @@ int se_gbm_linesearch_eval(se_ctx* ctx, const double* alpha, double* loss, doubl
   SE_REQUIRE(ctx, ctx->gbm.on, SE_ERR_STATE, "se_gbm_configure first");
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   const int dim = ctx->gbm.dim;
   GbmArgs a = gbm_args(ctx, false);
   if (ctx->ls_packed) {  // inside se_gbm_linesearch_brent: bit-identical 8 B/row view
@@ -1667,6 +1702,7 @@ int se_gbm_linesearch_stats(se_ctx* ctx, double* stats4) {
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.loss == SE_LOSS_SQUARED, SE_ERR_STATE, "squared loss only");
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   GbmArgs a = gbm_args(ctx, false);
   a.stats_from_r = ctx->gbm.r_current ? 1 : 0;
   a.ws = red_ws(ctx);
@@ -1682,6 +1718,7 @@ int se_gbm_update(se_ctx* ctx, const double* step, int flags, double* loss_sum, 
   const bool newton = (flags & SE_UPD_NEWTON) != 0;
   SE_REQUIRE(ctx, !newton || loss_has_hessian(ctx->gbm.loss), SE_ERR_ARG, "loss %d has no hessian", ctx->gbm.loss);
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   if (newton) SE_TRY(slot_alloc2d(ctx, SE_SLOT_WOUT, ctx->gbm.dim, ctx->gbm.n));
   GbmArgs a = gbm_args(ctx, false);
   const int mode = newton ? GBM_UPDATE_NEWTON : ((flags & SE_UPD_RESIDUAL) ? GBM_UPDATE_RESID : GBM_UPDATE);
@@ -1708,6 +1745,7 @@ int se_gbm_mean_loss(se_ctx* ctx, int which, double* out) {
   SE_REQUIRE(ctx, (which == 1 ? ctx->gbm.nv_global : ctx->gbm.n_global) > 0.0, SE_ERR_ARG,
              which == 1 ? "no validation rows on any rank" : "no training rows on any rank");
   SE_TRY(begin(ctx));
+  if (which == 0) SE_TRY(settle_f(ctx));
   GbmArgs a = gbm_args(ctx, which == 1);
   a.ws = red_ws(ctx);
   SE_TRY(gbm_launch(ctx, SE_KF_MEAN_LOSS, GBM_MEAN_LOSS, a, nullptr));
@@ -1768,6 +1806,7 @@ int linesearch_persist(se_ctx* ctx, double lo, double hi, double start, double r
                        int single, int parity, double* alpha, double* loss, int* n_eval) {
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   const int lossid = ctx->gbm.loss;
   const bool packed = gbm_linesearch_persist_packed(lossid);
   if (packed) SE_TRY(ensure_ls_view(ctx));
@@ -1858,6 +1897,7 @@ int se_gbm_linesearch_brent(se_ctx* ctx, double lo, double hi, double start, dou
                             int max_eval, double* alpha, double* loss, int* n_eval) {
   if (!ctx || !alpha) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.dim == 1, SE_ERR_STATE, "Brent line search needs dim == 1");
+  SE_TRY(settle_f(ctx));  // the packed view below reads F
   if (ctx->gbm.loss == SE_LOSS_SQUARED) {
     double st[4];
     SE_TRY(se_gbm_linesearch_stats(ctx, st));
@@ -1910,6 +1950,7 @@ int round_squared_device_brent(se_ctx* ctx, double learning_rate, double tol, in
                                double* loss_sum, int* n_eval) {
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   GbmArgs a = gbm_args(ctx, false);
   a.stats_from_r = ctx->gbm.r_current ? 1 : 0;
   a.ws = red_ws(ctx, kScalRound);  // stats -> d_scal[kScalRound..+2], summed across GPUs
@@ -1951,6 +1992,10 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
                         double* loss_sum, int* n_eval) {
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  const int write_r = (flags & SE_UPD_RESIDUAL) ? 1 : 0;
+  // residual mode reads r (or y and F on a round whose residual slot is not current) and leaves F owed; the eager
+  // form updates F itself and needs it current
+  if (!write_r) SE_TRY(settle_f(ctx));
   SqRoundArgs a;
   const auto& g = ctx->gbm;
   a.y = ctx->slot[SE_SLOT_Y].d;
@@ -1996,13 +2041,13 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   a.sync = ctx->d_fsync;
   a.epoch = ++ctx->fused_epoch;
   {
-    // tiles of 16 KB per array; y and F are prefetched: 32 KB per tile, over at most fused_ctas_per_sm * sms CTAs
+    // tiles of 16 KB per array; two arrays (r and h, or y and F) are prefetched: 32 KB per tile, over at most
+    // fused_ctas_per_sm * sms CTAs
     const double per_cta = ctx->fused_prefetch_mb * 1e6 / (32768.0 * (double)(ctx->fused_ctas_per_sm * ctx->sms));
     a.prefetch_tiles = per_cta < 0.0 ? 0 : (per_cta > 64.0 ? 64 : (int)(per_cta + 0.5));
   }
   a.timing = ctx->fused_timing;
   a.l2_mode = ctx->fused_l2_mode == 1 ? 1 : 0;
-  const int write_r = (flags & SE_UPD_RESIDUAL) ? 1 : 0;
   int grid = 0;
   void* wbase = nullptr;
   size_t wbytes = 0;
@@ -2021,6 +2066,8 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
                                                            &grid, wbase, wbytes));
   ctx->last_fused_grid = grid;
   ctx->gbm.r_current = write_r != 0;
+  const bool owed_before = ctx->gbm.f_owed;
+  if (write_r) ctx->gbm.f_owed = true;  // F = y - r from here on (unless the step turns out to be 0, below)
   double ls = 0.0;
   SE_TRY(fetch_scalars(ctx, kScalRound + 8, 1, &ls));
   double res[7];
@@ -2042,7 +2089,12 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   if (alpha) *alpha = res[4];
   if (n_eval) *n_eval = (int)fabs(res[6]);
   if (loss_sum) *loss_sum = ls;
-  if (res[6] < 0.0) return fail(ctx, SE_ERR_OPT, "Brent exceeded MaxEval(%d)", max_iter);
+  if (res[6] < 0.0) {
+    // the step was 0: F was not moved, so it is exactly as current as before the round (r = y - F when the round read
+    // y and F), and a download returns it bit for bit
+    ctx->gbm.f_owed = owed_before;
+    return fail(ctx, SE_ERR_OPT, "Brent exceeded MaxEval(%d)", max_iter);
+  }
   return SE_OK;
 }
 }  // namespace
@@ -2084,6 +2136,7 @@ int se_gbm_linesearch_eval2(se_ctx* ctx, double alpha, double* loss, double* d1,
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.dim == 1 && ctx->gbm.loss != SE_LOSS_LOGLOSS, SE_ERR_STATE, "needs a dim-1 scalar loss");
   SE_TRY(ensure_wsum(ctx));
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   GbmArgs a = gbm_args(ctx, false);
   a.coef[0] = (float)alpha;
   a.ws = red_ws(ctx);
@@ -2132,6 +2185,7 @@ int se_gbm_round_squared_async(se_ctx* ctx, double learning_rate) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.loss == SE_LOSS_SQUARED, SE_ERR_STATE, "squared loss only");
   SE_TRY(begin(ctx));
+  SE_TRY(settle_f(ctx));
   GbmArgs a = gbm_args(ctx, false);
   a.stats_from_r = ctx->gbm.r_current ? 1 : 0;
   a.ws = red_ws(ctx, kScalRound);  // stats -> d_scal[kScalRound..+2]
@@ -2647,6 +2701,7 @@ static int tree_predict_impl(se_ctx* ctx, int which, int n_nodes, const int32_t*
   }
   memcpy(hv, value, sizeof(float) * (size_t)n_nodes * n_out);
   SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
   if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   TreeArgs t;
   t.X = X.d; t.n = X.cols; t.ld = X.rows > 1 ? X.ld : X.cols; t.n_nodes = n_nodes;
@@ -2738,6 +2793,7 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
                "threshold): evaluate the members with se_tree_predict + se_agg_run instead");
   }
   BinState& B = ctx->bins[which];
+  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
   if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   ForestArgs a;
   a.X8 = B.d8; a.n = X.cols; a.ld8 = B.ld8;
@@ -2841,6 +2897,8 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
   SE_REQUIRE(ctx, O.d && out_row >= 0 && out_row < O.rows && O.cols == X.cols, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(begin(ctx));
   release_l2_persist(ctx);
+  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
+  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   float* hc = reinterpret_cast<float*>(ctx->h_small);
   int32_t* hcol = reinterpret_cast<int32_t*>(hc + n_coef);

@@ -402,6 +402,30 @@ __global__ void __launch_bounds__(kBlock) pack_signed_kernel(const float* __rest
   }
 }
 
+// F owed by the lazy squared-loss round: F = y - r, and r = y - F so that the pair is exactly what an eager update of
+// this F leaves (reading F and uploading it again then changes nothing downstream)
+__global__ void __launch_bounds__(kBlock) settle_f_kernel(const float* __restrict__ y, float* __restrict__ r,
+                                                         float* __restrict__ F, int64_t n) {
+  const int64_t n4 = n >> 2;
+  for (int64_t g = (int64_t)blockIdx.x * kBlock + threadIdx.x; g < n4; g += (int64_t)gridDim.x * kBlock) {
+    const float4 vy = ld_stream4(y + 4 * g), vr = ld_rw4(r + 4 * g);
+    float4 oF, oR;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      f4at(oF, e) = f4at(vy, e) - f4at(vr, e);
+      f4at(oR, e) = f4at(vy, e) - f4at(oF, e);
+    }
+    st_stream4(F + 4 * g, oF);
+    st_stream4(r + 4 * g, oR);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const int64_t i = (n4 << 2) + threadIdx.x;
+    const float f = y[i] - r[i];
+    F[i] = f;
+    r[i] = y[i] - f;
+  }
+}
+
 __global__ void sq_alpha_kernel(const double* stats, double* out) {
   const double s1 = stats[1], s2 = stats[2];
   double al = (s2 > 0.0) ? s1 / s2 : 1.0;
@@ -514,6 +538,11 @@ cudaError_t launch_gbm(int loss, int mode, const GbmArgs& a, int ctas_per_sm, in
 cudaError_t launch_gbm_pack_signed(const float* y, const float* F, const float* h, float* u, float* v, int64_t n,
                                    int sms, cudaStream_t st) {
   pack_signed_kernel<<<grid_for(n >> 2, kBlock, 4, sms), kBlock, 0, st>>>(y, F, h, u, v, n);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gbm_settle_f(const float* y, float* r, float* F, int64_t n, int sms, cudaStream_t st) {
+  settle_f_kernel<<<grid_for(n >> 2, kBlock, 4, sms), kBlock, 0, st>>>(y, r, F, n);
   return cudaGetLastError();
 }
 

@@ -7,9 +7,13 @@
 //    :368-385 of the reference) in ONE launch: statistics pass (8 B/row) -> last CTA folds the partials, sums them
 //    across GPUs over peer memory and runs Brent (se_brent.h, the same template as the host line search) -> the step
 //    is published through an acquire/release flag while every other CTA already has the first update tile's loads in
-//    flight -> fused F update + next pseudo-residuals + loss (20 B/row), walking the tiles in the opposite direction
-//    so that the statistics pass's tail of h is still in the L2 -> loss reduction + second exchange + host
+//    flight -> next pseudo-residuals r' = r - c h + loss (12 B/row), walking the tiles in the opposite direction
+//    so that the statistics pass's tail of r and h is still in the L2 -> loss reduction + second exchange + host
 //    mirror.  1 launch, 0 host round trips inside the round, the Brent latency hidden behind the preloads.
+//    The round (residual mode) does not read or write F: nothing reads it between rounds, and for the squared loss
+//    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api.cu settle_f).
+//    A round whose residual slot is not current (Y, F or R were just written) reads (y, F, h) instead of (r, h):
+//    r' = (y - F) - c h, 16 B/row.  Without residual mode the update is F' = F + c h (F, y, h read; F written).
 //
 //  * gbm_linesearch_persist_kernel — Brent's <= MaxEval evaluations of the line-search objective
 //    (boosting/GBMLoss.scala:50-74 through RDDLossFunction; GBMRegressor.scala:408-421) for the non-squared scalar
@@ -72,7 +76,8 @@ __device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
   const int rc = brent_core(f, a.lo, a.hi, a.start, a.rel, a.abs_tol, a.max_eval, &x, &fx, &evals);
   const double ne = (rc == kBrentOk) ? (double)evals : -(double)evals;  // negative: MaxEval exceeded
   a.out[4] = x, a.out[5] = fx, a.out[6] = ne;
-  // MaxEval exceeded: the host reports SE_ERR_OPT and F must stay untouched (F + 0*h == F, r is recomputed)
+  // MaxEval exceeded: the host reports SE_ERR_OPT and F must stay what it was (r - 0*h == r, F + 0*h == F; the host
+  // does not mark F as owed)
   const double step = (rc == kBrentOk) ? a.lr * x : 0.0;
   a.sync->x = step;
   st_release_gpu_u64(&a.sync->flag, a.epoch);  // the grid starts the update NOW; the host is served next
@@ -130,7 +135,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       ok[u] = g < n4;
       if (ok[u]) {
         if (a.stats_from_r) {
-          vy[u] = ld_rw4_p(a.r + 4 * g, pol_r_in);  // r is rewritten by phase B without being read again
+          vy[u] = ld_rw4_p(a.r + 4 * g, pol_r_in);  // read again and rewritten by phase B
         } else {
           vy[u] = ld_stream4_p(a.y + 4 * g, pol_keep);
           vF[u] = ld_rw4_p(a.F + 4 * g, pol_keep);
@@ -170,8 +175,11 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     if (threadIdx.x == 0) fused_round_brent<LOSS_REDUCE>(a);
   }
 
-  // ---- phase B: F' = F + step*h, r = y - F', Σ (y-F')²/2 — tiles in the opposite direction
-  float4 vy[U], vF[U], vh[U];
+  // ---- phase B, tiles in the opposite direction.  WRITE_R (residual mode): r' = r - step*h, Σ r'²/2; F is not
+  // touched (the host rebuilds it as y - r' when it is next accessed), or r' = (y - F) - step*h on a round whose
+  // residual slot is not current.  Otherwise: F' = F + step*h, Σ (y-F')²/2.
+  const bool from_r = WRITE_R && a.stats_from_r;
+  float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
   bool ok[U];
   auto load_tile = [&](int64_t i) {
     const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
@@ -180,8 +188,12 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       const int64_t g = base + (int64_t)u * kBlock;
       ok[u] = g < n4;
       if (ok[u]) {
-        vy[u] = ld_stream4_p(a.y + 4 * g, pol_stream);
-        vF[u] = ld_rw4_p(a.F + 4 * g, pol_stream);
+        if (from_r) {
+          vy[u] = ld_rw4_p(a.r + 4 * g, pol_stream);
+        } else {
+          vy[u] = ld_stream4_p(a.y + 4 * g, pol_stream);
+          vF[u] = ld_rw4_p(a.F + 4 * g, pol_stream);
+        }
         vh[u] = ld_stream4_p(a.h + 4 * g, pol_h_b);  // the update is h's last reader
       }
     }
@@ -190,8 +202,11 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   if (i >= 0) load_tile(i);  // in flight while the last CTA reduces, exchanges and runs Brent
   if (threadIdx.x == 0) {
     // The wait (partials fold + cross-GPU exchange + ~30 dependent fp64 Brent iterations) is turned into
-    // useful HBM time: every CTA pulls the y and F ranges of its next update tiles into the L2 with bulk prefetches
-    // (one instruction per 16 KB), bounded so that the whole grid stays within a.prefetch_tiles tiles per CTA.
+    // useful HBM time: every CTA pulls the ranges its next update tiles read (r and h, or y and F) into the L2 with
+    // bulk prefetches (one instruction per 16 KB), bounded so that the whole grid stays within a.prefetch_tiles tiles
+    // per CTA.
+    const float* pf0 = from_r ? a.r : a.y;
+    const float* pf1 = from_r ? a.h : a.F;
     int64_t pf = i - 1;
     int budget = a.prefetch_tiles;
     while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {
@@ -200,8 +215,8 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
         int64_t groups = n4 - g0;
         if (groups > tile) groups = tile;
         if (groups > 0) {
-          prefetch_l2_bulk(a.y + 4 * g0, (unsigned int)(groups * 16));
-          prefetch_l2_bulk(a.F + 4 * g0, (unsigned int)(groups * 16));
+          prefetch_l2_bulk(pf0 + 4 * g0, (unsigned int)(groups * 16));
+          prefetch_l2_bulk(pf1 + 4 * g0, (unsigned int)(groups * 16));
         }
         --pf;
         --budget;
@@ -218,18 +233,25 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     for (int u = 0; u < U; ++u) {
       if (!ok[u]) continue;
       const int64_t g = base + (int64_t)u * kBlock;
-      float4 oF, oR;
+      float4 o;
       float l_acc = 0.f;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float p = fmaf(coef, f4at(vh[u], e), f4at(vF[u], e));  // GBMRegressor.scala:434-441
-        const float d = f4at(vy[u], e) - p;
-        f4at(oF, e) = p;
-        f4at(oR, e) = d;                                             // -g(y, F') (:383)
+        float d;
+        if constexpr (WRITE_R) {
+          // -g(y, F + step*h) = (y - F) - step*h (GBMRegressor.scala:383, 434-441)
+          const float r = from_r ? f4at(vy[u], e) : f4at(vy[u], e) - f4at(vF[u], e);
+          d = fmaf(-coef, f4at(vh[u], e), r);
+          f4at(o, e) = d;
+        } else {
+          const float p = fmaf(coef, f4at(vh[u], e), f4at(vF[u], e));  // GBMRegressor.scala:434-441
+          d = f4at(vy[u], e) - p;
+          f4at(o, e) = p;
+        }
         if (LOSS_REDUCE) l_acc = fmaf(0.5f * d, d, l_acc);           // GBMLoss.scala:129-137
       }
-      st_stream4_p(a.F + 4 * g, oF, pol_stream);
-      if (WRITE_R) st_stream4_p(a.r + 4 * g, oR, pol_keep);  // the next statistics pass starts where this one ends
+      if (WRITE_R) st_stream4_p(a.r + 4 * g, o, pol_keep);  // the next statistics pass starts where this one ends
+      else st_stream4_p(a.F + 4 * g, o, pol_stream);
       if (LOSS_REDUCE) accb[0] += (double)l_acc;
     }
     --i;
@@ -237,10 +259,15 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   }
   if (blockIdx.x == 0 && threadIdx.x < (a.n & 3)) {
     const int64_t j = (n4 << 2) + threadIdx.x;
-    const float p = fmaf(coef, a.h[j], a.F[j]);
-    const float d = a.y[j] - p;
-    a.F[j] = p;
-    if (WRITE_R) a.r[j] = d;
+    float d;
+    if constexpr (WRITE_R) {
+      d = fmaf(-coef, a.h[j], from_r ? a.r[j] : a.y[j] - a.F[j]);
+      a.r[j] = d;
+    } else {
+      const float p = fmaf(coef, a.h[j], a.F[j]);
+      d = a.y[j] - p;
+      a.F[j] = p;
+    }
     accb[0] += (double)(0.5f * d * d);
   }
   if constexpr (LOSS_REDUCE) {

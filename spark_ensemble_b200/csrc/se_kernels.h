@@ -59,6 +59,9 @@ cudaError_t launch_gbm(int loss, int mode, const GbmArgs& a, int ctas_per_sm, in
 // Brent evaluation reads two arrays instead of three (launch_gbm GBM_EVAL with y == nullptr, F = u, h = v)
 cudaError_t launch_gbm_pack_signed(const float* y, const float* F, const float* h, float* u, float* v, int64_t n,
                                    int sms, cudaStream_t stream);
+// squared loss, F owed after a residual-mode fused round: F = y - r, then r = y - F (the residual an update of that F
+// would have left), 16 B/row
+cudaError_t launch_gbm_settle_f(const float* y, float* r, float* F, int64_t n, int sms, cudaStream_t stream);
 // LogLoss(K) for K > kMaxDim (se_gbm_generic.cu): coefficients, per-CTA partials [grid][K+1] and the K+1 sums live in
 // device buffers sized for K; the cross-GPU sum of `out` is an NCCL all-reduce issued by the caller
 struct GenericArgs {
@@ -88,6 +91,7 @@ struct FusedSync {
 };
 
 // One squared-loss boosting round in one launch: statistics -> (cross-GPU sum) -> Brent -> update + residual + loss.
+// write_r (residual mode): the update writes r' = r - c h only and leaves F for the host to rebuild as y - r'.
 struct SqRoundArgs {
   const float* y = nullptr;
   float* F = nullptr;
@@ -99,7 +103,7 @@ struct SqRoundArgs {
   int l2_hints = 0;
   int l2_mode = 0;         // 0: evict_normal / evict_first hints; 1: evict_last on r and h (experiment)
   int timing = 0;          // write %globaltimer stamps (us) to out[10..13]: start, statistics folded, step published, end
-  int prefetch_tiles = 0;  // y/F tiles of the update phase each CTA prefetches into L2 while it waits for the step
+  int prefetch_tiles = 0;  // update-phase tiles (r/h, or y/F) each CTA prefetches into L2 while it waits for the step
   double lr = 1.0, wsum = 1.0;                                   // learning rate, Σw (objective scale)
   double lo = 0.0, hi = 100.0, start = 1.0, rel = 1e-6, abs_tol = 1e-6;
   int max_eval = 100;
