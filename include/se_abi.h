@@ -291,7 +291,11 @@ enum se_agg_kind {
 SE_API int se_agg_configure(se_ctx* ctx, int kind, int num_models, int num_classes, int dim, int loss,
                      int64_t n);
 /* runs the aggregation over P.  weights: [M] (GBM regressor, boosting discrete) or [M][dim]
- * (GBM classifier) or NULL; init: [dim] or NULL. Fills RAW (+PROB, LABEL for classifiers). */
+ * (GBM classifier) or NULL; init: [dim] or NULL. Fills RAW (+PROB, LABEL for classifiers).
+ * LABEL is the first maximum of the class scores.  The vote kinds (bagging hard, boosting discrete) accept any number
+ * of classes: past the shared-memory histograms (K >= 199 plain, K >= 99 weighted) the histogram is kept in the RAW
+ * and PROB columns themselves, which is slower but equally exact.  SAMME.R (boosting real) sums lg2 max(p, EPSILON)
+ * in fp64 and forms PROB from those sums, so pure-leaf ensembles give equal probabilities to equal vote counts. */
 SE_API int se_agg_run(se_ctx* ctx, const double* weights, const double* init);
 
 /* ---- row sub-sampling: Spark's sampler restated for the host side that has no Spark ------------- */

@@ -181,6 +181,26 @@ def agg_boosting_real(P):
     return raw, softmax_cols(raw / (K - 1.0))
 
 
+# Pure-leaf closed forms.  A pure tree leaf returns a probability vector of exact 0s and one 1, so every clamped log
+# is 0 or -L with L = -log(EPSILON) = 52 ln 2, and the SAMME.R sums reduce to vote counts.
+L_EPS = -np.log(EPS)
+
+
+def samme_r_pure_leaf(K, wn, correct):
+    """SAMME.R weight of a row whose base model put probability 1 on one class: wn e^{-(K-1)L/K} when that class is
+    the label, wn e^{L/K} when it is not."""
+    return wn * np.where(correct, np.exp(-(K - 1.0) * L_EPS / K), np.exp(L_EPS / K))
+
+
+def boosting_real_pure_leaf(counts):
+    """SAMME.R aggregation of M one-hot models from the vote counts c[K][n]: raw_k = (K-1) L (c_k - M/K) and
+    prob = softmax(L c).  Independent of the order of summation: equal counts give equal values."""
+    counts = np.asarray(counts, dtype=np.float64)
+    K = counts.shape[0]
+    M = counts.sum(axis=0)
+    return (K - 1) * L_EPS * (counts - M / K), softmax_cols(L_EPS * counts)
+
+
 def agg_boosting_discrete(votes, a, K):
     M, n = votes.shape
     onehot = (np.arange(K)[None, :, None] == votes[:, None, :].astype(np.int64))

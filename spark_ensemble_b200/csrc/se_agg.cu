@@ -26,8 +26,14 @@ namespace {
 constexpr float kSparkEps = 2.220446049250313e-16f;
 constexpr int MU = 8;  // models loaded per batch: 8 independent 16 B requests per thread
 
-// out[c][i] = init_c + Σ_m a[m][c] · f(P[m][c][i]),  f = identity or log(max(·,ε))
+// lg2 max(p, ε): the clamp is the exact constant lg2 2^-52 = -52 (NaN clamps too), so the sums of pure-leaf outputs
+// (exact 0s and 1s) are exact multiples of 52 and equal vote counts give equal totals
+__device__ __forceinline__ float lg2_clamped(float p) { return (p > kSparkEps) ? lg2_approx(p) : -52.0f; }
+
+// out[c][i] = init_c + Σ_m a[m][c] · f(P[m][c][i]),  f = identity
 // P row (m,c) lives at P + (cols ? cols[m] : m*width + c) * ld.
+// LOGP (SAMME.R): f = lg2 max(·,ε), every term added in fp64 (a batch of fp32 sums of terms of ~-52 would lose 1e-5 of
+// the probabilities), and the fp64 total is stored as an fp32 pair: out = hi, out_lo = total - hi.
 template <bool LOGP>
 __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict__ P, int64_t n,
                                                         int64_t ld, int M, int width,
@@ -35,7 +41,7 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
                                                         const float* __restrict__ init,
                                                         const int32_t* __restrict__ cols,
                                                         float post_div, float* __restrict__ out,
-                                                        int64_t ld_out) {
+                                                        int64_t ld_out, float* __restrict__ out_lo = nullptr) {
   const int64_t n4 = n >> 2;
   for (int64_t g = (int64_t)blockIdx.x * kBlock + threadIdx.x; g < n4;
        g += (int64_t)gridDim.x * kBlock) {
@@ -58,15 +64,21 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
             wv[u] = a ? a[(int64_t)m * width + c] : 1.0f;
           }
         }
+        if constexpr (LOGP) {
+#pragma unroll
+          for (int u = 0; u < MU; ++u) {
+            if (m0 + u < M) {
+              d0 += (double)lg2_clamped(v[u].x); d1 += (double)lg2_clamped(v[u].y);
+              d2 += (double)lg2_clamped(v[u].z); d3 += (double)lg2_clamped(v[u].w);
+            }
+          }
+          continue;
+        }
         float4 s0 = make_float4(0.f, 0.f, 0.f, 0.f), s1 = s0;
 #pragma unroll
         for (int u = 0; u < MU; ++u) {
           if (m0 + u < M) {
-            float4 x = v[u];
-            if (LOGP) {
-              x.x = log_fast(fmaxf(x.x, kSparkEps)); x.y = log_fast(fmaxf(x.y, kSparkEps));
-              x.z = log_fast(fmaxf(x.z, kSparkEps)); x.w = log_fast(fmaxf(x.w, kSparkEps));
-            }
+            const float4 x = v[u];
             float4& s = (u & 1) ? s1 : s0;  // two accumulator sets: shorter dependency chains
             s.x = fmaf(wv[u], x.x, s.x); s.y = fmaf(wv[u], x.y, s.y);
             s.z = fmaf(wv[u], x.z, s.z); s.w = fmaf(wv[u], x.w, s.w);
@@ -78,6 +90,13 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
         } else {
           carry.x += s0.x + s1.x; carry.y += s0.y + s1.y; carry.z += s0.z + s1.z; carry.w += s0.w + s1.w;
         }
+      }
+      if constexpr (LOGP) {
+        const float4 hi = make_float4((float)d0, (float)d1, (float)d2, (float)d3);
+        st_stream4(out + c * ld_out + 4 * g, hi);
+        st_stream4(out_lo + c * ld_out + 4 * g, make_float4((float)(d0 - (double)hi.x), (float)(d1 - (double)hi.y),
+                                                            (float)(d2 - (double)hi.z), (float)(d3 - (double)hi.w)));
+        continue;
       }
       if (!wide) { d0 = (double)carry.x; d1 = (double)carry.y; d2 = (double)carry.z; d3 = (double)carry.w; }
       const double b = init ? (double)init[c] : 0.0;
@@ -95,9 +114,13 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
       double sd = init ? (double)init[c] : 0.0;
       for (int m = 0; m < M; ++m) {
         const int64_t rowi = cols ? (int64_t)cols[m] : (int64_t)m * width + c;
-        float x = P[rowi * ld + i];
-        if (LOGP) x = log_fast(fmaxf(x, kSparkEps));
-        sd += (double)((a ? a[(int64_t)m * width + c] : 1.0f) * x);
+        const float x = P[rowi * ld + i];
+        sd += LOGP ? (double)lg2_clamped(x) : (double)((a ? a[(int64_t)m * width + c] : 1.0f) * x);
+      }
+      if (LOGP) {
+        out[c * ld_out + i] = (float)sd;
+        out_lo[c * ld_out + i] = (float)(sd - (double)(float)sd);
+        continue;
       }
       if (post_div != 0.f) sd /= (double)post_div;
       out[c * ld_out + i] = (float)sd;
@@ -117,18 +140,43 @@ struct FinArgs {
   double inv_km1;  // 1 / (K - 1)
 };
 
-// raw value from the stage-1 sum.  Real: the mean is a shift common to all classes (soft-max invariant), so fp32 is
-// enough once the mean itself was accumulated in fp64; discrete: K·A_k − Σa subtracts nearly equal numbers and is
-// formed in fp64 before the single rounding to the fp32 output.
+// raw value from the stage-1 sum.  Discrete: K·A_k − Σa subtracts nearly equal numbers and is formed in fp64 before
+// the single rounding to the fp32 output.  (SAMME.R has its own epilogue, finalize_real_row.)
 template <class T>
 __device__ __forceinline__ float fin_raw(const FinArgs& f, T t, float mean_t) {
   switch (f.kind) {
-    case SE_AGG_BOOSTING_REAL:  // (K-1)(L_k − mean L)   BoostingClassifier.scala:355-360
-      return (float)(f.K - 1) * ((float)t - mean_t);
     case SE_AGG_BOOSTING_DISCRETE:  // +a on the vote, −a/(K-1) elsewhere   :371-376
       return (float)(((double)t * (double)f.K - f.sum_a) * f.inv_km1);  // one reciprocal instead of an fp64 division per class
     default: return (float)t;
   }
+}
+
+// SAMME.R epilogue.  get(c) returns T_c = Σ_m lg2 max(p_mc, ε) in fp64 (exact for pure leaves).  With L = T ln 2:
+// raw_c = (K-1)(L_c − mean L) (BoostingClassifier.scala:355-360) and prob = softmax(raw/(K-1)) = 2^(T_c − T_max) / Σ
+// (:342-346), formed from the fp64 differences, not from the rounded raw (|raw| reaches (K-1)·36·M, where one fp32 ulp
+// of raw is already 1e-5 of a probability).  First-maximum argmax of T, which orders the classes as raw does.
+// Three sweeps over the classes, each reading get(c) again: the third overwrites what the stage-1 sums were read from.
+template <class Get>
+__device__ __forceinline__ void finalize_real_row(const FinArgs& f, int64_t i, Get get) {
+  const int C = f.C;
+  double s = 0.0, tmax = -INFINITY;
+  int am = 0;
+  for (int c = 0; c < C; ++c) {
+    const double t = get(c);
+    s += t;
+    if (t > tmax) tmax = t, am = c;  // Vector.argmax: first maximum
+  }
+  const double mean = s / (double)C;
+  const double rs = (double)(f.K - 1) * 0.6931471805599453;
+  float ssum = 0.f;
+  for (int c = 0; c < C; ++c) ssum += ex2_approx((float)(get(c) - tmax));
+  const float inv = 1.0f / ssum;
+  for (int c = 0; c < C; ++c) {
+    const double t = get(c);
+    f.prob[c * f.ld + i] = ex2_approx((float)(t - tmax)) * inv;
+    f.raw[c * f.ld + i] = (float)(rs * (t - mean));
+  }
+  f.label[i] = (float)am;
 }
 
 // get(c) returns the stage-1 sum of class c for this row.  Two sweeps over the classes: (1) raw values with an
@@ -136,14 +184,8 @@ __device__ __forceinline__ float fin_raw(const FinArgs& f, T t, float mean_t) {
 template <class Get>
 __device__ __forceinline__ void finalize_row(const FinArgs& f, int64_t i, Get get) {
   const int C = f.C;
-  float mean_t = 0.f;
-  if (f.kind == SE_AGG_BOOSTING_REAL) {
-    double s = 0.0;
-    for (int c = 0; c < C; ++c) s += (double)get(c);
-    mean_t = (float)(s / (double)C);
-  }
-  const bool softmax = (f.kind == SE_AGG_BOOSTING_REAL || f.kind == SE_AGG_BOOSTING_DISCRETE ||
-                        f.kind == SE_AGG_GBM_CLASSIFIER);
+  const float mean_t = 0.f;
+  const bool softmax = (f.kind == SE_AGG_BOOSTING_DISCRETE || f.kind == SE_AGG_GBM_CLASSIFIER);
   // boosting: softmax(raw/(K-1)) (BoostingClassifier.scala:342-346); GBM logloss: softmax(raw) (GBMLoss.scala:258-261)
   const float sc = (f.kind == SE_AGG_GBM_CLASSIFIER) ? kLog2e : kLog2e / (float)(f.K - 1);
   float best = -INFINITY, ssum = 0.f;
@@ -241,6 +283,60 @@ __global__ void __launch_bounds__(kBlock) agg_votes_kernel(const float* __restri
       }
       f.label[i] = (float)am;
     }
+  }
+  if (bad_vote && f.bad_label != nullptr) *reinterpret_cast<volatile int*>(f.bad_label) = 1;
+}
+
+// Vote histogram for class counts whose shared-memory histogram does not fit (K + 1 bins x kBlock threads: K >= 99
+// weighted, K >= 199 plain).  Each row's histogram lives in its own RAW and PROB columns: RAW holds the fp32 sum of
+// the row's vote weights per class and PROB the rounding error of that sum (a two-sum per vote), so the weighted total
+// is good to ~2^-48 like the fp64 histogram; plain counts are exact integers in RAW.  The votes of a warp scatter over
+// K classes, so this is the slow path, kept for correctness at any K.
+__global__ void __launch_bounds__(kBlock) agg_votes_global_kernel(const float* __restrict__ votes, int64_t ld, int M,
+                                                                 const float* __restrict__ a, const FinArgs f) {
+  const int K = f.K;
+  bool bad_vote = false;
+  for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < f.n; i += (int64_t)gridDim.x * kBlock) {
+    float* hi = f.raw + i;
+    float* lo = f.prob + i;
+    for (int c = 0; c < K; ++c) hi[c * f.ld] = 0.f, lo[c * f.ld] = 0.f;
+    for (int m = 0; m < M; ++m) {
+      const float x = ld_stream1(votes + (int64_t)m * ld + i);
+      const int c = __float2int_rz(x);
+      const bool ok = ((unsigned)c < (unsigned)K) && ((float)c == x);  // a vote is a predicted class index
+      bad_vote = bad_vote || !ok;
+      if (!ok) continue;
+      const float w = a ? __ldg(a + m) : 1.0f;
+      const float s = hi[c * f.ld], t = s + w, bp = t - s;
+      hi[c * f.ld] = t;
+      lo[c * f.ld] += (s - (t - bp)) + (w - bp);
+    }
+    float best = -INFINITY;
+    int am = 0;
+    if (f.kind == SE_AGG_BAGGING_HARD) {
+      const float inv = 1.0f / (float)f.M;  // prob = raw·(1/M)  (BaggingClassifier.scala:285-287)
+      for (int c = 0; c < K; ++c) {
+        const float r = hi[c * f.ld];
+        if (r > best) best = r, am = c;  // Vector.argmax: first maximum
+        lo[c * f.ld] = r * inv;
+      }
+    } else {
+      const float sc = kLog2e / (float)(f.K - 1);  // prob = softmax(raw/(K-1))  (BoostingClassifier.scala:342-346)
+      for (int c = 0; c < K; ++c) {
+        const float r = fin_raw(f, (double)hi[c * f.ld] + (double)lo[c * f.ld], 0.f);
+        if (r > best) best = r, am = c;
+        hi[c * f.ld] = r;
+      }
+      double ssum = 0.0;  // up to thousands of terms of similar size: an fp32 sum drifts by 1e-5
+      for (int c = 0; c < K; ++c) {
+        const float e = ex2_approx((hi[c * f.ld] - best) * sc);
+        ssum += (double)e;
+        lo[c * f.ld] = e;
+      }
+      const float inv = (float)(1.0 / ssum);
+      for (int c = 0; c < K; ++c) lo[c * f.ld] *= inv;
+    }
+    f.label[i] = (float)am;
   }
   if (bad_vote && f.bad_label != nullptr) *reinterpret_cast<volatile int*>(f.bad_label) = 1;
 }
@@ -358,18 +454,9 @@ __device__ __forceinline__ void finalize_tile4(const FinArgs& f, float* T, int64
         if (row0 + j < f.n) base[row0 + j] = f4at(v, j);
     }
   };
-  float4 mean = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (f.kind == SE_AGG_BOOSTING_REAL) {
-    double m0 = 0.0, m1 = 0.0, m2 = 0.0, m3 = 0.0;
-    for (int c = 0; c < C; ++c) {
-      const float4 t = *reinterpret_cast<const float4*>(T + c * kAR);
-      m0 += (double)t.x, m1 += (double)t.y, m2 += (double)t.z, m3 += (double)t.w;
-    }
-    const double ic = 1.0 / (double)C;
-    mean = make_float4((float)(m0 * ic), (float)(m1 * ic), (float)(m2 * ic), (float)(m3 * ic));
-  }
-  const bool softmax = (f.kind == SE_AGG_BOOSTING_REAL || f.kind == SE_AGG_GBM_CLASSIFIER);
-  const float sc = (f.kind == SE_AGG_GBM_CLASSIFIER) ? kLog2e : kLog2e / (float)(f.K - 1);
+  const float4 mean = make_float4(0.f, 0.f, 0.f, 0.f);
+  const bool softmax = (f.kind == SE_AGG_GBM_CLASSIFIER);
+  const float sc = kLog2e;
   // pass 1: raw (kept in the tile, written to HBM), max and first argmax
   float4 best = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
   float4 am = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -410,8 +497,11 @@ __device__ __forceinline__ void finalize_tile4(const FinArgs& f, float* T, int64
   }
 }
 
-// dynamic shared memory (128-byte aligned): [stages][G*C][kAR] floats, then the running totals [C][kAR]
-template <int CMAX, int W>
+// dynamic shared memory (128-byte aligned): [stages][G*C][kAR] floats, then the running totals [C][kAR] (fp32, or
+// fp64 for LOGP)
+// LOGP (SAMME.R): every model's lg2 max(p, eps) is added straight into fp64 totals in shared memory: late in boosting
+// most terms are -52 (exact for pure leaves), and fp32 batch sums of them lose 1e-5 of the probabilities from M ~ 8.
+template <int CMAX, int W, bool LOGP>
 __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileArgs ta, const FinArgs f,
                                                              const __grid_constant__ CUtensorMap mapP) {
   constexpr int kAT = 32 * W, kAR = 128 * W;
@@ -423,6 +513,7 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
   const int stage_floats = box_rows * kAR;
   const int tid = threadIdx.x;
   float* total = ring + (size_t)S * stage_floats + 4 * tid;  // this thread's four columns
+  double* total_lg = reinterpret_cast<double*>(ring + (size_t)S * stage_floats) + 4 * tid;  // LOGP
   if (tid == 0) {
     for (int s = 0; s < S; ++s) mbar_init(&full[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -443,7 +534,6 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
   if (tid == 0)
     for (int s = 0; s < S && s < nbox; ++s) issue(s, s);
 
-  const float fold_scale = ta.logp ? kLn2 : 1.0f;  // logs are summed in the lg2 domain
   int stage = 0;
   uint32_t phase = 0;
   int64_t q = 0;
@@ -454,6 +544,12 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
     for (int c = 0; c < CMAX; ++c) acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
     int in_batch = 0;
     bool first_fold = true;
+    if constexpr (LOGP) {
+      for (int c = 0; c < C; ++c) {
+        double2* t = reinterpret_cast<double2*>(total_lg + c * kAR);
+        t[0] = make_double2(0.0, 0.0), t[1] = make_double2(0.0, 0.0);
+      }
+    }
     for (int step = 0; step < steps; ++step, ++q) {
       mbar_wait(&full[stage], phase);
       const float* box = ring + (size_t)stage * stage_floats + 4 * tid;
@@ -461,15 +557,22 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
       const int gcount = min(ta.G, M - m0);
       for (int g = 0; g < gcount; ++g) {
         const float* bg = box + g * C * kAR;
+        if constexpr (LOGP) {
+          for (int c = 0; c < C; ++c) {
+            const float4 x = *reinterpret_cast<const float4*>(bg + c * kAR);
+            double2* t = reinterpret_cast<double2*>(total_lg + c * kAR);
+            double2 t0 = t[0], t1 = t[1];
+            t0.x += (double)lg2_clamped(x.x), t0.y += (double)lg2_clamped(x.y);
+            t1.x += (double)lg2_clamped(x.z), t1.y += (double)lg2_clamped(x.w);
+            t[0] = t0, t[1] = t1;
+          }
+          continue;
+        }
         const float* wg = ta.a ? ta.a + (int64_t)(m0 + g) * C : nullptr;
 #pragma unroll
         for (int c = 0; c < CMAX; ++c) {
           if (c < C) {
-            float4 x = *reinterpret_cast<const float4*>(bg + c * kAR);
-            if (ta.logp) {
-              x.x = lg2_approx(fmaxf(x.x, kSparkEps)), x.y = lg2_approx(fmaxf(x.y, kSparkEps));
-              x.z = lg2_approx(fmaxf(x.z, kSparkEps)), x.w = lg2_approx(fmaxf(x.w, kSparkEps));
-            }
+            const float4 x = *reinterpret_cast<const float4*>(bg + c * kAR);
             const float wv = wg ? __ldg(wg + c) : 1.0f;
             acc[c].x = fmaf(wv, x.x, acc[c].x), acc[c].y = fmaf(wv, x.y, acc[c].y);
             acc[c].z = fmaf(wv, x.z, acc[c].z), acc[c].w = fmaf(wv, x.w, acc[c].w);
@@ -480,7 +583,7 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
       if (tid == 0 && q + S < nbox) issue(q + S, stage);
       if (++stage == S) stage = 0, phase ^= 1;
       in_batch += gcount;
-      if (in_batch >= 8 || step == steps - 1) {
+      if (!LOGP && (in_batch >= 8 || step == steps - 1)) {
         // fold the batch into the running totals: the rounding error stays at the magnitude of one batch
 #pragma unroll
         for (int c = 0; c < CMAX; ++c) {
@@ -492,8 +595,7 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
             } else {
               t = *reinterpret_cast<const float4*>(total + c * kAR);
             }
-            t.x = fmaf(acc[c].x, fold_scale, t.x), t.y = fmaf(acc[c].y, fold_scale, t.y);
-            t.z = fmaf(acc[c].z, fold_scale, t.z), t.w = fmaf(acc[c].w, fold_scale, t.w);
+            t.x += acc[c].x, t.y += acc[c].y, t.z += acc[c].z, t.w += acc[c].w;
             *reinterpret_cast<float4*>(total + c * kAR) = t;
             acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
           }
@@ -502,7 +604,14 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
         in_batch = 0;
       }
     }
-    if (row0 < f.n) finalize_tile4<kAR>(f, total, row0);
+    if (row0 < f.n) {
+      if constexpr (LOGP) {
+        for (int j = 0; j < 4; ++j)
+          if (row0 + j < f.n) finalize_real_row(f, row0 + j, [&](int c) { return total_lg[c * kAR + j]; });
+      } else {
+        finalize_tile4<kAR>(f, total, row0);
+      }
+    }
   }
 }
 
@@ -528,7 +637,10 @@ __global__ void __launch_bounds__(kBlock) agg_finalize_kernel(const FinArgs f) {
       f.label[i] = (res > r0) ? 1.0f : 0.0f;  // argmax, first maximum on ties
       continue;
     }
-    finalize_row(f, i, [&](int c) { return f.raw[c * f.ld + i]; });
+    if (f.kind == SE_AGG_BOOSTING_REAL)
+      finalize_real_row(f, i, [&](int c) { return (double)f.raw[c * f.ld + i] + (double)f.prob[c * f.ld + i]; });
+    else
+      finalize_row(f, i, [&](int c) { return f.raw[c * f.ld + i]; });
   }
 }
 
@@ -911,7 +1023,7 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   if (ta.G > 8) ta.G = 8;
   const int box_rows = ta.G * C;
   const size_t stage_bytes = (size_t)box_rows * kAR * sizeof(float);
-  const size_t total_bytes = (size_t)C * kAR * sizeof(float);
+  const size_t total_bytes = (size_t)C * kAR * (ta.logp ? sizeof(double) : sizeof(float));
   static const int forced_stages = [] { const char* e = getenv("SE_AGG_TILE_STAGES"); return e ? atoi(e) : 0; }();
   const int stages = forced_stages >= 1 && forced_stages <= kAggMaxStages ? forced_stages : 1;
   const size_t smem = total_bytes + stages * stage_bytes + 128;
@@ -925,14 +1037,15 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   const int64_t ntiles = (a.n + kAR - 1) / kAR;
   const int64_t cap = (int64_t)per_sm * sms;
   const int grid = (int)(ntiles < cap ? ntiles : cap);
-#define SE_CT(CM)                                                                                        \
+#define SE_CT(CM, LG)                                                                                    \
   {                                                                                                      \
-    auto kern = agg_class_tile_kernel<CM, warps>;                                                        \
+    auto kern = agg_class_tile_kernel<CM, warps, LG>;                                                    \
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);              \
     if (e != cudaSuccess) return e;                                                                      \
     kern<<<grid, kAT, smem, st>>>(ta, f, mapP);                                                          \
   }
-  if (C <= 4) SE_CT(4) else if (C <= 8) SE_CT(8) else if (C <= 16) SE_CT(16) else SE_CT(32)
+  if (ta.logp) SE_CT(32, true)  // no register batch: CMAX is unused
+  else if (C <= 4) SE_CT(4, false) else if (C <= 8) SE_CT(8, false) else if (C <= 16) SE_CT(16, false) else SE_CT(32, false)
 #undef SE_CT
   *launched = true;
   return cudaGetLastError();
@@ -1062,9 +1175,9 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
                                                        nullptr, 0.f, a.raw, a.ld_out);
       f.C = a.K;
       break;
-    case SE_AGG_BOOSTING_REAL:
+    case SE_AGG_BOOSTING_REAL:  // fp64 totals as (hi, lo) pairs in RAW and PROB, read back by finalize_real_row
       agg_sum_kernel<true><<<grid4, kBlock, 0, st>>>(a.P, a.n, a.ld, a.M, a.K, nullptr, nullptr,
-                                                      nullptr, 0.f, a.raw, a.ld_out);
+                                                      nullptr, 0.f, a.raw, a.ld_out, a.prob);
       f.C = a.K;
       break;
     case SE_AGG_BAGGING_HARD:
@@ -1084,14 +1197,17 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
       }
       const size_t hsz = weighted ? sizeof(double) : sizeof(float);
       const size_t smem = (size_t)(a.K + 1) * kBlock * hsz + (size_t)a.M * hsz;
-      if (smem > 200 * 1024) return cudaErrorInvalidValue;
+      f.C = a.K;
+      f.sum_a = a.sum_weights;
+      if (smem > 200 * 1024) {  // the histogram does not fit in shared memory: keep it in the output columns
+        agg_votes_global_kernel<<<grid1, kBlock, 0, st>>>(a.P, a.ld, a.M, weighted ? a.weights : nullptr, f);
+        return cudaGetLastError();
+      }
       auto kern = weighted ? agg_votes_kernel<double> : agg_votes_kernel<float>;
       if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
       }
-      f.C = a.K;
-      f.sum_a = a.sum_weights;
       kern<<<grid1, kBlock, smem, st>>>(a.P, a.ld, a.M, weighted ? a.weights : nullptr, f);
       return cudaGetLastError();  // epilogue fused: no separate finalize launch
     }

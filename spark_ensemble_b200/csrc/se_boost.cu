@@ -33,10 +33,17 @@ inline int grid_for(int64_t work_items, int64_t per_cta, int ctas_per_sm, int sm
   return (int)(units < want ? units : want);
 }
 
-// Σ_k code_k log max(p_k, ε) with code_y = 1, code_{k≠y} = -1/(K-1)  (BoostingClassifier.scala:218-224)
-//   = (1 + 1/(K-1))·log p_y − (1/(K-1))·Σ_k log p_k
+// lg2 max(p, ε): the clamp is the exact constant lg2 2^-52 = -52, not an SFU approximation of it (NaN clamps too)
+__device__ __forceinline__ float lg2_clamped(float p) { return (p > kSparkEps) ? lg2_approx(p) : -52.0f; }
+
+// loss = Σ_k code_k log max(p_k, ε) with code_y = 1, code_{k≠y} = -1/(K-1)  (BoostingClassifier.scala:218-224)
+//      = K/(K-1)·log p_y − (1/(K-1))·Σ_k log p_k,   so   −(K-1)/K·loss = ln 2·(Σ_k lg2 p_k / K − lg2 p_y)
+// and w' = wₙ·2^x with x = Σ/K − lg2 p_y in [-52, 52] (:226).  Late in boosting most p_k clamp to ε, so Σ is ~K terms
+// of -52: it is carried in fp64 (an fp32 sum loses ~1e-5 of the weight from K ~ 64), and x is split into an integer
+// power of two (exact) and a fraction in [-0.5, 0.5] for the SFU.
 struct RowState {
-  float best, sum_log, log_y;
+  float best, lg_y;
+  double sum_lg;
   int am;
 };
 
@@ -45,15 +52,20 @@ __device__ __forceinline__ void row_step(RowState& s, float p, int k, int yi) {
     s.best = p;
     s.am = k;
   }
-  const float lp = log_fast(fmaxf(p, kSparkEps));
-  s.sum_log += lp;
-  if (k == yi) s.log_y = lp;
+  const float lg = lg2_clamped(p);
+  s.sum_lg += (double)lg;
+  if (k == yi) s.lg_y = lg;
+}
+
+__device__ __forceinline__ float samme_r_weight(float wn, double sum_lg, float lg_y, double inv_k) {
+  const double x = fma(sum_lg, inv_k, -(double)lg_y);
+  const double xi = rint(x);
+  return wn * ex2_approx((float)(x - xi)) * __int_as_float(((int)xi + 127) << 23);
 }
 
 __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
   const int K = a.K;
-  const float inv_km1 = 1.0f / (float)(K - 1);
-  const float scale = -((float)(K - 1) / (float)K);
+  const double inv_k = 1.0 / (double)K;
   double acc[2] = {0.0, 0.0};
   const int64_t n4 = a.n >> 2;
   for (int64_t g = (int64_t)blockIdx.x * kBlock + threadIdx.x; g < n4;
@@ -64,7 +76,7 @@ __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
     int yi[4];
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      st[e].best = -INFINITY; st[e].sum_log = 0.f; st[e].log_y = 0.f; st[e].am = 0;
+      st[e].best = -INFINITY; st[e].sum_lg = 0.0; st[e].lg_y = 0.f; st[e].am = 0;
       yi[e] = (int)f4at(vy, e);  // compared only (validity is checked once per label upload)
     }
     for (int k0 = 0; k0 < K; k0 += KU) {
@@ -85,8 +97,7 @@ __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
     for (int e = 0; e < 4; ++e) {
       const float wn = f4at(vw, e) * a.inv_sum_w;  // :186
       err4 += (st[e].am != yi[e]) ? wn : 0.f;       // :202-209
-      const float loss = (1.0f + inv_km1) * st[e].log_y - inv_km1 * st[e].sum_log;
-      const float wo = wn * exp_fast(scale * loss);  // :226
+      const float wo = samme_r_weight(wn, st[e].sum_lg, st[e].lg_y, inv_k);  // :218-226
       f4at(out, e) = wo;
       sum4 += wo;
     }
@@ -96,12 +107,11 @@ __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
   }
   if (blockIdx.x == 0 && threadIdx.x < (a.n & 3)) {
     const int64_t i = (n4 << 2) + threadIdx.x;
-    RowState st{-INFINITY, 0.f, 0.f, 0};
+    RowState st{-INFINITY, 0.f, 0.0, 0};
     const int yi = (int)a.y[i];
     for (int k = 0; k < K; ++k) row_step(st, a.proba[(int64_t)k * a.ld + i], k, yi);
     const float wn = a.w[i] * a.inv_sum_w;
-    const float loss = (1.0f + inv_km1) * st.log_y - inv_km1 * st.sum_log;
-    const float wo = wn * exp_fast(scale * loss);
+    const float wo = samme_r_weight(wn, st.sum_lg, st.lg_y, inv_k);
     a.w[i] = wo;
     acc[0] += (st.am != yi) ? (double)wn : 0.0;
     acc[1] += (double)wo;
@@ -129,8 +139,7 @@ __global__ void __launch_bounds__(kRT) boost_real_tiled_kernel(const BoostArgs a
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const float inv_km1 = 1.0f / (float)(K - 1);
-  const float scale = -((float)(K - 1) / (float)K);
+  const double inv_k = 1.0 / (double)K;
   const int64_t ntiles = (a.n + kRR - 1) / kRR;
   double acc[2] = {0.0, 0.0};
   uint32_t it = 0;
@@ -149,10 +158,11 @@ __global__ void __launch_bounds__(kRT) boost_real_tiled_kernel(const BoostArgs a
     for (int e = 0; e < 4; ++e) yi[e] = min(max((int)f4at(vy, e), 0), K - 1);  // clamp = memory safety; validity checked once per upload
     mbar_wait(&bar, it & 1);
     const float* sP = tileP + 4 * tid;
-    float best[4], sum_lg[4];
+    float best[4];
+    double sum_lg[4];
     int am[4];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) best[e] = -INFINITY, sum_lg[e] = 0.f, am[e] = 0;
+    for (int e = 0; e < 4; ++e) best[e] = -INFINITY, sum_lg[e] = 0.0, am[e] = 0;
 #pragma unroll 2
     for (int k = 0; k < K; ++k) {
       const float4 p = *reinterpret_cast<const float4*>(sP + k * kRR);
@@ -160,7 +170,7 @@ __global__ void __launch_bounds__(kRT) boost_real_tiled_kernel(const BoostArgs a
       for (int e = 0; e < 4; ++e) {
         const float pe = f4at(p, e);
         if (pe > best[e]) best[e] = pe, am[e] = k;  // Vector.argmax: first maximum
-        sum_lg[e] += lg2_approx(fmaxf(pe, kSparkEps));
+        sum_lg[e] += (double)lg2_clamped(pe);
       }
     }
     float4 out;
@@ -168,10 +178,9 @@ __global__ void __launch_bounds__(kRT) boost_real_tiled_kernel(const BoostArgs a
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const bool in = row0 + e < a.n;
-      const float log_y = lg2_approx(fmaxf(sP[yi[e] * kRR + e], kSparkEps)) * kLn2;  // yi is clamped into [0, K)
-      const float wn = f4at(vw, e) * a.inv_sum_w;  // :186
-      const float loss = (1.0f + inv_km1) * log_y - inv_km1 * (sum_lg[e] * kLn2);  // :218-224
-      const float wo = wn * exp_fast(scale * loss);                                // :226
+      const float lg_y = lg2_clamped(sP[yi[e] * kRR + e]);  // yi is clamped into [0, K)
+      const float wn = f4at(vw, e) * a.inv_sum_w;          // :186
+      const float wo = samme_r_weight(wn, sum_lg[e], lg_y, inv_k);  // :218-226
       f4at(out, e) = wo;
       err4 += (in && am[e] != yi[e]) ? wn : 0.f;                                   // :202-209
       sum4 += in ? wo : 0.f;

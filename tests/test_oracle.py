@@ -225,6 +225,47 @@ def test_samme_r_matches_numpy_and_invariants(oracle, rng):
     assert 0 <= e <= 1 and np.all(out > 0)
 
 
+@pytest.mark.parametrize("K", [2, 5, 26, 201, 256])
+def test_samme_r_pure_leaf_closed_form(oracle, rng, K):
+    """One-hot base-model outputs (pure leaves): the C oracle's weights are wn e^{-(K-1)L/K} on rows whose vote is the
+    label and wn e^{L/K} elsewhere, L = -log(EPSILON), to 1e-12."""
+    n = 300
+    y = rng.integers(0, K, n)
+    vote = np.where(rng.random(n) < 0.6, y, (y + rng.integers(1, K, n)) % K)
+    P = (np.arange(K)[:, None] == vote[None, :]).astype(np.float64)
+    w = rng.random(n) + 0.1
+    sw = w.sum()
+    out, e, s = oracle.samme_r_update(K, y.astype(np.float64), w, sw, P)
+    want = NP.samme_r_pure_leaf(K, w / sw, vote == y)
+    np.testing.assert_allclose(out, want, rtol=1e-12, atol=0)
+    assert e == pytest.approx(np.sum((w / sw)[vote != y]), rel=1e-12)
+    assert s == pytest.approx(want.sum(), rel=1e-12)
+
+
+@pytest.mark.parametrize("K,M", [(2, 1), (2, 16), (5, 17), (26, 64), (33, 8), (40, 512)])
+def test_boosting_real_pure_leaf_closed_form(oracle, rng, K, M):
+    """M one-hot models: the C oracle's SAMME.R raw and probabilities are the vote-count closed form to 1e-12, and
+    classes with equal counts get equal probabilities (the rows alternate two classes, so half of them tie).
+    The oracle's probabilities are exponentials of differences of fp64 sums of M K terms of size L: where that
+    rounding bound, 4 M K L 2^-53, exceeds 1e-12 (M = 512), it is the tolerance."""
+    n = 200
+    votes = rng.integers(0, K, (M, n))
+    alt = rng.random(n) < 0.5
+    k1 = rng.integers(0, K, n)
+    k2 = (k1 + rng.integers(1, K, n)) % K
+    votes[:, alt] = np.where(np.arange(M)[:, None] % 2 == 0, k1[alt][None, :], k2[alt][None, :])
+    P = (np.arange(K)[None, :, None] == votes[:, None, :]).astype(np.float64)
+    counts = P.sum(axis=0)
+    raw, prob = oracle.agg_boosting_real(P)
+    rw, pw = NP.boosting_real_pure_leaf(counts)
+    assert np.all(np.abs(raw - rw) <= 1e-12 * np.abs(rw).max(axis=0))
+    ok = pw > 1e-300
+    np.testing.assert_allclose(prob[ok], pw[ok], rtol=max(1e-12, 4.0 * M * K * NP.L_EPS * 2.0 ** -53))
+    assert np.all(prob[~ok] <= 1e-300)
+    if M % 2 == 0:
+        np.testing.assert_array_equal(pw[k1[alt], np.flatnonzero(alt)], pw[k2[alt], np.flatnonzero(alt)])
+
+
 def test_samme_discrete_matches_numpy(oracle, rng):
     n, K = 1000, 5
     y = rng.integers(0, K, n).astype(np.float64)
