@@ -209,6 +209,8 @@ struct se_ctx {
   int fused_loss_reduce = 0;          // 1: reduce the train loss over the rows even when the closed form applies
   int fused_l2_mode = 0;              // experiment: 1 = evict_last on r/h, 2 = persisting window over r
   int fused_timing = 0;               // diagnostic: in-kernel %globaltimer stamps of the fused round
+  int fused_resident = 1;             // residual rounds reading r carry the statistics pass's tail in shared memory
+  double last_fused_resident_tiles = 0.0;  // tiles per CTA the last fused round carried in shared memory
   double last_fused_us[3] = {0, 0, 0};  // statistics phase, fold+exchange+Brent, update phase    // L2 budget of the update-phase prefetch issued while the grid waits for the step
   int ls_mode = 1;                    // non-squared line search: 0 one launch per evaluation (round-1 kernels), 1 one
                                       // persistent launch (device Brent), 2 host Brent over single-evaluation launches of
@@ -730,6 +732,7 @@ int se_ctx_create(int device, se_ctx** out) {
     cudaGetLastError();
   }
   if (const char* s = getenv("SE_FUSED_ROUND")) ctx->fused_round = atoi(s) != 0 ? 1 : 0;
+  if (const char* s = getenv("SE_FUSED_RESIDENT")) ctx->fused_resident = atoi(s) != 0;
   if (const char* s = getenv("SE_LS_MODE")) { const int v = atoi(s); if (v >= 0 && v <= 2) ctx->ls_mode = v; }
   if (const char* s = getenv("SE_LS_RESIDENT")) ctx->ls_resident = atoi(s) != 0;
   if (const char* s = getenv("SE_LS_RING")) { const int v = atoi(s); if (v >= 0 && v <= 4) ctx->ls_ring = v; }
@@ -878,21 +881,23 @@ int se_ctx_kernel_time_reset(se_ctx* ctx) {
 
 namespace {
 struct OptKey { const char* name; int id; };
-enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_L2_MODE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_PREFETCH_MB, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS, OPT_LS_RING, OPT_L2_PERSIST,
+enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_L2_MODE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_PREFETCH_MB, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS, OPT_LS_RING, OPT_L2_PERSIST,
        OPT_L2_PERSIST_FRAC, OPT_PEER_TIMEOUT_MS, OPT_ALTERNATE, OPT_L2_HINTS, OPT_CTAS_PER_SM, OPT_HOST_MIRROR,
        // read-only diagnostics
        OPT_LAST_ROUND_FUSED, OPT_LAST_LS_WORKERS, OPT_LAST_LS_PASSES, OPT_LAST_LS_HIT_RATIO, OPT_LAST_FUSED_GRID,
-       OPT_L2_PERSIST_MAX, OPT_L2_WINDOW_MAX, OPT_LAST_STAT0, OPT_LAST_STAT1, OPT_LAST_STAT2 };
+       OPT_LAST_FUSED_RESIDENT, OPT_L2_PERSIST_MAX, OPT_L2_WINDOW_MAX, OPT_LAST_STAT0, OPT_LAST_STAT1, OPT_LAST_STAT2 };
 const OptKey kOpts[] = {
   {"last_forest_chunks", OPT_LAST_FOREST_CHUNKS}, {"wm_fast", OPT_WM_FAST}, {"wm_list_cap", OPT_WM_LIST_CAP}, {"last_wm_mode", OPT_LAST_WM_MODE}, {"last_wm_deferred", OPT_LAST_WM_DEFERRED},
   {"tree_bins", OPT_TREE_BINS}, {"tree_mask", OPT_TREE_MASK}, {"last_tree_mask", OPT_LAST_TREE_MASK}, {"last_tree_binned", OPT_LAST_TREE_BINNED}, {"last_tree_rebinned_cols", OPT_LAST_TREE_REBINNED},
   {"fused_loss_reduce", OPT_FUSED_LOSS_REDUCE}, {"fused_l2_mode", OPT_FUSED_L2_MODE}, {"fused_timing", OPT_FUSED_TIMING}, {"last_fused_stats_us", OPT_LAST_FUSED_US0}, {"last_fused_brent_us", OPT_LAST_FUSED_US1},
   {"last_fused_update_us", OPT_LAST_FUSED_US2}, {"fused_prefetch_mb", OPT_FUSED_PREFETCH_MB}, {"fused_round", OPT_FUSED_ROUND}, {"fused_round_max_rows", OPT_FUSED_MAX_ROWS}, {"fused_ctas_per_sm", OPT_FUSED_CTAS},
+  {"fused_resident", OPT_FUSED_RESIDENT},
   {"ls_mode", OPT_LS_MODE}, {"ls_resident", OPT_LS_RESIDENT}, {"ls_ctas_per_sm", OPT_LS_CTAS}, {"ls_ring", OPT_LS_RING}, {"l2_persist", OPT_L2_PERSIST},
   {"l2_persist_frac", OPT_L2_PERSIST_FRAC}, {"peer_timeout_ms", OPT_PEER_TIMEOUT_MS}, {"alternate_passes", OPT_ALTERNATE},
   {"l2_hints", OPT_L2_HINTS}, {"ctas_per_sm", OPT_CTAS_PER_SM}, {"host_mirror", OPT_HOST_MIRROR},
   {"last_round_fused", OPT_LAST_ROUND_FUSED}, {"last_ls_workers", OPT_LAST_LS_WORKERS}, {"last_ls_passes", OPT_LAST_LS_PASSES},
   {"last_ls_hit_ratio", OPT_LAST_LS_HIT_RATIO}, {"last_fused_grid", OPT_LAST_FUSED_GRID},
+  {"last_fused_resident_tiles", OPT_LAST_FUSED_RESIDENT},
   {"l2_persist_max_bytes", OPT_L2_PERSIST_MAX}, {"l2_window_max_bytes", OPT_L2_WINDOW_MAX},
   {"last_round_stat0", OPT_LAST_STAT0}, {"last_round_stat1", OPT_LAST_STAT1}, {"last_round_stat2", OPT_LAST_STAT2},
 };
@@ -919,6 +924,7 @@ int se_ctx_set_option(se_ctx* ctx, const char* key, double value) {
     case OPT_FUSED_L2_MODE: SE_REQUIRE(ctx, iv >= 0 && iv <= 2, SE_ERR_ARG, "fused_l2_mode in {0,1,2}"); ctx->fused_l2_mode = iv; if (iv != 2) release_l2_persist(ctx); break;
     case OPT_FUSED_PREFETCH_MB: SE_REQUIRE(ctx, value >= 0.0 && value <= 512.0, SE_ERR_ARG, "fused_prefetch_mb in [0,512]"); ctx->fused_prefetch_mb = value; break;
     case OPT_FUSED_CTAS: SE_REQUIRE(ctx, iv >= 1 && iv <= 8, SE_ERR_ARG, "fused_ctas_per_sm in [1,8]"); ctx->fused_ctas_per_sm = iv; break;
+    case OPT_FUSED_RESIDENT: ctx->fused_resident = iv != 0; break;
     case OPT_LS_MODE: SE_REQUIRE(ctx, iv >= 0 && iv <= 2, SE_ERR_ARG, "ls_mode in {0,1,2}"); ctx->ls_mode = iv; break;
     case OPT_LS_RESIDENT: ctx->ls_resident = iv != 0; break;
     case OPT_LS_RING: SE_REQUIRE(ctx, iv >= 0 && iv <= 4, SE_ERR_ARG, "ls_ring in [0,4]"); ctx->ls_ring = iv; break;
@@ -969,6 +975,7 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_FUSED_US1: *value = ctx->last_fused_us[1]; break;
     case OPT_LAST_FUSED_US2: *value = ctx->last_fused_us[2]; break;
     case OPT_FUSED_CTAS: *value = ctx->fused_ctas_per_sm; break;
+    case OPT_FUSED_RESIDENT: *value = ctx->fused_resident; break;
     case OPT_LS_MODE: *value = ctx->ls_mode; break;
     case OPT_LS_RESIDENT: *value = ctx->ls_resident; break;
     case OPT_LS_RING: *value = ctx->ls_ring; break;
@@ -985,6 +992,7 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_LS_PASSES: *value = ctx->last_ls_passes; break;
     case OPT_LAST_LS_HIT_RATIO: *value = ctx->last_ls_hit_ratio; break;
     case OPT_LAST_FUSED_GRID: *value = ctx->last_fused_grid; break;
+    case OPT_LAST_FUSED_RESIDENT: *value = ctx->last_fused_resident_tiles; break;
     case OPT_L2_PERSIST_MAX: *value = (double)ctx->l2_persist_max; break;
     case OPT_L2_WINDOW_MAX: *value = (double)ctx->l2_window_max; break;
     case OPT_LAST_STAT0: *value = ctx->last_round_stats[0]; break;
@@ -2048,7 +2056,7 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   }
   a.timing = ctx->fused_timing;
   a.l2_mode = ctx->fused_l2_mode == 1 ? 1 : 0;
-  int grid = 0;
+  int grid = 0, resident_slots = 0;
   void* wbase = nullptr;
   size_t wbytes = 0;
   if (ctx->fused_l2_mode == 2 && ctx->l2_persist_max > 0 && ctx->l2_window_max > 0) {
@@ -2062,9 +2070,11 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
     wbase = a.r;
     ctx->l2_persist_dirty = true;
   }
-  SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->sms, ctx->fused_ctas_per_sm, ctx->stream,
-                                                           &grid, wbase, wbytes));
+  SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->fused_resident, ctx->sms,
+                                                           ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots,
+                                                           wbase, wbytes));
   ctx->last_fused_grid = grid;
+  ctx->last_fused_resident_tiles = resident_slots / 4.0;  // float4 groups per thread, U_SQ = 4 to a tile
   ctx->gbm.r_current = write_r != 0;
   const bool owed_before = ctx->gbm.f_owed;
   if (write_r) ctx->gbm.f_owed = true;  // F = y - r from here on (unless the step turns out to be 0, below)

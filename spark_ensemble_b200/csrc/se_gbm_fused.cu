@@ -8,8 +8,9 @@
 //    across GPUs over peer memory and runs Brent (se_brent.h, the same template as the host line search) -> the step
 //    is published through an acquire/release flag while every other CTA already has the first update tile's loads in
 //    flight -> next pseudo-residuals r' = r - c h + loss (12 B/row), walking the tiles in the opposite direction
-//    so that the statistics pass's tail of r and h is still in the L2 -> loss reduction + second exchange + host
-//    mirror.  1 launch, 0 host round trips inside the round, the Brent latency hidden behind the preloads.
+//    so that the statistics pass's tail of r and h is still on chip (residual rounds without a bag keep each CTA's
+//    last tile in registers and the groups before it in shared memory; otherwise the tail is in the L2) -> loss
+//    reduction + second exchange + host mirror.  1 launch, 0 host round trips inside the round.
 //    The round (residual mode) does not read or write F: nothing reads it between rounds, and for the squared loss
 //    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api.cu settle_f).
 //    A round whose residual slot is not current (Y, F or R were just written) reads (y, F, h) instead of (r, h):
@@ -63,6 +64,10 @@ __device__ __forceinline__ void prefetch_l2_bulk(const void* p, unsigned int byt
 
 // =================================================================================== squared-loss round, one launch
 constexpr int U_SQ = 4;  // float4 groups per thread per tile (as the two-launch kernels)
+// Residual-mode rounds that read r (no bag) carry phase A's tail into phase B on chip: the CTA's last tile stays in
+// registers and the groups before it in shared memory, one slot per float4 group of r and of h (8 KB per CTA), so
+// that a slot, not a whole 32 KB tile, is the unit the SM's shared memory is split into.
+constexpr int kSqSlotBytes = 2 * kBlock * 16;
 
 // The line search of the fused round, executed by ONE thread of the last CTA once the statistics are folded (and
 // summed across GPUs) while every other CTA waits for the step with its first update tile's loads in flight.
@@ -105,43 +110,61 @@ __device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
   }
 }
 
-template <bool WRITE_R, bool LOSS_REDUCE>
+// FROM_R (the path a fit and the benchmark take: residual mode, the residual slot current, no bag) is a compile-time
+// specialisation: it carries phase A's tail into phase B on chip (kSqSlotBytes) and has no y / F / bag arrays live.
+template <bool WRITE_R, bool LOSS_REDUCE, bool FROM_R>
 __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqRoundArgs a) {
+  static_assert(WRITE_R || !FROM_R, "FROM_R is a residual-mode round");
   constexpr int U = U_SQ;
+  extern __shared__ float4 s_res[];  // FROM_R: [slot][r, h][kBlock]
   __shared__ float s_coef;
+  __shared__ float4 s_brent_regs[2 * U];  // FROM_R: the Brent thread's carried groups while it runs Brent
   const int64_t n4 = a.n >> 2;
   constexpr int64_t tile = (int64_t)kBlock * U;
   const int64_t ntiles = (n4 + tile - 1) / tile;
   const int64_t G = gridDim.x;
   const int64_t cnt = (ntiles > (int64_t)blockIdx.x) ? (ntiles - 1 - blockIdx.x) / G + 1 : 0;  // tiles b, b+G, ...
-  const bool has_bag = (a.bag != nullptr);
+  const bool has_bag = !FROM_R && (a.bag != nullptr);
+  const bool stats_from_r = FROM_R || a.stats_from_r;
+  // FROM_R: group u of tile i has the flat index i*U + u.  The last tile (cnt-1) stays in registers, the S groups
+  // before it in shared memory: every group from p_res on is carried to phase B.
+  const int64_t S = FROM_R ? min((int64_t)a.resident_slots, (cnt > 0 ? cnt - 1 : 0) * U) : 0;
+  const int64_t p_res = (cnt - 1) * U - S;
   // l2_mode 1: r and h are the arrays worth keeping between phases / rounds (r: written by the update, read by the
   // next statistics pass; h: read by both phases) -> evict_last; y and F stream through -> evict_first
   const uint64_t pol_stream = l2_policy(a.l2_hints != 0);
   const uint64_t pol_keep = (a.l2_mode == 1) ? l2_policy_evict_last() : l2_policy(false);
   const uint64_t pol_r_in = (a.l2_mode == 1) ? pol_keep : pol_stream;
   const uint64_t pol_h_b = (a.l2_mode == 1) ? pol_keep : pol_stream;
+  // carried groups are served from chip in phase B: their L2 lines go first, so that the L2 keeps the groups before
+  // them, which phase B reads next
+  const uint64_t pol_carried = l2_policy(true);
 
   if (a.timing && blockIdx.x == 0 && threadIdx.x == 0) a.out[10] = global_timer_us();
   // ---- phase A: Σ(y-F)², Σh(y-F), Σh² (from the current residual slot when it is valid: 8 B/row)
   double acc[3] = {0.0, 0.0, 0.0};
-  for (int64_t i = 0; i < cnt; ++i) {
+  auto stats_tile = [&](int64_t i, float4 (&vy)[U], float4 (&vF)[U], float4 (&vh)[U], bool (&ok)[U]) {
     const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
-    float4 vy[U], vF[U], vh[U], vb[U];
-    bool ok[U];
+    float4 vb[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int64_t g = base + (int64_t)u * kBlock;
       ok[u] = g < n4;
       if (ok[u]) {
-        if (a.stats_from_r) {
-          vy[u] = ld_rw4_p(a.r + 4 * g, pol_r_in);  // read again and rewritten by phase B
+        if constexpr (FROM_R) {
+          const bool carried = i * U + u >= p_res;
+          vy[u] = ld_rw4_p(a.r + 4 * g, carried ? pol_carried : pol_r_in);
+          vh[u] = ld_stream4_p(a.h + 4 * g, carried ? pol_carried : pol_keep);
         } else {
-          vy[u] = ld_stream4_p(a.y + 4 * g, pol_keep);
-          vF[u] = ld_rw4_p(a.F + 4 * g, pol_keep);
+          if (stats_from_r) {
+            vy[u] = ld_rw4_p(a.r + 4 * g, pol_r_in);  // read again and rewritten by phase B
+          } else {
+            vy[u] = ld_stream4_p(a.y + 4 * g, pol_keep);
+            vF[u] = ld_rw4_p(a.F + 4 * g, pol_keep);
+          }
+          vh[u] = ld_stream4_p(a.h + 4 * g, pol_keep);   // re-read by phase B, starting from this pass's tail
+          if (has_bag) vb[u] = ld_stream4(a.bag + 4 * g);
         }
-        vh[u] = ld_stream4_p(a.h + 4 * g, pol_keep);   // re-read by phase B, starting from this pass's tail
-        if (has_bag) vb[u] = ld_stream4(a.bag + 4 * g);
       }
     }
 #pragma unroll
@@ -150,7 +173,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       float s0 = 0.f, s1 = 0.f, s2 = 0.f;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const float d = a.stats_from_r ? f4at(vy[u], e) : f4at(vy[u], e) - f4at(vF[u], e), h = f4at(vh[u], e);
+        const float d = stats_from_r ? f4at(vy[u], e) : f4at(vy[u], e) - f4at(vF[u], e), h = f4at(vh[u], e);
         const float c = has_bag ? f4at(vb[u], e) : 1.0f;
         s0 = fmaf(c * d, d, s0);
         s1 = fmaf(c * h, d, s1);
@@ -160,10 +183,35 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       acc[1] += (double)s1;
       acc[2] += (double)s2;
     }
+    if constexpr (FROM_R) {
+      if (i < cnt - 1) {  // each thread writes, and in phase B reads back, only its own slots: no barrier
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int64_t s = i * U + u - p_res;
+          if (s >= 0 && ok[u]) {
+            s_res[(2 * s) * kBlock + threadIdx.x] = vy[u];
+            s_res[(2 * s + 1) * kBlock + threadIdx.x] = vh[u];
+          }
+        }
+      }
+    }
+  };
+  // phase B's tile registers.  FROM_R: phase A loads into them, so that its last tile is where phase B starts; the
+  // other rounds keep phase A's tiles local, so that nothing is live across the wait but what phase B loads.
+  float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
+  bool ok[U];
+  for (int64_t i = 0; i < cnt; ++i) {
+    if constexpr (FROM_R) {
+      stats_tile(i, vy, vF, vh, ok);
+    } else {
+      float4 ty[U], tF[U], th[U];
+      bool tok[U];
+      stats_tile(i, ty, tF, th, tok);
+    }
   }
   if (blockIdx.x == 0 && threadIdx.x < (a.n & 3)) {
     const int64_t i = (n4 << 2) + threadIdx.x;
-    const float d = a.stats_from_r ? a.r[i] : a.y[i] - a.F[i], h = a.h[i];
+    const float d = stats_from_r ? a.r[i] : a.y[i] - a.F[i], h = a.h[i];
     const float c = has_bag ? a.bag[i] : 1.0f;
     acc[0] += (double)(c * d * d);
     acc[1] += (double)(c * h * d);
@@ -172,15 +220,26 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   const bool last = block_reduce_publish<3>(acc, a.ws_a);  // the last CTA also sums across GPUs (peer_exchange)
   if (last) {
     __syncthreads();  // a.out[0..2] were written by other threads of this CTA
-    if (threadIdx.x == 0) fused_round_brent<LOSS_REDUCE>(a);
+    if (threadIdx.x == 0) {
+      // FROM_R: Brent needs more registers than are left beside the carried tile; its thread parks that tile in
+      // shared memory meanwhile instead of spilling to local memory
+      if constexpr (FROM_R) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) s_brent_regs[u] = vy[u], s_brent_regs[U + u] = vh[u];
+      }
+      fused_round_brent<LOSS_REDUCE>(a);
+      if constexpr (FROM_R) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) vy[u] = s_brent_regs[u], vh[u] = s_brent_regs[U + u];
+      }
+    }
   }
 
   // ---- phase B, tiles in the opposite direction.  WRITE_R (residual mode): r' = r - step*h, Σ r'²/2; F is not
   // touched (the host rebuilds it as y - r' when it is next accessed), or r' = (y - F) - step*h on a round whose
-  // residual slot is not current.  Otherwise: F' = F + step*h, Σ (y-F')²/2.
-  const bool from_r = WRITE_R && a.stats_from_r;
-  float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
-  bool ok[U];
+  // residual slot is not current.  Otherwise: F' = F + step*h, Σ (y-F')²/2.  The order of the tiles, and so of the
+  // loss sum, is the same whether a tile comes from registers, shared memory or global memory.
+  const bool from_r = WRITE_R && stats_from_r;
   auto load_tile = [&](int64_t i) {
     const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
 #pragma unroll
@@ -188,6 +247,12 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       const int64_t g = base + (int64_t)u * kBlock;
       ok[u] = g < n4;
       if (ok[u]) {
+        const int64_t s = i * U + u - p_res;
+        if (FROM_R && s >= 0) {
+          vy[u] = s_res[(2 * s) * kBlock + threadIdx.x];
+          vh[u] = s_res[(2 * s + 1) * kBlock + threadIdx.x];
+          continue;
+        }
         if (from_r) {
           vy[u] = ld_rw4_p(a.r + 4 * g, pol_stream);
         } else {
@@ -199,7 +264,8 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     }
   };
   int64_t i = cnt - 1;
-  if (i >= 0) load_tile(i);  // in flight while the last CTA reduces, exchanges and runs Brent
+  // in flight while the last CTA reduces, exchanges and runs Brent (FROM_R: still in registers from phase A)
+  if (!FROM_R && i >= 0) load_tile(i);
   if (threadIdx.x == 0) {
     // The wait (partials fold + cross-GPU exchange + ~30 dependent fp64 Brent iterations) is turned into
     // useful HBM time: every CTA pulls the ranges its next update tiles read (r and h, or y and F) into the L2 with
@@ -208,6 +274,21 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     const float* pf0 = from_r ? a.r : a.y;
     const float* pf1 = from_r ? a.h : a.F;
     int64_t pf = i - 1;
+    if constexpr (FROM_R) {
+      // nothing of the carried tail is loaded: the loads issued before the wait are those of the first tile phase B
+      // reads from global memory (its groups below p_res)
+      pf = p_res > 0 ? (p_res - 1) / U : -1;
+      if (pf >= 0) {
+        const int64_t g0 = (blockIdx.x + pf * G) * tile;
+        int64_t groups = (p_res - pf * U) * kBlock;
+        if (groups > n4 - g0) groups = n4 - g0;
+        if (groups > 0) {
+          prefetch_l2_bulk(pf0 + 4 * g0, (unsigned int)(groups * 16));
+          prefetch_l2_bulk(pf1 + 4 * g0, (unsigned int)(groups * 16));
+        }
+        --pf;
+      }
+    }
     int budget = a.prefetch_tiles;
     while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {
       if (budget > 0 && pf >= 0) {
@@ -694,28 +775,84 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
 
 }  // namespace
 
-cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a, int write_r, int loss_reduce, int sms, int max_ctas_per_sm,
-                                      cudaStream_t st, int* grid_out, void* window_base, size_t window_bytes) {
-  static int blocks[4] = {-1, -1, -1, -1};
-  void (*kerns[4])(const SqRoundArgs) = {gbm_round_sq_fused_kernel<false, false>, gbm_round_sq_fused_kernel<false, true>,
-                                         gbm_round_sq_fused_kernel<true, false>, gbm_round_sq_fused_kernel<true, true>};
-  const int which = (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
-  if (blocks[which] < 0) {
-    cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks[which], kerns[which], kBlock, 0);
+cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int loss_reduce, int resident, int sms,
+                                      int max_ctas_per_sm, cudaStream_t st, int* grid_out, int* resident_slots_out,
+                                      void* window_base, size_t window_bytes) {
+  constexpr int kKerns = 6;
+  void (*kerns[kKerns])(const SqRoundArgs) = {
+      gbm_round_sq_fused_kernel<false, false, false>, gbm_round_sq_fused_kernel<false, true, false>,
+      gbm_round_sq_fused_kernel<true, false, false>,  gbm_round_sq_fused_kernel<true, true, false>,
+      gbm_round_sq_fused_kernel<true, false, true>,   gbm_round_sq_fused_kernel<true, true, true>};
+  const bool from_r = write_r && a0.stats_from_r && a0.bag == nullptr;
+  const int which = from_r ? 4 + (loss_reduce ? 1 : 0) : (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
+  // function attributes and occupancy are per DEVICE (a process may drive several GPUs, as in launch_ls)
+  constexpr int kMaxDev = 64;
+  struct KernInfo {
+    int blocks, max_dyn, static_smem;
+    // occupancy at the dynamic size of the last launch: consecutive rounds repeat it, and on small shards the host
+    // must issue the next launch within the current round's update phase
+    size_t dyn_checked;
+    int blocks_dyn;
+    bool ready;
+  };
+  static KernInfo info_dev[kMaxDev][kKerns] = {};
+  static int smem_per_sm_dev[kMaxDev];
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= kMaxDev) return cudaErrorInvalidDevice;
+  KernInfo& info = info_dev[dev][which];
+  if (!info.ready) {
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, kerns[which]);
     if (e != cudaSuccess) return e;
+    info.static_smem = (int)fa.sharedSizeBytes;
+    info.max_dyn = 0;
+    if (which >= 4) {  // the carry-over sizes its dynamic shared memory past the default 48 KB
+      int optin = 0;
+      cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+      info.max_dyn = optin - info.static_smem;
+      e = cudaFuncSetAttribute(kerns[which], cudaFuncAttributeMaxDynamicSharedMemorySize, info.max_dyn);
+      if (e != cudaSuccess) return e;
+    }
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&info.blocks, kerns[which], kBlock, 0);
+    if (e != cudaSuccess) return e;
+    cudaDeviceGetAttribute(&smem_per_sm_dev[dev], cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    info.ready = true;
   }
-  int per_sm = blocks[which];
+  int per_sm = info.blocks;
   if (per_sm > max_ctas_per_sm) per_sm = max_ctas_per_sm;
   if (per_sm < 1) return cudaErrorLaunchOutOfResources;
-  const int64_t ntiles = ((a.n >> 2) + (int64_t)kBlock * U_SQ - 1) / ((int64_t)kBlock * U_SQ);
+  const int64_t ntiles = ((a0.n >> 2) + (int64_t)kBlock * U_SQ - 1) / ((int64_t)kBlock * U_SQ);
   int64_t grid = (int64_t)per_sm * sms;
   if (grid > ntiles) grid = ntiles;
   if (grid < 1) grid = 1;
   if (grid > kMaxGridPartials / 2) grid = kMaxGridPartials / 2;
+  // carried slots per CTA: the SM's shared memory split between its co-resident CTAs (1 KB per CTA is reserved by
+  // the system), and no more than the busiest CTA has groups before its last tile
+  int64_t slots = 0;
+  if (from_r && resident) {
+    int64_t budget = (int64_t)smem_per_sm_dev[dev] / per_sm - 1024 - info.static_smem;
+    if (budget > info.max_dyn) budget = info.max_dyn;
+    slots = budget / kSqSlotBytes;
+    const int64_t per_cta = (ntiles + grid - 1) / grid;
+    if (slots > (per_cta - 1) * U_SQ) slots = (per_cta - 1) * U_SQ;
+    if (slots < 0) slots = 0;
+  }
+  const size_t dyn = (size_t)slots * kSqSlotBytes;
+  if (dyn > 0) {  // the whole grid must still be co-resident with this much shared memory per CTA
+    if (dyn != info.dyn_checked) {
+      cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&info.blocks_dyn, kerns[which], kBlock, dyn);
+      if (e != cudaSuccess) return e;
+      info.dyn_checked = dyn;
+    }
+    if ((int64_t)info.blocks_dyn * sms < grid) return cudaErrorCooperativeLaunchTooLarge;
+  }
+  SqRoundArgs a = a0;
+  a.resident_slots = (int)slots;
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3((unsigned)grid);
   lc.blockDim = dim3(kBlock);
-  lc.dynamicSmemBytes = 0;
+  lc.dynamicSmemBytes = dyn;
   lc.stream = st;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeCooperative;
@@ -733,6 +870,7 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a, int write_r, int los
   lc.attrs = attr;
   lc.numAttrs = na;
   if (grid_out) *grid_out = (int)grid;
+  if (resident_slots_out) *resident_slots_out = (int)slots;
   return cudaLaunchKernelEx(&lc, kerns[which], a);
 }
 

@@ -92,6 +92,8 @@ struct FusedSync {
 
 // One squared-loss boosting round in one launch: statistics -> (cross-GPU sum) -> Brent -> update + residual + loss.
 // write_r (residual mode): the update writes r' = r - c h only and leaves F for the host to rebuild as y - r'.
+// A residual-mode round that reads r (no bag) carries its statistics pass's last tile in registers and, with
+// `resident`, the groups before it in shared memory into the update pass; *resident_slots_out = groups per thread.
 struct SqRoundArgs {
   const float* y = nullptr;
   float* F = nullptr;
@@ -104,6 +106,7 @@ struct SqRoundArgs {
   int l2_mode = 0;         // 0: evict_normal / evict_first hints; 1: evict_last on r and h (experiment)
   int timing = 0;          // write %globaltimer stamps (us) to out[10..13]: start, statistics folded, step published, end
   int prefetch_tiles = 0;  // update-phase tiles (r/h, or y/F) each CTA prefetches into L2 while it waits for the step
+  int resident_slots = 0;  // set by the launcher: float4 groups of r and h per thread carried in shared memory
   double lr = 1.0, wsum = 1.0;                                   // learning rate, Σw (objective scale)
   double lo = 0.0, hi = 100.0, start = 1.0, rel = 1e-6, abs_tol = 1e-6;
   int max_eval = 100;
@@ -118,8 +121,9 @@ struct SqRoundArgs {
   FusedSync* sync = nullptr;
   unsigned long long epoch = 0;
 };
-cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a, int write_r, int loss_reduce, int sms, int max_ctas_per_sm,
-                                      cudaStream_t stream, int* grid_out, void* window_base = nullptr, size_t window_bytes = 0);
+cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a, int write_r, int loss_reduce, int resident, int sms,
+                                      int max_ctas_per_sm, cudaStream_t stream, int* grid_out, int* resident_slots_out,
+                                      void* window_base = nullptr, size_t window_bytes = 0);
 
 // Brent's whole line search for a dim-1 scalar loss in one launch (persistent workers + coordinator warp).
 struct LsArgs {
