@@ -1,0 +1,107 @@
+"""Device regression-tree fit (se_tree_fit): CUDA-event times per level and per tree, achieved bytes/s against the
+byte model of DESIGN.md §3 "Device tree fit", and GBM rounds/s with the device learner against the host learner.
+
+    python benchmarks/tree_fit_time.py [--rows 100000000] [--cols 128] [--gbm-rows 10000000] [--host-rows 1000000]
+
+The feature matrix of the tree timings is filled on the device (uniform), labels are normal; the split candidates
+come from the first 10000 rows of each column (the candidate rule's sample size at maxBins 32).  A level's time is
+the difference between the fit times of trees one level apart, so it includes everything a level launches."""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from spark_ensemble_b200 import _native as N  # noqa: E402
+from spark_ensemble_b200.context import Context  # noqa: E402
+from spark_ensemble_b200.learners import DeviceDecisionTreeRegressor, continuous_split_candidates  # noqa: E402
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        return q
+    except Exception as e:  # pragma: no cover
+        return f"unknown ({e})"
+
+
+def tree_times(n, d, max_bins, depths, reps):
+    out = {}
+    with Context(0) as ctx:
+        ctx.alloc(N.SLOT_X, d, n)
+        ctx.fill_synthetic(N.SLOT_X, "uniform", 1, 0.0, 1.0)
+        ctx.alloc(N.SLOT_R, 1, n)
+        ctx.fill_synthetic(N.SLOT_R, "normal", 2, 0.0, 1.0)
+        ctx.alloc(N.SLOT_H, 1, n)
+        m = min(n, 10000)
+        cands = [continuous_split_candidates(ctx.download(N.SLOT_X, count=m, offset=j * n), max_bins) for j in range(d)]
+        ctx.tree_fit_bins(cands)
+        sub = np.arange(d, dtype=np.int32)
+        for depth in depths:
+            ctx.tree_fit(N.SLOT_R, 0, subspace=sub, max_depth=depth, out_slot=N.SLOT_H)  # warm-up
+            ts = []
+            for _ in range(reps):
+                ctx.timer_start()
+                t = ctx.tree_fit(N.SLOT_R, 0, subspace=sub, max_depth=depth, out_slot=N.SLOT_H)
+                ts.append(ctx.timer_stop())
+            out[depth] = {"ms_median": float(np.median(ts)), "ms_min": float(np.min(ts)), "nodes": int(t["feature"].size)}
+    return out
+
+
+def gbm_rounds(n, d, learner, rounds, resident=True):
+    from spark_ensemble_b200.ensemble import DataFrame
+    from spark_ensemble_b200.regression import GBMRegressor
+    rng = np.random.default_rng(0)
+    X = rng.random((n, d), dtype=np.float32)
+    y = np.sin(6 * X[:, 0]) + X[:, 1] * X[:, 2] + 0.1 * rng.standard_normal(n)
+    df = DataFrame(features=X, label=y)
+    times = {}
+    for k in (1, rounds):
+        g = GBMRegressor().set("baseLearner", learner).set("numBaseLearners", k).set("residentFeatures", resident)
+        t0 = time.perf_counter()
+        g.fit(df)
+        times[k] = time.perf_counter() - t0
+    per_round = (times[rounds] - times[1]) / (rounds - 1)
+    return {"rows": n, "cols": d, "rounds": rounds, "fit_s": times[rounds], "s_per_round": per_round,
+            "rounds_per_s": 1.0 / per_round}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rows", type=int, default=100_000_000)
+    ap.add_argument("--cols", type=int, default=128)
+    ap.add_argument("--bins", type=int, default=32)
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--gbm-rows", type=int, default=10_000_000)
+    ap.add_argument("--gbm-cols", type=int, default=32)
+    ap.add_argument("--host-rows", type=int, default=1_000_000)
+    args = ap.parse_args()
+    res = {"card": card()}
+    n, d = args.rows, args.cols
+    tt = tree_times(n, d, args.bins, list(range(0, 7)), args.reps)
+    res["tree_ms"] = tt
+    bytes_level = n * (d + 4 + 2 + 2 + 1)  # ranks, labels, node index in and out, one gathered rank (no weights, no bag)
+    levels = {}
+    for L in range(6):
+        ms = tt[L + 1]["ms_median"] - tt[L]["ms_median"]
+        levels[L] = {"ms": ms, "model_bytes": bytes_level, "achieved_GBps": bytes_level / (ms * 1e-3) / 1e9}
+    res["levels"] = levels
+    res["byte_model_ms_per_level_at_3.06TBps"] = bytes_level / 3.06e12 * 1e3
+    print(json.dumps(res, indent=1), flush=True)
+    res["gbm_device"] = gbm_rounds(args.gbm_rows, args.gbm_cols, DeviceDecisionTreeRegressor(maxDepth=5), 20)
+    print(json.dumps({"gbm_device": res["gbm_device"]}), flush=True)
+    from spark_ensemble_b200.learners import DecisionTreeRegressor
+    res["gbm_host"] = gbm_rounds(args.host_rows, args.gbm_cols, DecisionTreeRegressor(maxDepth=5), 3)
+    print(json.dumps({"gbm_host": res["gbm_host"]}), flush=True)
+
+
+if __name__ == "__main__":
+    main()

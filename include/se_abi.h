@@ -344,6 +344,31 @@ SE_API int se_tree_predict_multi(se_ctx* ctx, int which, int n_nodes, const int3
 SE_API int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offsets, const int32_t* feature,
                              const float* threshold, const int32_t* left, const int32_t* right, const float* value,
                              const double* weights, double init, int out_slot, int out_row);
+/* ---- regression-tree fit on the device (DESIGN.md §3 "Device tree fit") ----------------------- */
+/* Sets the split candidates of a fit: column c of SE_SLOT_X (n_cols == its column count) gets the sorted, finite,
+ * strictly increasing thresholds[offsets[c] .. offsets[c+1]) (0..255 of them) as the edge list of the uint8 rank matrix
+ * the tree walks use, and is re-ranked on the device.  The rank matrix is shared with se_tree_predict / se_forest_predict,
+ * not duplicated.  Each column is marked as holding fit candidates; a walk that later inserts a threshold into such a
+ * column (e.g. a host-fitted tree in the same context) clears the mark, and se_tree_fit on it then fails with
+ * SE_ERR_STATE instead of binning against other edges. */
+SE_API int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const float* thresholds);
+/* Fits one regression tree: Spark's DecisionTreeRegressor (variance impurity, continuous features, level-wise best split
+ * over the candidates of se_tree_fit_bins, prune = true), restated in DESIGN.md §3.  Labels are row label_row of
+ * label_slot ([.][n]; SE_SLOT_R in a fit: reading it never rebuilds F); weights row weight_row of weight_slot, or all 1
+ * when weight_slot < 0; bag multiplicities from SE_SLOT_BAG when use_bag.  A node's statistics are fp64 sums over its
+ * rows of c, c·w, c·w·r and c·w·r².  In Newton mode pass SE_SLOT_WOUT: the device holds 1/2·h·w without the 1/S factor,
+ * which scales every weight alike, and no gain comparison, prediction or weight fraction depends on that scale.
+ * `subspace` maps the tree's feature index k to column subspace[k] of X (NULL: k itself), n_subspace >= 1.
+ * Bounds (SE_ERR_ARG): 0 <= max_depth <= 8, min_instances >= 1, 0 <= min_weight_fraction < 0.5.
+ * Returns the tree in the array form of se_tree_predict (BFS order, subspace-local feature, -1 for leaves; value = fp32
+ * of every node's prediction) in arrays of max_nodes entries, the gain of every internal node (gain may be NULL) and
+ * n_nodes.  Also writes the tree's output for every row, in the bag or not, into row out_row of out_slot; it equals
+ * se_tree_predict of the returned arrays bit for bit.  One device-to-host copy per call (the node records).
+ * Fails with SE_ERR_ARG when a communicator with more than one rank is attached (histograms are not all-reduced). */
+SE_API int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                       const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
+                       double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
+                       float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes);
 /* linear model: out = intercept + Σ_j coef[j]·X[subspace[j]] */
 SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,
                       const int32_t* subspace, int out_slot, int out_row);

@@ -140,6 +140,8 @@ NOT_BOUND = {
     "se_brent_minimize": "takes a C callback; the JVM side keeps commons-math3's BrentOptimizer (or calls gbmLinesearchBrent / gbmRound)",
     "se_slot_info": "returns a raw device pointer: not exposed to the JVM",
     "se_spark_bernoulli_sample": "restates Spark's BernoulliSampler for hosts WITHOUT Spark; the JVM side draws with Spark itself",
+    "se_tree_fit_bins": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
+    "se_tree_fit": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
 }
 
 HAND_CPP = r'''

@@ -16,7 +16,7 @@ from .ensemble import DataFrame, fit_dummy_classifier, java_string_hash, subspac
 from .gbm_engine import GBMEngine
 from .params import (Param, Params, ParamValidators, boosting_params, gbm_params, random_uid,
                      shared_classifier_params, shared_predictor_params, subbag_params)
-from .regression import _extract_instances, _split_validation, bag_counts
+from .regression import _check_device_learner, _extract_instances, _split_validation, bag_counts
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -115,6 +115,7 @@ class GBMClassifier(Params):
             if init_raw.shape[0] != dim:
                 raise ValueError("prior init needs every class present in the training labels")
 
+        device_fit = _check_device_learner(self, learner)
         from .sharded import make_context
         ctx = make_context(self.device, self("devices"))  # Param `devices`: rows sharded over several GPUs
         try:
@@ -131,17 +132,21 @@ class GBMClassifier(Params):
             i = v = 0
             while i < num_learners and v < self("numRounds"):  # :325
                 sub = subspaces[i]
-                r, wout = eng.fetch_residuals(newton)
-                imodels = []
-                for j in range(dim):  # one regressor per dimension (:377-411; Futures in the reference)
-                    fit_w = wout[j] if newton else w
-                    if counts is None:
-                        imodels.append(learner.fit(X[:, sub], r[j], fit_w))
-                    else:
-                        bw = counts[in_bag] if fit_w is None else counts[in_bag] * fit_w[in_bag]
-                        imodels.append(learner.fit(X[in_bag][:, sub], r[j][in_bag], bw))
-                for j in range(dim):
-                    eng.set_direction_from_model(j, imodels[j], sub, X)
+                if device_fit:  # each dimension's tree is fitted on the device and writes its own H row
+                    imodels = [eng.fit_direction(j, learner, sub, newton=newton, bag=counts is not None)
+                               for j in range(dim)]
+                else:
+                    r, wout = eng.fetch_residuals(newton)
+                    imodels = []
+                    for j in range(dim):  # one regressor per dimension (:377-411; Futures in the reference)
+                        fit_w = wout[j] if newton else w
+                        if counts is None:
+                            imodels.append(learner.fit(X[:, sub], r[j], fit_w))
+                        else:
+                            bw = counts[in_bag] if fit_w is None else counts[in_bag] * fit_w[in_bag]
+                            imodels.append(learner.fit(X[in_bag][:, sub], r[j][in_bag], bw))
+                    for j in range(dim):
+                        eng.set_direction_from_model(j, imodels[j], sub, X)
                 if self("optimizedWeights"):  # :413-431
                     if self("lineSearch") == "newton" and dim == 1:
                         a1, _, _ = eng.line_search_newton(self("tol"), self("maxIter"))

@@ -408,3 +408,37 @@ class Context:
         sub = None if subspace is None else np.ascontiguousarray(subspace, dtype=np.int32)
         self._ck(self._lib.se_linear_predict(self._h, int(validation), c.size, N.fptr(c), float(intercept),
                                              None if sub is None else N.iptr(sub), out_slot, out_row))
+
+    # ---- regression-tree fit on the device
+    def tree_fit_bins(self, candidates):
+        """Split candidates of a fit, one sorted fp32 list per column of SLOT_X (se_tree_fit_bins)."""
+        cands = [np.ascontiguousarray(c, dtype=np.float32).reshape(-1) for c in candidates]
+        offs = np.zeros(len(cands) + 1, dtype=np.int32)
+        offs[1:] = np.cumsum([c.size for c in cands])
+        thr = np.ascontiguousarray(np.concatenate(cands) if cands else np.zeros(0), dtype=np.float32)
+        self._ck(self._lib.se_tree_fit_bins(self._h, len(cands), N.iptr(offs), N.fptr(thr) if thr.size else None))
+
+    def tree_fit(self, label_slot: int, label_row: int = 0, weight_slot: int = -1, weight_row: int = 0,
+                 use_bag: bool = False, subspace=None, n_subspace: int | None = None, max_depth: int = 5,
+                 min_instances: int = 1, min_info_gain: float = 0.0, min_weight_fraction: float = 0.0,
+                 out_slot: int = N.SLOT_H, out_row: int = 0) -> dict:
+        """Fits one regression tree over the rank matrix (se_tree_fit) and writes its output for every row into
+        out_slot row out_row.  Returns the array form of se_tree_predict plus the gain of every internal node."""
+        sub = None if subspace is None else np.ascontiguousarray(subspace, dtype=np.int32)
+        ns = int(sub.size if sub is not None else n_subspace)
+        cap = (1 << (int(max_depth) + 1)) - 1 if 0 <= int(max_depth) <= 8 else 1
+        f = np.zeros(cap, dtype=np.int32)
+        t = np.zeros(cap, dtype=np.float32)
+        l = np.zeros(cap, dtype=np.int32)
+        r = np.zeros(cap, dtype=np.int32)
+        v = np.zeros(cap, dtype=np.float32)
+        g = np.zeros(cap, dtype=np.float64)
+        nn = C.c_int32()
+        self._ck(self._lib.se_tree_fit(self._h, int(label_slot), int(label_row), int(weight_slot), int(weight_row),
+                                       int(bool(use_bag)), None if sub is None else N.iptr(sub), ns, int(max_depth),
+                                       int(min_instances), float(min_info_gain), float(min_weight_fraction),
+                                       int(out_slot), int(out_row), cap, N.iptr(f), N.fptr(t), N.iptr(l), N.iptr(r),
+                                       N.fptr(v), N.dptr(g), C.byref(nn)))
+        k = nn.value
+        return {"feature": f[:k].copy(), "threshold": t[:k].copy(), "left": l[:k].copy(), "right": r[:k].copy(),
+                "value": v[:k].copy(), "gain": g[:k].copy()}

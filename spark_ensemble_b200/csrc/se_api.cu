@@ -109,6 +109,7 @@ struct BinState {
   bool valid = false;                      // X8 reflects the current contents of the slot for every column with edges
   std::vector<std::vector<float>> edges;   // per column
   std::vector<char> dirty;
+  std::vector<char> fit;                   // per column: the edges are exactly the candidates se_tree_fit_bins set
   float* d_edges = nullptr;                // [d][256]
   int32_t* d_nedges = nullptr;             // [d]
   int32_t* d_cols = nullptr;               // [d]
@@ -258,6 +259,18 @@ struct se_ctx {
   int tree_mask = 1;                  // shallow trees (<= 64 internal nodes): all-nodes comparison kernel over the rank matrix
   int last_tree_mask = 0;
   int last_tree_binned = 0, last_tree_rebinned_cols = 0;
+  // regression-tree fit (se_tree_fit): scratch kept across the rounds of a fit
+  struct {
+    uint16_t* d_nid = nullptr;        // two [nid_cap] node-index buffers (levels alternate)
+    int64_t nid_cap = 0;
+    double* d_hist = nullptr;
+    size_t hist_bytes = 0;
+    TreeFitNode* d_nodes = nullptr;   // [kTreeFitHeap]
+    uint2* d_dec = nullptr;           // [kTreeFitHeap]
+    int32_t* d_cols = nullptr;
+    int cols_cap = 0;
+    int smem_optin = 0;
+  } tf;
   std::string err;
   // stopwatch + per-kernel-family timing
   cudaEvent_t tm0 = nullptr, tm1 = nullptr;
@@ -773,6 +786,11 @@ int se_ctx_destroy(se_ctx* ctx) {
   free_bins(ctx->bins[1]);
   if (ctx->d_wm) cudaFree(ctx->d_wm);
   if (ctx->d_forest) cudaFree(ctx->d_forest);
+  if (ctx->tf.d_nid) cudaFree(ctx->tf.d_nid);
+  if (ctx->tf.d_hist) cudaFree(ctx->tf.d_hist);
+  if (ctx->tf.d_nodes) cudaFree(ctx->tf.d_nodes);
+  if (ctx->tf.d_dec) cudaFree(ctx->tf.d_dec);
+  if (ctx->tf.d_cols) cudaFree(ctx->tf.d_cols);
   if (ctx->big.d_coef) cudaFree(ctx->big.d_coef);
   if (ctx->big.h_coef) cudaFreeHost(ctx->big.h_coef);
   if (ctx->big.d_partials) cudaFree(ctx->big.d_partials);
@@ -2567,40 +2585,33 @@ namespace {
 // Makes the rank matrix of slot X cover every threshold of the given nodes (col[i] < 0: leaf): allocates it on first
 // use, inserts new thresholds into the per-column edge lists and re-ranks the columns that changed.  Returns 1 when the
 // matrix is ready, 0 when it cannot be used (disabled, no memory, NaN threshold, a column with more than 255 edges).
-int bins_prepare(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const int32_t* col, const float* thr) {
-  ctx->last_tree_rebinned_cols = 0;
-  if (!ctx->tree_bins || X.rows > 65535 || X.cols == 0) return 0;
-  BinState& B = ctx->bins[which];
+// Allocates the rank matrix of slot X on first use (or when the slot's shape changed).  False when there is no room.
+bool bins_ensure(BinState& B, const SlotBuf& X) {
   const int d = (int)X.rows;
-  if (!B.d8 || B.d != d || B.n != X.cols) {
+  if (B.d8 && B.d == d && B.n == X.cols) return true;
+  free_bins(B);
+  const int64_t ld8 = ((X.cols + 127) / 128) * 128;
+  bool ok = cudaMalloc(&B.d8, (size_t)d * (size_t)ld8) == cudaSuccess && cudaMalloc(&B.d_edges, sizeof(float) * 256 * (size_t)d) == cudaSuccess &&
+            cudaMalloc(&B.d_nedges, sizeof(int32_t) * (size_t)d) == cudaSuccess && cudaMalloc(&B.d_cols, sizeof(int32_t) * (size_t)d) == cudaSuccess;
+  if (!ok) {
+    cudaGetLastError();
     free_bins(B);
-    const int64_t ld8 = ((X.cols + 127) / 128) * 128;
-    bool ok = cudaMalloc(&B.d8, (size_t)d * (size_t)ld8) == cudaSuccess && cudaMalloc(&B.d_edges, sizeof(float) * 256 * (size_t)d) == cudaSuccess &&
-              cudaMalloc(&B.d_nedges, sizeof(int32_t) * (size_t)d) == cudaSuccess && cudaMalloc(&B.d_cols, sizeof(int32_t) * (size_t)d) == cudaSuccess;
-    if (!ok) {  // e.g. no room for another d x n bytes: keep walking the fp32 matrix
-      cudaGetLastError();
-      free_bins(B);
-      ctx->tree_bins = 0;
-      return 0;
-    }
-    B.ld8 = ld8; B.n = X.cols; B.d = d;
-    B.edges.assign((size_t)d, std::vector<float>());
-    B.dirty.assign((size_t)d, 0);
-    B.valid = true;
+    return false;
   }
+  B.ld8 = ld8; B.n = X.cols; B.d = d;
+  B.edges.assign((size_t)d, std::vector<float>());
+  B.dirty.assign((size_t)d, 0);
+  B.fit.assign((size_t)d, 0);
+  B.valid = true;
+  return true;
+}
+
+// Re-ranks every dirty column (and every column with edges when the slot was rewritten)
+int bins_rerank(se_ctx* ctx, BinState& B, const SlotBuf& X) {
+  const int d = B.d;
   if (!B.valid) {  // the slot was rewritten: every column that has edges must be re-ranked
     for (int c = 0; c < d; ++c) B.dirty[c] = B.edges[c].empty() ? 0 : 1;
     B.valid = true;
-  }
-  for (int i = 0; i < n_nodes; ++i) {
-    if (col[i] < 0) continue;
-    if (!(thr[i] == thr[i])) return 0;  // NaN threshold: leave it to the fp32 walk
-    std::vector<float>& E = B.edges[col[i]];
-    auto it = std::lower_bound(E.begin(), E.end(), thr[i]);
-    if (it != E.end() && *it == thr[i]) continue;
-    if (E.size() >= 255) return 0;      // this column needs more ranks than a byte holds
-    E.insert(it, thr[i]);
-    B.dirty[col[i]] = 1;
   }
   std::vector<int32_t> cols;
   for (int c = 0; c < d; ++c)
@@ -2609,7 +2620,8 @@ int bins_prepare(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const in
     std::vector<int32_t> ne((size_t)d);
     for (int c = 0; c < d; ++c) ne[c] = (int32_t)B.edges[c].size();
     for (int32_t c : cols)
-      SE_CUDA(ctx, cudaMemcpyAsync(B.d_edges + (size_t)c * 256, B.edges[c].data(), sizeof(float) * B.edges[c].size(), cudaMemcpyHostToDevice, ctx->stream));
+      if (!B.edges[c].empty())
+        SE_CUDA(ctx, cudaMemcpyAsync(B.d_edges + (size_t)c * 256, B.edges[c].data(), sizeof(float) * B.edges[c].size(), cudaMemcpyHostToDevice, ctx->stream));
     SE_CUDA(ctx, cudaMemcpyAsync(B.d_nedges, ne.data(), sizeof(int32_t) * (size_t)d, cudaMemcpyHostToDevice, ctx->stream));
     SE_CUDA(ctx, cudaMemcpyAsync(B.d_cols, cols.data(), sizeof(int32_t) * cols.size(), cudaMemcpyHostToDevice, ctx->stream));
     SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the host vectors above go out of scope
@@ -2620,6 +2632,29 @@ int bins_prepare(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const in
     for (int32_t c : cols) B.dirty[c] = 0;
     ctx->last_tree_rebinned_cols = (int)cols.size();
   }
+  return SE_OK;
+}
+
+int bins_prepare(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const int32_t* col, const float* thr) {
+  ctx->last_tree_rebinned_cols = 0;
+  if (!ctx->tree_bins || X.rows > 65535 || X.cols == 0) return 0;
+  BinState& B = ctx->bins[which];
+  if (!bins_ensure(B, X)) {  // e.g. no room for another d x n bytes: keep walking the fp32 matrix
+    ctx->tree_bins = 0;
+    return 0;
+  }
+  for (int i = 0; i < n_nodes; ++i) {
+    if (col[i] < 0) continue;
+    if (!(thr[i] == thr[i])) return 0;  // NaN threshold: leave it to the fp32 walk
+    std::vector<float>& E = B.edges[col[i]];
+    auto it = std::lower_bound(E.begin(), E.end(), thr[i]);
+    if (it != E.end() && *it == thr[i]) continue;
+    if (E.size() >= 255) return 0;      // this column needs more ranks than a byte holds
+    E.insert(it, thr[i]);
+    B.dirty[col[i]] = 1;
+    B.fit[col[i]] = 0;                  // no longer the fit's candidates: se_tree_fit refuses the column
+  }
+  SE_TRY(bins_rerank(ctx, B, X));
   return 1;
 }
 
@@ -2928,3 +2963,204 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
 }
 
 }  // extern "C"
+
+// ---- regression-tree fit over the rank matrix (se_tree_fit.cu) -----------------------------------
+int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const float* thresholds) {
+  if (!ctx || !offsets) return fail(ctx, SE_ERR_ARG, "null argument");
+  const SlotBuf& X = ctx->slot[SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
+  SE_REQUIRE(ctx, n_cols == X.rows, SE_ERR_ARG, "%d candidate lists for a feature matrix of %lld columns", n_cols, (long long)X.rows);
+  SE_REQUIRE(ctx, X.rows <= 65535, SE_ERR_ARG, "the rank matrix holds at most 65535 columns");
+  SE_REQUIRE(ctx, offsets[0] == 0, SE_ERR_ARG, "offsets[0] must be 0");
+  for (int c = 0; c < n_cols; ++c) {
+    const int32_t b = offsets[c], m = offsets[c + 1] - offsets[c];
+    SE_REQUIRE(ctx, m >= 0 && m <= 255, SE_ERR_ARG, "column %d: %d candidates (0..255 supported)", c, m);
+    SE_REQUIRE(ctx, m == 0 || thresholds, SE_ERR_ARG, "null thresholds");
+    for (int i = 0; i < m; ++i) {
+      SE_REQUIRE(ctx, isfinite(thresholds[b + i]), SE_ERR_ARG, "column %d: candidate %d is not finite", c, i);
+      SE_REQUIRE(ctx, i == 0 || thresholds[b + i - 1] < thresholds[b + i], SE_ERR_ARG,
+                 "column %d: candidates are not strictly increasing at %d", c, i);
+    }
+  }
+  SE_TRY(begin(ctx));
+  release_l2_persist(ctx);
+  BinState& B = ctx->bins[0];
+  SE_REQUIRE(ctx, bins_ensure(B, X), SE_ERR_CUDA, "no device memory for the rank matrix (%lld x %lld bytes)",
+             (long long)X.rows, (long long)X.cols);
+  for (int c = 0; c < n_cols; ++c) {
+    B.edges[c].assign(thresholds ? thresholds + offsets[c] : nullptr, thresholds ? thresholds + offsets[c + 1] : nullptr);
+    B.dirty[c] = 1;
+    B.fit[c] = 1;
+  }
+  SE_TRY(bins_rerank(ctx, B, X));
+  return end(ctx);
+}
+
+int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
+                double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
+                float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
+  if (!ctx || !feature || !threshold || !left || !right || !value || !n_nodes) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, max_depth >= 0 && max_depth <= 8, SE_ERR_ARG, "maxDepth %d outside [0, 8]", max_depth);
+  SE_REQUIRE(ctx, min_instances >= 1, SE_ERR_ARG, "minInstancesPerNode %d < 1", min_instances);
+  SE_REQUIRE(ctx, min_weight_fraction >= 0.0 && min_weight_fraction < 0.5, SE_ERR_ARG,
+             "minWeightFractionPerNode %g outside [0, 0.5)", min_weight_fraction);
+  SE_REQUIRE(ctx, !isnan(min_info_gain), SE_ERR_ARG, "minInfoGain is NaN");
+  SE_REQUIRE(ctx, !(ctx->comm && ctx->nranks > 1), SE_ERR_ARG,
+             "se_tree_fit fits on one GPU: its histograms are not all-reduced across %d ranks", ctx->nranks);
+  const SlotBuf& X = ctx->slot[SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
+  const int64_t n = X.cols;
+  auto row_of = [&](int slot, int row, const char* what, const float** p) -> int {
+    SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad %s slot %d", what, slot);
+    const SlotBuf& s = ctx->slot[slot];
+    SE_REQUIRE(ctx, s.d && s.cols == n && row >= 0 && row < s.rows, SE_ERR_STATE, "%s slot %d: no row %d of %lld values", what,
+               slot, row, (long long)n);
+    *p = s.d + (int64_t)row * (s.rows > 1 ? s.ld : s.cols);
+    return SE_OK;
+  };
+  const float *r = nullptr, *w = nullptr, *bag = nullptr, *outc = nullptr;
+  SE_TRY(row_of(label_slot, label_row, "label", &r));
+  if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &w));
+  if (use_bag) SE_TRY(row_of(SE_SLOT_BAG, 0, "bag", &bag));
+  SE_TRY(row_of(out_slot, out_row, "output", &outc));
+  SE_REQUIRE(ctx, n_subspace >= 1, SE_ERR_ARG, "empty subspace");
+  BinState& B = ctx->bins[0];
+  SE_REQUIRE(ctx, B.d8 && B.d == X.rows && B.n == X.cols, SE_ERR_STATE,
+             "no split candidates for this feature matrix: call se_tree_fit_bins first");
+  std::vector<int32_t> cols((size_t)n_subspace);
+  int maxc = 0;
+  for (int k = 0; k < n_subspace; ++k) {
+    const int32_t c = subspace ? subspace[k] : k;
+    SE_REQUIRE(ctx, c >= 0 && c < X.rows, SE_ERR_ARG, "subspace entry %d: column %d outside X with %lld columns", k, c,
+               (long long)X.rows);
+    SE_REQUIRE(ctx, B.fit[c], SE_ERR_STATE,
+               "column %d does not hold the fit's split candidates (never set, or a tree walk added a threshold to it): "
+               "call se_tree_fit_bins again", c);
+    cols[k] = c;
+    maxc = std::max(maxc, (int)B.edges[c].size());
+  }
+  const int nb = std::min(256, maxc + 2);  // ranks 0..maxc, then NaN (rank 255) in the last bin
+  SE_TRY(begin(ctx));
+  release_l2_persist(ctx);
+  if (label_slot == SE_SLOT_F || weight_slot == SE_SLOT_F || is_yfr(out_slot)) SE_TRY(settle_f(ctx));
+  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
+  SE_TRY(bins_rerank(ctx, B, X));  // X was rewritten since the candidates were set
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_small is reused below
+  // ---- scratch
+  auto& T = ctx->tf;
+  const int64_t nw = (n + 3) >> 2;
+  if (T.nid_cap < 4 * nw) {
+    if (T.d_nid) cudaFree(T.d_nid);
+    T.d_nid = nullptr; T.nid_cap = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_nid, sizeof(uint16_t) * 2 * 4 * (size_t)nw));
+    T.nid_cap = 4 * nw;
+  }
+  const int top = max_depth > 0 ? max_depth - 1 : 0;  // deepest level that is searched (or, at depth 0, only summed)
+  const size_t hist_bytes = ((size_t)1 << top) * (size_t)n_subspace * (size_t)nb * 4 * sizeof(double);
+  if (T.hist_bytes < hist_bytes) {
+    if (T.d_hist) cudaFree(T.d_hist);
+    T.d_hist = nullptr; T.hist_bytes = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_hist, hist_bytes));
+    T.hist_bytes = hist_bytes;
+  }
+  if (!T.d_nodes) {
+    SE_CUDA(ctx, cudaMalloc(&T.d_nodes, sizeof(TreeFitNode) * kTreeFitHeap));
+    SE_CUDA(ctx, cudaMalloc(&T.d_dec, sizeof(uint2) * kTreeFitHeap));
+    int optin = 0;
+    SE_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    T.smem_optin = optin;
+  }
+  if (T.cols_cap < n_subspace) {
+    if (T.d_cols) cudaFree(T.d_cols);
+    T.d_cols = nullptr; T.cols_cap = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_cols, sizeof(int32_t) * (size_t)n_subspace));
+    T.cols_cap = n_subspace;
+  }
+  SE_REQUIRE(ctx, sizeof(int32_t) * (size_t)n_subspace <= (size_t)kSmallBytes, SE_ERR_ARG, "subspace too large");
+  memcpy(ctx->h_small, cols.data(), sizeof(int32_t) * (size_t)n_subspace);
+  SE_CUDA(ctx, cudaMemcpyAsync(T.d_cols, ctx->h_small, sizeof(int32_t) * (size_t)n_subspace, cudaMemcpyHostToDevice, ctx->stream));
+  // ---- the fit: a fixed sequence of launches, no host round trip
+  TreeFitArgs a;
+  a.X8 = B.d8; a.ld8 = B.ld8; a.n = n;
+  a.cols = T.d_cols; a.n_edges = B.d_nedges; a.edges = B.d_edges;
+  a.S = n_subspace; a.nb = nb; a.max_depth = max_depth; a.search = max_depth > 0 ? 1 : 0;
+  a.has_w = w ? 1 : 0; a.r = r; a.w = w; a.bag = bag;
+  a.dec = T.d_dec; a.nodes = T.d_nodes; a.hist = T.d_hist;
+  a.min_instances = min_instances; a.min_info_gain = min_info_gain; a.min_weight_fraction = min_weight_fraction;
+  uint16_t* nid[2] = {T.d_nid, T.d_nid + T.nid_cap};
+  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, ctx->stream));
+  for (int L = 0; L <= top; ++L) {
+    a.L = L;
+    a.route = L >= 1;
+    a.nid_in = L >= 2 ? nid[(L - 1) & 1] : nullptr;
+    a.nid_out = L >= 1 ? nid[L & 1] : nullptr;
+    const size_t per_col = ((size_t)1 << L) * (size_t)nb * 4 * sizeof(double);
+    SE_CUDA(ctx, cudaMemsetAsync(T.d_hist, 0, per_col * (size_t)n_subspace, ctx->stream));
+    int smem_mode = 1, per_sm = 4;
+    size_t smem = 0;
+    if (per_col <= (size_t)kTreeFitSmemBudget) {
+      a.cb = (int)std::min<size_t>((size_t)n_subspace, kTreeFitSmemBudget / per_col);
+    } else if (per_col <= (size_t)T.smem_optin) {
+      a.cb = 1;
+      per_sm = per_col <= (size_t)T.smem_optin / 2 ? 2 : 1;
+    } else {  // one column's histogram of every node of the level does not fit: global fp64 atomics
+      smem_mode = 0;
+      a.cb = n_subspace;
+      per_sm = 8;
+    }
+    if (smem_mode) smem = per_col * (size_t)a.cb;
+    const int gx = smem_mode ? (n_subspace + a.cb - 1) / a.cb : 1;
+    int64_t gy = ((int64_t)ctx->sms * per_sm + gx - 1) / gx;
+    gy = std::min<int64_t>(gy, (nw + 255) / 256);
+    gy = std::max<int64_t>(std::min<int64_t>(gy, 65535), 1);
+    a.words_per_cta = (nw + gy - 1) / gy;
+    SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_hist(a, smem_mode, (int)gy, smem, ctx->stream));
+    SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_split(a, ctx->stream));
+  }
+  a.route = max_depth >= 1;
+  a.nid_in = max_depth >= 2 ? nid[(max_depth - 1) & 1] : nullptr;
+  a.nid_out = nullptr;
+  a.out = const_cast<float*>(outc);
+  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_out(a, ctx->sms, ctx->stream));
+  static_assert(sizeof(TreeFitNode) * kTreeFitHeap <= (size_t)kSmallBytes, "node records fit the staging buffer");
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->h_small, T.d_nodes, sizeof(TreeFitNode) * kTreeFitHeap, cudaMemcpyDeviceToHost, ctx->stream));
+  SE_TRY(end(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  // ---- prune (bottom-up: two leaf children with equal fp64 predictions) and number the nodes in BFS order
+  const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(ctx->h_small);
+  std::vector<char> leaf(kTreeFitHeap, 1);
+  std::vector<double> pred(kTreeFitHeap, 0.0);
+  std::vector<float> val(kTreeFitHeap, 0.f);
+  for (int h = 1; h < kTreeFitHeap; ++h) {
+    leaf[h] = R[h].state != 2;
+    pred[h] = R[h].pred;
+    val[h] = R[h].value;
+  }
+  for (int h = kTreeFitHeap / 2 - 1; h >= 1; --h) {
+    if (leaf[h] || !leaf[2 * h] || !leaf[2 * h + 1] || !(pred[2 * h] == pred[2 * h + 1])) continue;
+    leaf[h] = 1;
+    pred[h] = pred[2 * h];
+    val[h] = val[2 * h];
+  }
+  std::vector<int> order;
+  order.push_back(1);
+  for (size_t q = 0; q < order.size(); ++q)
+    if (!leaf[order[q]]) { order.push_back(2 * order[q]); order.push_back(2 * order[q] + 1); }
+  SE_REQUIRE(ctx, (int)order.size() <= max_nodes, SE_ERR_ARG, "the fitted tree has %d nodes, max_nodes is %d",
+             (int)order.size(), max_nodes);
+  std::vector<int> id(kTreeFitHeap, 0);
+  for (size_t q = 0; q < order.size(); ++q) id[order[q]] = (int)q;
+  for (size_t q = 0; q < order.size(); ++q) {
+    const int h = order[q];
+    const bool lf = leaf[h];
+    feature[q] = lf ? -1 : R[h].col;
+    threshold[q] = lf ? 0.f : R[h].thr;
+    left[q] = lf ? 0 : id[2 * h];
+    right[q] = lf ? 0 : id[2 * h + 1];
+    value[q] = val[h];
+    if (gain) gain[q] = lf ? 0.0 : R[h].gain;
+  }
+  *n_nodes = (int)order.size();
+  return SE_OK;
+}

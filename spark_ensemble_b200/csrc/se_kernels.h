@@ -273,6 +273,47 @@ struct ForestArgs {
 constexpr int kForestTile = 256;              // rows per CTA tile (one row per thread)
 constexpr int kForestSmemBudget = 54 * 1024;  // per CTA: four CTAs per SM (the walk is latency-bound: warps matter more than chunk size)
 cudaError_t launch_forest_predict(const ForestArgs& a, int sms, cudaStream_t s);
+// ---- regression-tree fit over the uint8 rank matrix (se_tree_fit.cu) -------------------------
+// Nodes are heap-indexed (root 1, children 2h, 2h + 1), so depth <= 8 needs 511 records.
+constexpr int kTreeFitHeap = 512;
+constexpr int kTreeFitSmemBudget = 56 * 1024;  // shared-memory histograms per CTA: four CTAs per SM
+struct TreeFitNode {                 // 64 B, downloaded once at the end of a fit
+  double cnt, w, s, q;               // rawCount, W, S, Q of the node's in-bag rows
+  double pred;                       // S / W
+  double gain;                       // of the chosen split (state 2)
+  int32_t state;                     // 0 unused, 1 leaf, 2 split
+  int32_t col, bin;                  // split: subspace-local column, left when rank <= bin
+  float thr;                         // split: the fp32 candidate
+  float value;                       // (float) pred
+  int32_t pad;
+};
+struct TreeFitArgs {
+  const uint8_t* X8 = nullptr;
+  int64_t ld8 = 0, n = 0;
+  const int32_t* cols = nullptr;     // device [S]: global column of subspace entry k
+  const int32_t* n_edges = nullptr;  // device [d]: candidates per column
+  const float* edges = nullptr;      // device [d][256]
+  int S = 0, nb = 0, L = 0, cb = 1, max_depth = 0;
+  int search = 1, route = 0, has_w = 0;
+  const float* r = nullptr;          // labels
+  const float* w = nullptr;          // weights (has_w)
+  const float* bag = nullptr;        // multiplicities or nullptr
+  const uint16_t* nid_in = nullptr;  // node of every row before this level's step (nullptr: the root)
+  uint16_t* nid_out = nullptr;       // after it (written by the first column block)
+  uint2* dec = nullptr;              // [kTreeFitHeap] x: global split column (~0: none), y: bin | open << 31
+  TreeFitNode* nodes = nullptr;      // [kTreeFitHeap]
+  double* hist = nullptr;            // [2^L][S][nb][4]
+  int64_t words_per_cta = 0;         // 4-row groups per CTA row range
+  int min_instances = 1;
+  double min_info_gain = 0.0, min_weight_fraction = 0.0;
+  float* out = nullptr;              // final pass: leaf value per row
+};
+cudaError_t launch_tree_fit_init(TreeFitNode* nodes, uint2* dec, cudaStream_t s);
+// smem_mode 1: shared-memory histograms of a.cb columns per CTA (smem bytes), folded into a.hist; 0: global atomics
+cudaError_t launch_tree_fit_hist(const TreeFitArgs& a, int smem_mode, int grid_y, size_t smem, cudaStream_t s);
+cudaError_t launch_tree_fit_split(const TreeFitArgs& a, cudaStream_t s);
+cudaError_t launch_tree_fit_out(const TreeFitArgs& a, int sms, cudaStream_t s);
+
 cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_coef,
                                   const float* coef, const int32_t* cols, float intercept,
                                   float* out, int sms, cudaStream_t s);

@@ -21,6 +21,8 @@ class GBMEngine:
         self.has_weights = has_weights
         ctx.gbm_configure(n, nv, dim, loss, param, has_weights)
         self._x_resident = False
+        self._X_host = None
+        self._fit_bins = None  # the device learner whose split candidates SLOT_X holds
 
     # ---- data in
     def load(self, y, w=None, F0=None, vy=None, vF0=None):
@@ -49,6 +51,8 @@ class GBMEngine:
         X = np.asarray(X)
         c.alloc(N.SLOT_X, X.shape[1], X.shape[0])
         c.upload_rowmajor(N.SLOT_X, X)  # transposed on the device, chunked + double buffered
+        self._X_host = X
+        self._fit_bins = None
         if Xv is not None and self.nv > 0:
             Xv = np.asarray(Xv)
             c.alloc(N.SLOT_VX, Xv.shape[1], Xv.shape[0])
@@ -63,6 +67,24 @@ class GBMEngine:
         r = self.ctx.download(N.SLOT_R, out=out).reshape(self.dim, self.n)
         wout = self.ctx.download(N.SLOT_WOUT).reshape(self.dim, self.n) if newton else None
         return r, wout
+
+    def fit_direction(self, j: int, learner, subspace, newton: bool = False, bag: bool = False):
+        """Fit the device tree learner on R row j (weights: WOUT row j in newton mode, else W when the fit has
+        weights; the bag's multiplicities when `bag`) and write its output into H row j.  The split candidates are
+        set once per fit, on the first call.  Nothing but the fitted tree crosses PCIe."""
+        if not self._x_resident:
+            raise ValueError("the device tree learner needs the features on the device (residentFeatures=True)")
+        c = self.ctx
+        if self._fit_bins is None:
+            c.tree_fit_bins(learner.split_candidates(self._X_host))
+            self._fit_bins = learner
+        if newton:
+            wslot, wrow = N.SLOT_WOUT, j
+        elif self.has_weights:
+            wslot, wrow = N.SLOT_W, 0
+        else:
+            wslot, wrow = -1, 0
+        return learner.fit_resident(c, N.SLOT_R, j, wslot, wrow, bag, subspace, N.SLOT_H, j)
 
     def set_direction(self, h, validation: bool = False):
         self.ctx.upload(N.SLOT_VH if validation else N.SLOT_H,

@@ -11,14 +11,19 @@ from __future__ import annotations
 import numpy as np
 
 
+def _floor_f32(t64: np.ndarray) -> np.ndarray:
+    """Largest fp32 <= each fp64 value, so `x <= t32` equals `x <= t64` for every fp32 x."""
+    t64 = np.asarray(t64, dtype=np.float64)
+    t32 = t64.astype(np.float32)
+    up = t32.astype(np.float64) > t64
+    t32[up] = np.nextafter(t32[up], np.float32(-np.inf))
+    return t32
+
+
 def _tree_arrays(tree) -> dict:
     t = tree.tree_
     leaf = t.children_left < 0
-    thr64 = t.threshold.astype(np.float64)
-    thr32 = thr64.astype(np.float32)
-    # largest fp32 <= fp64 threshold, so `x <= thr32` equals `x <= thr64` for every fp32 x
-    up = thr32.astype(np.float64) > thr64
-    thr32[up] = np.nextafter(thr32[up], np.float32(-np.inf))
+    thr32 = _floor_f32(t.threshold)
     return {
         "feature": np.where(leaf, -1, t.feature).astype(np.int32),
         "threshold": np.where(leaf, 0.0, thr32).astype(np.float32),
@@ -63,6 +68,156 @@ class DecisionTreeRegressor:
         sk.fit(np.asarray(X, dtype=np.float32), np.asarray(y, dtype=np.float64),
                sample_weight=None if w is None else np.asarray(w, dtype=np.float64))
         return DecisionTreeRegressionModel(sk)
+
+
+def continuous_split_candidates(values, max_bins: int) -> np.ndarray:
+    """Spark's findSplitsForContinuousFeature over one column's sample values (DESIGN.md §3 "Device tree fit"): sorted
+    distinct non-NaN values v_0 < ... < v_m with counts c_i (-0 counted as +0); every fp64 midpoint when m <= maxBins - 1,
+    else the midpoints where the running count passes the next multiple of N_s / maxBins.  Each midpoint is stored as the
+    largest fp32 below it; an infinite midpoint (a column holding +-inf) as +-FLT_MAX, so that it still separates the
+    infinite value from its finite neighbour and the lists stay finite."""
+    v = np.asarray(values, dtype=np.float64).reshape(-1)
+    v = v[~np.isnan(v)] + 0.0  # + 0.0 turns -0 into +0
+    vals, counts = np.unique(v, return_counts=True)
+    m = vals.size - 1
+    if m <= 0:
+        return np.zeros(0, dtype=np.float32)
+    mids = (vals[:-1] + vals[1:]) / 2.0
+    if m > max_bins - 1:
+        stride = counts.sum() / max_bins
+        cum = np.cumsum(counts)
+        keep = []
+        target = stride
+        for i in range(1, m + 1):  # the target moves only when a midpoint is emitted: sequential by nature
+            if abs(cum[i - 1] - target) < abs(cum[i] - target):
+                keep.append(i - 1)
+                target += stride
+        mids = mids[np.asarray(keep, dtype=np.int64)]
+    fmax = float(np.finfo(np.float32).max)
+    out = _floor_f32(np.clip(mids, -fmax, fmax))
+    return np.unique(out)  # sorted; clamping can only merge two candidates at the extremes
+
+
+class DeviceDecisionTreeRegressionModel(_Model):
+    """A regression tree fitted on the device, in the array form of se_tree_predict."""
+
+    def __init__(self, arrays: dict):
+        self._arrays = {k: np.asarray(v).copy() for k, v in arrays.items()}
+        self.numNodes = int(self._arrays["feature"].size)
+
+    def tree_arrays(self):
+        return {k: self._arrays[k] for k in ("feature", "threshold", "left", "right", "value")}
+
+    @property
+    def gains(self) -> np.ndarray:
+        return self._arrays["gain"]
+
+    def predict(self, X) -> np.ndarray:
+        """Host walk of the same arrays: left when x <= threshold (NaN goes right), fp32 features and values."""
+        X = np.asarray(X, dtype=np.float32)
+        f, t = self._arrays["feature"], self._arrays["threshold"]
+        l, r, v = self._arrays["left"], self._arrays["right"], self._arrays["value"]
+        node = np.zeros(X.shape[0], dtype=np.int64)
+        rows = np.arange(X.shape[0])
+        while True:
+            live = f[node] >= 0
+            if not live.any():
+                break
+            idx = rows[live]
+            nd = node[idx]
+            go_left = X[idx, f[nd]] <= t[nd]
+            node[idx] = np.where(go_left, l[nd], r[nd])
+        return v[node].astype(np.float64)
+
+
+class DeviceDecisionTreeRegressor:
+    """org.apache.spark.ml.regression.DecisionTreeRegressor fitted on the GPU: variance impurity, continuous features,
+    level-wise best split over at most maxBins - 1 candidates per column (se_tree_fit).  Params keep Spark's names and
+    defaults.  Inside GBMRegressor / GBMClassifier (residentFeatures=True) it fits on the device-resident residuals;
+    `fit` alone opens a context on `device`, uploads X, fits and closes it."""
+
+    device_learner = True
+
+    def __init__(self, maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1, minInfoGain: float = 0.0,
+                 minWeightFractionPerNode: float = 0.0, seed: int | None = None, device: int = 0):
+        from .ensemble import java_string_hash
+        self.maxDepth, self.maxBins = int(maxDepth), int(maxBins)
+        self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
+        self.minWeightFractionPerNode = float(minWeightFractionPerNode)
+        self.seed = java_string_hash("org.apache.spark.ml.regression.DecisionTreeRegressor") if seed is None else int(seed)
+        self.device = int(device)
+        self._check()
+
+    def _check(self):
+        if not 0 <= self.maxDepth <= 8:
+            raise ValueError(f"maxDepth must be in [0, 8], got {self.maxDepth}")
+        if not 2 <= self.maxBins <= 256:
+            raise ValueError(f"maxBins must be in [2, 256], got {self.maxBins}")
+        if self.minInstancesPerNode < 1:
+            raise ValueError(f"minInstancesPerNode must be >= 1, got {self.minInstancesPerNode}")
+        if not 0.0 <= self.minWeightFractionPerNode < 0.5:
+            raise ValueError(f"minWeightFractionPerNode must be in [0, 0.5), got {self.minWeightFractionPerNode}")
+
+    def copy(self, extra=None):
+        c = DeviceDecisionTreeRegressor(self.maxDepth, self.maxBins, self.minInstancesPerNode, self.minInfoGain,
+                                        self.minWeightFractionPerNode, self.seed, self.device)
+        for k, v in (extra or {}).items():
+            setattr(c, k, v)
+        c._check()
+        return c
+
+    def sample_rows(self, n: int):
+        """Rows the candidates are drawn from: all of them when n <= max(maxBins², 10000), else Spark's Bernoulli
+        sample at fraction max(maxBins², 10000) / n with this learner's seed.  None means every row."""
+        required = max(self.maxBins * self.maxBins, 10000)
+        if n <= required:
+            return None
+        import ctypes
+        from . import _native as N
+        c = np.zeros(n, dtype=np.float32)
+        s64 = int(self.seed) & 0xFFFFFFFFFFFFFFFF
+        s64 = s64 - (1 << 64) if s64 >= (1 << 63) else s64
+        N.check(N.load().se_spark_bernoulli_sample(ctypes.c_int64(s64), required / n, n, 0, N.fptr(c)))
+        return np.flatnonzero(c > 0)
+
+    def split_candidates(self, X) -> list:
+        """Split candidates of every column of X, computed once per fit from the feature values only."""
+        self._check()
+        X = np.asarray(X, dtype=np.float32)
+        rows = self.sample_rows(X.shape[0])
+        S = X if rows is None else X[rows]
+        return [continuous_split_candidates(S[:, j], self.maxBins) for j in range(X.shape[1])]
+
+    def fit_resident(self, ctx, label_slot: int, label_row: int, weight_slot: int, weight_row: int, use_bag: bool,
+                     subspace, out_slot: int, out_row: int) -> DeviceDecisionTreeRegressionModel:
+        """Fit over a context whose SLOT_X already holds this learner's candidates (Context.tree_fit_bins)."""
+        self._check()
+        t = ctx.tree_fit(label_slot, label_row, weight_slot, weight_row, use_bag, subspace=subspace,
+                         max_depth=self.maxDepth, min_instances=self.minInstancesPerNode,
+                         min_info_gain=self.minInfoGain, min_weight_fraction=self.minWeightFractionPerNode,
+                         out_slot=out_slot, out_row=out_row)
+        return DeviceDecisionTreeRegressionModel(t)
+
+    def fit(self, X, y, w=None) -> DeviceDecisionTreeRegressionModel:
+        from . import _native as N
+        from .context import Context
+        X = np.asarray(X, dtype=np.float32)
+        n, d = X.shape
+        if n == 0 or d == 0:
+            raise ValueError("DeviceDecisionTreeRegressor.fit needs at least one row and one column")
+        cands = self.split_candidates(X)
+        with Context(self.device) as ctx:
+            ctx.alloc(N.SLOT_X, d, n)
+            ctx.upload_rowmajor(N.SLOT_X, X)
+            ctx.alloc(N.SLOT_Y, n)
+            ctx.upload(N.SLOT_Y, np.asarray(y, dtype=np.float32))
+            if w is not None:
+                ctx.alloc(N.SLOT_W, n)
+                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
+            ctx.alloc(N.SLOT_H, n)
+            ctx.tree_fit_bins(cands)
+            return self.fit_resident(ctx, N.SLOT_Y, 0, N.SLOT_W if w is not None else -1, 0, False,
+                                     np.arange(d, dtype=np.int32), N.SLOT_H, 0)
 
 
 class DecisionTreeClassificationModel(_Model):

@@ -51,6 +51,18 @@ def bag_counts(n: int, subsample_ratio: float, replacement: bool, seed: int):
     return rng.poisson(subsample_ratio, n).astype(np.float32)
 
 
+def _check_device_learner(est: Params, learner) -> bool:
+    """True when the base learner fits on the device (learners.DeviceDecisionTreeRegressor).  It reads the residuals
+    and the features where they live, so it needs residentFeatures=True and a single GPU."""
+    if not getattr(learner, "device_learner", False):
+        return False
+    if not est("residentFeatures"):
+        raise ValueError("the device tree learner fits over the device-resident features: set residentFeatures=True")
+    if len(est("devices")) >= 2:
+        raise ValueError("the device tree learner fits on one GPU: `devices` must name at most one device")
+    return True
+
+
 def _split_validation(est: Params, dataset: DataFrame):
     vc = est("validationIndicatorCol") if est.isDefined("validationIndicatorCol") else ""
     if vc:
@@ -105,6 +117,8 @@ class GBMRegressor(Params):
         param = exact_quantile(y, self("alpha")) if loss == "huber" else self("alpha")
         newton = updates == "newton" and loss == "squared"  # HasScalarHessian among selectable losses :369
 
+        device_fit = _check_device_learner(self, learner)
+
         # Param `devices` with two or more GPUs: rows are sharded over one context per GPU (sharded.ShardedContext),
         # the per-round scalars are summed across GPUs inside the kernels; everything below is unchanged
         from .sharded import make_context
@@ -133,14 +147,17 @@ class GBMRegressor(Params):
                     ctx.gbm_set_loss_param(param)
                     eng.residuals(False)
                 sub = subspaces[i]
-                r, wout = eng.fetch_residuals(newton)
-                fit_w = wout[0] if newton else w
-                if counts is None:
-                    model = learner.fit(X[:, sub], r[0], fit_w)  # third party :387-396
-                else:  # the base learner sees the bag: row i with multiplicity c_i (== weight c_i·w_i)
-                    bw = counts[in_bag] if fit_w is None else counts[in_bag] * fit_w[in_bag]
-                    model = learner.fit(X[in_bag][:, sub], r[0][in_bag], bw)
-                eng.set_direction_from_model(0, model, sub, X)
+                if device_fit:  # the tree is fitted where the residuals live: only the tree comes back
+                    model = eng.fit_direction(0, learner, sub, newton=newton, bag=counts is not None)
+                else:
+                    r, wout = eng.fetch_residuals(newton)
+                    fit_w = wout[0] if newton else w
+                    if counts is None:
+                        model = learner.fit(X[:, sub], r[0], fit_w)  # third party :387-396
+                    else:  # the base learner sees the bag: row i with multiplicity c_i (== weight c_i·w_i)
+                        bw = counts[in_bag] if fit_w is None else counts[in_bag] * fit_w[in_bag]
+                        model = learner.fit(X[in_bag][:, sub], r[0][in_bag], bw)
+                    eng.set_direction_from_model(0, model, sub, X)
                 if self("optimizedWeights"):  # :398-425
                     if self("lineSearch") == "newton" and loss == "squared":
                         alpha, _, _ = eng.line_search_newton(self("tol"), self("maxIter"))
