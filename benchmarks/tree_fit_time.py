@@ -1,7 +1,10 @@
 """Device regression-tree fit (se_tree_fit): CUDA-event times per level and per tree, achieved bytes/s against the
 byte model of DESIGN.md §3 "Device tree fit", and GBM rounds/s with the device learner against the host learner.
+With --classes K, the same for the classification-tree fit (se_tree_fit_classifier, weighted, --impurity gini or
+entropy) and BoostingClassifier (SAMME) rounds/s with the device learner against the host learner.
 
     python benchmarks/tree_fit_time.py [--rows 100000000] [--cols 128] [--gbm-rows 10000000] [--host-rows 1000000]
+    python benchmarks/tree_fit_time.py --classes 26 [--impurity gini] [--rows ...] [--gbm-rows ...] [--host-rows ...]
 
 The feature matrix of the tree timings is filled on the device (uniform), labels are normal; the split candidates
 come from the first 10000 rows of each column (the candidate rule's sample size at maxBins 32).  A level's time is
@@ -33,24 +36,38 @@ def card():
         return f"unknown ({e})"
 
 
-def tree_times(n, d, max_bins, depths, reps):
+def tree_times(n, d, max_bins, depths, reps, classes=0, impurity="gini"):
     out = {}
     with Context(0) as ctx:
         ctx.alloc(N.SLOT_X, d, n)
         ctx.fill_synthetic(N.SLOT_X, "uniform", 1, 0.0, 1.0)
-        ctx.alloc(N.SLOT_R, 1, n)
-        ctx.fill_synthetic(N.SLOT_R, "normal", 2, 0.0, 1.0)
-        ctx.alloc(N.SLOT_H, 1, n)
+        if classes:  # labels: class indices drawn on the host; weights uniform in [0.5, 1.5)
+            ctx.alloc(N.SLOT_Y, 1, n)
+            ctx.upload(N.SLOT_Y, np.random.default_rng(2).integers(0, classes, n).astype(np.float32))
+            ctx.alloc(N.SLOT_W, 1, n)
+            ctx.fill_synthetic(N.SLOT_W, "uniform", 3, 0.5, 1.5)
+            ctx.alloc(N.SLOT_PRED, 1, n)
+        else:
+            ctx.alloc(N.SLOT_R, 1, n)
+            ctx.fill_synthetic(N.SLOT_R, "normal", 2, 0.0, 1.0)
+            ctx.alloc(N.SLOT_H, 1, n)
         m = min(n, 10000)
         cands = [continuous_split_candidates(ctx.download(N.SLOT_X, count=m, offset=j * n), max_bins) for j in range(d)]
         ctx.tree_fit_bins(cands)
         sub = np.arange(d, dtype=np.int32)
+
+        def fit(depth):
+            if classes:
+                return ctx.tree_fit_classifier(N.SLOT_Y, classes, weight_slot=N.SLOT_W, subspace=sub, impurity=impurity,
+                                               max_depth=depth, out_slot=N.SLOT_PRED)
+            return ctx.tree_fit(N.SLOT_R, 0, subspace=sub, max_depth=depth, out_slot=N.SLOT_H)
+
         for depth in depths:
-            ctx.tree_fit(N.SLOT_R, 0, subspace=sub, max_depth=depth, out_slot=N.SLOT_H)  # warm-up
+            fit(depth)  # warm-up
             ts = []
             for _ in range(reps):
                 ctx.timer_start()
-                t = ctx.tree_fit(N.SLOT_R, 0, subspace=sub, max_depth=depth, out_slot=N.SLOT_H)
+                t = fit(depth)
                 ts.append(ctx.timer_stop())
             out[depth] = {"ms_median": float(np.median(ts)), "ms_min": float(np.min(ts)), "nodes": int(t["feature"].size)}
     return out
@@ -74,6 +91,48 @@ def gbm_rounds(n, d, learner, rounds, resident=True):
             "rounds_per_s": 1.0 / per_round}
 
 
+def boosting_rounds(n, d, K, learner, rounds):
+    from spark_ensemble_b200.classification import BoostingClassifier
+    from spark_ensemble_b200.ensemble import DataFrame
+    rng = np.random.default_rng(0)
+    X = rng.random((n, d), dtype=np.float32)
+    z = np.sin(6 * X[:, 0]) + X[:, 1] * X[:, 2] + 0.3 * rng.standard_normal(n)
+    y = np.digitize(z, np.quantile(z, np.linspace(0, 1, K + 1)[1:-1])).astype(np.float64)
+    df = DataFrame(features=X, label=y, weight=rng.uniform(0.5, 1.5, n))
+    times = {}
+    for k in (1, rounds):
+        b = BoostingClassifier().set("baseLearner", learner).set("numBaseLearners", k).set("residentFeatures", True)
+        b.set("weightCol", "weight")
+        t0 = time.perf_counter()
+        m = b.fit(df)
+        times[k] = time.perf_counter() - t0
+    per_round = (times[rounds] - times[1]) / (rounds - 1)
+    return {"rows": n, "cols": d, "classes": K, "rounds": rounds, "fitted_rounds": len(m.trainingHistory),
+            "fit_s": times[rounds], "s_per_round": per_round, "rounds_per_s": 1.0 / per_round}
+
+
+def main_classes(args):
+    from spark_ensemble_b200.learners import DecisionTreeClassifier, DeviceDecisionTreeClassifier
+    K = args.classes
+    res = {"card": card(), "classes": K, "impurity": args.impurity}
+    n, d = args.rows, args.cols
+    tt = tree_times(n, d, args.bins, list(range(0, 7)), args.reps, classes=K, impurity=args.impurity)
+    res["tree_ms"] = tt
+    bytes_level = n * (d + 4 + 4 + 2 + 2 + 1)  # ranks, labels, weights, node index in and out, one gathered rank
+    levels = {}
+    for L in range(6):
+        ms = tt[L + 1]["ms_median"] - tt[L]["ms_median"]
+        levels[L] = {"ms": ms, "model_bytes": bytes_level, "achieved_GBps": bytes_level / (ms * 1e-3) / 1e9}
+    res["levels"] = levels
+    res["byte_model_ms_per_level_at_3.06TBps"] = bytes_level / 3.06e12 * 1e3
+    print(json.dumps(res, indent=1), flush=True)
+    dev = DeviceDecisionTreeClassifier(maxDepth=5, impurity=args.impurity)
+    res["boost_device"] = boosting_rounds(args.gbm_rows, args.gbm_cols, K, dev, 10)
+    print(json.dumps({"boost_device": res["boost_device"]}), flush=True)
+    res["boost_host"] = boosting_rounds(args.host_rows, args.gbm_cols, K, DecisionTreeClassifier(maxDepth=5), 3)
+    print(json.dumps({"boost_host": res["boost_host"]}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rows", type=int, default=100_000_000)
@@ -83,7 +142,11 @@ def main():
     ap.add_argument("--gbm-rows", type=int, default=10_000_000)
     ap.add_argument("--gbm-cols", type=int, default=32)
     ap.add_argument("--host-rows", type=int, default=1_000_000)
+    ap.add_argument("--classes", type=int, default=0, help="classification fit with this many classes (2..64)")
+    ap.add_argument("--impurity", default="gini", choices=("gini", "entropy"))
     args = ap.parse_args()
+    if args.classes:
+        return main_classes(args)
     res = {"card": card()}
     n, d = args.rows, args.cols
     tt = tree_times(n, d, args.bins, list(range(0, 7)), args.reps)

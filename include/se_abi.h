@@ -369,6 +369,27 @@ SE_API int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_sl
                        const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
                        double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
                        float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes);
+/* ---- classification-tree fit on the device (DESIGN.md §3 "Device classification-tree fit") -------- */
+enum se_tree_impurity { SE_IMPURITY_GINI = 0, SE_IMPURITY_ENTROPY = 1 };
+enum se_tree_out { SE_TREE_OUT_LABEL = 0, SE_TREE_OUT_PROBA = 1 };
+/* Fits one classification tree: Spark's DecisionTreeClassifier (gini or entropy impurity, continuous features,
+ * level-wise best split over the candidates of se_tree_fit_bins, prune = true), restated in DESIGN.md §3.  The
+ * arguments are se_tree_fit's, plus: labels are class indices 0..num_classes-1 (clamped into that range on the device;
+ * SE_SLOT_Y is validated once per upload and the call fails with SE_ERR_ARG on a bad label); 2 <= num_classes <= 64.
+ * A node's statistics are fp64 rawCount Σ c and class weights n_k = Σ c·w over its rows of label k.  A weight row that
+ * is a common multiple of the intended weights (e.g. SE_SLOT_BW, not divided by Σw) gives the same splits up to rounding.
+ * Pruning merges two leaf children with equal labels into a leaf with that label and the PARENT's class weights.
+ * out_kind SE_TREE_OUT_LABEL writes every row's label into row out_row of out_slot (as se_tree_predict of `value`);
+ * SE_TREE_OUT_PROBA writes its K probabilities into rows out_row .. out_row + K - 1 (as se_tree_predict_multi of
+ * `proba`), bit for bit.  Returns the tree in BFS order: feature / threshold / left / right as se_tree_fit, value =
+ * label, proba [n_nodes][K] = fp32 of n_k / W (all 0 when W == 0), class_weights [n_nodes][K] (may be NULL), gain (may
+ * be NULL), n_nodes.  Bounds (SE_ERR_ARG) as se_tree_fit, plus num_classes and impurity. */
+SE_API int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row,
+                                  int use_bag, const int32_t* subspace, int n_subspace, int num_classes, int impurity,
+                                  int max_depth, int min_instances, double min_info_gain, double min_weight_fraction,
+                                  int out_kind, int out_slot, int out_row, int max_nodes, int32_t* feature,
+                                  float* threshold, int32_t* left, int32_t* right, float* value, float* proba,
+                                  double* class_weights, double* gain, int* n_nodes);
 /* linear model: out = intercept + Σ_j coef[j]·X[subspace[j]] */
 SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,
                       const int32_t* subspace, int out_slot, int out_row);

@@ -142,6 +142,7 @@ NOT_BOUND = {
     "se_spark_bernoulli_sample": "restates Spark's BernoulliSampler for hosts WITHOUT Spark; the JVM side draws with Spark itself",
     "se_tree_fit_bins": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
     "se_tree_fit": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
+    "se_tree_fit_classifier": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
 }
 
 HAND_CPP = r'''

@@ -117,6 +117,8 @@ PROTOTYPES = {
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,
                     _ip, _fp, _ip, _ip, _fp, _dp, C.POINTER(_i32)],
+    "se_tree_fit_classifier": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _i32, _i32, _d, _d, _i32,
+                               _i32, _i32, _i32, _ip, _fp, _ip, _ip, _fp, _fp, _dp, _dp, C.POINTER(_i32)],
 }
 _RESTYPES = {"se_last_error": C.c_char_p}
 

@@ -252,6 +252,7 @@ class BoostingClassifier(Params):
         _validate_labels(y, K)
         real = self("algorithm").lower() == "real"
         learner = self("baseLearner")
+        device_fit = _check_device_learner(self, learner)
         models, est_weights, history = [], [], []
         ctx = Context(self.device)
         try:
@@ -260,18 +261,28 @@ class BoostingClassifier(Params):
             if resident:  # column-major X in HBM: fitted trees are evaluated on device (no K x n upload per round)
                 ctx.alloc(N.SLOT_X, X.shape[1], n)
                 ctx.upload_rowmajor(N.SLOT_X, X)
+            if device_fit:  # the device learner's split candidates, set once for every round
+                ctx.tree_fit_bins(learner.split_candidates(X))
+                all_cols = np.arange(X.shape[1], dtype=np.int32)
             ctx.upload(N.SLOT_Y, y)
             ctx.upload(N.SLOT_BW, np.ones(n) if w is None else w)  # boostingWeights = instances.map(_.weight) :168
             sum_w = ctx.slot_sum(N.SLOT_BW)  # :175
             i, done = 0, False
             while i < self("numBaseLearners") and not done and sum_w > 0:  # :180
-                wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)  # weight = boostingWeight / sumWeights :184-187
-                model = learner.fit(X, y, wn, num_classes=K)    # third party :189-195
+                if device_fit:  # fitted on SLOT_Y / SLOT_BW where they live, straight into SLOT_PROBA or SLOT_PRED;
+                    # the splits are invariant under the common 1 / sumWeights scale of :184-187
+                    model = learner.fit_resident(ctx, K, N.SLOT_Y, 0, N.SLOT_BW, 0, False, all_cols,
+                                                 N.SLOT_PROBA if real else N.SLOT_PRED, 0, proba=real)
+                else:
+                    wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)  # weight = boostingWeight / sumWeights :184-187
+                    model = learner.fit(X, y, wn, num_classes=K)    # third party :189-195
                 if real:  # SAMME.R :198-230
                     if not hasattr(model, "predictProbability"):
                         raise RuntimeError('algorithm "real" is not compatible with base learner')  # :261-263
                     t = model.tree_arrays() if resident else None
-                    if t is not None:
+                    if device_fit:
+                        pass  # the device fit wrote SLOT_PROBA
+                    elif t is not None:
                         ctx.tree_predict_multi(t, N.SLOT_PROBA)
                     else:
                         P = model.predictProbability(X)
@@ -283,7 +294,9 @@ class BoostingClassifier(Params):
                     models.append(model)
                 else:  # SAMME :231-260
                     t = model.tree_arrays() if resident else None
-                    if t is not None:
+                    if device_fit:
+                        pass  # the device fit wrote SLOT_PRED
+                    elif t is not None:
                         ctx.tree_predict(t, N.SLOT_PRED, 0)
                     else:
                         ctx.upload(N.SLOT_PRED, model.predict(X))

@@ -442,3 +442,38 @@ class Context:
         k = nn.value
         return {"feature": f[:k].copy(), "threshold": t[:k].copy(), "left": l[:k].copy(), "right": r[:k].copy(),
                 "value": v[:k].copy(), "gain": g[:k].copy()}
+
+    def tree_fit_classifier(self, label_slot: int, num_classes: int, label_row: int = 0, weight_slot: int = -1,
+                            weight_row: int = 0, use_bag: bool = False, subspace=None, n_subspace: int | None = None,
+                            impurity: str = "gini", max_depth: int = 5, min_instances: int = 1,
+                            min_info_gain: float = 0.0, min_weight_fraction: float = 0.0, proba: bool = False,
+                            out_slot: int = N.SLOT_PRED, out_row: int = 0) -> dict:
+        """Fits one classification tree over the rank matrix (se_tree_fit_classifier) and writes, for every row, its
+        label into out_slot row out_row, or (proba) its K class probabilities into rows out_row .. out_row + K - 1.
+        Returns the array form of se_tree_predict / se_tree_predict_multi ("value" = label, "values" [n, K]
+        probabilities) plus the fp64 class weights ("class_weights" [n, K]) and gains of every node."""
+        imp = {"gini": 0, "entropy": 1}.get(str(impurity).lower())
+        if imp is None:
+            raise ValueError(f"impurity must be gini or entropy, got {impurity!r}")
+        sub = None if subspace is None else np.ascontiguousarray(subspace, dtype=np.int32)
+        ns = int(sub.size if sub is not None else n_subspace)
+        K = int(num_classes)
+        cap = (1 << (int(max_depth) + 1)) - 1 if 0 <= int(max_depth) <= 8 else 1
+        kk = max(K, 1) if 0 < K <= 64 else 1
+        f = np.zeros(cap, dtype=np.int32)
+        t = np.zeros(cap, dtype=np.float32)
+        l = np.zeros(cap, dtype=np.int32)
+        r = np.zeros(cap, dtype=np.int32)
+        v = np.zeros(cap, dtype=np.float32)
+        p = np.zeros((cap, kk), dtype=np.float32)
+        cw = np.zeros((cap, kk), dtype=np.float64)
+        g = np.zeros(cap, dtype=np.float64)
+        nn = C.c_int32()
+        self._ck(self._lib.se_tree_fit_classifier(
+            self._h, int(label_slot), int(label_row), int(weight_slot), int(weight_row), int(bool(use_bag)),
+            None if sub is None else N.iptr(sub), ns, K, imp, int(max_depth), int(min_instances), float(min_info_gain),
+            float(min_weight_fraction), int(bool(proba)), int(out_slot), int(out_row), cap, N.iptr(f), N.fptr(t),
+            N.iptr(l), N.iptr(r), N.fptr(v), N.fptr(p), N.dptr(cw), N.dptr(g), C.byref(nn)))
+        k = nn.value
+        return {"feature": f[:k].copy(), "threshold": t[:k].copy(), "left": l[:k].copy(), "right": r[:k].copy(),
+                "value": v[:k].copy(), "values": p[:k].copy(), "class_weights": cw[:k].copy(), "gain": g[:k].copy()}

@@ -270,6 +270,9 @@ struct se_ctx {
     int32_t* d_cols = nullptr;
     int cols_cap = 0;
     int smem_optin = 0;
+    double* d_cw = nullptr;           // classification: [kTreeFitHeap][kTreeFitMaxClasses]
+    float* d_prob = nullptr;          // [kTreeFitHeap][kTreeFitMaxClasses]
+    int4* d_prn = nullptr;            // [kTreeFitHeap]
   } tf;
   std::string err;
   // stopwatch + per-kernel-family timing
@@ -791,6 +794,9 @@ int se_ctx_destroy(se_ctx* ctx) {
   if (ctx->tf.d_nodes) cudaFree(ctx->tf.d_nodes);
   if (ctx->tf.d_dec) cudaFree(ctx->tf.d_dec);
   if (ctx->tf.d_cols) cudaFree(ctx->tf.d_cols);
+  if (ctx->tf.d_cw) cudaFree(ctx->tf.d_cw);
+  if (ctx->tf.d_prob) cudaFree(ctx->tf.d_prob);
+  if (ctx->tf.d_prn) cudaFree(ctx->tf.d_prn);
   if (ctx->big.d_coef) cudaFree(ctx->big.d_coef);
   if (ctx->big.h_coef) cudaFreeHost(ctx->big.h_coef);
   if (ctx->big.d_partials) cudaFree(ctx->big.d_partials);
@@ -2996,11 +3002,14 @@ int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const floa
   return end(ctx);
 }
 
-int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
-                const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
-                double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
-                float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
-  if (!ctx || !feature || !threshold || !left || !right || !value || !n_nodes) return fail(ctx, SE_ERR_ARG, "null argument");
+namespace {
+// The part of a fit that se_tree_fit and se_tree_fit_classifier share: argument checks, scratch, the level loop with
+// its shared-memory / global-atomics choice, the classifier's pruning, the out kernel and the download of the node
+// records into h_small: [kTreeFitHeap] TreeFitNode, then for K >= 2 the class weights ([kTreeFitHeap][K] double), the
+// probabilities ([kTreeFitHeap][K] float) and the pruning table ([kTreeFitHeap] int4).  K == 0: regression.
+int tree_fit_run(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot, int label_row, int weight_slot,
+                 int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth, int min_instances,
+                 double min_info_gain, double min_weight_fraction, int out_slot, int out_row) {
   SE_REQUIRE(ctx, max_depth >= 0 && max_depth <= 8, SE_ERR_ARG, "maxDepth %d outside [0, 8]", max_depth);
   SE_REQUIRE(ctx, min_instances >= 1, SE_ERR_ARG, "minInstancesPerNode %d < 1", min_instances);
   SE_REQUIRE(ctx, min_weight_fraction >= 0.0 && min_weight_fraction < 0.5, SE_ERR_ARG,
@@ -3024,6 +3033,8 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
   if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &w));
   if (use_bag) SE_TRY(row_of(SE_SLOT_BAG, 0, "bag", &bag));
   SE_TRY(row_of(out_slot, out_row, "output", &outc));
+  SE_REQUIRE(ctx, !out_proba || out_row + K <= ctx->slot[out_slot].rows, SE_ERR_STATE,
+             "output slot %d: no rows %d..%d for the class probabilities", out_slot, out_row, out_row + K - 1);
   SE_REQUIRE(ctx, n_subspace >= 1, SE_ERR_ARG, "empty subspace");
   BinState& B = ctx->bins[0];
   SE_REQUIRE(ctx, B.d8 && B.d == X.rows && B.n == X.cols, SE_ERR_STATE,
@@ -3057,7 +3068,8 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
     T.nid_cap = 4 * nw;
   }
   const int top = max_depth > 0 ? max_depth - 1 : 0;  // deepest level that is searched (or, at depth 0, only summed)
-  const size_t hist_bytes = ((size_t)1 << top) * (size_t)n_subspace * (size_t)nb * 4 * sizeof(double);
+  const int sw = K > 0 ? K + (w ? 1 : 0) : 4;  // doubles per histogram bin
+  const size_t hist_bytes = ((size_t)1 << top) * (size_t)n_subspace * (size_t)nb * (size_t)sw * sizeof(double);
   if (T.hist_bytes < hist_bytes) {
     if (T.d_hist) cudaFree(T.d_hist);
     T.d_hist = nullptr; T.hist_bytes = 0;
@@ -3070,6 +3082,11 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
     int optin = 0;
     SE_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     T.smem_optin = optin;
+  }
+  if (K > 0 && !T.d_cw) {
+    SE_CUDA(ctx, cudaMalloc(&T.d_cw, sizeof(double) * kTreeFitHeap * kTreeFitMaxClasses));
+    SE_CUDA(ctx, cudaMalloc(&T.d_prob, sizeof(float) * kTreeFitHeap * kTreeFitMaxClasses));
+    SE_CUDA(ctx, cudaMalloc(&T.d_prn, sizeof(int4) * kTreeFitHeap));
   }
   if (T.cols_cap < n_subspace) {
     if (T.d_cols) cudaFree(T.d_cols);
@@ -3088,6 +3105,9 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
   a.has_w = w ? 1 : 0; a.r = r; a.w = w; a.bag = bag;
   a.dec = T.d_dec; a.nodes = T.d_nodes; a.hist = T.d_hist;
   a.min_instances = min_instances; a.min_info_gain = min_info_gain; a.min_weight_fraction = min_weight_fraction;
+  a.K = K; a.sw = sw; a.entropy = entropy; a.out_proba = out_proba;
+  a.cw = T.d_cw; a.prob = T.d_prob; a.prn = T.d_prn;
+  if (K > 0 && label_slot == SE_SLOT_Y) SE_TRY(ensure_labels_checked(ctx, 0, K, n));  // class indices, checked per upload
   uint16_t* nid[2] = {T.d_nid, T.d_nid + T.nid_cap};
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, ctx->stream));
   for (int L = 0; L <= top; ++L) {
@@ -3095,7 +3115,7 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
     a.route = L >= 1;
     a.nid_in = L >= 2 ? nid[(L - 1) & 1] : nullptr;
     a.nid_out = L >= 1 ? nid[L & 1] : nullptr;
-    const size_t per_col = ((size_t)1 << L) * (size_t)nb * 4 * sizeof(double);
+    const size_t per_col = ((size_t)1 << L) * (size_t)nb * (size_t)sw * sizeof(double);
     SE_CUDA(ctx, cudaMemsetAsync(T.d_hist, 0, per_col * (size_t)n_subspace, ctx->stream));
     int smem_mode = 1, per_sm = 4;
     size_t smem = 0;
@@ -3122,11 +3142,38 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
   a.nid_in = max_depth >= 2 ? nid[(max_depth - 1) & 1] : nullptr;
   a.nid_out = nullptr;
   a.out = const_cast<float*>(outc);
+  {
+    const SlotBuf& O = ctx->slot[out_slot];
+    a.ld_out = O.rows > 1 ? O.ld : O.cols;
+  }
+  if (K > 0) SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_prune(a, ctx->stream));
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_out(a, ctx->sms, ctx->stream));
-  static_assert(sizeof(TreeFitNode) * kTreeFitHeap <= (size_t)kSmallBytes, "node records fit the staging buffer");
-  SE_CUDA(ctx, cudaMemcpyAsync(ctx->h_small, T.d_nodes, sizeof(TreeFitNode) * kTreeFitHeap, cudaMemcpyDeviceToHost, ctx->stream));
+  static_assert(sizeof(TreeFitNode) * kTreeFitHeap + (sizeof(double) + sizeof(float)) * kTreeFitHeap * kTreeFitMaxClasses +
+                        sizeof(int4) * kTreeFitHeap <= (size_t)kSmallBytes,
+                "node records fit the staging buffer");
+  char* hs = reinterpret_cast<char*>(ctx->h_small);
+  size_t off = sizeof(TreeFitNode) * kTreeFitHeap;
+  SE_CUDA(ctx, cudaMemcpyAsync(hs, T.d_nodes, off, cudaMemcpyDeviceToHost, ctx->stream));
+  if (K > 0) {
+    const size_t cwb = sizeof(double) * kTreeFitHeap * (size_t)K, pb = sizeof(float) * kTreeFitHeap * (size_t)K;
+    SE_CUDA(ctx, cudaMemcpyAsync(hs + off, T.d_cw, cwb, cudaMemcpyDeviceToHost, ctx->stream));
+    SE_CUDA(ctx, cudaMemcpyAsync(hs + off + cwb, T.d_prob, pb, cudaMemcpyDeviceToHost, ctx->stream));
+    SE_CUDA(ctx, cudaMemcpyAsync(hs + off + cwb + pb, T.d_prn, sizeof(int4) * kTreeFitHeap, cudaMemcpyDeviceToHost, ctx->stream));
+  }
   SE_TRY(end(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (K > 0) SE_TRY(check_labels(ctx));  // a label outside [0, K) was clamped: the fit is invalid
+  return SE_OK;
+}
+}  // namespace
+
+int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
+                double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
+                float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
+  if (!ctx || !feature || !threshold || !left || !right || !value || !n_nodes) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_TRY(tree_fit_run(ctx, 0, 0, 0, label_slot, label_row, weight_slot, weight_row, use_bag, subspace, n_subspace,
+                      max_depth, min_instances, min_info_gain, min_weight_fraction, out_slot, out_row));
   // ---- prune (bottom-up: two leaf children with equal fp64 predictions) and number the nodes in BFS order
   const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(ctx->h_small);
   std::vector<char> leaf(kTreeFitHeap, 1);
@@ -3159,6 +3206,55 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
     left[q] = lf ? 0 : id[2 * h];
     right[q] = lf ? 0 : id[2 * h + 1];
     value[q] = val[h];
+    if (gain) gain[q] = lf ? 0.0 : R[h].gain;
+  }
+  *n_nodes = (int)order.size();
+  return SE_OK;
+}
+
+// ---- classification-tree fit over the rank matrix (se_tree_fit.cu) -------------------------------
+int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                           const int32_t* subspace, int n_subspace, int num_classes, int impurity, int max_depth,
+                           int min_instances, double min_info_gain, double min_weight_fraction, int out_kind,
+                           int out_slot, int out_row, int max_nodes, int32_t* feature, float* threshold, int32_t* left,
+                           int32_t* right, float* value, float* proba, double* class_weights, double* gain,
+                           int* n_nodes) {
+  if (!ctx || !feature || !threshold || !left || !right || !value || !proba || !n_nodes)
+    return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= kTreeFitMaxClasses, SE_ERR_ARG, "numClasses %d outside [2, %d]",
+             num_classes, kTreeFitMaxClasses);
+  SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
+  SE_REQUIRE(ctx, out_kind == SE_TREE_OUT_LABEL || out_kind == SE_TREE_OUT_PROBA, SE_ERR_ARG, "bad output kind %d", out_kind);
+  const int K = num_classes;
+  SE_TRY(tree_fit_run(ctx, K, impurity == SE_IMPURITY_ENTROPY, out_kind == SE_TREE_OUT_PROBA, label_slot, label_row,
+                      weight_slot, weight_row, use_bag, subspace, n_subspace, max_depth, min_instances, min_info_gain,
+                      min_weight_fraction, out_slot, out_row));
+  // the device pruned the tree (tree_prune_cls_kernel): number what is left in BFS order
+  const char* hs = reinterpret_cast<const char*>(ctx->h_small);
+  const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(hs);
+  const double* CW = reinterpret_cast<const double*>(hs + sizeof(TreeFitNode) * kTreeFitHeap);
+  const float* PR = reinterpret_cast<const float*>(CW + (size_t)kTreeFitHeap * K);
+  const int4* PN = reinterpret_cast<const int4*>(PR + (size_t)kTreeFitHeap * K);
+  std::vector<int> order;
+  order.push_back(1);
+  for (size_t q = 0; q < order.size(); ++q)
+    if (!PN[order[q]].z) { order.push_back(2 * order[q]); order.push_back(2 * order[q] + 1); }
+  SE_REQUIRE(ctx, (int)order.size() <= max_nodes, SE_ERR_ARG, "the fitted tree has %d nodes, max_nodes is %d",
+             (int)order.size(), max_nodes);
+  std::vector<int> id(kTreeFitHeap, 0);
+  for (size_t q = 0; q < order.size(); ++q) id[order[q]] = (int)q;
+  for (size_t q = 0; q < order.size(); ++q) {
+    const int h = order[q];
+    const bool lf = PN[h].z != 0;
+    feature[q] = lf ? -1 : R[h].col;
+    threshold[q] = lf ? 0.f : R[h].thr;
+    left[q] = lf ? 0 : id[2 * h];
+    right[q] = lf ? 0 : id[2 * h + 1];
+    value[q] = (float)PN[h].y;  // a merged leaf keeps its children's label ...
+    for (int k = 0; k < K; ++k) {  // ... and its own statistics
+      proba[q * K + k] = PR[(size_t)h * K + k];
+      if (class_weights) class_weights[q * K + k] = CW[(size_t)h * K + k];
+    }
     if (gain) gain[q] = lf ? 0.0 : R[h].gain;
   }
   *n_nodes = (int)order.size();

@@ -273,13 +273,14 @@ struct ForestArgs {
 constexpr int kForestTile = 256;              // rows per CTA tile (one row per thread)
 constexpr int kForestSmemBudget = 54 * 1024;  // per CTA: four CTAs per SM (the walk is latency-bound: warps matter more than chunk size)
 cudaError_t launch_forest_predict(const ForestArgs& a, int sms, cudaStream_t s);
-// ---- regression-tree fit over the uint8 rank matrix (se_tree_fit.cu) -------------------------
+// ---- regression- and classification-tree fit over the uint8 rank matrix (se_tree_fit.cu) -----
 // Nodes are heap-indexed (root 1, children 2h, 2h + 1), so depth <= 8 needs 511 records.
 constexpr int kTreeFitHeap = 512;
 constexpr int kTreeFitSmemBudget = 56 * 1024;  // shared-memory histograms per CTA: four CTAs per SM
+constexpr int kTreeFitMaxClasses = 64;         // classification: two classes per lane of the split search's warp
 struct TreeFitNode {                 // 64 B, downloaded once at the end of a fit
-  double cnt, w, s, q;               // rawCount, W, S, Q of the node's in-bag rows
-  double pred;                       // S / W
+  double cnt, w, s, q;               // rawCount, W, S, Q of the node's in-bag rows (classification: s, q unused)
+  double pred;                       // S / W (classification: the label)
   double gain;                       // of the chosen split (state 2)
   int32_t state;                     // 0 unused, 1 leaf, 2 split
   int32_t col, bin;                  // split: subspace-local column, left when rank <= bin
@@ -302,16 +303,25 @@ struct TreeFitArgs {
   uint16_t* nid_out = nullptr;       // after it (written by the first column block)
   uint2* dec = nullptr;              // [kTreeFitHeap] x: global split column (~0: none), y: bin | open << 31
   TreeFitNode* nodes = nullptr;      // [kTreeFitHeap]
-  double* hist = nullptr;            // [2^L][S][nb][4]
+  double* hist = nullptr;            // [2^L][S][nb][sw]
   int64_t words_per_cta = 0;         // 4-row groups per CTA row range
   int min_instances = 1;
   double min_info_gain = 0.0, min_weight_fraction = 0.0;
-  float* out = nullptr;              // final pass: leaf value per row
+  float* out = nullptr;              // final pass: leaf value per row (classification: label, or K rows of ld_out)
+  // classification (K >= 2; K == 0 is the regression fit): labels in `r` are class indices
+  int K = 0, sw = 4;                 // sw: doubles per histogram bin (regression 4; classification K, + 1 when has_w)
+  int entropy = 0, out_proba = 0;
+  int64_t ld_out = 0;
+  double* cw = nullptr;              // [kTreeFitHeap][K] class weights of every node
+  float* prob = nullptr;             // [kTreeFitHeap][K] fp32 of cw / W (all 0 when W == 0)
+  int4* prn = nullptr;               // [kTreeFitHeap] after pruning: x the node whose statistics a row at h outputs,
+                                     // y its label, z 1 when h is a leaf of the pruned tree
 };
 cudaError_t launch_tree_fit_init(TreeFitNode* nodes, uint2* dec, cudaStream_t s);
 // smem_mode 1: shared-memory histograms of a.cb columns per CTA (smem bytes), folded into a.hist; 0: global atomics
 cudaError_t launch_tree_fit_hist(const TreeFitArgs& a, int smem_mode, int grid_y, size_t smem, cudaStream_t s);
 cudaError_t launch_tree_fit_split(const TreeFitArgs& a, cudaStream_t s);
+cudaError_t launch_tree_fit_prune(const TreeFitArgs& a, cudaStream_t s);  // classification only
 cudaError_t launch_tree_fit_out(const TreeFitArgs& a, int sms, cudaStream_t s);
 
 cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_coef,

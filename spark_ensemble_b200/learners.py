@@ -130,23 +130,10 @@ class DeviceDecisionTreeRegressionModel(_Model):
         return v[node].astype(np.float64)
 
 
-class DeviceDecisionTreeRegressor:
-    """org.apache.spark.ml.regression.DecisionTreeRegressor fitted on the GPU: variance impurity, continuous features,
-    level-wise best split over at most maxBins - 1 candidates per column (se_tree_fit).  Params keep Spark's names and
-    defaults.  Inside GBMRegressor / GBMClassifier (residentFeatures=True) it fits on the device-resident residuals;
-    `fit` alone opens a context on `device`, uploads X, fits and closes it."""
+class _DeviceTreeLearner:
+    """What the device tree learners share: the tree Params' validators and the split candidates of a fit."""
 
     device_learner = True
-
-    def __init__(self, maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1, minInfoGain: float = 0.0,
-                 minWeightFractionPerNode: float = 0.0, seed: int | None = None, device: int = 0):
-        from .ensemble import java_string_hash
-        self.maxDepth, self.maxBins = int(maxDepth), int(maxBins)
-        self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
-        self.minWeightFractionPerNode = float(minWeightFractionPerNode)
-        self.seed = java_string_hash("org.apache.spark.ml.regression.DecisionTreeRegressor") if seed is None else int(seed)
-        self.device = int(device)
-        self._check()
 
     def _check(self):
         if not 0 <= self.maxDepth <= 8:
@@ -157,14 +144,6 @@ class DeviceDecisionTreeRegressor:
             raise ValueError(f"minInstancesPerNode must be >= 1, got {self.minInstancesPerNode}")
         if not 0.0 <= self.minWeightFractionPerNode < 0.5:
             raise ValueError(f"minWeightFractionPerNode must be in [0, 0.5), got {self.minWeightFractionPerNode}")
-
-    def copy(self, extra=None):
-        c = DeviceDecisionTreeRegressor(self.maxDepth, self.maxBins, self.minInstancesPerNode, self.minInfoGain,
-                                        self.minWeightFractionPerNode, self.seed, self.device)
-        for k, v in (extra or {}).items():
-            setattr(c, k, v)
-        c._check()
-        return c
 
     def sample_rows(self, n: int):
         """Rows the candidates are drawn from: all of them when n <= max(maxBins², 10000), else Spark's Bernoulli
@@ -187,6 +166,31 @@ class DeviceDecisionTreeRegressor:
         rows = self.sample_rows(X.shape[0])
         S = X if rows is None else X[rows]
         return [continuous_split_candidates(S[:, j], self.maxBins) for j in range(X.shape[1])]
+
+
+class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
+    """org.apache.spark.ml.regression.DecisionTreeRegressor fitted on the GPU: variance impurity, continuous features,
+    level-wise best split over at most maxBins - 1 candidates per column (se_tree_fit).  Params keep Spark's names and
+    defaults.  Inside GBMRegressor / GBMClassifier (residentFeatures=True) it fits on the device-resident residuals;
+    `fit` alone opens a context on `device`, uploads X, fits and closes it."""
+
+    def __init__(self, maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1, minInfoGain: float = 0.0,
+                 minWeightFractionPerNode: float = 0.0, seed: int | None = None, device: int = 0):
+        from .ensemble import java_string_hash
+        self.maxDepth, self.maxBins = int(maxDepth), int(maxBins)
+        self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
+        self.minWeightFractionPerNode = float(minWeightFractionPerNode)
+        self.seed = java_string_hash("org.apache.spark.ml.regression.DecisionTreeRegressor") if seed is None else int(seed)
+        self.device = int(device)
+        self._check()
+
+    def copy(self, extra=None):
+        c = DeviceDecisionTreeRegressor(self.maxDepth, self.maxBins, self.minInstancesPerNode, self.minInfoGain,
+                                        self.minWeightFractionPerNode, self.seed, self.device)
+        for k, v in (extra or {}).items():
+            setattr(c, k, v)
+        c._check()
+        return c
 
     def fit_resident(self, ctx, label_slot: int, label_row: int, weight_slot: int, weight_row: int, use_bag: bool,
                      subspace, out_slot: int, out_row: int) -> DeviceDecisionTreeRegressionModel:
@@ -262,6 +266,128 @@ class DecisionTreeClassifier:
         yi = np.asarray(y).astype(int)
         sk.fit(np.asarray(X, dtype=np.float32), yi, sample_weight=None if w is None else np.asarray(w, dtype=np.float64))
         return DecisionTreeClassificationModel(sk, int(num_classes or (yi.max() + 1)))
+
+
+class DeviceDecisionTreeClassificationModel(_Model):
+    """A classification tree fitted on the device, in the array form of se_tree_predict ("value": the label) and
+    se_tree_predict_multi ("values": [n_nodes, K] class probabilities), as DecisionTreeClassificationModel gives."""
+
+    def __init__(self, arrays: dict, num_classes: int):
+        self._arrays = {k: np.asarray(v).copy() for k, v in arrays.items()}
+        self.numClasses = int(num_classes)
+        self.numNodes = int(self._arrays["feature"].size)
+
+    def tree_arrays(self):
+        return {k: self._arrays[k] for k in ("feature", "threshold", "left", "right", "value", "values")}
+
+    @property
+    def gains(self) -> np.ndarray:
+        return self._arrays["gain"]
+
+    @property
+    def class_weights(self) -> np.ndarray:
+        return self._arrays["class_weights"]
+
+    def _leaf(self, X) -> np.ndarray:
+        """Host walk of the arrays: left when x <= threshold (NaN goes right), fp32 features."""
+        X = np.asarray(X, dtype=np.float32)
+        f, t = self._arrays["feature"], self._arrays["threshold"]
+        l, r = self._arrays["left"], self._arrays["right"]
+        node = np.zeros(X.shape[0], dtype=np.int64)
+        rows = np.arange(X.shape[0])
+        while True:
+            live = f[node] >= 0
+            if not live.any():
+                break
+            idx = rows[live]
+            nd = node[idx]
+            go_left = X[idx, f[nd]] <= t[nd]
+            node[idx] = np.where(go_left, l[nd], r[nd])
+        return node
+
+    def predict(self, X) -> np.ndarray:
+        return self._arrays["value"][self._leaf(X)].astype(np.float64)
+
+    def predictProbability(self, X) -> np.ndarray:
+        return self._arrays["values"][self._leaf(X)].astype(np.float64)
+
+
+class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
+    """org.apache.spark.ml.classification.DecisionTreeClassifier fitted on the GPU: gini or entropy impurity,
+    continuous features, level-wise best split over at most maxBins - 1 candidates per column, Spark's pruning
+    (se_tree_fit_classifier).  Params keep Spark's names and defaults; 2..64 classes.  Inside BoostingClassifier
+    (residentFeatures=True) it fits on the device-resident labels and boosting weights; `fit` alone opens a context on
+    `device`, uploads X, fits and closes it (BaggingClassifier uses it that way)."""
+
+    def __init__(self, maxDepth: int = 5, maxBins: int = 32, impurity: str = "gini", minInstancesPerNode: int = 1,
+                 minInfoGain: float = 0.0, minWeightFractionPerNode: float = 0.0, seed: int | None = None,
+                 device: int = 0):
+        from .ensemble import java_string_hash
+        self.maxDepth, self.maxBins, self.impurity = int(maxDepth), int(maxBins), str(impurity)
+        self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
+        self.minWeightFractionPerNode = float(minWeightFractionPerNode)
+        self.seed = (java_string_hash("org.apache.spark.ml.classification.DecisionTreeClassifier") if seed is None
+                     else int(seed))
+        self.device = int(device)
+        self._check()
+
+    def _check(self):
+        super()._check()
+        if self.impurity.lower() not in ("gini", "entropy"):
+            raise ValueError(f"impurity must be gini or entropy, got {self.impurity!r}")
+
+    def copy(self, extra=None):
+        c = DeviceDecisionTreeClassifier(self.maxDepth, self.maxBins, self.impurity, self.minInstancesPerNode,
+                                         self.minInfoGain, self.minWeightFractionPerNode, self.seed, self.device)
+        for k, v in (extra or {}).items():
+            setattr(c, k, v)
+        c._check()
+        return c
+
+    @staticmethod
+    def _check_classes(K: int):
+        if not 2 <= K <= 64:
+            raise ValueError(f"the device classification tree supports 2..64 classes, got {K}")
+
+    def fit_resident(self, ctx, num_classes: int, label_slot: int, label_row: int, weight_slot: int, weight_row: int,
+                     use_bag: bool, subspace, out_slot: int, out_row: int,
+                     proba: bool = False) -> DeviceDecisionTreeClassificationModel:
+        """Fit over a context whose SLOT_X already holds this learner's candidates (Context.tree_fit_bins); writes
+        every row's label (or, with proba, its K probabilities from row out_row on) into out_slot."""
+        self._check()
+        self._check_classes(int(num_classes))
+        t = ctx.tree_fit_classifier(label_slot, num_classes, label_row, weight_slot, weight_row, use_bag,
+                                    subspace=subspace, impurity=self.impurity.lower(), max_depth=self.maxDepth,
+                                    min_instances=self.minInstancesPerNode, min_info_gain=self.minInfoGain,
+                                    min_weight_fraction=self.minWeightFractionPerNode, proba=proba,
+                                    out_slot=out_slot, out_row=out_row)
+        return DeviceDecisionTreeClassificationModel(t, num_classes)
+
+    def fit(self, X, y, w=None, num_classes: int | None = None) -> DeviceDecisionTreeClassificationModel:
+        from . import _native as N
+        from .context import Context
+        X = np.asarray(X, dtype=np.float32)
+        n, d = X.shape
+        if n == 0 or d == 0:
+            raise ValueError("DeviceDecisionTreeClassifier.fit needs at least one row and one column")
+        y = np.asarray(y, dtype=np.float64).reshape(-1)
+        K = int(num_classes) if num_classes is not None else int(y.max()) + 1
+        if y.size != n or np.any(y < 0) or np.any(y != np.floor(y)) or np.any(y >= K):
+            raise ValueError(f"labels must be integer class indices in [0, {K}) and one per row")
+        self._check_classes(K)
+        cands = self.split_candidates(X)
+        with Context(self.device) as ctx:
+            ctx.alloc(N.SLOT_X, d, n)
+            ctx.upload_rowmajor(N.SLOT_X, X)
+            ctx.alloc(N.SLOT_Y, n)
+            ctx.upload(N.SLOT_Y, y.astype(np.float32))
+            if w is not None:
+                ctx.alloc(N.SLOT_W, n)
+                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
+            ctx.alloc(N.SLOT_PRED, n)
+            ctx.tree_fit_bins(cands)
+            return self.fit_resident(ctx, K, N.SLOT_Y, 0, N.SLOT_W if w is not None else -1, 0, False,
+                                     np.arange(d, dtype=np.int32), N.SLOT_PRED, 0)
 
 
 class LinearRegressionModel(_Model):

@@ -52,13 +52,14 @@ def bag_counts(n: int, subsample_ratio: float, replacement: bool, seed: int):
 
 
 def _check_device_learner(est: Params, learner) -> bool:
-    """True when the base learner fits on the device (learners.DeviceDecisionTreeRegressor).  It reads the residuals
-    and the features where they live, so it needs residentFeatures=True and a single GPU."""
+    """True when the base learner fits on the device (learners.DeviceDecisionTreeRegressor / Classifier).  It reads
+    the residuals (or labels and boosting weights) and the features where they live, so it needs
+    residentFeatures=True and a single GPU (estimators without a `devices` Param run on one)."""
     if not getattr(learner, "device_learner", False):
         return False
     if not est("residentFeatures"):
         raise ValueError("the device tree learner fits over the device-resident features: set residentFeatures=True")
-    if len(est("devices")) >= 2:
+    if est.hasParam("devices") and len(est("devices")) >= 2:
         raise ValueError("the device tree learner fits on one GPU: `devices` must name at most one device")
     return True
 
