@@ -41,8 +41,9 @@ def _data(n, d, K, seed, special=False, exact=False):
 
 
 def _fit(ctx, X, y, K, *, w=None, bag=None, sub=None, impurity="gini", max_depth=3, max_bins=32, min_instances=1,
-         min_info_gain=0.0, min_weight_fraction=0.0):
-    """Device fits (label and probability outputs) and the oracle fit of the same problem."""
+         min_info_gain=0.0, min_weight_fraction=0.0, exact=False):
+    """Device fits (label and probability outputs) and the oracle fit of the same problem.  Every node of both device
+    trees is audited (np_tree_cls.audit) from the rows it receives, whatever the near ties."""
     from spark_ensemble_b200 import _native as N
     from spark_ensemble_b200.learners import DeviceDecisionTreeClassifier
     n, d = X.shape
@@ -74,6 +75,10 @@ def _fit(ctx, X, y, K, *, w=None, bag=None, sub=None, impurity="gini", max_depth
     np.testing.assert_array_equal(out.view(np.uint32), ctx.download(N.SLOT_RAW).view(np.uint32))
     ctx.tree_predict_multi(tp, N.SLOT_P, subspace=sub)
     np.testing.assert_array_equal(outp.view(np.uint32), ctx.download(N.SLOT_P).reshape(K, n).view(np.uint32))
+    params = dict(num_classes=K, impurity=impurity, max_depth=max_depth, min_instances=min_instances,
+                  min_info_gain=min_info_gain, min_weight_fraction=min_weight_fraction)
+    assert TC.audit(t, X, cands, sub, y, w, bag, params, out=out, exact=exact) == t["feature"].size
+    assert TC.audit(tp, X, cands, sub, y, w, bag, params, out_proba=outp, exact=exact) == tp["feature"].size
     ranks = [T.ranks(X[:, c], cands[c]) for c in sub]
     o = TC.fit(ranks, [cands[c].size for c in sub], y, K, w=w, counts=bag, impurity_kind=impurity,
                max_depth=max_depth, min_instances=min_instances, min_info_gain=min_info_gain,
@@ -150,6 +155,7 @@ def test_device_fit_matches_oracle(ctx, n, S, K, impurity, depth, bins, weighted
     t, out, outp, o, ranks, cands = _fit(ctx, X, y, K, w=w, bag=counts, sub=sub, impurity=impurity, max_depth=depth,
                                          max_bins=bins)
     done, skipped = _compare(t, o, ranks, cands, np.arange(n), counts=counts)
+    print(f"nodes {t['feature'].size}: all audited, {done} compared with the restatement, {skipped} subtrees skipped")
     assert done >= 1
     if n >= 100:
         assert skipped <= (done // 3 if n < 10000 else max(1, done // 10)), (done, skipped)
@@ -169,7 +175,7 @@ def _exact(ctx, seed, impurity):
     K = 3
     X, y = _data(4096, 3, K, seed=seed, exact=True)
     X = np.concatenate([X[:, :1], X], axis=1)  # column 1 duplicates column 0
-    t, out, outp, o, ranks, cands = _fit(ctx, X, y, K, impurity=impurity, max_depth=6, max_bins=8)
+    t, out, outp, o, ranks, cands = _fit(ctx, X, y, K, impurity=impurity, max_depth=6, max_bins=8, exact=True)
     done, skipped = _compare(t, o, ranks, cands, np.arange(X.shape[0]))
     assert skipped <= max(1, done // 10)
     assert 1 not in set(t["feature"].tolist()), "the duplicated column must lose every tie to the first"

@@ -202,6 +202,129 @@ def test_validity_rules_bind():
     np.testing.assert_array_equal(t["proba"][0], np.float32([(y == 0).mean(), (y == 1).mean()]))
 
 
+# ---- the audit of a fitted tree (oracle/np_tree_cls.audit) ----------------------------------------------------
+@pytest.mark.parametrize("seed,K,kind,weighted,bagged", [(0, 3, "gini", False, False), (1, 5, "entropy", True, False),
+                                                         (2, 2, "gini", True, True), (3, 26, "entropy", False, True)])
+def test_audit_passes_restatement_fits_and_fails_each_corruption(seed, K, kind, weighted, bagged):
+    rng = np.random.default_rng(400 + seed)
+    n, d = 4000, 5
+    X = rng.standard_normal((n, d)).astype(np.float32)
+    X[rng.random((n, d)) < 0.03] = np.nan
+    z = np.sin(2 * np.nan_to_num(X[:, 1])) + np.nan_to_num(X[:, 3]) ** 2 + 0.4 * rng.standard_normal(n)
+    y = np.minimum(np.digitize(z, np.quantile(z, np.linspace(0, 1, K + 1)[1:-1])), K - 1).astype(np.float32)
+    w = rng.uniform(0.25, 4.0, n).astype(np.float32) if weighted else None
+    c = rng.poisson(1.0, n).astype(np.float32) if bagged else None
+    cands = [T.candidates(X[:, j], 32) for j in range(d)]
+    sub = np.array([4, 1, 0, 3], np.int32)
+    R = [T.ranks(X[:, j], cands[j]) for j in sub]
+    params = dict(num_classes=K, impurity=kind, max_depth=4, min_instances=1, min_info_gain=0.0,
+                  min_weight_fraction=0.0)
+    o = TC.fit(R, [cands[j].size for j in sub], y, K, w=w, counts=c, impurity_kind=kind, max_depth=4)
+    a = TC.arrays(o, [cands[j] for j in sub])
+    leaf = TC.leaf_of(o, R)
+    assert TC.audit(a, X, cands, sub, y, w, c, params, out=o["label"][leaf], out_proba=o["proba"][leaf].T) == \
+        a["feature"].size
+    f = a["feature"]
+    splits, leaves = np.flatnonzero(f >= 0), np.flatnonzero(f < 0)
+    muts = []
+    b = {k: v.copy() for k, v in a.items()}
+    i = next(i for i in leaves if b["values"][i].max() > 0.1)
+    kk = int(np.argmax(b["values"][i]))
+    b["values"][i, kk] += 4 * np.spacing(b["values"][i, kk])
+    muts.append(("probability + 4 ulps", b))
+    b = {k: v.copy() for k, v in a.items()}
+    cc = cands[sub[f[0]]]
+    j = int(np.searchsorted(cc, b["threshold"][0]))
+    b["threshold"][0] = cc[j + 1] if j + 1 < cc.size else cc[j - 1]
+    muts.append(("threshold on the neighbouring candidate", b))
+    b = {k: v.copy() for k, v in a.items()}
+    i = splits[0]
+    b["left"][i], b["right"][i] = a["right"][i], a["left"][i]
+    muts.append(("children swapped", b))
+    b = {k: v.copy() for k, v in a.items()}
+    cw = (np.ones(n) if c is None else c.astype(np.float64)) * (np.ones(n) if w is None else w)
+    ib = np.flatnonzero(cw > 0)
+    cnt = np.ones(n) if c is None else c.astype(np.float64)
+    gains = []
+    for k in range(len(R)):
+        g = TC._column_gains(R[k][ib], y.astype(np.int64)[ib], cnt[ib], cw[ib], K, cands[sub[k]].size, kind, params,
+                             cw.sum())
+        gains += [(float(g[jj]), k, int(jj)) for jj in np.flatnonzero(np.isfinite(g))]
+    gains.sort(key=lambda x: (-x[0], x[1], x[2]))
+    g2, k2, j2 = next(x for x in gains if x[1] != f[0])
+    assert gains[0][0] - g2 > 1e-6
+    b["feature"][0], b["threshold"][0] = k2, cands[sub[k2]][j2]
+    muts.append(("root split on the runner-up column", b))
+    b = {k: v.copy() for k, v in a.items()}
+    b["class_weights"][0, int(np.argmax(b["class_weights"][0]))] *= 1 + 1e-9
+    muts.append(("class weight x (1 + 1e-9)", b))
+    b = {k: v.copy() for k, v in a.items()}
+    i = next(i for i in leaves if np.sort(b["values"][i])[-1] - np.sort(b["values"][i])[-2] > 0.01)
+    b["value"][i] = np.argsort(b["values"][i])[-2]
+    muts.append(("label of the second-largest class", b))
+    for i in splits:  # a pruned tree's internal nodes all have leaves of two labels below them
+        b, q = T.cut(a, i)
+        b["value"][q] = TC.label_of(b["class_weights"][q])
+        muts.append((f"internal node {i} collapsed into a leaf with its own statistics", b))
+    for name, b in muts:
+        with pytest.raises(AssertionError):
+            TC.audit(b, X, cands, sub, y, w, c, params)
+            pytest.fail(f"the audit accepted: {name}")
+
+
+def test_audit_merged_leaf_and_zero_weight_root():
+    """The hand-worked cascade (one merged leaf with the root's distribution) passes; the same leaf with a child's
+    distribution, or with a label the subtree does not give, fails.  A root without in-bag weight is label 0 with
+    all-zero probabilities."""
+    X, y = _groups({(0, 0): (2, 0), (0, 1): (2, 1), (1, 0): (3, 3), (1, 1): (1, 0)})
+    cands = [T.candidates(X[:, j], 256) for j in range(2)]
+    R = [T.ranks(X[:, j], cands[j]) for j in range(2)]
+    o = TC.fit(R, [x.size for x in cands], y, 2, max_depth=2)
+    a = TC.arrays(o, cands)
+    params = dict(num_classes=2, max_depth=2)
+    assert TC.audit(a, X, cands, [0, 1], y, params=params, exact=True) == 1
+    b = {k: v.copy() for k, v in a.items()}
+    b["values"][0] = np.float32([1.0, 0.0])
+    b["class_weights"][0] = [2.0, 0.0]
+    with pytest.raises(AssertionError):
+        TC.audit(b, X, cands, [0, 1], y, params=params)
+    # the same data with the (1, 1) row of class 1: the root keeps its split, a leaf there is wrong
+    X2, y2 = _groups({(0, 0): (2, 0), (0, 1): (2, 1), (1, 0): (3, 3), (1, 1): (0, 1)})
+    with pytest.raises(AssertionError):
+        TC.audit(dict(a, class_weights=np.array([[7.0, 5.0]]), values=np.float32([[7 / 12, 5 / 12]])), X2, cands,
+                 [0, 1], y2, params=params)
+    zero = dict(a, class_weights=np.zeros((1, 2)), values=np.zeros((1, 2), np.float32), value=np.zeros(1, np.float32))
+    TC.audit(zero, X, cands, [0, 1], y, w=np.zeros(12, np.float32), params=params, exact=True)
+
+
+@pytest.mark.parametrize("kind,weighted", [("gini", False), ("entropy", True)])
+def test_audit_fails_every_wrongly_collapsed_subtree(kind, weighted):
+    """Small deep nodes of integer labels meet near ties often.  A tie below an internal node must not excuse
+    collapsing it: every internal node of restatement fits, made a leaf with its own statistics, fails the audit."""
+    collapsed = 0
+    for seed in range(6):
+        rng = np.random.default_rng(500 + seed)
+        n, d, K = 1500, 4, 3
+        X = rng.standard_normal((n, d)).astype(np.float32)
+        z = np.sin(2 * X[:, 0]) + X[:, 1] * X[:, 2] + 0.5 * rng.standard_normal(n)
+        y = np.minimum(np.digitize(z, np.quantile(z, [1 / 3, 2 / 3])), K - 1).astype(np.float32)
+        w = rng.uniform(0.25, 4.0, n).astype(np.float32) if weighted else None
+        cands = [T.candidates(X[:, j], 32) for j in range(d)]
+        R = [T.ranks(X[:, j], cands[j]) for j in range(d)]
+        o = TC.fit(R, [x.size for x in cands], y, K, w=w, impurity_kind=kind, max_depth=5)
+        a = TC.arrays(o, cands)
+        params = dict(num_classes=K, impurity=kind, max_depth=5)
+        TC.audit(a, X, cands, np.arange(d), y, w, params=params)
+        for i in np.flatnonzero(a["feature"] >= 0):
+            b, q = T.cut(a, i)
+            b["value"][q] = TC.label_of(b["class_weights"][q])
+            with pytest.raises(AssertionError):
+                TC.audit(b, X, cands, np.arange(d), y, w, params=params)
+                pytest.fail(f"seed {seed}: the audit accepted internal node {i} collapsed into a leaf")
+            collapsed += 1
+    assert collapsed > 100
+
+
 # ---- Params ----------------------------------------------------------------------------------------------------
 def test_device_classifier_params():
     from spark_ensemble_b200.ensemble import java_string_hash

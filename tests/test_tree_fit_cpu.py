@@ -225,6 +225,104 @@ def test_validity_rules_bind():
     assert t["feature"].tolist() == [-1] and abs(t["pred"][0] - y.astype(np.float64).mean()) < 1e-12
 
 
+# ---- the audit of a fitted tree (oracle/np_tree.audit) --------------------------------------------------------
+def _audit_problem(seed, weighted, bagged):
+    rng = np.random.default_rng(300 + seed)
+    n, d = 3000, 5
+    X = rng.standard_normal((n, d)).astype(np.float32)
+    X[rng.random((n, d)) < 0.03] = np.nan
+    z = np.nan_to_num(X)
+    r = (np.sin(2 * z[:, 1]) + z[:, 3] ** 2 + 0.3 * rng.standard_normal(n)).astype(np.float32)
+    w = rng.uniform(0.25, 4.0, n).astype(np.float32) if weighted else None
+    c = rng.poisson(1.0, n).astype(np.float32) if bagged else None
+    cands = [T.candidates(X[:, j], 32) for j in range(d)]
+    sub = np.array([4, 1, 0, 3], np.int32)
+    R = [T.ranks(X[:, j], cands[j]) for j in sub]
+    params = dict(max_depth=4, min_instances=1, min_info_gain=0.0, min_weight_fraction=0.0)
+    o = T.fit(R, [cands[j].size for j in sub], r, w=w, counts=c, **params)
+    return T.arrays(o, [cands[j] for j in sub]), X, cands, sub, r, w, c, params, T.predict(o, R), R
+
+
+def _mutations(a, X, cands, sub, r, w, c, params, R):
+    """The tree with one thing wrong, five ways: (name, arrays)."""
+    f, left, right = a["feature"], a["left"], a["right"]
+    splits = np.flatnonzero(f >= 0)
+    leaves = np.flatnonzero(f < 0)
+    out = []
+    b = a.copy()
+    b["value"] = b["value"].copy()
+    i = leaves[0]
+    b["value"][i] = np.float32(b["value"][i]) + 4 * np.spacing(np.float32(b["value"][i]))
+    out.append(("leaf value + 4 ulps", b))
+    b = {k: v.copy() for k, v in a.items()}
+    i = splits[0]
+    cc = cands[sub[f[i]]]
+    j = int(np.searchsorted(cc, b["threshold"][i]))
+    b["threshold"][i] = cc[j + 1] if j + 1 < cc.size else cc[j - 1]
+    out.append(("threshold on the neighbouring candidate", b))
+    b = {k: v.copy() for k, v in a.items()}
+    i = next(i for i in splits if abs(a["value"][left[i]] - a["value"][right[i]]) > 1e-3)
+    b["left"][i], b["right"][i] = a["right"][i], a["left"][i]
+    out.append(("children swapped", b))
+    b = {k: v.copy() for k, v in a.items()}
+    cw = (np.ones(r.size) if c is None else c.astype(np.float64)) * (np.ones(r.size) if w is None else w)
+    ib = np.flatnonzero(cw > 0) if c is not None else np.arange(r.size)
+    cand = T._node_search(R, [cands[j].size for j in sub], ib, np.ones(r.size) if c is None else c.astype(np.float64),
+                          cw, r.astype(np.float64), params, cw.sum())
+    g, k2, j2 = next(x for x in cand if x[1] != f[0])
+    assert cand[0][0] - g > 1e-6
+    b["feature"][0], b["threshold"][0] = k2, cands[sub[k2]][j2]
+    out.append(("root split on the runner-up column", b))
+    for i in splits:  # the value stays fp32(S/W) of the node's rows: only the missing split is wrong
+        out.append((f"internal node {i} collapsed into a leaf", T.cut(a, i)[0]))
+    return out
+
+
+@pytest.mark.parametrize("seed,weighted,bagged", [(0, False, False), (1, True, False), (2, True, True)])
+def test_audit_passes_restatement_fits_and_fails_each_corruption(seed, weighted, bagged):
+    a, X, cands, sub, r, w, c, params, pred, R = _audit_problem(seed, weighted, bagged)
+    assert T.audit(a, X, cands, sub, r, w, c, params, out=pred.astype(np.float32)) == a["feature"].size
+    for name, b in _mutations(a, X, cands, sub, r, w, c, params, R):
+        with pytest.raises(AssertionError):
+            T.audit(b, X, cands, sub, r, w, c, params)
+            pytest.fail(f"the audit accepted: {name}")
+
+
+def test_audit_exact_and_degenerate_fits():
+    """Dyadic data: values exact, so a 1-ulp error fails; a root without in-bag weight is a NaN leaf; a pure node
+    split by a rounding-positive gain passes (Spark's rule) while a false leaf with a real gain does not."""
+    rng = np.random.default_rng(9)
+    X = rng.integers(0, 8, (2000, 3)).astype(np.float32)
+    r = (rng.integers(-8, 8, 2000) / 4).astype(np.float32)
+    cands = [T.candidates(X[:, j], 8) for j in range(3)]
+    sub = np.arange(3)
+    R = [T.ranks(X[:, j], cands[j]) for j in sub]
+    params = dict(max_depth=5)
+    o = T.fit(R, [x.size for x in cands], r, max_depth=5)
+    a = T.arrays(o, cands)
+    T.audit(a, X, cands, sub, r, params=params, exact=True)
+    b = {k: v.copy() for k, v in a.items()}
+    i = np.flatnonzero((a["feature"] < 0) & (a["value"] != 0))[0]
+    b["value"][i] = np.nextafter(b["value"][i], np.float32(np.inf))
+    T.audit(b, X, cands, sub, r, params=params)  # 1 ulp passes on inexact data ...
+    with pytest.raises(AssertionError):
+        T.audit(b, X, cands, sub, r, params=params, exact=True)  # ... not on exact data
+    leaf = {"feature": np.array([-1], np.int32), "threshold": np.zeros(1, np.float32), "left": np.zeros(1, np.int32),
+            "right": np.zeros(1, np.int32), "value": np.array([np.nan], np.float32), "gain": np.zeros(1)}
+    T.audit(leaf, X, cands, sub, r, counts=np.zeros(2000, np.float32), params=params)
+    T.audit(leaf, X, cands, sub, r, w=np.zeros(2000, np.float32), params=params)
+    with pytest.raises(AssertionError):  # the root has a real split: a leaf there is wrong
+        T.audit(dict(leaf, value=np.float32([r.astype(np.float64).mean()])), X, cands, sub, r, params=params)
+    # a pure node (quantile residuals {0.9, -0.1} all equal) split on a noise-level gain passes the audit
+    q = np.float32(0.9) * np.ones(64, np.float32)
+    Xq = np.arange(64, dtype=np.float32)[:, None]
+    cq = [T.candidates(Xq[:, 0], 4)]
+    t1 = {"feature": np.array([0, -1, -1], np.int32), "threshold": np.array([cq[0][0], 0, 0], np.float32),
+          "left": np.array([1, 0, 0], np.int32), "right": np.array([2, 0, 0], np.int32),
+          "value": np.full(3, q[0], np.float32), "gain": np.array([1e-18, 0, 0])}
+    T.audit(t1, Xq, cq, [0], q, params=dict(max_depth=1))
+
+
 # ---- Params ----------------------------------------------------------------------------------------------------
 def test_device_learner_params():
     m = Lr.DeviceDecisionTreeRegressor()
