@@ -344,6 +344,27 @@ SE_API int se_tree_predict_multi(se_ctx* ctx, int which, int n_nodes, const int3
 SE_API int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offsets, const int32_t* feature,
                              const float* threshold, const int32_t* left, const int32_t* right, const float* value,
                              const double* weights, double init, int out_slot, int out_row);
+/* A classifier ensemble of trees in ONE pass, with se_agg_run's epilogue: every row walks every tree over the uint8 rank
+ * matrix, keeps its class totals on chip (fp64, carried in fp64 between chunks of trees) and is finished into RAW, PROB
+ * and LABEL as se_agg_configure + se_agg_run would lay them out — without the [M][K][n] member outputs (SE_SLOT_P is not
+ * allocated).  kind, num_classes, dim and loss mean what they mean for se_agg_configure; only the classifier kinds:
+ *   SE_AGG_GBM_CLASSIFIER     tree t adds weights[t] · value(leaf) to class tree_class[t] (the GBM dimension, [0, dim));
+ *                             totals start at init[0 .. dim) (NULL: 0); dim 1 with 2 classes gives raw = (-F, F)
+ *   SE_AGG_BAGGING_HARD       1 to class value(leaf)
+ *   SE_AGG_BOOSTING_DISCRETE  (float) weights[t] to class value(leaf)
+ *   SE_AGG_BAGGING_SOFT       probs[leaf][k] to every class k
+ *   SE_AGG_BOOSTING_REAL      lg2 max(probs[leaf][k], EPSILON) to every class k (the terms se_agg_run adds)
+ * Trees as se_forest_predict (offsets, tree-local children, GLOBAL columns of X); probs is [total nodes][num_classes]
+ * (bagging soft, boosting real; else may be NULL); tree_class is [n_trees] (GBM only).  Every term is added in fp64 in
+ * model order.  Fails with SE_ERR_STATE, with se_forest_predict's message, when the rank matrix cannot hold the
+ * forest's thresholds (evaluate the members then); with SE_ERR_ARG on a malformed tree, a leaf label that is not a class
+ * index in [0, num_classes) (raised on the device, as se_agg_run does for a bad vote), num_classes above
+ * SE_FOREST_AGG_MAX_CLASSES or a regression kind. */
+#define SE_FOREST_AGG_MAX_CLASSES 32
+SE_API int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, int loss, int n_trees,
+                         const int32_t* offsets, const int32_t* feature, const float* threshold, const int32_t* left,
+                         const int32_t* right, const float* value, const float* probs, const int32_t* tree_class,
+                         const double* weights, const double* init);
 /* ---- regression-tree fit on the device (DESIGN.md §3 "Device tree fit") ----------------------- */
 /* Sets the split candidates of a fit: column c of SE_SLOT_X (n_cols == its column count) gets the sorted, finite,
  * strictly increasing thresholds[offsets[c] .. offsets[c+1]) (0..255 of them) as the edge list of the uint8 rank matrix

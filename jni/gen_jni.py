@@ -111,6 +111,11 @@ TABLE = [
                                             ("threshold", "in_f32"), ("left", "in_i32"), ("right", "in_i32"), ("value", "in_f32"),
                                             ("weights", "in_f64"), ("init", "f64"), ("outSlot", "i32"), ("outRow", "i32")],
      "GBMRegressionModel.predict / BaggingRegressionModel.predict for tree members: init + sum of weight * tree(x) in one pass"),
+    ("forestAgg", "se_forest_agg", [("ctx", "ctx"), ("which", "i32"), ("kind", "i32"), ("numClasses", "i32"), ("dim", "i32"),
+                                    ("loss", "i32"), ("nTrees", "i32"), ("offsets", "in_i32"), ("feature", "in_i32"),
+                                    ("threshold", "in_f32"), ("left", "in_i32"), ("right", "in_i32"), ("value", "in_f32"),
+                                    ("probs", "in_f32"), ("treeClass", "in_i32"), ("weights", "in_f64"), ("init", "in_f64")],
+     "predictRaw / probability / prediction of a classifier ensemble of trees in one pass, without member outputs"),
     ("linearPredict", "se_linear_predict", [("ctx", "ctx"), ("which", "i32"), ("nCoef", "i32"), ("coef", "in_f32"), ("intercept", "f32"),
                                             ("subspace", "in_i32"), ("outSlot", "i32"), ("outRow", "i32")], ""),
 ]

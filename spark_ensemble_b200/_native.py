@@ -29,6 +29,7 @@ UPD_RESIDUAL, UPD_NEWTON, UPD_LOSS = 1, 2, 4
 (AGG_GBM_REGRESSOR, AGG_BAGGING_REGRESSOR, AGG_GBM_CLASSIFIER, AGG_BAGGING_SOFT, AGG_BAGGING_HARD,
  AGG_BOOSTING_REAL, AGG_BOOSTING_DISCRETE, AGG_BOOSTING_REG_MEDIAN, AGG_BOOSTING_REG_MEAN) = range(9)
 R2_LOSS = {"exponential": 0, "linear": 1, "squared": 2}
+FOREST_AGG_MAX_CLASSES = 32  # SE_FOREST_AGG_MAX_CLASSES: se_forest_agg's class limit
 
 # enum se_kernel_family
 KERNEL_FAMILIES = ["sq_stats", "eval", "update", "resid", "mean_loss", "boost_real", "boost_err",
@@ -113,6 +114,7 @@ PROTOTYPES = {
     "se_tree_predict": [_vp, _i32, _i32, _ip, _fp, _ip, _ip, _fp, _ip, _i32, _i32, _i32],
     "se_tree_predict_multi": [_vp, _i32, _i32, _ip, _fp, _ip, _ip, _fp, _i32, _ip, _i32, _i32],
     "se_forest_predict": [_vp, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _dp, _d, _i32, _i32],
+    "se_forest_agg": [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _fp, _ip, _dp, _dp],
     "se_linear_predict": [_vp, _i32, _i32, _fp, _f, _ip, _i32, _i32],
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,

@@ -16,7 +16,8 @@ from .ensemble import DataFrame, fit_dummy_classifier, java_string_hash, subspac
 from .gbm_engine import GBMEngine
 from .params import (Param, Params, ParamValidators, boosting_params, gbm_params, random_uid,
                      shared_classifier_params, shared_predictor_params, subbag_params)
-from .regression import _check_device_learner, _extract_instances, _split_validation, bag_counts
+from .regression import (_check_device_learner, _device_trees, _extract_instances, _rank_matrix_full,
+                         _resident_context, _split_validation, bag_counts)
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -68,6 +69,21 @@ class _ClassifierModelBase(Params):
         label = ctx.download(N.SLOT_LABEL).astype(np.float64)
         C = self._out_classes
         return raw.reshape(C, -1).T, prob.reshape(C, -1).T, label
+
+    def _forest_agg_resident(self, X, kind: int, trees, **kw):
+        """Scores the tree members in one pass over the device-resident features (se_forest_agg): no member output
+        is computed on the host or stacked.  None when the forest is outside the kernel's reach (more than
+        FOREST_AGG_MAX_CLASSES classes, or more than 255 thresholds in a column): the caller scores member by member."""
+        if trees is None or self.numClasses > N.FOREST_AGG_MAX_CLASSES:
+            return None
+        with _resident_context(self.device, X) as ctx:
+            try:
+                ctx.forest_agg(kind, self.numClasses, trees, **kw)
+            except N.NativeError as e:
+                if _rank_matrix_full(e):
+                    return None
+                raise
+            return self._fetch(ctx)
 
 
 # ================================================================================ GBMClassifier
@@ -221,6 +237,13 @@ class GBMClassificationModel(_ClassifierModelBase):
 
     def _raw_prob_label(self, X):
         n, M, dim = X.shape[0], self.numModels, self.dim
+        out = self._forest_agg_resident(
+            X, N.AGG_GBM_CLASSIFIER, _device_trees(self, [m for ms in self.models for m in ms]),
+            weights=np.concatenate([np.asarray(wt, dtype=np.float64).reshape(dim) for wt in self.weights]) if M else None,
+            init=self.init, tree_class=np.tile(np.arange(dim, dtype=np.int32), M), dim=dim, loss=self("loss").lower(),
+            subspaces=[s for s in self.subspaces[:M] for _ in range(dim)])
+        if out is not None:
+            return out
         P = np.zeros((max(M, 1), dim, n), dtype=np.float32)
         for i in range(M):
             Xs = X[:, self.subspaces[i]]
@@ -348,6 +371,10 @@ class BoostingClassificationModel(_ClassifierModelBase):
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         real = self("algorithm").lower() == "real"
+        out = self._forest_agg_resident(X, N.AGG_BOOSTING_REAL if real else N.AGG_BOOSTING_DISCRETE,
+                                        _device_trees(self, self.models), weights=None if real else self.weights)
+        if out is not None:
+            return out
         with Context(self.device) as ctx:
             if real:
                 P = np.zeros((max(M, 1), K, n), dtype=np.float32)
@@ -401,8 +428,10 @@ _pbagc = [Param("numBaseLearners", "number of base learners", ParamValidators.gt
           Param("baseLearner", "base learner"),
           Param("votingStrategy", "voting strategy, (case-insensitive). Supported options: soft,hard",
                 lambda v: v.lower() in ("soft", "hard"), str),
-          Param("parallelism", "threads", ParamValidators.gtEq(1), int)]
+          Param("parallelism", "threads", ParamValidators.gtEq(1), int),
+          Param("residentFeatures", "evaluate base models on device over the HBM-resident feature matrix", convert=bool)]
 _BAG_CLS_DEFAULTS = {**_d, **_dc, **_ds, "numBaseLearners": 10, "votingStrategy": "hard", "parallelism": 1,
+                     "residentFeatures": False,
                      "seed": java_string_hash("org.apache.spark.ml.classification.BaggingClassifier")}
 BaggingClassifier._declare(_p + _pc + _ps + _pbagc, _BAG_CLS_DEFAULTS)
 
@@ -422,6 +451,10 @@ class BaggingClassificationModel(_ClassifierModelBase):
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         soft = self("votingStrategy").lower() == "soft"
+        out = self._forest_agg_resident(X, N.AGG_BAGGING_SOFT if soft else N.AGG_BAGGING_HARD,
+                                        _device_trees(self, self.models), subspaces=self.subspaces)
+        if out is not None:
+            return out
         with Context(self.device) as ctx:
             if soft:
                 P = np.zeros((M, K, n), dtype=np.float32)

@@ -12,6 +12,34 @@ import numpy as np
 from . import _native as N
 
 
+def _pack_forest(trees, subspaces=None, width: int = 0):
+    """Concatenated node arrays of a list of trees (se_forest_predict / se_forest_agg form): offsets, GLOBAL column
+    per node (each tree's subspace applied), threshold, tree-local children, value, and with width > 0 the
+    [n_nodes, width] "values" of every tree stacked."""
+    offs = np.zeros(len(trees) + 1, dtype=np.int32)
+    f, t, l, r, v, p = [], [], [], [], [], []
+    for i, tr in enumerate(trees):
+        fi = np.asarray(tr["feature"], dtype=np.int32)
+        if subspaces is not None and subspaces[i] is not None:
+            sub = np.asarray(subspaces[i], dtype=np.int32)
+            if np.any(fi >= sub.size):
+                raise ValueError(f"tree {i}: feature index outside its subspace")
+            fi = np.where(fi >= 0, sub[np.maximum(fi, 0)], fi).astype(np.int32)
+        f.append(fi)
+        t.append(np.asarray(tr["threshold"], dtype=np.float32))
+        l.append(np.asarray(tr["left"], dtype=np.int32))
+        r.append(np.asarray(tr["right"], dtype=np.int32))
+        v.append(np.asarray(tr["value"], dtype=np.float32))
+        if width:
+            pi = np.asarray(tr["values"], dtype=np.float32)
+            if pi.shape != (fi.size, width):
+                raise ValueError(f"tree {i}: values must be [n_nodes, {width}], got {pi.shape}")
+            p.append(pi)
+        offs[i + 1] = offs[i] + fi.size
+    f, t, l, r, v = (np.ascontiguousarray(np.concatenate(a)) for a in (f, t, l, r, v))
+    return offs, f, t, l, r, v, (np.ascontiguousarray(np.concatenate(p)) if width else None)
+
+
 class Context:
     def __init__(self, device: int = 0):
         self._lib = N.load()
@@ -379,28 +407,33 @@ class Context:
         """out = init + sum_t weights[t] * tree_t(x) for a list of regression trees (dicts as in tree_predict) in one
         pass over the resident feature matrix (se_forest_predict: GBMRegressionModel.predict,
         regression/GBMRegressor.scala:531-539).  `subspaces[t]` maps tree t's feature indices to columns of X."""
-        offs = np.zeros(len(trees) + 1, dtype=np.int32)
-        f, t, l, r, v = [], [], [], [], []
-        for i, tr in enumerate(trees):
-            fi = np.asarray(tr["feature"], dtype=np.int32)
-            if subspaces is not None and subspaces[i] is not None:
-                sub = np.asarray(subspaces[i], dtype=np.int32)
-                if np.any(fi >= sub.size):
-                    raise ValueError(f"tree {i}: feature index outside its subspace")
-                fi = np.where(fi >= 0, sub[np.maximum(fi, 0)], fi).astype(np.int32)
-            f.append(fi)
-            t.append(np.asarray(tr["threshold"], dtype=np.float32))
-            l.append(np.asarray(tr["left"], dtype=np.int32))
-            r.append(np.asarray(tr["right"], dtype=np.int32))
-            v.append(np.asarray(tr["value"], dtype=np.float32))
-            offs[i + 1] = offs[i] + fi.size
-        f, t, l, r, v = (np.ascontiguousarray(np.concatenate(a)) for a in (f, t, l, r, v))
+        offs, f, t, l, r, v, _ = _pack_forest(trees, subspaces)
         w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float64)
         if w is not None and w.size != len(trees):
             raise ValueError("one weight per tree")
         self._ck(self._lib.se_forest_predict(self._h, int(validation), len(trees), N.iptr(offs), N.iptr(f), N.fptr(t),
                                              N.iptr(l), N.iptr(r), N.fptr(v), None if w is None else N.dptr(w),
                                              float(init), out_slot, out_row))
+
+    def forest_agg(self, kind: int, num_classes: int, trees, weights=None, init=None, tree_class=None, dim: int = 1,
+                   loss=0, validation: bool = False, subspaces=None):
+        """A classifier ensemble of trees scored in one pass over the resident feature matrix, straight into RAW,
+        PROB and LABEL as agg_configure + agg_run lay them out, with no member-output matrix (se_forest_agg).
+        Trees are dicts as in tree_predict; bagging soft and boosting real also need "values" ([n_nodes, K] leaf
+        probabilities).  `tree_class[t]` is tree t's GBM dimension, `subspaces[t]` maps its feature indices to
+        columns of X."""
+        vec = kind in (N.AGG_BAGGING_SOFT, N.AGG_BOOSTING_REAL)
+        offs, f, t, l, r, v, p = _pack_forest(trees, subspaces, num_classes if vec else 0)
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        if w is not None and w.size != len(trees):
+            raise ValueError("one weight per tree")
+        cls = None if tree_class is None else np.ascontiguousarray(tree_class, dtype=np.int32)
+        ini = None if init is None else np.ascontiguousarray(np.atleast_1d(init), dtype=np.float64)
+        lid = N.LOSS[loss] if isinstance(loss, str) else int(loss)
+        self._ck(self._lib.se_forest_agg(self._h, int(validation), int(kind), int(num_classes), int(dim), lid, len(trees),
+                                         N.iptr(offs), N.iptr(f), N.fptr(t), N.iptr(l), N.iptr(r), N.fptr(v),
+                                         None if p is None else N.fptr(p), None if cls is None else N.iptr(cls),
+                                         None if w is None else N.dptr(w), None if ini is None else N.dptr(ini)))
 
     def linear_predict(self, coef, intercept: float, out_slot: int, out_row: int = 0,
                        validation: bool = False, subspace=None):

@@ -615,26 +615,30 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
   }
 }
 
+// Binary GBM classifier with dim 1 (GBMClassifier.scala:583-584 + GBMLoss.scala:284-289,311-316): raw = (−F, F) from
+// the one total F = res.
+__device__ __forceinline__ void finalize_binary_row(const FinArgs& f, int64_t i, float res) {
+  const float r0 = -res;
+  // p1 = 1/(1+e^x), p0 = 1 - p1 with x = raw(0) (bernoulli) or -2 raw(0) (exponential); both
+  // formed from t = e^-|x| so the small one keeps full relative precision
+  const float x = (f.loss == SE_LOSS_EXPONENTIAL) ? -2.0f * r0 : r0;
+  const float t = exp_neg_fast(-fabsf(x));
+  const float inv = rcp_approx(1.0f + t);
+  const float p1 = (x >= 0.f) ? t * inv : inv;
+  const float p0 = (x >= 0.f) ? inv : t * inv;
+  f.raw[i] = r0;
+  f.raw[f.ld + i] = res;
+  f.prob[i] = p0;
+  f.prob[f.ld + i] = p1;
+  f.label[i] = (res > r0) ? 1.0f : 0.0f;  // argmax, first maximum on ties
+}
+
 // Stage 2 for the sum-based kinds: per-row epilogue on tmp[C][n] (in RAW) -> raw, prob, label.
 __global__ void __launch_bounds__(kBlock) agg_finalize_kernel(const FinArgs f) {
   for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < f.n;
        i += (int64_t)gridDim.x * kBlock) {
     if (f.kind == SE_AGG_GBM_CLASSIFIER && f.dim == 1 && f.K == 2) {
-      // GBMClassifier.scala:583-584 + GBMLoss.scala:284-289,311-316 (raw(0) = −F)
-      const float res = f.raw[i];
-      const float r0 = -res;
-      // p1 = 1/(1+e^x), p0 = 1 - p1 with x = raw(0) (bernoulli) or -2 raw(0) (exponential); both
-      // formed from t = e^-|x| so the small one keeps full relative precision
-      const float x = (f.loss == SE_LOSS_EXPONENTIAL) ? -2.0f * r0 : r0;
-      const float t = exp_neg_fast(-fabsf(x));
-      const float inv = rcp_approx(1.0f + t);
-      const float p1 = (x >= 0.f) ? t * inv : inv;
-      const float p0 = (x >= 0.f) ? inv : t * inv;
-      f.raw[i] = r0;
-      f.raw[f.ld + i] = res;
-      f.prob[i] = p0;
-      f.prob[f.ld + i] = p1;
-      f.label[i] = (res > r0) ? 1.0f : 0.0f;  // argmax, first maximum on ties
+      finalize_binary_row(f, i, f.raw[i]);
       continue;
     }
     if (f.kind == SE_AGG_BOOSTING_REAL)
@@ -1051,6 +1055,102 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   return cudaGetLastError();
 }
 
+// ---- a classifier forest in one pass (se_forest_agg) -------------------------------------------------------------
+// What tree t adds to its row's class totals, for its leaf node `leaf` (chunk-local node index):
+//   kFaTreeClass  GBM classifier: w_t · value(leaf) to class cls_t                (GBMClassifier.scala:567-589)
+//   kFaVote       bagging hard / boosting discrete: w_t (1 for hard) to class value(leaf) (BaggingClassifier.scala:
+//                 260-283, BoostingClassifier.scala:366-382); a value that is not a class index raises bad_label
+//   kFaSoft       bagging soft: p_leaf,k to every class k                         (BaggingClassifier.scala:260-287)
+//   kFaReal       boosting real: lg2_clamped(p_leaf,k) to every class k           (BoostingClassifier.scala:348-364)
+// Every term is added in fp64 in model order, so SAMME.R totals equal the member route's sums term for term.
+enum { kFaTreeClass = 0, kFaVote = 1, kFaSoft = 2, kFaReal = 3 };
+static_assert(kForestAggMaxClasses == SE_FOREST_AGG_MAX_CLASSES, "the kernel's class limit is the ABI's");
+
+template <int MODE>
+__global__ void __launch_bounds__(kForestAggTile) forest_agg_kernel(const ForestAggArgs g, const FinArgs fin) {
+  constexpr int TILE = kForestAggTile;
+  extern __shared__ __align__(16) unsigned char fsm[];
+  const ForestArgs& a = g.f;
+  for (int i = threadIdx.x; i < a.blob_bytes / 16; i += TILE)
+    reinterpret_cast<uint4*>(fsm)[i] = __ldg(reinterpret_cast<const uint4*>(a.blob) + i);
+  const double* s_w = reinterpret_cast<const double*>(fsm);
+  const unsigned long long* s_coloff = reinterpret_cast<const unsigned long long*>(fsm + a.off_coloff);
+  const uint2* s_nodes = reinterpret_cast<const uint2*>(fsm + a.off_nodes);
+  const int* s_toff = reinterpret_cast<const int*>(fsm + a.off_treeoff);
+  const int* s_cls = reinterpret_cast<const int*>(fsm + a.off_treecls);
+  const float* s_val = reinterpret_cast<const float*>(fsm + a.off_values);
+  unsigned char* s_rank = fsm + a.off_ranks;
+  double* s_tot = reinterpret_cast<double*>(s_rank + (size_t)a.C * TILE);  // [C][TILE]: off_ranks and C * TILE are 8-aligned
+  const int C = g.C, K = g.K;
+  bool bad_vote = false;
+  const int64_t ntiles = (a.n + TILE - 1) / TILE;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    __syncthreads();  // the packed trees are staged (first tile) / the previous tile's walks are over
+    const int64_t row0 = tile * TILE;
+    for (int i = threadIdx.x; i < a.C * (TILE / 4); i += TILE) {
+      const int c = i / (TILE / 4), q = i % (TILE / 4);
+      const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
+      uint32_t v = 0;
+      if (r < a.ld8) v = __ldg(reinterpret_cast<const uint32_t*>(a.X8 + s_coloff[c] + r));
+      *reinterpret_cast<uint32_t*>(s_rank + c * TILE + 4 * q) = v;
+    }
+    __syncthreads();
+    const int64_t row = row0 + threadIdx.x;
+    if (row >= a.n) continue;
+    double* tot = s_tot + threadIdx.x;  // this row's totals: own column, no synchronisation
+    for (int c = 0; c < C; ++c) tot[c * TILE] = g.first ? g.init[c] : g.acc[c * g.ld_acc + row];
+    const unsigned char* myr = s_rank + threadIdx.x;
+    auto add = [&](int t, int leaf) {
+      const int node = s_toff[t] + leaf;
+      if constexpr (MODE == kFaTreeClass) {
+        tot[s_cls[t] * TILE] += s_w[t] * (double)s_val[node];
+      } else if constexpr (MODE == kFaVote) {
+        const float v = s_val[node];
+        const int c = __float2int_rz(v);
+        const bool ok = ((unsigned)c < (unsigned)K) && ((float)c == v);  // a vote is a predicted class index
+        bad_vote = bad_vote || !ok;
+        if (ok) tot[c * TILE] += s_w[t];
+      } else {
+        const float* p = g.probs + (size_t)node * K;
+        for (int k = 0; k < K; ++k) {
+          const float pk = __ldg(p + k);
+          tot[k * TILE] += (MODE == kFaReal) ? (double)lg2_clamped(pk) : (double)pk;
+        }
+      }
+    };
+    int t = 0;
+    for (; t + 1 < a.T; t += 2) {  // two independent walks in flight, terms added in model order
+      const uint2* n0 = s_nodes + s_toff[t];
+      const uint2* n1 = s_nodes + s_toff[t + 1];
+      int d0 = 0, d1 = 0;
+      bool l0 = true, l1 = true;
+      while (l0 || l1) {
+        if (l0) forest_step<TILE>(n0, myr, d0, l0);
+        if (l1) forest_step<TILE>(n1, myr, d1, l1);
+      }
+      add(t, d0);
+      add(t + 1, d1);
+    }
+    if (t < a.T) {
+      const uint2* n0 = s_nodes + s_toff[t];
+      int d0 = 0;
+      bool l0 = true;
+      while (l0) forest_step<TILE>(n0, myr, d0, l0);
+      add(t, d0);
+    }
+    if (!g.last) {
+      for (int c = 0; c < C; ++c) g.acc[c * g.ld_acc + row] = tot[c * TILE];
+    } else if (MODE == kFaTreeClass && g.dim == 1 && g.K == 2) {
+      finalize_binary_row(fin, row, (float)tot[0]);
+    } else if (MODE == kFaReal) {
+      finalize_real_row(fin, row, [&](int c) { return tot[c * TILE]; });
+    } else {
+      finalize_row(fin, row, [&](int c) { return tot[c * TILE]; });
+    }
+  }
+  if (bad_vote && g.bad_label != nullptr) *reinterpret_cast<volatile int*>(g.bad_label) = 1;
+}
+
 }  // namespace
 
 cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t st) {
@@ -1220,6 +1320,45 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
     f.sum_a = a.sum_weights;
   }
   agg_finalize_kernel<<<grid1, kBlock, 0, st>>>(f);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_forest_agg(const ForestAggArgs& g, int sms, cudaStream_t st) {
+  const ForestArgs& a = g.f;
+  const size_t smem = (size_t)a.off_ranks + (size_t)a.C * kForestAggTile + (size_t)g.C * kForestAggTile * sizeof(double);
+  if (a.T < 1 || a.C < 0 || g.C < 1 || g.C > kForestAggMaxClasses || smem > 220 * 1024 || (a.blob_bytes & 15) != 0)
+    return cudaErrorInvalidValue;
+  FinArgs f{};
+  f.kind = g.kind; f.C = g.C; f.K = g.K; f.dim = g.dim; f.loss = g.loss; f.M = g.M;
+  f.sum_a = g.sum_a;
+  f.n = a.n; f.ld = g.ld_out; f.raw = g.raw; f.prob = g.prob; f.label = g.label;
+  f.bad_label = g.bad_label;
+  f.inv_km1 = 1.0 / (double)((g.K > 1 ? g.K : 2) - 1);
+  int per_sm = (int)((220 * 1024) / (smem + 1024));
+  if (per_sm < 1) per_sm = 1;
+  if (per_sm > 16) per_sm = 16;
+  int64_t need = (a.n + kForestAggTile - 1) / kForestAggTile;
+  if (need < 1) need = 1;
+  const int64_t cap = (int64_t)sms * per_sm;
+  const int grid = (int)(need < cap ? need : cap);
+#define SE_FA(MODE)                                                                                              \
+  {                                                                                                              \
+    auto kern = forest_agg_kernel<MODE>;                                                                         \
+    if (smem > 48 * 1024) {                                                                                      \
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
+      if (e != cudaSuccess) return e;                                                                            \
+    }                                                                                                            \
+    kern<<<grid, kForestAggTile, smem, st>>>(g, f);                                                              \
+  }
+  switch (g.kind) {
+    case SE_AGG_GBM_CLASSIFIER: SE_FA(kFaTreeClass) break;
+    case SE_AGG_BAGGING_HARD:
+    case SE_AGG_BOOSTING_DISCRETE: SE_FA(kFaVote) break;
+    case SE_AGG_BAGGING_SOFT: SE_FA(kFaSoft) break;
+    case SE_AGG_BOOSTING_REAL: SE_FA(kFaReal) break;
+    default: return cudaErrorInvalidValue;
+  }
+#undef SE_FA
   return cudaGetLastError();
 }
 

@@ -248,8 +248,12 @@ struct se_ctx {
   // binned (uint8) copies of X / VX for the tree walk
   BinState bins[2];
   int tree_bins = 1;                  // 0: always walk the fp32 matrix
-  unsigned char* d_forest = nullptr;  // packed chunk of trees for se_forest_predict
+  unsigned char* d_forest = nullptr;  // packed chunk of trees for se_forest_predict / se_forest_agg
   size_t forest_cap = 0;
+  float* d_forest_p = nullptr;        // se_forest_agg: leaf class probabilities of every node [nodes][K]
+  size_t forest_p_cap = 0;            // floats
+  double* d_forest_acc = nullptr;     // se_forest_agg: fp64 class totals carried between chunks [C][n]
+  size_t forest_acc_cap = 0;          // doubles
   int last_forest_chunks = 0;
   int wm_fast = 1;                    // weighted median (M <= 64, weights >= 0): keys-only sort + margin check, exact kernel for the rest
   int64_t wm_list_cap = 0;            // deferred-row list capacity (0: n / 4)
@@ -789,6 +793,8 @@ int se_ctx_destroy(se_ctx* ctx) {
   free_bins(ctx->bins[1]);
   if (ctx->d_wm) cudaFree(ctx->d_wm);
   if (ctx->d_forest) cudaFree(ctx->d_forest);
+  if (ctx->d_forest_p) cudaFree(ctx->d_forest_p);
+  if (ctx->d_forest_acc) cudaFree(ctx->d_forest_acc);
   if (ctx->tf.d_nid) cudaFree(ctx->tf.d_nid);
   if (ctx->tf.d_hist) cudaFree(ctx->tf.d_hist);
   if (ctx->tf.d_nodes) cudaFree(ctx->tf.d_nodes);
@@ -2787,6 +2793,173 @@ int se_tree_predict_multi(se_ctx* ctx, int which, int n_nodes, const int32_t* fe
                            out_slot, 0);
 }
 
+// ---- forests in one pass over the rank matrix (se_forest_predict, se_forest_agg) ----------------------------------
+namespace {
+// Every member must be a tree rooted at its first node, with tree-local child indices and GLOBAL column indices of X
+// (d columns): anything else could send the device walk out of the tree or around a cycle.
+int forest_check(se_ctx* ctx, int64_t d, int n_trees, const int32_t* offsets, const int32_t* feature, const int32_t* left,
+                 const int32_t* right) {
+  SE_REQUIRE(ctx, offsets[0] == 0, SE_ERR_ARG, "offsets[0] must be 0");
+  const int64_t total = offsets[n_trees];
+  SE_REQUIRE(ctx, total >= n_trees && total <= (1 << 26), SE_ERR_ARG, "bad node count %lld", (long long)total);
+  std::vector<char> seen;
+  std::vector<int32_t> stack;
+  for (int t = 0; t < n_trees; ++t) {
+    const int32_t b = offsets[t], nn = offsets[t + 1] - offsets[t];
+    SE_REQUIRE(ctx, nn >= 1 && nn <= 65535, SE_ERR_ARG, "tree %d: %d nodes (1..65535 supported)", t, nn);
+    for (int i = 0; i < nn; ++i) {
+      if (feature[b + i] < 0) continue;
+      SE_REQUIRE(ctx, feature[b + i] < d, SE_ERR_ARG, "tree %d node %d: column %d outside X with %lld columns", t, i,
+                 feature[b + i], (long long)d);
+      SE_REQUIRE(ctx, left[b + i] >= 0 && left[b + i] < nn && right[b + i] >= 0 && right[b + i] < nn, SE_ERR_ARG,
+                 "tree %d node %d: bad child", t, i);
+    }
+    seen.assign((size_t)nn, 0);
+    stack.clear();
+    stack.push_back(0);
+    seen[0] = 1;
+    while (!stack.empty()) {
+      const int32_t i = stack.back();
+      stack.pop_back();
+      if (feature[b + i] < 0) continue;
+      for (const int32_t c : {left[b + i], right[b + i]}) {
+        SE_REQUIRE(ctx, !seen[c], SE_ERR_ARG, "tree %d: node %d is reached twice: not a tree", t, c);
+        seen[c] = 1;
+        stack.push_back(c);
+      }
+    }
+  }
+  return SE_OK;
+}
+
+// Makes the rank matrix of X cover every threshold of the forest; SE_ERR_STATE when it cannot (a column with more than
+// 255 distinct thresholds, a NaN threshold, tree_bins off).
+int forest_bins(se_ctx* ctx, int which, const SlotBuf& X, int n_trees, const int32_t* offsets, const int32_t* feature,
+                const float* threshold) {
+  const int rc = bins_prepare(ctx, which, X, offsets[n_trees], feature, threshold);
+  if (rc < 0) return rc;
+  SE_REQUIRE(ctx, rc == 1, SE_ERR_STATE,
+             "the forest kernel needs the uint8 rank matrix (tree_bins on, <= 255 distinct thresholds per column, no NaN "
+             "threshold): evaluate the members with se_tree_predict + se_agg_run instead");
+  return SE_OK;
+}
+
+// Trees [t0, t1) run as one launch; cols are the global columns they use (local column c = cols[c]).
+struct ForestChunk {
+  int t0 = 0, t1 = 0;
+  size_t nodes = 0;
+  std::vector<int32_t> cols;
+};
+
+size_t forest_pad(size_t v, size_t to) { return (v + to - 1) / to * to; }
+
+// Blob layout of a chunk (ForestArgs): T trees, C columns, Nn nodes, with or without the per-tree class array.
+void forest_layout(size_t T, size_t C, size_t Nn, bool cls, ForestArgs& a) {
+  a.T = (int)T; a.C = (int)C;
+  a.off_coloff = (int)(8 * T);
+  a.off_nodes = a.off_coloff + (int)(8 * C);
+  a.off_treeoff = a.off_nodes + (int)(8 * Nn);
+  a.off_treecls = cls ? a.off_treeoff + (int)forest_pad(4 * (T + 1), 8) : 0;
+  a.off_values = (cls ? a.off_treecls + (int)forest_pad(4 * T, 8) : a.off_treeoff + (int)forest_pad(4 * (T + 1), 8));
+  a.blob_bytes = (int)forest_pad((size_t)a.off_values + 4 * Nn, 16);
+  a.off_ranks = a.blob_bytes;
+}
+
+// Cuts the forest into chunks of consecutive trees whose blob, plus the ranks of their columns ([C][tile] bytes), plus
+// `fixed` bytes the kernel keeps for itself fit one CTA's shared memory.  A chunk grows tree by tree under the
+// four-CTAs-per-SM budget; a member that does not fit it alone gets two, then one CTA per SM.
+int forest_plan(se_ctx* ctx, int64_t d, int n_trees, const int32_t* offsets, const int32_t* feature, bool cls, int tile,
+                size_t fixed, std::vector<ForestChunk>& chunks) {
+  chunks.clear();
+  std::vector<int32_t> local((size_t)d, -1);  // global column -> local column of the current chunk
+  std::vector<int32_t> used;
+  int t0 = 0;
+  while (t0 < n_trees) {
+    size_t nodes = 0;
+    int t1 = t0;
+    for (const size_t budget : {(size_t)kForestSmemBudget, (size_t)(100 * 1024), (size_t)(216 * 1024)}) {
+      for (int32_t c : used) local[c] = -1;
+      used.clear();
+      nodes = 0;
+      for (t1 = t0; t1 < n_trees; ++t1) {
+        const int32_t b = offsets[t1], nn = offsets[t1 + 1] - offsets[t1];
+        std::vector<int32_t> added;
+        for (int i = 0; i < nn; ++i) {
+          const int32_t c = feature[b + i];
+          if (c >= 0 && local[c] < 0) { local[c] = (int32_t)(used.size() + added.size()); added.push_back(c); }
+        }
+        ForestArgs a;
+        forest_layout((size_t)(t1 - t0 + 1), used.size() + added.size(), nodes + (size_t)nn, cls, a);
+        const size_t bytes = (size_t)a.blob_bytes + (size_t)a.C * tile + fixed;
+        if (bytes > budget || a.C > 65535) {
+          for (int32_t c : added) local[c] = -1;
+          break;
+        }
+        used.insert(used.end(), added.begin(), added.end());
+        nodes += (size_t)nn;
+      }
+      if (t1 > t0) break;
+    }
+    SE_REQUIRE(ctx, t1 > t0, SE_ERR_ARG, "tree %d alone (%d nodes) does not fit the forest kernel's shared memory", t0,
+               offsets[t0 + 1] - offsets[t0]);
+    ForestChunk ch;
+    ch.t0 = t0; ch.t1 = t1; ch.nodes = nodes; ch.cols = used;
+    chunks.push_back(std::move(ch));
+    t0 = t1;
+  }
+  return SE_OK;
+}
+
+// Packs a chunk (weights NULL: all 1; tree_class NULL: no class array) into ctx->d_forest and sets the layout fields of
+// `a`.  Returns once the copy is done: the blob is pageable host memory and d_forest is reused by the next chunk.
+int forest_upload_chunk(se_ctx* ctx, const BinState& B, const ForestChunk& ch, const int32_t* offsets,
+                        const int32_t* feature, const float* threshold, const int32_t* left, const int32_t* right,
+                        const float* value, const double* weights, const int32_t* tree_class, ForestArgs& a) {
+  const size_t T = (size_t)(ch.t1 - ch.t0), C = ch.cols.size();
+  forest_layout(T, C, ch.nodes, tree_class != nullptr, a);
+  std::vector<unsigned char> blob((size_t)a.blob_bytes, 0);
+  std::vector<int32_t> local((size_t)B.d, -1);
+  for (size_t c = 0; c < C; ++c) local[ch.cols[c]] = (int32_t)c;
+  double* bw = reinterpret_cast<double*>(blob.data());
+  unsigned long long* bco = reinterpret_cast<unsigned long long*>(blob.data() + a.off_coloff);
+  uint2* bn = reinterpret_cast<uint2*>(blob.data() + a.off_nodes);
+  int32_t* bto = reinterpret_cast<int32_t*>(blob.data() + a.off_treeoff);
+  int32_t* bcl = reinterpret_cast<int32_t*>(blob.data() + a.off_treecls);
+  float* bv = reinterpret_cast<float*>(blob.data() + a.off_values);
+  for (size_t c = 0; c < C; ++c) bco[c] = (unsigned long long)ch.cols[c] * (unsigned long long)B.ld8;
+  size_t at = 0;
+  for (int t = ch.t0; t < ch.t1; ++t) {
+    const int32_t b = offsets[t], nn = offsets[t + 1] - offsets[t];
+    bw[t - ch.t0] = weights ? weights[t] : 1.0;
+    bto[t - ch.t0] = (int32_t)at;
+    if (tree_class) bcl[t - ch.t0] = tree_class[t];
+    for (int i = 0; i < nn; ++i) {
+      const int32_t c = feature[b + i];
+      bv[at + i] = value[b + i];
+      if (c < 0) { bn[at + i] = make_uint2(0x80000000u, 0u); continue; }
+      const std::vector<float>& E = B.edges[c];
+      const uint32_t j = (uint32_t)(std::lower_bound(E.begin(), E.end(), threshold[b + i]) - E.begin());  // x <= t_j <=> rank <= j
+      bn[at + i] = make_uint2((uint32_t)local[c] | (j << 16), (uint32_t)left[b + i] | ((uint32_t)right[b + i] << 16));
+    }
+    at += (size_t)nn;
+  }
+  bto[T] = (int32_t)at;
+  // the previous chunk's kernel may still be reading d_forest
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (ctx->forest_cap < (size_t)a.blob_bytes) {
+    if (ctx->d_forest) cudaFree(ctx->d_forest);
+    ctx->d_forest = nullptr; ctx->forest_cap = 0;
+    SE_CUDA(ctx, cudaMalloc(&ctx->d_forest, (size_t)a.blob_bytes));
+    ctx->forest_cap = (size_t)a.blob_bytes;
+  }
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_forest, blob.data(), (size_t)a.blob_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  a.blob = ctx->d_forest;
+  a.X8 = B.d8; a.ld8 = B.ld8;
+  return SE_OK;
+}
+}  // namespace
+
 // Σ_t weights[t] · tree_t(x) + init for every row in one pass over the rank matrix per chunk of trees
 // (GBMRegressionModel.predict, regression/GBMRegressor.scala:531-539; BaggingRegressionModel.predict,
 // regression/BaggingRegressor.scala:221-228 with weights 1 / M).
@@ -2800,141 +2973,120 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
   const SlotBuf& O = ctx->slot[out_slot];
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
   SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
-  SE_REQUIRE(ctx, offsets[0] == 0, SE_ERR_ARG, "offsets[0] must be 0");
-  const int64_t total = offsets[n_trees];
-  SE_REQUIRE(ctx, total >= n_trees && total <= (1 << 26), SE_ERR_ARG, "bad node count %lld", (long long)total);
-  // every member must be a tree rooted at its first node, with tree-local child indices and GLOBAL column indices
-  {
-    std::vector<char> seen;
-    std::vector<int32_t> stack;
-    for (int t = 0; t < n_trees; ++t) {
-      const int32_t b = offsets[t], nn = offsets[t + 1] - offsets[t];
-      SE_REQUIRE(ctx, nn >= 1 && nn <= 65535, SE_ERR_ARG, "tree %d: %d nodes (1..65535 supported)", t, nn);
-      for (int i = 0; i < nn; ++i) {
-        if (feature[b + i] < 0) continue;
-        SE_REQUIRE(ctx, feature[b + i] < X.rows, SE_ERR_ARG, "tree %d node %d: column %d outside X with %lld columns", t, i,
-                   feature[b + i], (long long)X.rows);
-        SE_REQUIRE(ctx, left[b + i] >= 0 && left[b + i] < nn && right[b + i] >= 0 && right[b + i] < nn, SE_ERR_ARG,
-                   "tree %d node %d: bad child", t, i);
-      }
-      seen.assign((size_t)nn, 0);
-      stack.clear();
-      stack.push_back(0);
-      seen[0] = 1;
-      while (!stack.empty()) {
-        const int32_t i = stack.back();
-        stack.pop_back();
-        if (feature[b + i] < 0) continue;
-        for (const int32_t c : {left[b + i], right[b + i]}) {
-          SE_REQUIRE(ctx, !seen[c], SE_ERR_ARG, "tree %d: node %d is reached twice: not a tree", t, c);
-          seen[c] = 1;
-          stack.push_back(c);
-        }
-      }
-    }
-  }
+  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
   SE_TRY(begin(ctx));
   release_l2_persist(ctx);
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  {
-    const int rc = bins_prepare(ctx, which, X, (int)total, feature, threshold);
-    if (rc < 0) return rc;
-    SE_REQUIRE(ctx, rc == 1, SE_ERR_STATE,
-               "the forest kernel needs the uint8 rank matrix (tree_bins on, <= 255 distinct thresholds per column, no NaN "
-               "threshold): evaluate the members with se_tree_predict + se_agg_run instead");
-  }
-  BinState& B = ctx->bins[which];
+  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
+  const BinState& B = ctx->bins[which];
+  std::vector<ForestChunk> chunks;
+  SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, false, kForestTile, 0, chunks));
   if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
   if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   ForestArgs a;
-  a.X8 = B.d8; a.n = X.cols; a.ld8 = B.ld8;
+  a.n = X.cols;
   a.out = O.d + (int64_t)out_row * (O.rows > 1 ? O.ld : O.cols);
   a.init = init;
-  auto pad = [](size_t v, size_t to) { return (v + to - 1) / to * to; };
-  std::vector<int32_t> local((size_t)X.rows, -1);  // global column -> local column of the current chunk
-  std::vector<int32_t> used;
-  std::vector<unsigned char> blob;
-  int chunks = 0;
-  int t0 = 0;
-  while (t0 < n_trees) {
-    // grow the chunk tree by tree while columns x 256 ranks + packed trees fit the shared-memory budget
-    size_t nodes = 0;
-    int t1 = t0;
-    // a member that does not fit the four-CTAs-per-SM budget alone gets two, then one CTA per SM
-    for (const size_t budget : {(size_t)kForestSmemBudget, (size_t)(100 * 1024), (size_t)(216 * 1024)}) {
-    for (int32_t c : used) local[c] = -1;
-    used.clear();
-    nodes = 0;
-    for (t1 = t0; t1 < n_trees; ++t1) {
-      const int32_t b = offsets[t1], nn = offsets[t1 + 1] - offsets[t1];
-      std::vector<int32_t> added;
-      for (int i = 0; i < nn; ++i) {
-        const int32_t c = feature[b + i];
-        if (c >= 0 && local[c] < 0) { local[c] = (int32_t)(used.size() + added.size()); added.push_back(c); }
-      }
-      const size_t T = (size_t)(t1 - t0 + 1), C = used.size() + added.size(), Nn = nodes + (size_t)nn;
-      const size_t bytes = pad(8 * T + 8 * C + 8 * Nn + pad(4 * (T + 1), 8) + pad(4 * Nn, 16), 16) + C * kForestTile;
-      if (bytes > budget || C > 65535) {
-        for (int32_t c : added) local[c] = -1;
-        break;
-      }
-      used.insert(used.end(), added.begin(), added.end());
-      nodes = Nn;
-    }
-    if (t1 > t0) break;
-    }
-    SE_REQUIRE(ctx, t1 > t0, SE_ERR_ARG, "tree %d alone (%d nodes) does not fit the forest kernel's shared memory", t0,
-               offsets[t0 + 1] - offsets[t0]);
-    const size_t T = (size_t)(t1 - t0), C = used.size(), Nn = nodes;
-    a.T = (int)T; a.C = (int)C;
-    a.off_coloff = (int)(8 * T);
-    a.off_nodes = a.off_coloff + (int)(8 * C);
-    a.off_treeoff = a.off_nodes + (int)(8 * Nn);
-    a.off_values = a.off_treeoff + (int)pad(4 * (T + 1), 8);
-    a.blob_bytes = (int)pad((size_t)a.off_values + 4 * Nn, 16);
-    a.off_ranks = a.blob_bytes;
-    blob.assign((size_t)a.blob_bytes, 0);
-    double* bw = reinterpret_cast<double*>(blob.data());
-    unsigned long long* bco = reinterpret_cast<unsigned long long*>(blob.data() + a.off_coloff);
-    uint2* bn = reinterpret_cast<uint2*>(blob.data() + a.off_nodes);
-    int32_t* bto = reinterpret_cast<int32_t*>(blob.data() + a.off_treeoff);
-    float* bv = reinterpret_cast<float*>(blob.data() + a.off_values);
-    for (size_t c = 0; c < C; ++c) bco[c] = (unsigned long long)used[c] * (unsigned long long)B.ld8;
-    size_t at = 0;
-    for (int t = t0; t < t1; ++t) {
-      const int32_t b = offsets[t], nn = offsets[t + 1] - offsets[t];
-      bw[t - t0] = weights ? weights[t] : 1.0;
-      bto[t - t0] = (int32_t)at;
-      for (int i = 0; i < nn; ++i) {
-        const int32_t c = feature[b + i];
-        bv[at + i] = value[b + i];
-        if (c < 0) { bn[at + i] = make_uint2(0x80000000u, 0u); continue; }
-        const std::vector<float>& E = B.edges[c];
-        const uint32_t j = (uint32_t)(std::lower_bound(E.begin(), E.end(), threshold[b + i]) - E.begin());  // x <= t_j <=> rank <= j
-        bn[at + i] = make_uint2((uint32_t)local[c] | (j << 16), (uint32_t)left[b + i] | ((uint32_t)right[b + i] << 16));
-      }
-      at += (size_t)nn;
-    }
-    bto[T] = (int32_t)at;
-    if (ctx->forest_cap < (size_t)a.blob_bytes) {
-      if (ctx->d_forest) cudaFree(ctx->d_forest);
-      ctx->d_forest = nullptr; ctx->forest_cap = 0;
-      SE_CUDA(ctx, cudaMalloc(&ctx->d_forest, (size_t)a.blob_bytes));
-      ctx->forest_cap = (size_t)a.blob_bytes;
-    }
-    // the previous chunk's kernel may still be reading d_forest
-    SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_forest, blob.data(), (size_t)a.blob_bytes, cudaMemcpyHostToDevice, ctx->stream));
-    SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // blob is pageable host memory reused by the next chunk
-    a.blob = ctx->d_forest;
-    a.accumulate = chunks > 0 ? 1 : 0;
+  for (size_t k = 0; k < chunks.size(); ++k) {
+    SE_TRY(forest_upload_chunk(ctx, B, chunks[k], offsets, feature, threshold, left, right, value, weights, nullptr, a));
+    a.accumulate = k > 0 ? 1 : 0;
     SE_LAUNCH_T(ctx, SE_KF_TREE, launch_forest_predict(a, ctx->sms, ctx->stream));
-    ++chunks;
-    t0 = t1;
   }
-  ctx->last_forest_chunks = chunks;
+  ctx->last_forest_chunks = (int)chunks.size();
   ctx->last_tree_binned = 1;
   return end(ctx);
+}
+
+// A classifier ensemble of trees in one pass with the aggregation's epilogue (see se_abi.h).
+int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, int loss, int n_trees, const int32_t* offsets,
+                  const int32_t* feature, const float* threshold, const int32_t* left, const int32_t* right,
+                  const float* value, const float* probs, const int32_t* tree_class, const double* weights,
+                  const double* init) {
+  if (!ctx || !offsets || !feature || !threshold || !left || !right || !value) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= (1 << 20), SE_ERR_ARG, "bad tree count %d", n_trees);
+  SE_REQUIRE(ctx, kind == SE_AGG_GBM_CLASSIFIER || kind == SE_AGG_BAGGING_SOFT || kind == SE_AGG_BAGGING_HARD ||
+                      kind == SE_AGG_BOOSTING_REAL || kind == SE_AGG_BOOSTING_DISCRETE,
+             SE_ERR_ARG, "se_forest_agg serves the classifier kinds (2..6), got %d", kind);
+  SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= SE_FOREST_AGG_MAX_CLASSES, SE_ERR_ARG,
+             "se_forest_agg supports 2..%d classes, got %d", SE_FOREST_AGG_MAX_CLASSES, num_classes);
+  const bool gbm = (kind == SE_AGG_GBM_CLASSIFIER);
+  const bool vec = (kind == SE_AGG_BAGGING_SOFT || kind == SE_AGG_BOOSTING_REAL);
+  if (gbm) {
+    SE_REQUIRE(ctx, dim >= 1 && dim <= SE_FOREST_AGG_MAX_CLASSES && (dim > 1 || num_classes == 2), SE_ERR_ARG,
+               "bad dim %d for %d classes", dim, num_classes);
+    SE_REQUIRE(ctx, tree_class && weights, SE_ERR_ARG, "the GBM classifier needs tree_class and weights");
+    for (int t = 0; t < n_trees; ++t)
+      SE_REQUIRE(ctx, tree_class[t] >= 0 && tree_class[t] < dim, SE_ERR_ARG, "tree %d: class %d outside [0, %d)", t,
+                 tree_class[t], dim);
+  }
+  SE_REQUIRE(ctx, !vec || probs, SE_ERR_ARG, "bagging soft / boosting real need the leaf probabilities");
+  SE_REQUIRE(ctx, kind != SE_AGG_BOOSTING_DISCRETE || weights, SE_ERR_ARG, "boosting discrete needs the weights");
+  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
+  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
+  const int C = gbm ? dim : num_classes;               // totals per row
+  const int out_c = (gbm && dim == 1) ? 2 : C;         // classes of RAW / PROB
+  const int64_t n = X.cols;
+  SE_TRY(slot_alloc2d(ctx, SE_SLOT_RAW, out_c, n));
+  SE_TRY(slot_alloc2d(ctx, SE_SLOT_PROB, out_c, n));
+  SE_TRY(slot_alloc2d(ctx, SE_SLOT_LABEL, 1, n));
+  SE_TRY(begin(ctx));
+  release_l2_persist(ctx);
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
+  const BinState& B = ctx->bins[which];
+  std::vector<ForestChunk> chunks;
+  SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, gbm, kForestAggTile,
+                     (size_t)C * kForestAggTile * sizeof(double), chunks));
+  const int64_t total_nodes = offsets[n_trees];
+  if (vec) {  // every node's K probabilities, read by the kernel through L1 at the leaf it reaches
+    const size_t need = (size_t)total_nodes * (size_t)num_classes;
+    if (ctx->forest_p_cap < need) {
+      if (ctx->d_forest_p) cudaFree(ctx->d_forest_p);
+      ctx->d_forest_p = nullptr; ctx->forest_p_cap = 0;
+      SE_CUDA(ctx, cudaMalloc(&ctx->d_forest_p, sizeof(float) * need));
+      ctx->forest_p_cap = need;
+    }
+    SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_forest_p, probs, sizeof(float) * need, cudaMemcpyHostToDevice, ctx->stream));
+  }
+  const int64_t ld_acc = ((n + 31) / 32) * 32;
+  if (chunks.size() > 1 && ctx->forest_acc_cap < (size_t)C * (size_t)ld_acc) {
+    if (ctx->d_forest_acc) cudaFree(ctx->d_forest_acc);
+    ctx->d_forest_acc = nullptr; ctx->forest_acc_cap = 0;
+    SE_CUDA(ctx, cudaMalloc(&ctx->d_forest_acc, sizeof(double) * (size_t)C * (size_t)ld_acc));
+    ctx->forest_acc_cap = (size_t)C * (size_t)ld_acc;
+  }
+  // the vote weights are narrowed to fp32 as se_agg_run does, and Σa is the sum of what the kernel adds
+  std::vector<double> w((size_t)n_trees, 1.0);
+  double sum_a = 0.0;
+  for (int t = 0; t < n_trees; ++t) {
+    if (kind == SE_AGG_BOOSTING_DISCRETE) w[t] = (double)(float)weights[t];
+    else if (gbm) w[t] = weights[t];
+    sum_a += w[t];
+  }
+  ForestAggArgs g;
+  g.f.n = n;
+  g.kind = kind; g.K = num_classes; g.C = C; g.dim = gbm ? dim : 1; g.loss = loss; g.M = n_trees;
+  g.sum_a = sum_a;
+  for (int c = 0; c < C; ++c) g.init[c] = (gbm && init) ? init[c] : 0.0;
+  g.acc = ctx->d_forest_acc; g.ld_acc = ld_acc;
+  const SlotBuf& R = ctx->slot[SE_SLOT_RAW];
+  g.raw = R.d; g.prob = ctx->slot[SE_SLOT_PROB].d; g.label = ctx->slot[SE_SLOT_LABEL].d;
+  g.ld_out = R.rows > 1 ? R.ld : R.cols;
+  g.bad_label = ctx->d_bad_label;
+  for (size_t k = 0; k < chunks.size(); ++k) {
+    SE_TRY(forest_upload_chunk(ctx, B, chunks[k], offsets, feature, threshold, left, right, value, w.data(),
+                               gbm ? tree_class : nullptr, g.f));
+    g.probs = vec ? ctx->d_forest_p + (size_t)offsets[chunks[k].t0] * (size_t)num_classes : nullptr;
+    g.first = k == 0 ? 1 : 0;
+    g.last = k + 1 == chunks.size() ? 1 : 0;
+    SE_LAUNCH_T(ctx, SE_KF_TREE, launch_forest_agg(g, ctx->sms, ctx->stream));
+  }
+  ctx->last_forest_chunks = (int)chunks.size();
+  ctx->last_tree_binned = 1;
+  SE_TRY(end(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return check_labels(ctx);  // a leaf label that is not a class index in [0, K)
 }
 
 int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,

@@ -257,15 +257,16 @@ cudaError_t launch_tree_predict_binned(const TreeArgs& a, const uint8_t* X8, con
 //   [off_coloff)   uint64   byte offset of local column c in X8 (column * ld8), c < C
 //   [off_nodes)    uint2    nodes: x = local column | rank threshold << 16 | leaf << 31, y = left | right << 16 (tree-local)
 //   [off_treeoff)  int32    first node of tree t (T + 1 entries)
+//   [off_treecls)  int32    class of tree t (T entries; se_forest_agg's GBM classifier only, else off_treecls == 0)
 //   [off_values)   float    leaf value per node
-//   [off_ranks)    uint8    (shared memory only) the tile's ranks, [C][256]
+//   [off_ranks)    uint8    (shared memory only) the tile's ranks, [C][tile rows]
 struct ForestArgs {
   const uint8_t* X8 = nullptr;
   int64_t n = 0, ld8 = 0;
   const unsigned char* blob = nullptr;
   int blob_bytes = 0;  // multiple of 16
   int T = 0, C = 0;
-  int off_coloff = 0, off_nodes = 0, off_treeoff = 0, off_values = 0, off_ranks = 0;
+  int off_coloff = 0, off_nodes = 0, off_treeoff = 0, off_treecls = 0, off_values = 0, off_ranks = 0;
   double init = 0.0;
   int accumulate = 0;
   float* out = nullptr;
@@ -273,6 +274,40 @@ struct ForestArgs {
 constexpr int kForestTile = 256;              // rows per CTA tile (one row per thread)
 constexpr int kForestSmemBudget = 54 * 1024;  // per CTA: four CTAs per SM (the walk is latency-bound: warps matter more than chunk size)
 cudaError_t launch_forest_predict(const ForestArgs& a, int sms, cudaStream_t s);
+
+// One level of a packed tree for the row whose ranks start at myr (rank of local column c at myr[c * TILE]).
+template <int TILE>
+__device__ __forceinline__ void forest_step(const uint2* __restrict__ nodes, const unsigned char* __restrict__ myr, int& nd,
+                                            bool& live) {
+  const uint2 w = nodes[nd];
+  live = (w.x >> 31) == 0;
+  if (live) {
+    const uint32_t rank = myr[(w.x & 0xFFFFu) * TILE];
+    nd = (int)((rank <= ((w.x >> 16) & 0xFFu)) ? (w.y & 0xFFFFu) : (w.y >> 16));
+  }
+}
+
+// A classifier forest in ONE pass with the aggregation's epilogue (se_forest_agg, se_agg.cu): the chunk's trees are
+// staged as for forest_predict_kernel, each row's C class totals are fp64 in shared memory ([C][kForestAggTile] after
+// the ranks), carried between chunks in `acc` ([C][ld_acc] fp64) and finished by finalize_row / finalize_real_row.
+constexpr int kForestAggTile = 128;        // rows per CTA tile: C x 128 fp64 totals (32 KB at the class limit)
+constexpr int kForestAggMaxClasses = 32;   // SE_FOREST_AGG_MAX_CLASSES
+struct ForestAggArgs {
+  ForestArgs f;                  // the chunk (f.init, f.accumulate and f.out unused)
+  int kind = 0, K = 0, C = 0, dim = 1, loss = 0, M = 0;
+  double sum_a = 0.0;            // Σ of the tree weights (boosting discrete epilogue)
+  double init[kForestAggMaxClasses] = {};  // GBM classifier: the totals of the first chunk start here
+  const float* probs = nullptr;  // [chunk nodes][K] leaf class probabilities (bagging soft, boosting real), read through L1
+  double* acc = nullptr;         // [C][ld_acc] totals between chunks
+  int64_t ld_acc = 0;
+  int first = 1, last = 1;       // the chunk starts from init / finishes the rows
+  float* raw = nullptr;
+  float* prob = nullptr;
+  float* label = nullptr;
+  int64_t ld_out = 0;
+  int* bad_label = nullptr;
+};
+cudaError_t launch_forest_agg(const ForestAggArgs& a, int sms, cudaStream_t s);
 // ---- regression- and classification-tree fit over the uint8 rank matrix (se_tree_fit.cu) -----
 // Nodes are heap-indexed (root 1, children 2h, 2h + 1), so depth <= 8 needs 511 records.
 constexpr int kTreeFitHeap = 512;

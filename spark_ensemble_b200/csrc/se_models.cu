@@ -327,16 +327,6 @@ __global__ void __launch_bounds__(kBlock, 4) tree_predict_mask_kernel(const Tree
 // (C x 256 bytes), keeps the packed trees next to it, and every thread walks ALL trees for its row out of shared
 // memory, two trees interleaved, accumulating w_t · leaf in fp64 in model order like the reference's loop: the rank
 // matrix is read once per chunk of trees and no intermediate is written.
-__device__ __forceinline__ void forest_step(const uint2* __restrict__ nodes, const unsigned char* __restrict__ myr, int& nd,
-                                            bool& live) {
-  const uint2 w = nodes[nd];
-  live = (w.x >> 31) == 0;
-  if (live) {
-    const uint32_t rank = myr[(w.x & 0xFFFFu) * kForestTile];
-    nd = (int)((rank <= ((w.x >> 16) & 0xFFu)) ? (w.y & 0xFFFFu) : (w.y >> 16));
-  }
-}
-
 __global__ void __launch_bounds__(kForestTile) forest_predict_kernel(const ForestArgs a) {
   extern __shared__ __align__(16) unsigned char fsm[];
   for (int i = threadIdx.x; i < a.blob_bytes / 16; i += kForestTile)
@@ -370,8 +360,8 @@ __global__ void __launch_bounds__(kForestTile) forest_predict_kernel(const Fores
         int d0 = 0, d1 = 0;
         bool l0 = true, l1 = true;
         while (l0 || l1) {
-          if (l0) forest_step(n0, myr, d0, l0);
-          if (l1) forest_step(n1, myr, d1, l1);
+          if (l0) forest_step<kForestTile>(n0, myr, d0, l0);
+          if (l1) forest_step<kForestTile>(n1, myr, d1, l1);
         }
         acc += s_w[t] * (double)s_val[s_toff[t] + d0];  // model order (GBMRegressor.scala:534-537)
         acc += s_w[t + 1] * (double)s_val[s_toff[t + 1] + d1];
@@ -380,7 +370,7 @@ __global__ void __launch_bounds__(kForestTile) forest_predict_kernel(const Fores
         const uint2* n0 = s_nodes + s_toff[t];
         int d0 = 0;
         bool l0 = true;
-        while (l0) forest_step(n0, myr, d0, l0);
+        while (l0) forest_step<kForestTile>(n0, myr, d0, l0);
         acc += s_w[t] * (double)s_val[s_toff[t] + d0];
       }
       a.out[row] = (float)acc;

@@ -218,6 +218,53 @@ _GBM_REG_DEFAULTS = {**_d, **_ds, **_db, **_dg, "loss": "squared", "alpha": 0.9,
 GBMRegressor._declare(_p + _ps + _pb + _pg + _preg, _GBM_REG_DEFAULTS)
 
 
+def _device_trees(model: Params, members) -> list | None:
+    """The tree arrays of every member when the model scores them on the device: residentFeatures is set, there is
+    at least one member, and every member exposes tree_arrays().  None keeps the member-by-member route."""
+    if not model("residentFeatures") or not members:
+        return None
+    trees = []
+    for m in members:
+        fn = getattr(m, "tree_arrays", None)
+        t = fn() if fn is not None else None
+        if t is None:
+            return None
+        trees.append(t)
+    return trees
+
+
+def _resident_context(device: int, X) -> Context:
+    """A context whose SLOT_X holds the rows of X column-major: the matrix the forest kernels walk."""
+    X = np.asarray(X, dtype=np.float32)
+    ctx = Context(device)
+    try:
+        ctx.alloc(N.SLOT_X, X.shape[1], X.shape[0])
+        ctx.upload_rowmajor(N.SLOT_X, X)
+    except BaseException:
+        ctx.close()
+        raise
+    return ctx
+
+
+def _rank_matrix_full(e: N.NativeError) -> bool:
+    """The forest's thresholds do not fit the uint8 rank matrix (more than 255 in a column): score member by member."""
+    return e.code == N.SE_ERR_STATE
+
+
+def _forest_sum_resident(model: Params, X, trees, subspaces, weights, init: float) -> np.ndarray | None:
+    """init + Σ_t weights[t] · tree_t(x) through se_forest_predict; None when the rank matrix cannot hold the trees."""
+    n = X.shape[0]
+    with _resident_context(model.device, X) as ctx:
+        ctx.alloc(N.SLOT_RAW, 1, n)
+        try:
+            ctx.forest_predict(trees, N.SLOT_RAW, weights=weights, init=init, subspaces=subspaces)
+        except N.NativeError as e:
+            if _rank_matrix_full(e):
+                return None
+            raise
+        return ctx.download(N.SLOT_RAW).astype(np.float64)
+
+
 def _stack_model_outputs(models, subspaces, X, extra=None) -> np.ndarray:
     rows = [] if extra is None else [extra]
     for m, s in zip(models, subspaces):
@@ -240,7 +287,20 @@ class GBMRegressionModel(Params):
         self.device = device
         self.parent = None
 
+    def _aggregate_resident(self, X) -> np.ndarray | None:
+        """One pass over the device-resident features when every member (and a tree init) is a tree."""
+        const_init = hasattr(self.init, "prediction")
+        trees = _device_trees(self, self.models if const_init else [self.init] + self.models)
+        if trees is None:
+            return None
+        subs = list(self.subspaces) if const_init else [None] + list(self.subspaces)
+        w = self.weights if const_init else np.concatenate([[1.0], self.weights])
+        return _forest_sum_resident(self, X, trees, subs, w, self.init.prediction if const_init else 0.0)
+
     def _aggregate(self, X) -> np.ndarray:
+        out = self._aggregate_resident(X)
+        if out is not None:
+            return out
         n = X.shape[0]
         const_init = hasattr(self.init, "prediction")
         P = _stack_model_outputs(self.models, self.subspaces, X,
@@ -298,8 +358,9 @@ class BaggingRegressor(Params):
 _pbag = [Param("numBaseLearners", "number of base learners", ParamValidators.gtEq(1), int),
          Param("baseLearner", "base learner"),
          Param("parallelism", "the number of threads to use when running parallel algorithms (>= 1)",
-               ParamValidators.gtEq(1), int)]
-_BAG_REG_DEFAULTS = {**_d, **_ds, "numBaseLearners": 10, "parallelism": 1,
+               ParamValidators.gtEq(1), int),
+         Param("residentFeatures", "evaluate base models on device over the HBM-resident feature matrix", convert=bool)]
+_BAG_REG_DEFAULTS = {**_d, **_ds, "numBaseLearners": 10, "parallelism": 1, "residentFeatures": False,
                      "seed": java_string_hash("org.apache.spark.ml.regression.BaggingRegressor")}
 BaggingRegressor._declare(_p + _ps + _pbag, _BAG_REG_DEFAULTS)
 
@@ -315,6 +376,11 @@ class BaggingRegressionModel(Params):
         self.parent = None
 
     def _aggregate(self, X) -> np.ndarray:
+        trees = _device_trees(self, self.models)
+        if trees is not None:  # (Σ_t tree_t(x)) / M in one pass over the device-resident features
+            s = _forest_sum_resident(self, X, trees, self.subspaces, None, 0.0)
+            if s is not None:
+                return s / self.numModels
         P = _stack_model_outputs(self.models, self.subspaces, X)
         with Context(self.device) as ctx:
             ctx.agg_configure(N.AGG_BAGGING_REGRESSOR, P.shape[0], 0, 1, 0, X.shape[0])
@@ -386,8 +452,9 @@ _pbr = [Param("lossType", "loss function, exponential by default (case-insensiti
               lambda v: v.lower() in ("exponential", "squared", "linear"), str),
         Param("votingStrategy", "voting strategy, (case-insensitive). Supported options: median,mean",
               lambda v: v.lower() in ("median", "mean"), str),
-        Param("seed", "random seed", convert=int)]
-_BOOST_REG_DEFAULTS = {**_d, **_db, "lossType": "exponential", "votingStrategy": "median",
+        Param("seed", "random seed", convert=int),
+        Param("residentFeatures", "evaluate base models on device over the HBM-resident feature matrix", convert=bool)]
+_BOOST_REG_DEFAULTS = {**_d, **_db, "lossType": "exponential", "votingStrategy": "median", "residentFeatures": False,
                        "seed": java_string_hash("org.apache.spark.ml.regression.BoostingRegressor")}
 BoostingRegressor._declare(_p + _pb + _pbr, _BOOST_REG_DEFAULTS)
 
@@ -404,9 +471,30 @@ class BoostingRegressionModel(Params):
         self.device = device
         self.parent = None
 
+    def _aggregate_resident(self, X, median: bool) -> np.ndarray | None:
+        """Members evaluated over the device-resident features when every one is a tree: the weighted mean in one
+        forest pass; for the median each tree writes its row of SLOT_P on the device before the aggregation."""
+        trees = _device_trees(self, self.models)
+        if trees is None:
+            return None
+        if not median:
+            s = _forest_sum_resident(self, X, trees, None, self.weights, 0.0)
+            return None if s is None else s / float(np.sum(self.weights))
+        n = X.shape[0]
+        with _resident_context(self.device, X) as ctx:
+            ctx.agg_configure(N.AGG_BOOSTING_REG_MEDIAN, len(trees), 0, 1, 0, n)
+            for i, t in enumerate(trees):
+                ctx.tree_predict(t, N.SLOT_P, i)
+            ctx.agg_run(self.weights)
+            return ctx.download(N.SLOT_RAW).astype(np.float64)
+
     def _aggregate(self, X) -> np.ndarray:
+        median = self("votingStrategy").lower() == "median"
+        out = self._aggregate_resident(X, median)
+        if out is not None:
+            return out
         P = np.ascontiguousarray(np.stack([m.predict(X) for m in self.models]), dtype=np.float32)
-        kind = N.AGG_BOOSTING_REG_MEDIAN if self("votingStrategy").lower() == "median" else N.AGG_BOOSTING_REG_MEAN
+        kind = N.AGG_BOOSTING_REG_MEDIAN if median else N.AGG_BOOSTING_REG_MEAN
         with Context(self.device) as ctx:
             ctx.agg_configure(kind, P.shape[0], 0, 1, 0, X.shape[0])
             ctx.upload(N.SLOT_P, P)
