@@ -385,7 +385,12 @@ SE_API int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, con
  * of every node's prediction) in arrays of max_nodes entries, the gain of every internal node (gain may be NULL) and
  * n_nodes.  Also writes the tree's output for every row, in the bag or not, into row out_row of out_slot; it equals
  * se_tree_predict of the returned arrays bit for bit.  One device-to-host copy per call (the node records).
- * Fails with SE_ERR_ARG when a communicator with more than one rank is attached (histograms are not all-reduced). */
+ * With a communicator of two or more ranks attached the call is COLLECTIVE: every rank calls it with the same
+ * arguments, after se_tree_fit_bins with the same candidates; each level's fp64 histogram is all-reduced (NCCL), so
+ * every rank returns the tree of the union of the ranks' rows and writes its own rows' output.  Before the first
+ * histogram collective the ranks agree on the fit's shape: when one rank fails its own checks (a rank with no rows
+ * included) or the ranks differ in max_depth, the subspace, the candidates, the validity rules, K, weights or bag,
+ * every rank fails — that rank with its own error, the others with SE_ERR_ARG. */
 SE_API int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
                        const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
                        double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
@@ -404,7 +409,8 @@ enum se_tree_out { SE_TREE_OUT_LABEL = 0, SE_TREE_OUT_PROBA = 1 };
  * SE_TREE_OUT_PROBA writes its K probabilities into rows out_row .. out_row + K - 1 (as se_tree_predict_multi of
  * `proba`), bit for bit.  Returns the tree in BFS order: feature / threshold / left / right as se_tree_fit, value =
  * label, proba [n_nodes][K] = fp32 of n_k / W (all 0 when W == 0), class_weights [n_nodes][K] (may be NULL), gain (may
- * be NULL), n_nodes.  Bounds (SE_ERR_ARG) as se_tree_fit, plus num_classes and impurity. */
+ * be NULL), n_nodes.  Bounds (SE_ERR_ARG) as se_tree_fit, plus num_classes and impurity.  Collective under a
+ * communicator, as se_tree_fit (impurity and num_classes included in what the ranks must agree on). */
 SE_API int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row,
                                   int use_bag, const int32_t* subspace, int n_subspace, int num_classes, int impurity,
                                   int max_depth, int min_instances, double min_info_gain, double min_weight_fraction,

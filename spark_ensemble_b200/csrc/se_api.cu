@@ -3155,20 +3155,33 @@ int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const floa
 }
 
 namespace {
-// The part of a fit that se_tree_fit and se_tree_fit_classifier share: argument checks, scratch, the level loop with
-// its shared-memory / global-atomics choice, the classifier's pruning, the out kernel and the download of the node
-// records into h_small: [kTreeFitHeap] TreeFitNode, then for K >= 2 the class weights ([kTreeFitHeap][K] double), the
-// probabilities ([kTreeFitHeap][K] float) and the pruning table ([kTreeFitHeap] int4).  K == 0: regression.
-int tree_fit_run(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot, int label_row, int weight_slot,
-                 int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth, int min_instances,
-                 double min_info_gain, double min_weight_fraction, int out_slot, int out_row) {
+// What the local part of a fit (tree_fit_prepare) hands to its level loop.
+struct TreeFitPlan {
+  const float *r = nullptr, *w = nullptr, *bag = nullptr, *outc = nullptr;
+  int64_t n = 0, nw = 0;
+  int nb = 0, sw = 0, top = 0;
+  uint32_t hash = 0;  // 24 bits: the subspace, its columns' candidates and the validity rules
+};
+
+// FNV-1a over 32-bit words
+inline uint32_t fnv_words(uint32_t h, const void* p, size_t words) {
+  const uint32_t* q = static_cast<const uint32_t*>(p);
+  for (size_t i = 0; i < words; ++i)
+    for (int b = 0; b < 4; ++b) h = (h ^ ((q[i] >> (8 * b)) & 0xFFu)) * 16777619u;
+  return h;
+}
+
+// The checks, the scratch and the uploads of a fit: everything that depends on this rank alone.  Under a communicator
+// its failure is not returned to the caller straight away: tree_fit_agree tells every rank first.
+int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot, int label_row, int weight_slot,
+                     int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth,
+                     int min_instances, double min_info_gain, double min_weight_fraction, int out_slot, int out_row,
+                     TreeFitPlan& P) {
   SE_REQUIRE(ctx, max_depth >= 0 && max_depth <= 8, SE_ERR_ARG, "maxDepth %d outside [0, 8]", max_depth);
   SE_REQUIRE(ctx, min_instances >= 1, SE_ERR_ARG, "minInstancesPerNode %d < 1", min_instances);
   SE_REQUIRE(ctx, min_weight_fraction >= 0.0 && min_weight_fraction < 0.5, SE_ERR_ARG,
              "minWeightFractionPerNode %g outside [0, 0.5)", min_weight_fraction);
   SE_REQUIRE(ctx, !isnan(min_info_gain), SE_ERR_ARG, "minInfoGain is NaN");
-  SE_REQUIRE(ctx, !(ctx->comm && ctx->nranks > 1), SE_ERR_ARG,
-             "se_tree_fit fits on one GPU: its histograms are not all-reduced across %d ranks", ctx->nranks);
   const SlotBuf& X = ctx->slot[SE_SLOT_X];
   SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
   const int64_t n = X.cols;
@@ -3249,7 +3262,89 @@ int tree_fit_run(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot,
   SE_REQUIRE(ctx, sizeof(int32_t) * (size_t)n_subspace <= (size_t)kSmallBytes, SE_ERR_ARG, "subspace too large");
   memcpy(ctx->h_small, cols.data(), sizeof(int32_t) * (size_t)n_subspace);
   SE_CUDA(ctx, cudaMemcpyAsync(T.d_cols, ctx->h_small, sizeof(int32_t) * (size_t)n_subspace, cudaMemcpyHostToDevice, ctx->stream));
+  if (K > 0 && label_slot == SE_SLOT_Y) SE_TRY(ensure_labels_checked(ctx, 0, K, n));  // class indices, checked per upload
+  uint32_t h = 2166136261u;
+  h = fnv_words(h, cols.data(), cols.size());
+  for (int32_t c : cols) {
+    const uint32_t m = (uint32_t)B.edges[c].size();
+    h = fnv_words(h, &m, 1);
+    h = fnv_words(h, B.edges[c].data(), m);
+  }
+  const int32_t rules[2] = {min_instances, entropy};
+  const double frac[2] = {min_info_gain, min_weight_fraction};
+  h = fnv_words(h, rules, 2);
+  h = fnv_words(h, frac, sizeof(frac) / 4);
+  P.r = r; P.w = w; P.bag = bag; P.outc = outc;
+  P.n = n; P.nw = nw; P.nb = nb; P.sw = sw; P.top = top;
+  P.hash = (h ^ (h >> 24)) & 0xFFFFFFu;
+  return SE_OK;
+}
+
+// Under a communicator of two or more ranks, one max all-reduce of the fit's shape and of its negation, before the
+// first histogram collective: every rank learns the minimum and maximum of each entry, and every rank fails when one
+// rank failed its own checks (rc) or when any entry differs.  Without it a rank that stops alone would leave its peers
+// blocked in the first histogram all-reduce.  The failing rank keeps its own error; its peers get SE_ERR_ARG.
+int tree_fit_agree(se_ctx* ctx, int rc, const double* shape, int count) {
+  static const char* const names[] = {"failed", "maxDepth", "the subspace size", "the bins per column",
+                                      "the doubles per bin", "numClasses", "the weights", "the bag",
+                                      "the subspace, its candidates or the validity rules (hash)"};
+  constexpr int kMax = 16;
+  const std::string local = ctx->err;
+  double v[2 * kMax];
+  for (int i = 0; i < count; ++i) {
+    v[i] = i == 0 ? (rc != SE_OK ? 1.0 : 0.0) : shape[i];
+    v[count + i] = -v[i];
+  }
+  SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  for (int i = 0; i < 2 * count; ++i) ctx->h_scal[kScalHost + i] = v[i];
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_scal + kScalHost, ctx->h_scal + kScalHost, sizeof(double) * 2 * count,
+                               cudaMemcpyHostToDevice, ctx->stream));
+  NcclApi& api = nccl();
+  const int nr = api.AllReduce(ctx->d_scal + kScalHost, ctx->d_scal + kScalHost, (size_t)(2 * count), kNcclFloat64,
+                               kNcclMax, ctx->comm, ctx->stream);
+  if (nr != 0) return fail(ctx, SE_ERR_NCCL, "ncclAllReduce: %s", api.GetErrorString(nr));
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->h_scal + kScalHost, ctx->d_scal + kScalHost, sizeof(double) * 2 * count,
+                               cudaMemcpyDeviceToHost, ctx->stream));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < 2 * count; ++i) v[i] = ctx->h_scal[kScalHost + i];
+  if (rc != SE_OK) return fail(ctx, rc, "%s", local.c_str());
+  SE_REQUIRE(ctx, v[0] == 0.0, SE_ERR_ARG, "ranks disagree on the fit: another rank failed its own checks");
+  for (int i = 1; i < count; ++i)
+    SE_REQUIRE(ctx, v[i] == -v[count + i], SE_ERR_ARG, "ranks disagree on the fit: %s is %.17g on one rank, %.17g on another",
+               names[i], -v[count + i], v[i]);
+  return SE_OK;
+}
+
+// The part of a fit that se_tree_fit and se_tree_fit_classifier share: argument checks, scratch, the level loop with
+// its shared-memory / global-atomics choice, the classifier's pruning, the out kernel and the download of the node
+// records into h_small: [kTreeFitHeap] TreeFitNode, then for K >= 2 the class weights ([kTreeFitHeap][K] double), the
+// probabilities ([kTreeFitHeap][K] float) and the pruning table ([kTreeFitHeap] int4).  K == 0: regression.  rc0 is
+// the caller's own checks.
+//
+// Under a communicator the fit is collective: each level's histogram is summed over the ranks (one fp64 NCCL
+// all-reduce between the histogram and the split kernels), so every rank splits on the histogram of the union of the
+// shards and writes its own rows' output.  The collective sequence is fixed by the shape tree_fit_agree checks.
+int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int label_slot, int label_row,
+                 int weight_slot, int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth,
+                 int min_instances, double min_info_gain, double min_weight_fraction, int out_slot, int out_row) {
+  TreeFitPlan P;
+  int rc = rc0 != SE_OK ? rc0
+                        : tree_fit_prepare(ctx, K, entropy, out_proba, label_slot, label_row, weight_slot, weight_row,
+                                           use_bag, subspace, n_subspace, max_depth, min_instances, min_info_gain,
+                                           min_weight_fraction, out_slot, out_row, P);
+  const bool collective = ctx->comm && ctx->nranks > 1;
+  if (collective) {
+    const double shape[] = {0.0, (double)max_depth, (double)n_subspace, (double)P.nb, (double)P.sw, (double)K,
+                            P.w ? 1.0 : 0.0, P.bag ? 1.0 : 0.0, (double)P.hash};
+    rc = tree_fit_agree(ctx, rc, shape, (int)(sizeof(shape) / sizeof(shape[0])));
+  }
+  if (rc != SE_OK) return rc;
   // ---- the fit: a fixed sequence of launches, no host round trip
+  auto& T = ctx->tf;
+  BinState& B = ctx->bins[0];
+  const int64_t n = P.n, nw = P.nw;
+  const int nb = P.nb, sw = P.sw, top = P.top;
+  const float *r = P.r, *w = P.w, *bag = P.bag, *outc = P.outc;
   TreeFitArgs a;
   a.X8 = B.d8; a.ld8 = B.ld8; a.n = n;
   a.cols = T.d_cols; a.n_edges = B.d_nedges; a.edges = B.d_edges;
@@ -3259,7 +3354,6 @@ int tree_fit_run(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot,
   a.min_instances = min_instances; a.min_info_gain = min_info_gain; a.min_weight_fraction = min_weight_fraction;
   a.K = K; a.sw = sw; a.entropy = entropy; a.out_proba = out_proba;
   a.cw = T.d_cw; a.prob = T.d_prob; a.prn = T.d_prn;
-  if (K > 0 && label_slot == SE_SLOT_Y) SE_TRY(ensure_labels_checked(ctx, 0, K, n));  // class indices, checked per upload
   uint16_t* nid[2] = {T.d_nid, T.d_nid + T.nid_cap};
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, ctx->stream));
   for (int L = 0; L <= top; ++L) {
@@ -3288,6 +3382,12 @@ int tree_fit_run(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot,
     gy = std::max<int64_t>(std::min<int64_t>(gy, 65535), 1);
     a.words_per_cta = (nw + gy - 1) / gy;
     SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_hist(a, smem_mode, (int)gy, smem, ctx->stream));
+    if (collective) {  // the level's histogram over the union of the shards, bit-identical on every rank
+      NcclApi& api = nccl();
+      const int nr = api.AllReduce(T.d_hist, T.d_hist, per_col / sizeof(double) * (size_t)n_subspace, kNcclFloat64,
+                                   kNcclSum, ctx->comm, ctx->stream);
+      if (nr != 0) return fail(ctx, SE_ERR_NCCL, "ncclAllReduce: %s", api.GetErrorString(nr));
+    }
     SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_split(a, ctx->stream));
   }
   a.route = max_depth >= 1;
@@ -3323,8 +3423,10 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
                 const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
                 double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
                 float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
-  if (!ctx || !feature || !threshold || !left || !right || !value || !n_nodes) return fail(ctx, SE_ERR_ARG, "null argument");
-  SE_TRY(tree_fit_run(ctx, 0, 0, 0, label_slot, label_row, weight_slot, weight_row, use_bag, subspace, n_subspace,
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  const int rc0 = (!feature || !threshold || !left || !right || !value || !n_nodes) ? fail(ctx, SE_ERR_ARG, "null argument")
+                                                                                    : SE_OK;
+  SE_TRY(tree_fit_run(ctx, rc0, 0, 0, 0, label_slot, label_row, weight_slot, weight_row, use_bag, subspace, n_subspace,
                       max_depth, min_instances, min_info_gain, min_weight_fraction, out_slot, out_row));
   // ---- prune (bottom-up: two leaf children with equal fp64 predictions) and number the nodes in BFS order
   const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(ctx->h_small);
@@ -3371,16 +3473,19 @@ int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weigh
                            int out_slot, int out_row, int max_nodes, int32_t* feature, float* threshold, int32_t* left,
                            int32_t* right, float* value, float* proba, double* class_weights, double* gain,
                            int* n_nodes) {
-  if (!ctx || !feature || !threshold || !left || !right || !value || !proba || !n_nodes)
-    return fail(ctx, SE_ERR_ARG, "null argument");
-  SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= kTreeFitMaxClasses, SE_ERR_ARG, "numClasses %d outside [2, %d]",
-             num_classes, kTreeFitMaxClasses);
-  SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
-  SE_REQUIRE(ctx, out_kind == SE_TREE_OUT_LABEL || out_kind == SE_TREE_OUT_PROBA, SE_ERR_ARG, "bad output kind %d", out_kind);
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  auto checks = [&]() -> int {  // this rank's own: under a communicator tree_fit_run tells the other ranks
+    SE_REQUIRE(ctx, feature && threshold && left && right && value && proba && n_nodes, SE_ERR_ARG, "null argument");
+    SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= kTreeFitMaxClasses, SE_ERR_ARG, "numClasses %d outside [2, %d]",
+               num_classes, kTreeFitMaxClasses);
+    SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
+    SE_REQUIRE(ctx, out_kind == SE_TREE_OUT_LABEL || out_kind == SE_TREE_OUT_PROBA, SE_ERR_ARG, "bad output kind %d", out_kind);
+    return SE_OK;
+  };
   const int K = num_classes;
-  SE_TRY(tree_fit_run(ctx, K, impurity == SE_IMPURITY_ENTROPY, out_kind == SE_TREE_OUT_PROBA, label_slot, label_row,
-                      weight_slot, weight_row, use_bag, subspace, n_subspace, max_depth, min_instances, min_info_gain,
-                      min_weight_fraction, out_slot, out_row));
+  SE_TRY(tree_fit_run(ctx, checks(), K, impurity == SE_IMPURITY_ENTROPY, out_kind == SE_TREE_OUT_PROBA, label_slot,
+                      label_row, weight_slot, weight_row, use_bag, subspace, n_subspace, max_depth, min_instances,
+                      min_info_gain, min_weight_fraction, out_slot, out_row));
   // the device pruned the tree (tree_prune_cls_kernel): number what is left in BFS order
   const char* hs = reinterpret_cast<const char*>(ctx->h_small);
   const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(hs);

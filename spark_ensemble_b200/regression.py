@@ -54,13 +54,23 @@ def bag_counts(n: int, subsample_ratio: float, replacement: bool, seed: int):
 def _check_device_learner(est: Params, learner) -> bool:
     """True when the base learner fits on the device (learners.DeviceDecisionTreeRegressor / Classifier).  It reads
     the residuals (or labels and boosting weights) and the features where they live, so it needs
-    residentFeatures=True and a single GPU (estimators without a `devices` Param run on one)."""
+    residentFeatures=True.  With Param `devices` naming two or more GPUs it fits over all of their rows at once
+    (sharded.ShardedContext.tree_fit: each level's histogram is all-reduced across the GPUs)."""
     if not getattr(learner, "device_learner", False):
         return False
     if not est("residentFeatures"):
         raise ValueError("the device tree learner fits over the device-resident features: set residentFeatures=True")
-    if est.hasParam("devices") and len(est("devices")) >= 2:
-        raise ValueError("the device tree learner fits on one GPU: `devices` must name at most one device")
+    devices = [int(d) for d in est("devices")] if est.hasParam("devices") else []
+    if len(devices) >= 2:  # every rank joins each level's all-reduce: the GPUs must exist and be distinct (NCCL)
+        from . import _native as N
+        if len(set(devices)) != len(devices):
+            raise ValueError(f"the device tree learner shards its fit over `devices`, which must name distinct GPUs: "
+                             f"{devices}")
+        visible = N.device_count()
+        missing = [d for d in devices if d >= visible]
+        if missing:
+            raise ValueError(f"the device tree learner shards its fit over `devices` {devices}, but GPU {missing[0]} is "
+                             f"not one of the {visible} visible")
     return True
 
 

@@ -40,6 +40,7 @@ class ShardedContext:
     # ---- plumbing
     def _all(self, fn):
         futs = [self._pool.submit(fn, r, c) for r, c in enumerate(self.ctxs)]
+        cf.wait(futs)  # every rank has returned before an error is raised: no call of theirs is still running
         return [f.result() for f in futs]
 
     def _total(self, slot: int) -> int:
@@ -217,6 +218,17 @@ class ShardedContext:
 
     def linear_predict(self, coef, intercept, out_slot, out_row=0, validation=False, subspace=None):
         self._all(lambda r, c: c.linear_predict(coef, intercept, out_slot, out_row, validation=validation, subspace=subspace))
+
+    # ---- device tree fit: each level's histogram is all-reduced, so every rank fits the tree of the whole rows
+    def tree_fit_bins(self, candidates):
+        self._all(lambda r, c: c.tree_fit_bins(candidates))
+
+    def tree_fit(self, *a, **k):
+        res = self._all(lambda r, c: c.tree_fit(*a, **k))
+        for t in res[1:]:
+            assert t.keys() == res[0].keys() and all(np.array_equal(t[key], res[0][key]) for key in t), \
+                "ranks disagree on the fitted tree (their histograms must be bit-identical)"
+        return res[0]
 
 
 def make_context(device: int = 0, devices=None):
