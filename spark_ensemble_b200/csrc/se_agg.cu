@@ -11,8 +11,6 @@
 // All of them are one streaming pass over the stacked base-model outputs P (the only large operand:
 // 4·M·width B/row) followed by a tiny per-row epilogue.  Stage 1 (sum / vote histogram) is the
 // HBM-bound kernel; stage 2 (finalize) touches only C values per row.
-#include <stdlib.h>
-
 #include "se_kernels.h"
 #include "se_loss.cuh"
 #include "se_tma.cuh"
@@ -421,20 +419,18 @@ __global__ void __launch_bounds__(kBlock) agg_hard_votes_packed_kernel(const flo
 // ------------------------------------------------------------------ class-wide sums through TMA tiles
 // For the classifiers every row needs all C class sums before its epilogue (argmax, soft-max).  The streaming path
 // (agg_sum_kernel + agg_finalize_kernel) round-trips a [C][n] intermediate through HBM and, per ncu, is
-// instruction-bound: 15.8 instructions per element in stage 1 and 55 per (row, class) in the epilogue.  Here a W-warp
-// CTA owns 128 W rows; the stacked model outputs arrive as 2-D tensor-map TMA boxes of G models x C classes x 128 W
-// rows; a thread owns four rows and keeps the C x 4 sums of the current batch of <= 8 models in REGISTERS (one 128-bit
+// instruction-bound: 15.8 instructions per element in stage 1 and 55 per (row, class) in the epilogue.  Here a one-warp
+// CTA owns 128 rows; the stacked model outputs arrive as 2-D tensor-map TMA boxes of G models x C classes x 128 rows;
+// a thread owns four rows and keeps the C x 4 sums of the current batch of <= 8 models in REGISTERS (one 128-bit
 // shared-memory read and 4 FMAs — plus 4 lg2 for SAMME.R — per class and model); each batch is folded into the
-// tile's running totals [C][128 W] in shared memory (own columns only), and the epilogue runs out of shared memory
+// tile's running totals [C][128] in shared memory (own columns only), and the epilogue runs out of shared memory
 // with 128-bit stores: P is read once, nothing is re-read.  Latency is covered by the other resident CTAs (up to 8
 // per SM), not by per-CTA double buffering.
-// W warps per CTA: 32 W threads, tiles of 128 W rows
-constexpr int kAggMaxStages = 4;
+constexpr int kClassTileRows = 128;  // one warp per CTA, four rows per thread
 
 struct ClassTileArgs {
   int M, C;          // models, classes
   int G;             // models per TMA box
-  int stages;
   int logp;          // f = log max(p, eps) (boosting real)
   const float* a;    // weights [M][C] (GBM classifier) or null
   const float* init; // [C] or null
@@ -497,44 +493,41 @@ __device__ __forceinline__ void finalize_tile4(const FinArgs& f, float* T, int64
   }
 }
 
-// dynamic shared memory (128-byte aligned): [stages][G*C][kAR] floats, then the running totals [C][kAR] (fp32, or
+// dynamic shared memory (128-byte aligned): [G*C][kAR] floats (one box), then the running totals [C][kAR] (fp32, or
 // fp64 for LOGP)
 // LOGP (SAMME.R): every model's lg2 max(p, eps) is added straight into fp64 totals in shared memory: late in boosting
 // most terms are -52 (exact for pure leaves), and fp32 batch sums of them lose 1e-5 of the probabilities from M ~ 8.
-template <int CMAX, int W, bool LOGP>
-__global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileArgs ta, const FinArgs f,
-                                                             const __grid_constant__ CUtensorMap mapP) {
-  constexpr int kAT = 32 * W, kAR = 128 * W;
+template <int CMAX, bool LOGP>
+__global__ void __launch_bounds__(32) agg_class_tile_kernel(const ClassTileArgs ta, const FinArgs f,
+                                                         const __grid_constant__ CUtensorMap mapP) {
+  constexpr int kAR = kClassTileRows;
   extern __shared__ __align__(128) unsigned char smem_dyn[];
-  float* ring = reinterpret_cast<float*>(smem_dyn + ((128u - (smem_u32(smem_dyn) & 127u)) & 127u));
-  __shared__ __align__(8) uint64_t full[kAggMaxStages];
-  const int C = ta.C, M = ta.M, S = ta.stages;
+  float* stage = reinterpret_cast<float*>(smem_dyn + ((128u - (smem_u32(smem_dyn) & 127u)) & 127u));
+  __shared__ __align__(8) uint64_t full;
+  const int C = ta.C, M = ta.M;
   const int box_rows = ta.G * C;
   const int stage_floats = box_rows * kAR;
   const int tid = threadIdx.x;
-  float* total = ring + (size_t)S * stage_floats + 4 * tid;  // this thread's four columns
-  double* total_lg = reinterpret_cast<double*>(ring + (size_t)S * stage_floats) + 4 * tid;  // LOGP
+  float* total = stage + stage_floats + 4 * tid;  // this thread's four columns
+  double* total_lg = reinterpret_cast<double*>(stage + stage_floats) + 4 * tid;  // LOGP
   if (tid == 0) {
-    for (int s = 0; s < S; ++s) mbar_init(&full[s], 1);
+    mbar_init(&full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  (void)kAT;
   const int64_t ntiles = (f.n + kAR - 1) / kAR;
   const int64_t my_tiles = (ntiles > blockIdx.x) ? (ntiles - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
   const int steps = (M + ta.G - 1) / ta.G;            // boxes per tile
   const int64_t nbox = my_tiles * steps;              // boxes this CTA consumes, in order
-  auto issue = [&](int64_t q, int stage) {            // one elected thread
+  auto issue = [&](int64_t q) {                       // one elected thread
     const int64_t tile = blockIdx.x + (q / steps) * gridDim.x;
     const int step = (int)(q % steps);
-    mbar_expect_tx(&full[stage], (uint32_t)(stage_floats * sizeof(float)));
-    tma_load_tile_at(ring + (size_t)stage * stage_floats, &mapP, (int)(tile * kAR), step * box_rows, &full[stage]);
+    mbar_expect_tx(&full, (uint32_t)(stage_floats * sizeof(float)));
+    tma_load_tile_at(stage, &mapP, (int)(tile * kAR), step * box_rows, &full);
   };
-  if (tid == 0)
-    for (int s = 0; s < S && s < nbox; ++s) issue(s, s);
+  if (tid == 0 && nbox > 0) issue(0);
 
-  int stage = 0;
   uint32_t phase = 0;
   int64_t q = 0;
   for (int64_t ti = 0; ti < my_tiles; ++ti) {
@@ -551,8 +544,8 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
       }
     }
     for (int step = 0; step < steps; ++step, ++q) {
-      mbar_wait(&full[stage], phase);
-      const float* box = ring + (size_t)stage * stage_floats + 4 * tid;
+      mbar_wait(&full, phase);
+      const float* box = stage + 4 * tid;
       const int m0 = step * ta.G;
       const int gcount = min(ta.G, M - m0);
       for (int g = 0; g < gcount; ++g) {
@@ -580,8 +573,8 @@ __global__ void __launch_bounds__(32 * W) agg_class_tile_kernel(const ClassTileA
         }
       }
       __syncthreads();  // every thread is done with the box: the stage can be refilled
-      if (tid == 0 && q + S < nbox) issue(q + S, stage);
-      if (++stage == S) stage = 0, phase ^= 1;
+      if (tid == 0 && q + 1 < nbox) issue(q + 1);
+      phase ^= 1;
       in_batch += gcount;
       if (!LOGP && (in_batch >= 8 || step == steps - 1)) {
         // fold the batch into the running totals: the rounding error stays at the magnitude of one batch
@@ -999,15 +992,13 @@ inline int grid_rows(int64_t items, int64_t per_cta, int ctas_per_sm, int sms) {
   return (int)(need < cap ? need : cap);
 }
 
-// class-wide sum kinds through the tile kernel (2 <= C <= 32 classes, the tile and >= 2 stages fit in shared memory)
+// class-wide sum kinds through the tile kernel (2 <= C <= 32 classes, the tile fits in shared memory)
 cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int sms, cudaStream_t st, bool* launched) {
   *launched = false;
-  static const int enabled = [] { const char* e = getenv("SE_AGG_TILE"); return e ? atoi(e) : 1; }();
-  if (!enabled || a.M < 1 || a.n < 1 || a.n >= (int64_t)0x7fffff00) return cudaSuccess;
+  if (a.M < 1 || a.n < 1 || a.n >= (int64_t)0x7fffff00) return cudaSuccess;
   // one warp per CTA (128-row tiles), one stage: shared memory bounds occupancy and what counts is the number of
   // boxes in flight per SM (more warps or stages per CTA leave fewer CTAs resident)
-  constexpr int warps = 1;
-  const int kAT = 32 * warps, kAR = 128 * warps;
+  constexpr int kAR = kClassTileRows;
   ClassTileArgs ta{};
   FinArgs f = f0;
   ta.M = a.M;
@@ -1028,10 +1019,7 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   const int box_rows = ta.G * C;
   const size_t stage_bytes = (size_t)box_rows * kAR * sizeof(float);
   const size_t total_bytes = (size_t)C * kAR * (ta.logp ? sizeof(double) : sizeof(float));
-  static const int forced_stages = [] { const char* e = getenv("SE_AGG_TILE_STAGES"); return e ? atoi(e) : 0; }();
-  const int stages = forced_stages >= 1 && forced_stages <= kAggMaxStages ? forced_stages : 1;
-  const size_t smem = total_bytes + stages * stage_bytes + 128;
-  ta.stages = stages;
+  const size_t smem = total_bytes + stage_bytes + 128;
   CUtensorMap mapP;
   cudaError_t e = make_tile_map_rows(&mapP, a.P, a.n, a.ld, (int64_t)a.M * C, kAR, box_rows);
   if (e != cudaSuccess) return e;
@@ -1043,10 +1031,10 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   const int grid = (int)(ntiles < cap ? ntiles : cap);
 #define SE_CT(CM, LG)                                                                                    \
   {                                                                                                      \
-    auto kern = agg_class_tile_kernel<CM, warps, LG>;                                                    \
+    auto kern = agg_class_tile_kernel<CM, LG>;                                                           \
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);              \
     if (e != cudaSuccess) return e;                                                                      \
-    kern<<<grid, kAT, smem, st>>>(ta, f, mapP);                                                          \
+    kern<<<grid, 32, smem, st>>>(ta, f, mapP);                                                           \
   }
   if (ta.logp) SE_CT(32, true)  // no register batch: CMAX is unused
   else if (C <= 4) SE_CT(4, false) else if (C <= 8) SE_CT(8, false) else if (C <= 16) SE_CT(16, false) else SE_CT(32, false)
@@ -1283,8 +1271,7 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
     case SE_AGG_BAGGING_HARD:
     case SE_AGG_BOOSTING_DISCRETE: {
       const bool weighted = (a.kind == SE_AGG_BOOSTING_DISCRETE);
-      static const bool packed_ok = [] { const char* e = getenv("SE_VOTES_PACKED"); return !(e && atoi(e) == 0); }();
-      if (!weighted && packed_ok && a.M <= 255 && (size_t)((a.K + 3) / 4) * kVR * kBlock * 4 <= 160 * 1024) {
+      if (!weighted && a.M <= 255 && (size_t)((a.K + 3) / 4) * kVR * kBlock * 4 <= 160 * 1024) {
         const size_t psmem = (size_t)((a.K + 3) / 4) * kVR * kBlock * sizeof(uint32_t);
         if (psmem > 48 * 1024) {
           cudaError_t e = cudaFuncSetAttribute(agg_hard_votes_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem);

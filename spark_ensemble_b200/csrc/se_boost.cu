@@ -5,8 +5,6 @@
 // passes over zipped RDDs per round; here SAMME.R is ONE pass (P[K][n] read once: 4K+8 B read, 4 B
 // written per row) that also produces both scalars, and SAMME is the two passes its data dependence
 // (β needs the error first) requires.  Weights are updated in place.
-#include <stdlib.h>
-
 #include "se_kernels.h"
 #include "se_loss.cuh"
 #include "se_tma.cuh"
@@ -127,6 +125,7 @@ __global__ void __launch_bounds__(kBlock) boost_real_kernel(const BoostArgs a) {
 // log p_y is picked from the tile afterwards.  Same arithmetic as boost_real_kernel (BoostingClassifier.scala:198-230).
 constexpr int kRT = 64;        // threads per CTA
 constexpr int kRR = 4 * kRT;   // rows per tile
+constexpr int kSammeTiledMinK = 5;  // SAMME.R: K <= 4 streams through registers (boost_real_kernel), wider K in tiles
 
 __global__ void __launch_bounds__(kRT) boost_real_tiled_kernel(const BoostArgs a, const __grid_constant__ CUtensorMap mapP) {
   extern __shared__ __align__(128) unsigned char smem_dyn[];
@@ -370,9 +369,8 @@ cudaError_t launch_boostreg_update(const BoostRegArgs& a, int ctas_per_sm, int s
 }
 
 cudaError_t launch_boost_real(const BoostArgs& a, int ctas_per_sm, int sms, cudaStream_t s) {
-  static const int tiled_min_k = [] { const char* e = getenv("SE_SAMME_TILED_MIN_K"); return e ? atoi(e) : 5; }();
   const size_t tile_bytes = (size_t)a.K * kRR * sizeof(float);
-  if (a.K >= tiled_min_k && a.n > 0 && a.n < (int64_t)0x7fffff00 && tile_bytes <= 200 * 1024) {
+  if (a.K >= kSammeTiledMinK && a.n > 0 && a.n < (int64_t)0x7fffff00 && tile_bytes <= 200 * 1024) {
     CUtensorMap mapP;
     cudaError_t e = make_tile_map(&mapP, a.proba, a.n, a.ld, a.K, kRR);
     if (e != cudaSuccess) return e;

@@ -10,8 +10,6 @@
 // computing (U x 3 independent 16 B requests in flight per thread), evaluates the loss in fp32,
 // accumulates sums in fp64, and the grid finishes with the deterministic last-CTA reduction from
 // se_common.cuh.  HBM-bound: K1 (update+residual+loss) moves 20 B/row, K2 (eval) 12 B/row.
-#include <stdlib.h>
-
 #include "se_kernels.h"
 #include "se_loss.cuh"
 
@@ -20,6 +18,7 @@ namespace se {
 namespace {
 
 constexpr int U_SCALAR = 4;  // float4 groups per thread per tile (cheap losses: pure streaming)
+constexpr int kLoglossTiledMinK = 5;  // LogLoss: K <= 4 classes per row in registers, wider K in TMA tiles
 
 // Transcendental-heavy losses spend ~30 instructions per row: with U = 4 (76-80 registers, 3 CTAs/SM) the
 // warps of an SM bunch up in the same load-then-compute phase (few eligible warps per cycle, low issue
@@ -522,17 +521,10 @@ cudaError_t launch_gbm(int loss, int mode, const GbmArgs& a, int ctas_per_sm, in
   }
   const int K = a.dim;
   if (K < 1 || K > kMaxDim) return cudaErrorInvalidValue;
-  // K classes per row in registers up to `staged_min_k - 1`; wider K goes through the TMA-tiled kernels (se_gbm_tiled.cu)
-  static const int staged_min_k = [] {
-    const char* e = getenv("SE_LOGLOSS_STAGED_MIN_K");
-    const int v = e ? atoi(e) : 5;
-    return v < 2 ? 2 : (v > 9 ? 9 : v);  // the register kernels exist for K <= 8 only
-  }();
-  if (K >= staged_min_k) return launch_gbm_logloss_tiled(mode, a, sms, st);
+  if (K >= kLoglossTiledMinK) return launch_gbm_logloss_tiled(mode, a, sms, st);
   if (ctas_per_sm > 4) ctas_per_sm = 4;  // register-resident K <= 4 kernels
   if (K <= 2) return launch_logloss_k<2, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
-  if (K <= 4) return launch_logloss_k<4, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
-  return launch_logloss_k<8, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
+  return launch_logloss_k<4, 4>(mode, a, grid_for((a.n + 3) / 4, kBlock, ctas_per_sm, sms), st);
 }
 
 cudaError_t launch_gbm_pack_signed(const float* y, const float* F, const float* h, float* u, float* v, int64_t n,

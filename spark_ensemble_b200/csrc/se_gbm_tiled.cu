@@ -17,8 +17,6 @@
 // e_y / s = softmax_y - 1 keeps full relative precision on well-fitted rows).
 // About 8 instructions per (row, class) instead of ~37 for the one-row-per-thread form which was
 // issue-bound, far from the HBM roofline in eval mode.
-#include <stdlib.h>
-
 #include "se_kernels.h"
 #include "se_loss.cuh"
 #include "se_tma.cuh"
@@ -42,7 +40,7 @@ struct TiledTraits {
   static constexpr bool kReduce = kSumLoss || kNewton;
 };
 
-// dynamic shared memory (128-byte aligned): [stage][ {F,h} ][K][kTR] floats
+// dynamic shared memory (128-byte aligned): [ {F,h} ][K][kTR] floats
 template <int KMAX, int MODE, int W>
 __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs a,
                                                                 const __grid_constant__ CUtensorMap mapF,
@@ -52,19 +50,18 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
   extern __shared__ __align__(128) unsigned char smem_dyn[];
   // TMA tile destinations must be 128-byte aligned; the offset is applied to the shared array itself so that
   // the compiler keeps shared-memory addressing (LDS/STS) for everything derived from it
-  float* stage_base = reinterpret_cast<float*>(smem_dyn + ((128u - (smem_u32(smem_dyn) & 127u)) & 127u));
+  float* stage = reinterpret_cast<float*>(smem_dyn + ((128u - (smem_u32(smem_dyn) & 127u)) & 127u));
   const int K = a.dim;
   constexpr int kArrays = T::kReadH ? 2 : 1;
   const int stage_floats = kArrays * K * kTR;
-  __shared__ __align__(8) uint64_t bars[2];
+  __shared__ __align__(8) uint64_t bar;
   __shared__ float s_coef[kMaxDim];
   __shared__ __align__(16) float s_scale[T::kPerClassAcc ? kTR : 4];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (int k = tid; k < K; k += kTT) s_coef[k] = a.coef[k];
   if (tid == 0) {
-    mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
+    mbar_init(&bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -72,14 +69,6 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
   const int64_t ntiles = (a.n + kTR - 1) / kTR;
   const int64_t ld = a.ld;
   const bool has_w = (a.w != nullptr);
-  const bool two_stage = (a.stages >= 2);
-
-  auto issue = [&](int64_t tile, int stage) {  // one elected thread: the whole stage in <= 2 instructions
-    float* dst = stage_base + (size_t)stage * stage_floats;
-    mbar_expect_tx(&bars[stage], (uint32_t)(stage_floats * sizeof(float)));
-    tma_load_tile(dst, &mapF, (int)(tile * kTR), &bars[stage]);
-    if (T::kReadH) tma_load_tile(dst + K * kTR, &mapH, (int)(tile * kTR), &bars[stage]);
-  };
 
   constexpr int NRED = T::kPerClassAcc ? KMAX + 1 : 1;
   constexpr int kAcc = T::kPerClassAcc ? KMAX / W : 1;
@@ -88,16 +77,13 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
 #pragma unroll
   for (int kk = 0; kk < kAcc; ++kk) acc_c[kk] = 0.0;
 
-  int64_t tile = blockIdx.x;
-  if (two_stage && tid == 0 && tile < ntiles) issue(tile, 0);
   uint32_t it = 0;
-  for (; tile < ntiles; tile += gridDim.x, ++it) {
-    const int stage = two_stage ? (it & 1) : 0;
-    const int64_t next = tile + gridDim.x;
-    if (two_stage) {
-      if (tid == 0 && next < ntiles) issue(next, stage ^ 1);  // that stage was released by the barrier below
-    } else if (tid == 0) {
-      issue(tile, 0);  // single stage: the other resident CTAs of the SM cover this tile's load latency
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+    // one elected thread loads the whole tile in <= 2 instructions; the other resident CTAs of the SM cover its latency
+    if (tid == 0) {
+      mbar_expect_tx(&bar, (uint32_t)(stage_floats * sizeof(float)));
+      tma_load_tile(stage, &mapF, (int)(tile * kTR), &bar);
+      if (T::kReadH) tma_load_tile(stage + K * kTR, &mapH, (int)(tile * kTR), &bar);
     }
     const int64_t row0 = tile * kTR + 4 * tid;
     const bool any_in = row0 < a.n;
@@ -115,8 +101,8 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
       yi[j] = in[j] ? min(max((int)f4at(y4, j), 0), K - 1) : 0;  // clamp = memory safety; validity is checked once per label upload
       if (!in[j]) f4at(c4, j) = 0.f;
     }
-    mbar_wait(&bars[stage], two_stage ? ((it >> 1) & 1) : (it & 1));
-    float* sF = stage_base + (size_t)stage * stage_floats + 4 * tid;
+    mbar_wait(&bar, it & 1);
+    float* sF = stage + 4 * tid;
     const float* sH = sF + K * kTR;
 
     // ---- A1: p = F + c_k h (GBMLoss.scala:56-59), running max and argmax (first maximum); p replaces F in shared memory
@@ -192,7 +178,7 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
       float4 sc[W];
 #pragma unroll
       for (int q = 0; q < W; ++q) sc[q] = lds4(s_scale + 128 * q + 4 * lane);
-      const float* tE = stage_base + (size_t)stage * stage_floats + 4 * lane;
+      const float* tE = stage + 4 * lane;
       const float* tH = tE + K * kTR;
 #pragma unroll
       for (int kk = 0; kk < kAcc; ++kk) {
@@ -238,7 +224,7 @@ __global__ void __launch_bounds__(32 * W) gbm_logloss_tiled_kernel(const GbmArgs
         }
       }
       __syncthreads();
-      const float* tE = stage_base + (size_t)stage * stage_floats + 4 * lane;
+      const float* tE = stage + 4 * lane;
 #pragma unroll
       for (int kk = 0; kk < kAcc; ++kk) {
         const int k = warp + W * kk;
@@ -333,12 +319,7 @@ cudaError_t launch_tiled_k(int mode, const GbmArgs& a, int sms, cudaStream_t st)
   }
   const size_t stage_bytes = (size_t)(read_h ? 2 : 1) * K * kTR * sizeof(float);
   // one stage: with shared memory bounding occupancy, more resident CTAs beat double buffering at every K
-  // SE_LOGLOSS_STAGES=2 for experiments
-  static const int forced_stages = [] { const char* s = getenv("SE_LOGLOSS_STAGES"); return s ? atoi(s) : 0; }();
-  const int stages = forced_stages >= 2 ? 2 : 1;
-  GbmArgs args = a;
-  args.stages = stages;
-  const size_t smem = stages * stage_bytes + 128;
+  const size_t smem = stage_bytes + 128;
   int per_sm = (int)((228 * 1024) / (smem + 2560));  // + static shared memory and the 1 KB the system reserves per CTA
   if (per_sm < 1) return cudaErrorInvalidValue;
   if (per_sm > 16 / W) per_sm = 16 / W;  // at most 16 resident warps per SM
@@ -352,7 +333,7 @@ cudaError_t launch_tiled_k(int mode, const GbmArgs& a, int sms, cudaStream_t st)
     auto kern = gbm_logloss_tiled_kernel<KMAX, M, W>;                                                     \
     e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);             \
     if (e != cudaSuccess) return e;                                                                     \
-    kern<<<grid, kTT, smem, st>>>(args, mapF, mapH);                                                    \
+    kern<<<grid, kTT, smem, st>>>(a, mapF, mapH);                                                       \
     break;                                                                                              \
   }
   switch (mode) {

@@ -43,7 +43,6 @@ struct GbmArgs {
   // step = (float)(lr64 * *dev_alpha) when non-null: alpha comes from the on-device line search (se_brent.cu)
   const double* dev_alpha = nullptr;
   double lr64 = 1.0;
-  int stages = 1;  // tiled logloss kernel: shared-memory stages (1, or 2 for experiments)
   int stats_from_r = 0;  // squared-loss statistics read the current residual slot r = y - F (8 B/row) instead of y, F (12 B/row)
   int l2_hints = 0; // L2-sized shard: evict_first for the arrays the next pass does not re-read (se_common.cuh)
   int reverse = 0; // walk the tiles from the end: consecutive passes alternate direction so the tail of one

@@ -6,8 +6,6 @@
 // fitted model here means h never crosses PCIe (SURVEY.md §8f-1).  Supported: binary decision trees
 // with continuous splits (Spark ContinuousSplit.shouldGoLeft: x <= threshold goes left) and linear
 // models.  HasSubBag.slice (ensemble/HasSubBag.scala:81-84) is folded into the feature->column map.
-#include <stdlib.h>
-
 #include "se_kernels.h"
 
 namespace se {
@@ -212,11 +210,7 @@ __global__ void __launch_bounds__(kBlock, MINB) tree_predict_binned_kernel(const
 // INDEPENDENT vector loads (no level-to-level dependency, one wavefront per 128 rows instead of one per sector), four
 // byte-compares at a time in SWAR form, and the per-row walk reads its decision bits from shared memory.
 //   bit j of a row = rank(x[col_j]) <= t_j; internal node ordinals j are assigned in node order by warp 0.
-constexpr int kTreeMaskWords = 4;
-template <int RW> struct MaskVec;
-template <> struct MaskVec<1> { using type = uint32_t; };
-template <> struct MaskVec<2> { using type = uint2; };
-template <> struct MaskVec<4> { using type = uint4; };
+constexpr int RW = 4;  // words of 4 consecutive rows per thread, fetched as ONE 16-byte load per node
 
 __device__ __forceinline__ uint32_t bytes_le(uint32_t x, uint32_t t, uint32_t t_hi) {
   // bit 7 of every byte lane: x_byte <= t_byte.  Low 7 bits: (t_lo + 128) - x_lo keeps bit 7 iff t_lo >= x_lo (no
@@ -225,10 +219,8 @@ __device__ __forceinline__ uint32_t bytes_le(uint32_t x, uint32_t t, uint32_t t_
   return (~x & t) | (~(x ^ t) & d);
 }
 
-template <int RW>  // RW words of 4 consecutive rows per thread, fetched as ONE 4*RW-byte load per node
 __global__ void __launch_bounds__(kBlock, 4) tree_predict_mask_kernel(const TreeArgs a, const uint8_t* __restrict__ X8,
                                                                       const uint4* __restrict__ nodes) {
-  using V = typename MaskVec<RW>::type;
   __shared__ unsigned long long s_off[64];
   __shared__ uint32_t s_thr[64];
   __shared__ uint32_t s_walk[256];  // ordinal | left << 8 | right << 16 | leaf << 31
@@ -283,7 +275,7 @@ __global__ void __launch_bounds__(kBlock, 4) tree_predict_mask_kernel(const Tree
       for (int s = 0; s < 8; ++s) {
         const int j = 8 * k + s;
         const uint32_t t = s_thr[j];
-        const V v = __ldg(reinterpret_cast<const V*>(row + s_off[j]));
+        const uint4 v = __ldg(reinterpret_cast<const uint4*>(row + s_off[j]));
         const uint32_t* xs = reinterpret_cast<const uint32_t*>(&v);
 #pragma unroll
         for (int w = 0; w < RW; ++w) {
@@ -291,7 +283,7 @@ __global__ void __launch_bounds__(kBlock, 4) tree_predict_mask_kernel(const Tree
           acc[w] |= (s == 7 ? le : (le >> (7 - s))) & (0x01010101u << s);
         }
       }
-      *reinterpret_cast<V*>(&s_acc[k][tid * RW]) = *reinterpret_cast<const V*>(acc);
+      *reinterpret_cast<uint4*>(&s_acc[k][tid * RW]) = *reinterpret_cast<const uint4*>(acc);
     }
     // the thread reads back only what it stored itself: no barrier
 #pragma unroll
@@ -454,43 +446,24 @@ cudaError_t launch_tree_predict_binned(const TreeArgs& a, const uint8_t* X8, con
                                        int sms, cudaStream_t st) {
   const size_t smem = (size_t)a.n_nodes * (sizeof(uint4) + sizeof(float));
   if (smem > 200 * 1024) return cudaErrorInvalidValue;
-  static const int variant = [] { const char* e = getenv("SE_TREE_VARIANT"); return e ? atoi(e) : 0; }();
-  const int64_t ngroups = (a.n + TV - 1) / TV;
-  // shallow trees: all node comparisons from coalesced column reads, then a walk over bits (tree_predict_mask_kernel)
-  // SE_TREE_VARIANT: 0 default, 1-5 and 9 walk variants, 10/11/12 all-nodes kernel with 1/2/4 words per thread
-  if (mask_mode && n_internal <= 64 && a.n_nodes <= 256 && (variant == 0 || variant >= 10)) {
-    const int rw = variant == 10 ? 1 : variant == 11 ? 2 : variant == 12 ? 4 : kTreeMaskWords;
-    const int64_t need0 = (a.n + 4 * rw - 1) / (4 * rw);
-    int64_t need = (need0 + kBlock - 1) / kBlock;
-    if (need < 1) need = 1;
-    const int64_t cap = (int64_t)sms * 16;
-    const int grid = (int)(need < cap ? need : cap);
-    if (rw == 1) tree_predict_mask_kernel<1><<<grid, kBlock, 0, st>>>(a, X8, nodes);
-    else if (rw == 2) tree_predict_mask_kernel<2><<<grid, kBlock, 0, st>>>(a, X8, nodes);
-    else tree_predict_mask_kernel<4><<<grid, kBlock, 0, st>>>(a, X8, nodes);
+  // shallow trees: all node comparisons from coalesced column reads, then a walk over bits (tree_predict_mask_kernel);
+  // deeper ones walk the rank matrix level by level (tree_predict_binned_kernel)
+  const bool all_nodes = mask_mode && n_internal <= 64 && a.n_nodes <= 256;
+  const int64_t rows_per_thread = all_nodes ? 4 * RW : TV;
+  int64_t need = ((a.n + rows_per_thread - 1) / rows_per_thread + kBlock - 1) / kBlock;
+  if (need < 1) need = 1;
+  const int64_t cap = (int64_t)sms * 16;
+  const int grid = (int)(need < cap ? need : cap);
+  if (all_nodes) {
+    tree_predict_mask_kernel<<<grid, kBlock, 0, st>>>(a, X8, nodes);
     return cudaGetLastError();
   }
-#define SE_TREE_LAUNCH(W, MINB)                                                                                      \
-  do {                                                                                                               \
-    auto kern = tree_predict_binned_kernel<W, MINB>;                                                                 \
-    if (smem > 48 * 1024) {                                                                                          \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);            \
-      if (e != cudaSuccess) return e;                                                                                \
-    }                                                                                                                \
-    int64_t need = (ngroups + (int64_t)kBlock * W - 1) / ((int64_t)kBlock * W);                                      \
-    if (need < 1) need = 1;                                                                                          \
-    const int64_t cap = (int64_t)sms * 16;                                                                           \
-    kern<<<(int)(need < cap ? need : cap), kBlock, smem, st>>>(a, X8, nodes);                                        \
-  } while (0)
-  switch (variant) {
-    case 1: SE_TREE_LAUNCH(1, 8); break;
-    case 2: SE_TREE_LAUNCH(2, 4); break;
-    case 3: SE_TREE_LAUNCH(2, 3); break;
-    case 4: SE_TREE_LAUNCH(4, 2); break;
-    case 5: SE_TREE_LAUNCH(1, 6); break;
-    default: SE_TREE_LAUNCH(1, 4); break;
+  auto kern = tree_predict_binned_kernel<1, 4>;
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
   }
-#undef SE_TREE_LAUNCH
+  kern<<<grid, kBlock, smem, st>>>(a, X8, nodes);
   return cudaGetLastError();
 }
 
