@@ -365,6 +365,20 @@ SE_API int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int 
                          const int32_t* offsets, const int32_t* feature, const float* threshold, const int32_t* left,
                          const int32_t* right, const float* value, const float* probs, const int32_t* tree_class,
                          const double* weights, const double* init);
+/* The weighted median of a forest of 1..SE_FOREST_MEDIAN_MAX_TREES regression trees in ONE pass:
+ * out[row] = Utils.weightedMedian(tree_t(x) in model order, weights) (ensemble/Utils.scala:26-40,
+ * BoostingRegressionModel.predict with votingStrategy "median", regression/BoostingRegressor.scala:333-337), written to
+ * row out_row of out_slot.  Trees as se_forest_predict (offsets, tree-local children, GLOBAL columns of X), one fp64
+ * weight per tree.  Every row walks every tree over the uint8 rank matrix and keeps its M leaf values on chip: no
+ * [M][n] member outputs (SE_SLOT_P is not used).  The result is bit for bit what se_tree_predict per member into
+ * SE_SLOT_P followed by se_agg_run(SE_AGG_BOOSTING_REG_MEDIAN) gives for the same trees and weights, including -0, NaN
+ * leaves, ties and weights that are negative or not finite.  Fails with SE_ERR_ARG above SE_FOREST_MEDIAN_MAX_TREES
+ * trees or on a malformed tree, and with SE_ERR_STATE, with se_forest_predict's message, when the rank matrix cannot
+ * hold the forest's thresholds: evaluate the members with se_tree_predict + se_agg_run then. */
+#define SE_FOREST_MEDIAN_MAX_TREES 64
+SE_API int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets, const int32_t* feature,
+                            const float* threshold, const int32_t* left, const int32_t* right, const float* value,
+                            const double* weights, int out_slot, int out_row);
 /* ---- regression-tree fit on the device (DESIGN.md §3 "Device tree fit") ----------------------- */
 /* Sets the split candidates of a fit: column c of SE_SLOT_X (n_cols == its column count) gets the sorted, finite,
  * strictly increasing thresholds[offsets[c] .. offsets[c+1]) (0..255 of them) as the edge list of the uint8 rank matrix

@@ -116,6 +116,10 @@ TABLE = [
                                     ("threshold", "in_f32"), ("left", "in_i32"), ("right", "in_i32"), ("value", "in_f32"),
                                     ("probs", "in_f32"), ("treeClass", "in_i32"), ("weights", "in_f64"), ("init", "in_f64")],
      "predictRaw / probability / prediction of a classifier ensemble of trees in one pass, without member outputs"),
+    ("forestMedian", "se_forest_median", [("ctx", "ctx"), ("which", "i32"), ("nTrees", "i32"), ("offsets", "in_i32"), ("feature", "in_i32"),
+                                          ("threshold", "in_f32"), ("left", "in_i32"), ("right", "in_i32"), ("value", "in_f32"),
+                                          ("weights", "in_f64"), ("outSlot", "i32"), ("outRow", "i32")],
+     "BoostingRegressionModel.predict (median) for 1..64 tree members: the weighted median in one pass, without member outputs"),
     ("linearPredict", "se_linear_predict", [("ctx", "ctx"), ("which", "i32"), ("nCoef", "i32"), ("coef", "in_f32"), ("intercept", "f32"),
                                             ("subspace", "in_i32"), ("outSlot", "i32"), ("outRow", "i32")], ""),
 ]

@@ -30,6 +30,7 @@ UPD_RESIDUAL, UPD_NEWTON, UPD_LOSS = 1, 2, 4
  AGG_BOOSTING_REAL, AGG_BOOSTING_DISCRETE, AGG_BOOSTING_REG_MEDIAN, AGG_BOOSTING_REG_MEAN) = range(9)
 R2_LOSS = {"exponential": 0, "linear": 1, "squared": 2}
 FOREST_AGG_MAX_CLASSES = 32  # SE_FOREST_AGG_MAX_CLASSES: se_forest_agg's class limit
+FOREST_MEDIAN_MAX_TREES = 64  # SE_FOREST_MEDIAN_MAX_TREES: se_forest_median's tree limit
 
 # enum se_kernel_family
 KERNEL_FAMILIES = ["sq_stats", "eval", "update", "resid", "mean_loss", "boost_real", "boost_err",
@@ -115,6 +116,7 @@ PROTOTYPES = {
     "se_tree_predict_multi": [_vp, _i32, _i32, _ip, _fp, _ip, _ip, _fp, _i32, _ip, _i32, _i32],
     "se_forest_predict": [_vp, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _dp, _d, _i32, _i32],
     "se_forest_agg": [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _fp, _ip, _dp, _dp],
+    "se_forest_median": [_vp, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _dp, _i32, _i32],
     "se_linear_predict": [_vp, _i32, _i32, _fp, _f, _ip, _i32, _i32],
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,

@@ -415,6 +415,18 @@ class Context:
                                              N.iptr(l), N.iptr(r), N.fptr(v), None if w is None else N.dptr(w),
                                              float(init), out_slot, out_row))
 
+    def forest_median(self, trees, out_slot: int, weights, out_row: int = 0, validation: bool = False, subspaces=None):
+        """out = the weighted median of tree_t(x) (BoostingRegressionModel.predict with votingStrategy "median",
+        ensemble/Utils.scala:26-40) for 1..64 regression trees in one pass over the resident feature matrix
+        (se_forest_median): bit for bit what tree_predict per member into SLOT_P + agg_run(AGG_BOOSTING_REG_MEDIAN)
+        gives.  `subspaces[t]` maps tree t's feature indices to columns of X."""
+        offs, f, t, l, r, v, _ = _pack_forest(trees, subspaces)
+        w = np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        if w.size != len(trees):
+            raise ValueError("one weight per tree")
+        self._ck(self._lib.se_forest_median(self._h, int(validation), len(trees), N.iptr(offs), N.iptr(f), N.fptr(t),
+                                            N.iptr(l), N.iptr(r), N.fptr(v), N.dptr(w), out_slot, out_row))
+
     def forest_agg(self, kind: int, num_classes: int, trees, weights=None, init=None, tree_class=None, dim: int = 1,
                    loss=0, validation: bool = False, subspaces=None):
         """A classifier ensemble of trees scored in one pass over the resident feature matrix, straight into RAW,

@@ -1139,6 +1139,138 @@ __global__ void __launch_bounds__(kForestAggTile) forest_agg_kernel(const Forest
   if (bad_vote && g.bad_label != nullptr) *reinterpret_cast<volatile int*>(g.bad_label) = 1;
 }
 
+// ---- the weighted median of a regression forest in one pass (se_forest_median) -----------------------------------
+// The member route writes every tree's outputs to SE_SLOT_P ([M][n], 4·M B per row) and reads them back in
+// agg_wmedian_fast_kernel / agg_wmedian_list_kernel.  Here the row's M leaf values go to its own column of shared
+// memory instead, chunk after chunk, and the same decisions are taken on them: the keys-only sort and model-order
+// bisection, and the exact (key, model) sort with sorted-order sums for the rows inside the margin (mode 1) or for all
+// rows (mode 0: a weight that is negative or not finite, or the fast path switched off).  So every row picks the
+// member route's value, bit for bit.
+static_assert(kForestMedianMaxTrees == SE_FOREST_MEDIAN_MAX_TREES, "the kernel's tree limit is the ABI's");
+
+// (min blocks 1: with the default bounds ptxas spilled a few bytes at MP = 1; shared memory holds the CTAs per SM to
+// four at most anyway)
+template <int MP>
+__global__ void __launch_bounds__(kForestMedianTile, 1) forest_median_kernel(const __grid_constant__ ForestMedianArgs g) {
+  constexpr int TILE = kForestMedianTile;
+  constexpr int LOG = (MP == 1) ? 0 : (MP == 2) ? 1 : (MP == 4) ? 2 : (MP == 8) ? 3 : (MP == 16) ? 4 : (MP == 32) ? 5 : 6;
+  extern __shared__ __align__(16) unsigned char fsm[];
+  __shared__ double s_a[kForestMedianMaxTrees];
+  for (int m = threadIdx.x; m < kForestMedianMaxTrees; m += TILE) s_a[m] = (m < g.M) ? g.w[m] : 0.0;
+  const int M = g.M;
+  float* vals = reinterpret_cast<float*>(fsm + g.vals_off) + threadIdx.x;  // this row's leaf values: own column
+  const unsigned char* myr = fsm + threadIdx.x;  // + the chunk's blob_bytes: this row's ranks
+  const double half = 0.5 * g.total;
+  const int64_t ntiles = (g.n + TILE - 1) / TILE;
+  for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    const int64_t row0 = tile * TILE, row = row0 + threadIdx.x;
+    const bool in = row < g.n;
+    for (int k = 0; k < g.n_chunks; ++k) {
+      const ForestMedianChunk ch = g.chunk[k];  // a copy: a reference into the parameters spilled at MP = 16
+      const unsigned char* blob = g.blob + ch.blob_off;
+      __syncthreads();  // the previous chunk's (or tile's) walks are over
+      if (g.n_chunks > 1 || tile == blockIdx.x)  // one chunk stays staged for every tile of the CTA
+        for (int i = threadIdx.x; i < ch.blob_bytes / 16; i += TILE)
+          reinterpret_cast<uint4*>(fsm)[i] = __ldg(reinterpret_cast<const uint4*>(blob) + i);
+      const unsigned long long* coloff = reinterpret_cast<const unsigned long long*>(blob + ch.off_coloff);
+      unsigned char* s_rank = fsm + ch.blob_bytes;
+      for (int i = threadIdx.x; i < ch.C * (TILE / 4); i += TILE) {
+        const int c = i / (TILE / 4), q = i % (TILE / 4);
+        const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
+        uint32_t v = 0;
+        if (r < g.ld8) v = __ldg(reinterpret_cast<const uint32_t*>(g.X8 + __ldg(coloff + c) + r));
+        *reinterpret_cast<uint32_t*>(s_rank + c * TILE + 4 * q) = v;
+      }
+      __syncthreads();
+      if (!in) continue;
+      const uint2* s_nodes = reinterpret_cast<const uint2*>(fsm + ch.off_nodes);
+      const int* s_toff = reinterpret_cast<const int*>(fsm + ch.off_treeoff);
+      const float* s_val = reinterpret_cast<const float*>(fsm + ch.off_values);
+      const unsigned char* r8 = myr + ch.blob_bytes;
+      float* v = vals + (size_t)ch.t0 * TILE;
+      int t = 0;
+      for (; t + 1 < ch.T; t += 2) {  // two independent walks in flight
+        const uint2* n0 = s_nodes + s_toff[t];
+        const uint2* n1 = s_nodes + s_toff[t + 1];
+        int d0 = 0, d1 = 0;
+        bool l0 = true, l1 = true;
+        while (l0 || l1) {
+          if (l0) forest_step<TILE>(n0, r8, d0, l0);
+          if (l1) forest_step<TILE>(n1, r8, d1, l1);
+        }
+        v[t * TILE] = s_val[s_toff[t] + d0];
+        v[(t + 1) * TILE] = s_val[s_toff[t + 1] + d1];
+      }
+      if (t < ch.T) {
+        const uint2* n0 = s_nodes + s_toff[t];
+        int d0 = 0;
+        bool l0 = true;
+        while (l0) forest_step<TILE>(n0, r8, d0, l0);
+        v[t * TILE] = s_val[s_toff[t] + d0];
+      }
+    }
+    // agg_wmedian_fast_kernel on the row's values (modes 1 and 2)
+    uint32_t pick = 0;
+    bool exact = (g.mode == 0);
+    if constexpr (MP == 1) {  // one tree: both routes return its value (one weight is always "all equal": no margin)
+      pick = wm_key(vals[0]);
+      exact = false;
+    } else if (in && g.mode != 0) {
+      uint32_t key[MP], s[MP];
+#pragma unroll
+      for (int m = 0; m < MP; ++m) {
+        key[m] = 0xFFFFFFFFu;  // padding sorts last and carries weight 0
+        if (m < M) key[m] = wm_key(vals[m * TILE]);
+        s[m] = key[m];
+      }
+      sortnet_oddeven<MP>(s, [](uint32_t& x, uint32_t& y) {
+        const uint32_t lo = min(x, y), hi = max(x, y);
+        x = lo;
+        y = hi;
+      });
+      uint32_t t = 0, v_hi = s[MP - 1];
+      double c_lo = 0.0, c_hi = g.total;
+      auto probe = [&](uint32_t v) {
+        double c = 0.0;
+#pragma unroll
+        for (int m = 0; m < MP; ++m) {
+          const double b = __hiloint2double((key[m] <= v) ? 0x3ff00000 : 0, 0);
+          c = fma(g.w[m], b, c);
+        }
+        const bool right = !(c >= half);
+        c_lo = right ? c : c_lo;
+        c_hi = right ? c_hi : c;
+        v_hi = right ? v_hi : v;
+        t = 2u * t + (right ? 1u : 0u);
+      };
+      if constexpr (LOG > 0) probe(wm_candidate<MP, 0>(s, t));
+      if constexpr (LOG > 1) probe(wm_candidate<MP, 1>(s, t));
+      if constexpr (LOG > 2) probe(wm_candidate<MP, 2>(s, t));
+      if constexpr (LOG > 3) probe(wm_candidate<MP, 3>(s, t));
+      if constexpr (LOG > 4) probe(wm_candidate<MP, 4>(s, t));
+      if constexpr (LOG > 5) probe(wm_candidate<MP, 5>(s, t));
+      const bool safe = (c_hi - half > g.tau) && (half - c_lo > g.tau);
+      pick = v_hi;
+      exact = (g.mode == 1) && !safe;
+    }
+    // the exact (key, model) sort and sorted-order sums, as agg_wmedian_list_kernel / agg_wmedian_reg_kernel
+    if (in && exact) {
+      unsigned long long w[MP];
+#pragma unroll
+      for (int m = 0; m < MP; ++m) {
+        w[m] = ~0ull;
+        if (m < M) w[m] = ((unsigned long long)wm_key(vals[m * TILE]) << 32) | (unsigned long long)(unsigned)m;
+      }
+      pick = (uint32_t)(wm_exact_pick<MP>(w, M, s_a) >> 32);
+    }
+    if (in) g.out[row] = wm_unkey(pick);
+    if (g.mode == 1 && g.deferred != nullptr) {  // rows inside the margin, for se_ctx_get_option("last_wm_deferred")
+      const unsigned mask = __ballot_sync(0xffffffffu, in && exact);
+      if (mask && (threadIdx.x & 31) == __ffs(mask) - 1) atomicAdd(g.deferred, (unsigned)__popc(mask));
+    }
+  }
+}
+
 }  // namespace
 
 cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t st) {
@@ -1346,6 +1478,54 @@ cudaError_t launch_forest_agg(const ForestAggArgs& g, int sms, cudaStream_t st) 
     default: return cudaErrorInvalidValue;
   }
 #undef SE_FA
+  return cudaGetLastError();
+}
+
+cudaError_t forest_median_ctas_per_sm(int M, int* ctas) {
+  int Mp = 1;
+  while (Mp < M) Mp <<= 1;
+  cudaFuncAttributes fa{};
+  cudaError_t e = cudaErrorInvalidValue;
+  switch (Mp) {
+#define SE_FM(MPV) case MPV: e = cudaFuncGetAttributes(&fa, forest_median_kernel<MPV>); break;
+    SE_FM(1) SE_FM(2) SE_FM(4) SE_FM(8) SE_FM(16) SE_FM(32) SE_FM(64)
+#undef SE_FM
+    default: break;
+  }
+  if (e != cudaSuccess) return e;
+  const int regs = (fa.numRegs + 7) / 8 * 8;  // allocated per thread in units of 8
+  *ctas = regs > 0 ? 65536 / (regs * kForestMedianTile) : 16;
+  if (*ctas < 1) *ctas = 1;
+  return cudaSuccess;
+}
+
+cudaError_t launch_forest_median(const ForestMedianArgs& g, size_t smem, int sms, cudaStream_t st) {
+  if (g.M < 1 || g.M > kForestMedianMaxTrees || g.n_chunks < 1 || g.n_chunks > g.M || smem > 220 * 1024)
+    return cudaErrorInvalidValue;
+  int per_sm = (int)((228 * 1024) / (smem + sizeof(double) * kForestMedianMaxTrees + 1024));
+  if (per_sm < 1) per_sm = 1;
+  if (per_sm > 16) per_sm = 16;
+  int64_t need = (g.n + kForestMedianTile - 1) / kForestMedianTile;
+  if (need < 1) need = 1;
+  const int64_t cap = (int64_t)sms * per_sm;
+  const int grid = (int)(need < cap ? need : cap);
+  int Mp = 1;
+  while (Mp < g.M) Mp <<= 1;
+  switch (Mp) {
+#define SE_FM(MPV)                                                                                               \
+  case MPV: {                                                                                                    \
+    auto kern = forest_median_kernel<MPV>;                                                                       \
+    if (smem > 48 * 1024) {                                                                                      \
+      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
+      if (e != cudaSuccess) return e;                                                                            \
+    }                                                                                                            \
+    kern<<<grid, kForestMedianTile, smem, st>>>(g);                                                              \
+    break;                                                                                                       \
+  }
+    SE_FM(1) SE_FM(2) SE_FM(4) SE_FM(8) SE_FM(16) SE_FM(32) SE_FM(64)
+#undef SE_FM
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

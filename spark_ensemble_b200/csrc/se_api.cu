@@ -2869,7 +2869,7 @@ void forest_layout(size_t T, size_t C, size_t Nn, bool cls, ForestArgs& a) {
 // `fixed` bytes the kernel keeps for itself fit one CTA's shared memory.  A chunk grows tree by tree under the
 // four-CTAs-per-SM budget; a member that does not fit it alone gets two, then one CTA per SM.
 int forest_plan(se_ctx* ctx, int64_t d, int n_trees, const int32_t* offsets, const int32_t* feature, bool cls, int tile,
-                size_t fixed, std::vector<ForestChunk>& chunks) {
+                size_t fixed, std::vector<ForestChunk>& chunks, size_t first_budget = kForestSmemBudget) {
   chunks.clear();
   std::vector<int32_t> local((size_t)d, -1);  // global column -> local column of the current chunk
   std::vector<int32_t> used;
@@ -2877,7 +2877,7 @@ int forest_plan(se_ctx* ctx, int64_t d, int n_trees, const int32_t* offsets, con
   while (t0 < n_trees) {
     size_t nodes = 0;
     int t1 = t0;
-    for (const size_t budget : {(size_t)kForestSmemBudget, (size_t)(100 * 1024), (size_t)(216 * 1024)}) {
+    for (const size_t budget : {first_budget, std::max(first_budget, (size_t)(100 * 1024)), (size_t)(216 * 1024)}) {
       for (int32_t c : used) local[c] = -1;
       used.clear();
       nodes = 0;
@@ -2910,14 +2910,13 @@ int forest_plan(se_ctx* ctx, int64_t d, int n_trees, const int32_t* offsets, con
   return SE_OK;
 }
 
-// Packs a chunk (weights NULL: all 1; tree_class NULL: no class array) into ctx->d_forest and sets the layout fields of
-// `a`.  Returns once the copy is done: the blob is pageable host memory and d_forest is reused by the next chunk.
-int forest_upload_chunk(se_ctx* ctx, const BinState& B, const ForestChunk& ch, const int32_t* offsets,
-                        const int32_t* feature, const float* threshold, const int32_t* left, const int32_t* right,
-                        const float* value, const double* weights, const int32_t* tree_class, ForestArgs& a) {
+// Packs a chunk (weights NULL: all 1; tree_class NULL: no class array) into `blob` and sets the layout fields of `a`.
+void forest_pack_chunk(const BinState& B, const ForestChunk& ch, const int32_t* offsets, const int32_t* feature,
+                       const float* threshold, const int32_t* left, const int32_t* right, const float* value,
+                       const double* weights, const int32_t* tree_class, ForestArgs& a, std::vector<unsigned char>& blob) {
   const size_t T = (size_t)(ch.t1 - ch.t0), C = ch.cols.size();
   forest_layout(T, C, ch.nodes, tree_class != nullptr, a);
-  std::vector<unsigned char> blob((size_t)a.blob_bytes, 0);
+  blob.assign((size_t)a.blob_bytes, 0);
   std::vector<int32_t> local((size_t)B.d, -1);
   for (size_t c = 0; c < C; ++c) local[ch.cols[c]] = (int32_t)c;
   double* bw = reinterpret_cast<double*>(blob.data());
@@ -2944,16 +2943,30 @@ int forest_upload_chunk(se_ctx* ctx, const BinState& B, const ForestChunk& ch, c
     at += (size_t)nn;
   }
   bto[T] = (int32_t)at;
-  // the previous chunk's kernel may still be reading d_forest
+}
+
+// Copies `bytes` of pageable host memory into ctx->d_forest.  Returns once the copy is done: the previous chunk's kernel
+// may still be reading d_forest before it, and the next chunk reuses it after it.
+int forest_upload(se_ctx* ctx, const unsigned char* host, size_t bytes) {
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ctx->forest_cap < (size_t)a.blob_bytes) {
+  if (ctx->forest_cap < bytes) {
     if (ctx->d_forest) cudaFree(ctx->d_forest);
     ctx->d_forest = nullptr; ctx->forest_cap = 0;
-    SE_CUDA(ctx, cudaMalloc(&ctx->d_forest, (size_t)a.blob_bytes));
-    ctx->forest_cap = (size_t)a.blob_bytes;
+    SE_CUDA(ctx, cudaMalloc(&ctx->d_forest, bytes));
+    ctx->forest_cap = bytes;
   }
-  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_forest, blob.data(), (size_t)a.blob_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_forest, host, bytes, cudaMemcpyHostToDevice, ctx->stream));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return SE_OK;
+}
+
+// Packs a chunk into ctx->d_forest and sets the layout fields of `a`.
+int forest_upload_chunk(se_ctx* ctx, const BinState& B, const ForestChunk& ch, const int32_t* offsets,
+                        const int32_t* feature, const float* threshold, const int32_t* left, const int32_t* right,
+                        const float* value, const double* weights, const int32_t* tree_class, ForestArgs& a) {
+  std::vector<unsigned char> blob;
+  forest_pack_chunk(B, ch, offsets, feature, threshold, left, right, value, weights, tree_class, a, blob);
+  SE_TRY(forest_upload(ctx, blob.data(), blob.size()));
   a.blob = ctx->d_forest;
   a.X8 = B.d8; a.ld8 = B.ld8;
   return SE_OK;
@@ -3087,6 +3100,94 @@ int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, in
   SE_TRY(end(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return check_labels(ctx);  // a leaf label that is not a class index in [0, K)
+}
+
+// The weighted median of at most 64 regression trees in one pass, the value se_tree_predict per member into SE_SLOT_P
+// followed by se_agg_run(SE_AGG_BOOSTING_REG_MEDIAN) gives (see se_abi.h).
+int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets, const int32_t* feature,
+                     const float* threshold, const int32_t* left, const int32_t* right, const float* value,
+                     const double* weights, int out_slot, int out_row) {
+  if (!ctx || !offsets || !feature || !threshold || !left || !right || !value || !weights)
+    return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= SE_FOREST_MEDIAN_MAX_TREES, SE_ERR_ARG,
+             "se_forest_median serves 1..%d trees, got %d: evaluate the members with se_tree_predict + se_agg_run",
+             SE_FOREST_MEDIAN_MAX_TREES, n_trees);
+  SE_REQUIRE(ctx, out_slot >= 0 && out_slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad out slot");
+  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
+  const SlotBuf& O = ctx->slot[out_slot];
+  SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
+  SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
+  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
+  SE_TRY(begin(ctx));
+  release_l2_persist(ctx);
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
+  const BinState& B = ctx->bins[which];
+  const size_t vals_bytes = (size_t)n_trees * kForestMedianTile * sizeof(float);
+  // chunks as large as the CTAs its registers let an SM hold can use: every chunk beyond the first re-stages its trees
+  // for each tile, and the median's registers (up to 252 at 64 trees) cap the CTAs per SM below four already
+  int ctas = 0;
+  SE_CUDA(ctx, forest_median_ctas_per_sm(n_trees, &ctas));
+  if (ctas > 4) ctas = 4;
+  const size_t budget = std::min((size_t)(216 * 1024), (size_t)(228 * 1024) / (size_t)ctas - 1024 - 512 - 16);
+  std::vector<ForestChunk> chunks;
+  SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, false, kForestMedianTile, vals_bytes, chunks, budget));
+  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
+  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
+  // every chunk's packed trees in one buffer: the kernel walks them all for each tile
+  ForestMedianArgs g;
+  g.n = X.cols;
+  g.X8 = B.d8; g.ld8 = B.ld8;
+  g.M = n_trees;
+  g.n_chunks = (int)chunks.size();
+  std::vector<unsigned char> all, blob;
+  size_t stage = 0;  // the largest chunk's blob + ranks
+  for (size_t k = 0; k < chunks.size(); ++k) {
+    ForestArgs a;
+    forest_pack_chunk(B, chunks[k], offsets, feature, threshold, left, right, value, nullptr, nullptr, a, blob);
+    ForestMedianChunk& c = g.chunk[k];
+    c.blob_off = (int)all.size(); c.blob_bytes = a.blob_bytes;
+    c.T = a.T; c.C = a.C; c.t0 = chunks[k].t0;
+    c.off_coloff = a.off_coloff; c.off_nodes = a.off_nodes; c.off_treeoff = a.off_treeoff; c.off_values = a.off_values;
+    all.insert(all.end(), blob.begin(), blob.end());  // blob_bytes is a multiple of 16: every chunk stays aligned
+    stage = std::max(stage, (size_t)a.blob_bytes + (size_t)a.C * kForestMedianTile);
+  }
+  g.vals_off = (int)forest_pad(stage, 16);
+  SE_TRY(forest_upload(ctx, all.data(), all.size()));
+  g.blob = ctx->d_forest;
+  // the weights as se_agg_run takes them: the fast path when every weight is finite and >= 0 (without a margin when
+  // they are all equal), the exact sort for every row otherwise
+  g.mode = 0;
+  if (ctx->wm_fast) {
+    bool ok = true, equal = true;
+    for (int t = 0; t < n_trees; ++t) {
+      ok = ok && (weights[t] >= 0.0) && (weights[t] <= 1.7976931348623157e308);
+      equal = equal && (weights[t] == weights[0]);
+    }
+    if (ok) g.mode = equal ? 2 : 1;
+  }
+  g.total = 0.0;
+  for (int m = 0; m < kForestMedianMaxTrees; ++m) {
+    g.w[m] = (m < n_trees) ? weights[m] : 0.0;
+    g.total += g.w[m];  // model order, like the kernel's own sums
+  }
+  g.tau = (g.mode == 1) ? 8.0 * (double)n_trees * 1.1102230246251565e-16 * g.total : -1.0;
+  if (g.mode == 1) {
+    if (ctx->wm_alloc < 1) {
+      if (ctx->d_wm) cudaFree(ctx->d_wm);
+      ctx->d_wm = nullptr;
+      SE_CUDA(ctx, cudaMalloc(&ctx->d_wm, sizeof(unsigned int)));
+      ctx->wm_alloc = 1;
+    }
+    SE_CUDA(ctx, cudaMemsetAsync(ctx->d_wm, 0, sizeof(unsigned int), ctx->stream));
+    g.deferred = ctx->d_wm;
+  }
+  g.out = O.d + (int64_t)out_row * (O.rows > 1 ? O.ld : O.cols);
+  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_forest_median(g, (size_t)g.vals_off + vals_bytes, ctx->sms, ctx->stream));
+  ctx->last_wm_mode = g.mode;
+  ctx->last_forest_chunks = (int)chunks.size();
+  ctx->last_tree_binned = 1;
+  return end(ctx);
 }
 
 int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,

@@ -307,6 +307,34 @@ struct ForestAggArgs {
   int* bad_label = nullptr;
 };
 cudaError_t launch_forest_agg(const ForestAggArgs& a, int sms, cudaStream_t s);
+// The weighted median of a forest of at most 64 regression trees in ONE pass (se_forest_median, se_agg.cu): a CTA walks
+// every chunk of trees over its 128-row tile in turn, re-staging the chunk's packed trees and ranks as
+// forest_predict_kernel stages them, and keeps each row's M leaf values in its own column of shared memory
+// ([M][kForestMedianTile] fp32 at vals_off) until the last chunk; the median is then taken as agg_wmedian_fast_kernel
+// takes it, and the rows inside its rounding margin (mode 1) or every row (mode 0) by wm_exact_pick on the same values.
+constexpr int kForestMedianTile = 128;
+constexpr int kForestMedianMaxTrees = 64;  // SE_FOREST_MEDIAN_MAX_TREES
+struct ForestMedianChunk {
+  int blob_off = 0, blob_bytes = 0;  // the chunk's packed trees at blob + blob_off (ForestArgs layout, multiple of 16)
+  int T = 0, C = 0, t0 = 0;          // its trees are t0 .. t0 + T - 1 of the forest, over C local columns
+  int off_coloff = 0, off_nodes = 0, off_treeoff = 0, off_values = 0;
+};
+struct ForestMedianArgs {
+  const uint8_t* X8 = nullptr;
+  int64_t n = 0, ld8 = 0;
+  const unsigned char* blob = nullptr;
+  int n_chunks = 0, M = 0;
+  int vals_off = 0;               // shared-memory byte offset of the leaf values: past every chunk's blob and ranks
+  int mode = 0;                   // 0: exact sort for every row; 1: fast path + margin; 2: all weights equal, no margin
+  double total = 0.0, tau = -1.0; // Σ weights in model order, the margin 8·M·2⁻⁵³·total (mode 1)
+  double w[kForestMedianMaxTrees] = {};
+  ForestMedianChunk chunk[kForestMedianMaxTrees];
+  unsigned int* deferred = nullptr;  // mode 1: counts the rows resolved by the exact sort (nullable)
+  float* out = nullptr;
+};
+cudaError_t launch_forest_median(const ForestMedianArgs& a, size_t smem, int sms, cudaStream_t s);
+// CTAs of the kernel for M trees one SM can hold by its registers alone (>= 1)
+cudaError_t forest_median_ctas_per_sm(int M, int* ctas);
 // ---- regression- and classification-tree fit over the uint8 rank matrix (se_tree_fit.cu) -----
 // Nodes are heap-indexed (root 1, children 2h, 2h + 1), so depth <= 8 needs 511 records.
 constexpr int kTreeFitHeap = 512;

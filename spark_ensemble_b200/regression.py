@@ -422,18 +422,30 @@ class BoostingRegressor(Params):
         n = y.shape[0]
         loss_type = self("lossType").lower()
         learner = self("baseLearner")
+        # A device learner fits where the boosting weights live when the features are resident.  Without
+        # residentFeatures it keeps the learner.fit route below (its own context per round) rather than raising.
+        device_fit = bool(self("residentFeatures")) and getattr(learner, "device_learner", False)
         models, est_weights, history = [], [], []
         ctx = Context(self.device)
         try:
             ctx.boostreg_configure(n)
+            if device_fit:  # X once, and the learner's split candidates once for every round
+                ctx.alloc(N.SLOT_X, X.shape[1], n)
+                ctx.upload_rowmajor(N.SLOT_X, X)
+                ctx.tree_fit_bins(learner.split_candidates(X))
+                all_cols = np.arange(X.shape[1], dtype=np.int32)
             ctx.upload(N.SLOT_Y, y)
             ctx.upload(N.SLOT_BW, np.ones(n) if w is None else w)  # :205
             sum_w = ctx.slot_sum(N.SLOT_BW)                          # :212
             i, best, done = 0, 0, False
             while i < self("numBaseLearners") and not done and sum_w > 0:  # :218
-                wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)     # :222-225
-                model = learner.fit(X, y, wn)                        # third party :231-233
-                ctx.upload(N.SLOT_PRED, model.predict(X))
+                if device_fit:  # fitted on SLOT_Y / SLOT_BW where they live, straight into SLOT_PRED; the splits are
+                    # invariant under the common 1 / sumWeights scale of :222-225
+                    model = learner.fit_resident(ctx, N.SLOT_Y, 0, N.SLOT_BW, 0, False, all_cols, N.SLOT_PRED, 0)
+                else:
+                    wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)  # :222-225
+                    model = learner.fit(X, y, wn)                     # third party :231-233
+                    ctx.upload(N.SLOT_PRED, model.predict(X))
                 max_error = ctx.boostreg_max_error()                 # :235-238
                 if max_error == 0:                                   # :240-243
                     best, done = i, True
@@ -483,7 +495,8 @@ class BoostingRegressionModel(Params):
 
     def _aggregate_resident(self, X, median: bool) -> np.ndarray | None:
         """Members evaluated over the device-resident features when every one is a tree: the weighted mean in one
-        forest pass; for the median each tree writes its row of SLOT_P on the device before the aggregation."""
+        forest pass, and the median of at most 64 trees too (se_forest_median).  Above 64 trees, or when the rank
+        matrix cannot hold the thresholds, each tree writes its row of SLOT_P on the device before the aggregation."""
         trees = _device_trees(self, self.models)
         if trees is None:
             return None
@@ -491,6 +504,15 @@ class BoostingRegressionModel(Params):
             s = _forest_sum_resident(self, X, trees, None, self.weights, 0.0)
             return None if s is None else s / float(np.sum(self.weights))
         n = X.shape[0]
+        if len(trees) <= N.FOREST_MEDIAN_MAX_TREES:
+            with _resident_context(self.device, X) as ctx:
+                ctx.alloc(N.SLOT_RAW, 1, n)
+                try:
+                    ctx.forest_median(trees, N.SLOT_RAW, self.weights)
+                    return ctx.download(N.SLOT_RAW).astype(np.float64)
+                except N.NativeError as e:
+                    if not _rank_matrix_full(e):
+                        raise
         with _resident_context(self.device, X) as ctx:
             ctx.agg_configure(N.AGG_BOOSTING_REG_MEDIAN, len(trees), 0, 1, 0, n)
             for i, t in enumerate(trees):
