@@ -43,9 +43,8 @@ for n in (100_000_000, 50_000_000, 25_000_000, 12_500_000, 6_250_000):
     ctx.copy_slot(N.SLOT_H, N.SLOT_F)   # h = 0.5 y + N(0, 0.5)
     ctx.fill(N.SLOT_F, 0.0)
     ctx.gbm_pseudo_residuals(False)
-    for fused, l2m, res in ((1, 0, 1), (1, 0, 0), (0, 0, 1)):
+    for fused, res in ((1, 1), (1, 0), (0, 1)):
         ctx.set_option("fused_round", fused)
-        ctx.set_option("fused_l2_mode", l2m)
         ctx.set_option("fused_resident", res)
         ctx.set_option("fused_timing", 0)
         for _ in range(5):
@@ -61,7 +60,7 @@ for n in (100_000_000, 50_000_000, 25_000_000, 12_500_000, 6_250_000):
         for _ in range(50):
             ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
         kt = ctx.kernel_times(); ctx.kernel_timing(False)
-        out = {"rows": n, "fused": fused, "l2_mode": l2m, "fused_resident": res, "wall_us_per_round": wall,
+        out = {"rows": n, "fused": fused, "fused_resident": res, "wall_us_per_round": wall,
                "kernel_event_us": {k: 1e3 * v["ms"] / v["launches"] for k, v in kt.items()}}
         if fused:
             ctx.set_option("fused_timing", 1)

@@ -38,20 +38,16 @@ def main():
     args = ap.parse_args()
     ctx = Context(0)
     res = []
-    print("persisting L2 max", ctx.get_option("l2_persist_max_bytes") / 1e6, "MB; window max",
-          ctx.get_option("l2_window_max_bytes") / 1e6, "MB", flush=True)
     for n in args.rows:
         ctx.gbm_configure(n, 0, 1, args.loss, 0.0, False)
         ctx.fill_synthetic(N.SLOT_Y, "bernoulli", 1, 0.4, 1.0)
         ctx.fill(N.SLOT_F, 0.0)
         ctx.fill_synthetic(N.SLOT_H, "normal", 3, 0.0, 1.0)
         variants = [("per-eval launches (round 1)", dict(ls_mode=0)),
-                    ("persistent", dict(ls_mode=1, l2_persist=0, ls_resident=1, ls_ctas_per_sm=4)),
-                    ("persistent no-resident", dict(ls_mode=1, l2_persist=0, ls_resident=0, ls_ctas_per_sm=4)),
-                    ("persistent 3 CTAs/SM", dict(ls_mode=1, l2_persist=0, ls_resident=1, ls_ctas_per_sm=3)),
-                    ("persistent 2 CTAs/SM", dict(ls_mode=1, l2_persist=0, ls_resident=1, ls_ctas_per_sm=2)),
-                    ("persistent + L2 persisting window (carve-out released after each search)",
-                     dict(ls_mode=1, l2_persist=1, ls_resident=1, ls_ctas_per_sm=4))]
+                    ("persistent", dict(ls_mode=1, ls_resident=1, ls_ctas_per_sm=4)),
+                    ("persistent no-resident", dict(ls_mode=1, ls_resident=0, ls_ctas_per_sm=4)),
+                    ("persistent 3 CTAs/SM", dict(ls_mode=1, ls_resident=1, ls_ctas_per_sm=3)),
+                    ("persistent 2 CTAs/SM", dict(ls_mode=1, ls_resident=1, ls_ctas_per_sm=2))]
         for name, opts in variants:
             ctx.fill(N.SLOT_F, 0.0)
             for k, v in opts.items():
@@ -63,7 +59,7 @@ def main():
             ctx.kernel_timing(False)
             r = {"rows": n, "loss": args.loss, "variant": name, "ms_per_round": ms, "evals": ev,
                  "kernel_ms_per_round": {k: v["ms"] / (args.rounds + 2) for k, v in kt.items()},
-                 "workers": ctx.get_option("last_ls_workers"), "hit_ratio": ctx.get_option("last_ls_hit_ratio")}
+                 "workers": ctx.get_option("last_ls_workers")}
             res.append(r)
             print(json.dumps(r), flush=True)
     for n in args.squared_rows:
@@ -71,10 +67,7 @@ def main():
         ctx.fill_synthetic(N.SLOT_Y, "normal", 1, 0.0, 1.0)
         ctx.fill_synthetic(N.SLOT_H, "normal", 3, 0.0, 1.0)
         for name, opts in (("two launches + host Brent", dict(fused_round=0)),
-                           ("one cooperative launch, no prefetch", dict(fused_round=1, fused_ctas_per_sm=3, fused_prefetch_mb=0)),
-                           ("one cooperative launch, prefetch 32 MB", dict(fused_round=1, fused_ctas_per_sm=3, fused_prefetch_mb=32)),
-                           ("one cooperative launch, prefetch 64 MB", dict(fused_round=1, fused_ctas_per_sm=3, fused_prefetch_mb=64)),
-                           ("one cooperative launch, prefetch 96 MB", dict(fused_round=1, fused_ctas_per_sm=3, fused_prefetch_mb=96))):
+                           ("one cooperative launch", dict(fused_round=1, fused_ctas_per_sm=3))):
             ctx.fill(N.SLOT_F, 0.0)
             ctx.gbm_pseudo_residuals(False)
             for k, v in opts.items():

@@ -115,20 +115,20 @@ SE_API int se_ctx_kernel_timing(se_ctx* ctx, int on);
 SE_API int se_ctx_kernel_time(se_ctx* ctx, int family, double* total_ms, int64_t* launches);
 SE_API int se_ctx_kernel_time_reset(se_ctx* ctx);
 /* Tunables and diagnostics by name (doubles).  Settable: "fused_round" (-1 auto by shard size / 0 / 1: squared-loss
- * round in ONE cooperative launch), "fused_round_max_rows", "fused_ctas_per_sm", "fused_prefetch_mb", "fused_resident" (that
+ * round in ONE cooperative launch), "fused_round_max_rows", "fused_ctas_per_sm", "fused_resident" (that
  * round, reading the residual without a bag, carries its statistics pass's tail into the update in shared memory
  * [default 1]), "ls_mode" (non-squared Brent line
  * search: 0 = one launch per evaluation, 1 = one persistent launch with Brent on the device [default], 2 = host Brent
  * over single-evaluation launches of the persistent kernel — bit-identical to 1, for tests), "ls_resident",
- * "ls_ctas_per_sm", "ls_ring" (cp.async ring stages for the streamed tiles, 0 = register prefetch [default]), "l2_persist", "l2_persist_frac", "peer_timeout_ms" (spin bound of the fused peer exchange,
+ * "ls_ctas_per_sm", "peer_timeout_ms" (spin bound of the fused peer exchange,
  * 0 = forever), "alternate_passes", "l2_hints", "ctas_per_sm", "host_mirror", "tree_bins" (uint8 rank matrix for tree
  * walks), "tree_mask" (all-nodes kernel for trees of <= 64 internal nodes), "wm_fast" (weighted median, M <= 64 and
  * weights >= 0: keys-only sort + margin-checked model-order sums, exact kernel for the deferred rows), "wm_list_cap"
  * (deferred-row list capacity, 0 = rows / 4).  Read-only: "last_tree_binned", "last_tree_mask", "last_wm_mode" (0 exact,
  * 1 fast with margin, 2 equal weights), "last_wm_deferred" (synchronises), "last_round_fused",
- * "last_ls_workers", "last_ls_passes", "last_ls_hit_ratio", "last_fused_grid", "last_fused_resident_tiles" (tiles per
- * CTA the last one-launch round carried in shared memory), "l2_persist_max_bytes",
- * "l2_window_max_bytes".  Unknown keys fail with SE_ERR_ARG. */
+ * "last_ls_workers", "last_ls_passes", "last_ls_hit_ratio" (kept for compatibility, always 0), "last_fused_grid",
+ * "last_fused_resident_tiles" (tiles per CTA the last one-launch round carried in shared memory).  Unknown keys fail
+ * with SE_ERR_ARG. */
 SE_API int se_ctx_set_option(se_ctx* ctx, const char* key, double value);
 SE_API int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value);
 /* pinned (page-locked) host memory for the buffers handed to se_upload/se_download (JNI: wrap in a

@@ -109,7 +109,7 @@ class Context:
         self._ck(self._lib.se_ctx_kernel_time_reset(self._h))
 
     def set_option(self, key: str, value: float):
-        """Tunables by name (se_ctx_set_option): fused_round, ls_mode, l2_persist, peer_timeout_ms, ..."""
+        """Tunables by name (se_ctx_set_option): fused_round, ls_mode, ls_resident, peer_timeout_ms, ..."""
         self._ck(self._lib.se_ctx_set_option(self._h, key.encode(), float(value)))
 
     def get_option(self, key: str) -> float:

@@ -206,31 +206,20 @@ struct se_ctx {
   int fused_round = -1;               // squared-loss round in one launch: -1 by shard size, 0 off, 1 on
   int64_t fused_round_max_rows = (int64_t)1 << 40;  // no size limit by default
   int fused_ctas_per_sm = 3;
-  double fused_prefetch_mb = 0.0;     // off by default
   int fused_loss_reduce = 0;          // 1: reduce the train loss over the rows even when the closed form applies
-  int fused_l2_mode = 0;              // experiment: 1 = evict_last on r/h, 2 = persisting window over r
   int fused_timing = 0;               // diagnostic: in-kernel %globaltimer stamps of the fused round
   int fused_resident = 1;             // residual rounds reading r carry the statistics pass's tail in shared memory
   double last_fused_resident_tiles = 0.0;  // tiles per CTA the last fused round carried in shared memory
-  double last_fused_us[3] = {0, 0, 0};  // statistics phase, fold+exchange+Brent, update phase    // L2 budget of the update-phase prefetch issued while the grid waits for the step
+  double last_fused_us[3] = {0, 0, 0};  // statistics phase, fold+exchange+Brent, update phase
   int ls_mode = 1;                    // non-squared line search: 0 one launch per evaluation (round-1 kernels), 1 one
                                       // persistent launch (device Brent), 2 host Brent over single-evaluation launches of
                                       // the persistent kernel (bit-identity check of mode 1)
   int ls_resident = 1;                // workers keep their first tiles in shared memory
   int ls_ctas_per_sm = 4;
-  int ls_ring = 0;                    // cp.async ring stages for the streamed tiles (0 off = register prefetch, 2..4)
-  int l2_persist = 0;                 // mark the packed line-search view as L2-persisting.  OFF by default: while a
-                                      // carve-out is configured, every STREAMING kernel works with a smaller L2
-  size_t l2_persist_max = 0;          // cudaDevAttrMaxPersistingL2CacheSize
-  size_t l2_window_max = 0;           // cudaDevAttrMaxAccessPolicyWindowSize
-  size_t l2_persist_set = 0;          // current cudaLimitPersistingL2CacheSize
-  double l2_persist_frac = 0.75;      // fraction of the persisting carve-out the window is sized for
-  bool l2_persist_dirty = false;      // persisting lines may be resident: reset before unrelated kernels
   int clock_khz = 1965000;
   double peer_timeout_ms = 120000.0;  // spin bound of the fused peer exchange (0 = wait forever)
   // diagnostics of the last call (se_ctx_get_option)
   int last_round_fused = 0, last_ls_workers = 0, last_ls_resident = 0, last_ls_passes = 0, last_fused_grid = 0;
-  double last_ls_hit_ratio = 0.0;
   double last_round_stats[3] = {0.0, 0.0, 0.0};
   // newton updates: SE_SLOT_WOUT holds 1/2 hc w; the 1/S_j of each dimension is applied on download
   std::vector<float> wout_scale;
@@ -596,19 +585,6 @@ int for_segments(se_ctx* ctx, const SlotBuf& s, int64_t count, int64_t offset, F
   return SE_OK;
 }
 
-// Release L2 lines a previous line search marked as persisting (they would otherwise keep occupying the carve-out
-// while unrelated kernels stream through a smaller L2).
-int release_l2_persist(se_ctx* ctx) {
-  if (!ctx->l2_persist_dirty) return SE_OK;
-  ctx->l2_persist_dirty = false;
-  cudaCtxResetPersistingL2Cache();
-  // the carve-out itself (not only the lines in it) slows streaming kernels down: give the L2 back
-  cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, 0);
-  ctx->l2_persist_set = 0;
-  cudaGetLastError();
-  return SE_OK;
-}
-
 int ensure_counts(se_ctx* ctx) {
   if (ctx->gbm.counts_valid) return SE_OK;
   SE_CUDA(ctx, cudaSetDevice(ctx->device));  // callers may run before begin(): launches below need the right device
@@ -745,18 +721,10 @@ int se_ctx_create(int device, se_ctx** out) {
   SE_CREATE_CUDA(cudaMalloc(&ctx->d_fsync, sizeof(FusedSync)));
   SE_CREATE_CUDA(cudaMemset(ctx->d_fsync, 0, sizeof(FusedSync)));
   ctx->clock_khz = prop.clockRate > 0 ? prop.clockRate : 1965000;
-  {
-    int v = 0;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxPersistingL2CacheSize, device) == cudaSuccess && v > 0) ctx->l2_persist_max = (size_t)v;
-    if (cudaDeviceGetAttribute(&v, cudaDevAttrMaxAccessPolicyWindowSize, device) == cudaSuccess && v > 0) ctx->l2_window_max = (size_t)v;
-    cudaGetLastError();
-  }
   if (const char* s = getenv("SE_FUSED_ROUND")) ctx->fused_round = atoi(s) != 0 ? 1 : 0;
   if (const char* s = getenv("SE_FUSED_RESIDENT")) ctx->fused_resident = atoi(s) != 0;
   if (const char* s = getenv("SE_LS_MODE")) { const int v = atoi(s); if (v >= 0 && v <= 2) ctx->ls_mode = v; }
   if (const char* s = getenv("SE_LS_RESIDENT")) ctx->ls_resident = atoi(s) != 0;
-  if (const char* s = getenv("SE_LS_RING")) { const int v = atoi(s); if (v >= 0 && v <= 4) ctx->ls_ring = v; }
-  if (const char* s = getenv("SE_L2_PERSIST")) ctx->l2_persist = atoi(s) != 0;
   if (const char* s = getenv("SE_PEER_TIMEOUT_MS")) { const double v = atof(s); if (v >= 0.0) ctx->peer_timeout_ms = v; }
   SE_CREATE_CUDA(cudaHostAlloc(&ctx->h_mirror, sizeof(double) * (kMboxPayload + 8), cudaHostAllocMapped));
   memset(ctx->h_mirror, 0, sizeof(double) * (kMboxPayload + 8));
@@ -911,24 +879,23 @@ int se_ctx_kernel_time_reset(se_ctx* ctx) {
 
 namespace {
 struct OptKey { const char* name; int id; };
-enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_L2_MODE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_PREFETCH_MB, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS, OPT_LS_RING, OPT_L2_PERSIST,
-       OPT_L2_PERSIST_FRAC, OPT_PEER_TIMEOUT_MS, OPT_ALTERNATE, OPT_L2_HINTS, OPT_CTAS_PER_SM, OPT_HOST_MIRROR,
+enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS,
+       OPT_PEER_TIMEOUT_MS, OPT_ALTERNATE, OPT_L2_HINTS, OPT_CTAS_PER_SM, OPT_HOST_MIRROR,
        // read-only diagnostics
        OPT_LAST_ROUND_FUSED, OPT_LAST_LS_WORKERS, OPT_LAST_LS_PASSES, OPT_LAST_LS_HIT_RATIO, OPT_LAST_FUSED_GRID,
-       OPT_LAST_FUSED_RESIDENT, OPT_L2_PERSIST_MAX, OPT_L2_WINDOW_MAX, OPT_LAST_STAT0, OPT_LAST_STAT1, OPT_LAST_STAT2 };
+       OPT_LAST_FUSED_RESIDENT, OPT_LAST_STAT0, OPT_LAST_STAT1, OPT_LAST_STAT2 };
 const OptKey kOpts[] = {
   {"last_forest_chunks", OPT_LAST_FOREST_CHUNKS}, {"wm_fast", OPT_WM_FAST}, {"wm_list_cap", OPT_WM_LIST_CAP}, {"last_wm_mode", OPT_LAST_WM_MODE}, {"last_wm_deferred", OPT_LAST_WM_DEFERRED},
   {"tree_bins", OPT_TREE_BINS}, {"tree_mask", OPT_TREE_MASK}, {"last_tree_mask", OPT_LAST_TREE_MASK}, {"last_tree_binned", OPT_LAST_TREE_BINNED}, {"last_tree_rebinned_cols", OPT_LAST_TREE_REBINNED},
-  {"fused_loss_reduce", OPT_FUSED_LOSS_REDUCE}, {"fused_l2_mode", OPT_FUSED_L2_MODE}, {"fused_timing", OPT_FUSED_TIMING}, {"last_fused_stats_us", OPT_LAST_FUSED_US0}, {"last_fused_brent_us", OPT_LAST_FUSED_US1},
-  {"last_fused_update_us", OPT_LAST_FUSED_US2}, {"fused_prefetch_mb", OPT_FUSED_PREFETCH_MB}, {"fused_round", OPT_FUSED_ROUND}, {"fused_round_max_rows", OPT_FUSED_MAX_ROWS}, {"fused_ctas_per_sm", OPT_FUSED_CTAS},
+  {"fused_loss_reduce", OPT_FUSED_LOSS_REDUCE}, {"fused_timing", OPT_FUSED_TIMING}, {"last_fused_stats_us", OPT_LAST_FUSED_US0}, {"last_fused_brent_us", OPT_LAST_FUSED_US1},
+  {"last_fused_update_us", OPT_LAST_FUSED_US2}, {"fused_round", OPT_FUSED_ROUND}, {"fused_round_max_rows", OPT_FUSED_MAX_ROWS}, {"fused_ctas_per_sm", OPT_FUSED_CTAS},
   {"fused_resident", OPT_FUSED_RESIDENT},
-  {"ls_mode", OPT_LS_MODE}, {"ls_resident", OPT_LS_RESIDENT}, {"ls_ctas_per_sm", OPT_LS_CTAS}, {"ls_ring", OPT_LS_RING}, {"l2_persist", OPT_L2_PERSIST},
-  {"l2_persist_frac", OPT_L2_PERSIST_FRAC}, {"peer_timeout_ms", OPT_PEER_TIMEOUT_MS}, {"alternate_passes", OPT_ALTERNATE},
+  {"ls_mode", OPT_LS_MODE}, {"ls_resident", OPT_LS_RESIDENT}, {"ls_ctas_per_sm", OPT_LS_CTAS},
+  {"peer_timeout_ms", OPT_PEER_TIMEOUT_MS}, {"alternate_passes", OPT_ALTERNATE},
   {"l2_hints", OPT_L2_HINTS}, {"ctas_per_sm", OPT_CTAS_PER_SM}, {"host_mirror", OPT_HOST_MIRROR},
   {"last_round_fused", OPT_LAST_ROUND_FUSED}, {"last_ls_workers", OPT_LAST_LS_WORKERS}, {"last_ls_passes", OPT_LAST_LS_PASSES},
   {"last_ls_hit_ratio", OPT_LAST_LS_HIT_RATIO}, {"last_fused_grid", OPT_LAST_FUSED_GRID},
   {"last_fused_resident_tiles", OPT_LAST_FUSED_RESIDENT},
-  {"l2_persist_max_bytes", OPT_L2_PERSIST_MAX}, {"l2_window_max_bytes", OPT_L2_WINDOW_MAX},
   {"last_round_stat0", OPT_LAST_STAT0}, {"last_round_stat1", OPT_LAST_STAT1}, {"last_round_stat2", OPT_LAST_STAT2},
 };
 int opt_id(const char* key) {
@@ -951,16 +918,11 @@ int se_ctx_set_option(se_ctx* ctx, const char* key, double value) {
     case OPT_TREE_MASK: ctx->tree_mask = iv != 0; break;
     case OPT_WM_FAST: ctx->wm_fast = iv != 0; break;
     case OPT_WM_LIST_CAP: SE_REQUIRE(ctx, value >= 0 && value < 2147483000.0, SE_ERR_ARG, "wm_list_cap in [0, 2^31)"); ctx->wm_list_cap = (int64_t)value; break;
-    case OPT_FUSED_L2_MODE: SE_REQUIRE(ctx, iv >= 0 && iv <= 2, SE_ERR_ARG, "fused_l2_mode in {0,1,2}"); ctx->fused_l2_mode = iv; if (iv != 2) release_l2_persist(ctx); break;
-    case OPT_FUSED_PREFETCH_MB: SE_REQUIRE(ctx, value >= 0.0 && value <= 512.0, SE_ERR_ARG, "fused_prefetch_mb in [0,512]"); ctx->fused_prefetch_mb = value; break;
     case OPT_FUSED_CTAS: SE_REQUIRE(ctx, iv >= 1 && iv <= 8, SE_ERR_ARG, "fused_ctas_per_sm in [1,8]"); ctx->fused_ctas_per_sm = iv; break;
     case OPT_FUSED_RESIDENT: ctx->fused_resident = iv != 0; break;
     case OPT_LS_MODE: SE_REQUIRE(ctx, iv >= 0 && iv <= 2, SE_ERR_ARG, "ls_mode in {0,1,2}"); ctx->ls_mode = iv; break;
     case OPT_LS_RESIDENT: ctx->ls_resident = iv != 0; break;
-    case OPT_LS_RING: SE_REQUIRE(ctx, iv >= 0 && iv <= 4, SE_ERR_ARG, "ls_ring in [0,4]"); ctx->ls_ring = iv; break;
     case OPT_LS_CTAS: SE_REQUIRE(ctx, iv >= 1 && iv <= 8, SE_ERR_ARG, "ls_ctas_per_sm in [1,8]"); ctx->ls_ctas_per_sm = iv; break;
-    case OPT_L2_PERSIST: ctx->l2_persist = iv != 0; break;
-    case OPT_L2_PERSIST_FRAC: SE_REQUIRE(ctx, value > 0.0 && value <= 1.0, SE_ERR_ARG, "l2_persist_frac in (0,1]"); ctx->l2_persist_frac = value; break;
     case OPT_PEER_TIMEOUT_MS: SE_REQUIRE(ctx, value >= 0.0, SE_ERR_ARG, "peer_timeout_ms >= 0"); ctx->peer_timeout_ms = value; break;
     case OPT_ALTERNATE: ctx->alternate = iv != 0; break;
     case OPT_L2_HINTS: ctx->l2_hints = value < 0 ? -1 : (iv != 0); break;
@@ -976,7 +938,6 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
   switch (opt_id(key)) {
     case OPT_FUSED_ROUND: *value = ctx->fused_round; break;
     case OPT_FUSED_MAX_ROWS: *value = (double)ctx->fused_round_max_rows; break;
-    case OPT_FUSED_PREFETCH_MB: *value = ctx->fused_prefetch_mb; break;
     case OPT_FUSED_TIMING: *value = ctx->fused_timing; break;
     case OPT_FUSED_LOSS_REDUCE: *value = ctx->fused_loss_reduce; break;
     case OPT_TREE_BINS: *value = ctx->tree_bins; break;
@@ -1000,7 +961,6 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_TREE_MASK: *value = ctx->last_tree_mask; break;
     case OPT_LAST_TREE_BINNED: *value = ctx->last_tree_binned; break;
     case OPT_LAST_TREE_REBINNED: *value = ctx->last_tree_rebinned_cols; break;
-    case OPT_FUSED_L2_MODE: *value = ctx->fused_l2_mode; break;
     case OPT_LAST_FUSED_US0: *value = ctx->last_fused_us[0]; break;
     case OPT_LAST_FUSED_US1: *value = ctx->last_fused_us[1]; break;
     case OPT_LAST_FUSED_US2: *value = ctx->last_fused_us[2]; break;
@@ -1008,10 +968,7 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_FUSED_RESIDENT: *value = ctx->fused_resident; break;
     case OPT_LS_MODE: *value = ctx->ls_mode; break;
     case OPT_LS_RESIDENT: *value = ctx->ls_resident; break;
-    case OPT_LS_RING: *value = ctx->ls_ring; break;
     case OPT_LS_CTAS: *value = ctx->ls_ctas_per_sm; break;
-    case OPT_L2_PERSIST: *value = ctx->l2_persist; break;
-    case OPT_L2_PERSIST_FRAC: *value = ctx->l2_persist_frac; break;
     case OPT_PEER_TIMEOUT_MS: *value = ctx->peer_timeout_ms; break;
     case OPT_ALTERNATE: *value = ctx->alternate; break;
     case OPT_L2_HINTS: *value = ctx->l2_hints; break;
@@ -1020,11 +977,9 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_ROUND_FUSED: *value = ctx->last_round_fused; break;
     case OPT_LAST_LS_WORKERS: *value = ctx->last_ls_workers; break;
     case OPT_LAST_LS_PASSES: *value = ctx->last_ls_passes; break;
-    case OPT_LAST_LS_HIT_RATIO: *value = ctx->last_ls_hit_ratio; break;
+    case OPT_LAST_LS_HIT_RATIO: *value = 0.0; break;  // kept for compatibility: no L2 window is ever requested
     case OPT_LAST_FUSED_GRID: *value = ctx->last_fused_grid; break;
     case OPT_LAST_FUSED_RESIDENT: *value = ctx->last_fused_resident_tiles; break;
-    case OPT_L2_PERSIST_MAX: *value = (double)ctx->l2_persist_max; break;
-    case OPT_L2_WINDOW_MAX: *value = (double)ctx->l2_window_max; break;
     case OPT_LAST_STAT0: *value = ctx->last_round_stats[0]; break;
     case OPT_LAST_STAT1: *value = ctx->last_round_stats[1]; break;
     case OPT_LAST_STAT2: *value = ctx->last_round_stats[2]; break;
@@ -1555,7 +1510,6 @@ int se_gbm_configure(se_ctx* ctx, int64_t n_train, int64_t n_valid, int dim, int
   g.r_current = false;
   g.wsum_valid = false; g.counts_valid = false;
   ctx->y_state[0] = ctx->y_state[1] = 0;
-  release_l2_persist(ctx);
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_Y, 1, n_train));
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_F, dim, n_train));
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_H, dim, n_train));
@@ -1830,7 +1784,7 @@ int ensure_ls_view(se_ctx* ctx) {
   if (ctx->d_ls_u) cudaFree(ctx->d_ls_u);
   ctx->d_ls_u = ctx->d_ls_v = nullptr;
   ctx->ls_cap = 0;
-  // one allocation for both halves: a single L2 access-policy window covers the whole view
+  // one allocation for both halves, v starting on a 256-byte boundary
   const size_t half = ((size_t)ctx->gbm.n + 32 + 63) / 64 * 64;
   SE_CUDA(ctx, cudaMalloc(&ctx->d_ls_u, sizeof(float) * 2 * half));
   ctx->d_ls_v = ctx->d_ls_u + half;
@@ -1873,24 +1827,6 @@ int linesearch_persist(se_ctx* ctx, double lo, double hi, double start, double r
   // tiles resident and shorten the per-evaluation rendezvous; large shards want more CTAs in flight
   cfg.max_ctas_per_sm = (ctx->ls_ctas_per_sm == 4 && ctx->gbm.n <= 8000000) ? 3 : ctx->ls_ctas_per_sm;
   cfg.resident = ctx->ls_resident;
-  cfg.ring = ctx->ls_ring;
-  ctx->last_ls_hit_ratio = 0.0;
-  if (packed && !single && ctx->l2_persist && ctx->l2_persist_max > 0 && ctx->l2_window_max > 0) {
-    if (ctx->l2_persist_set != ctx->l2_persist_max) {
-      if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, ctx->l2_persist_max) == cudaSuccess) ctx->l2_persist_set = ctx->l2_persist_max;
-      cudaGetLastError();
-    }
-    if (ctx->l2_persist_set > 0) {
-      size_t bytes = sizeof(float) * (size_t)(ctx->d_ls_v - ctx->d_ls_u) + sizeof(float) * (size_t)ctx->gbm.n;  // [u .. end of v)
-      if (bytes > ctx->l2_window_max) bytes = ctx->l2_window_max;
-      cfg.window_base = ctx->d_ls_u;
-      cfg.window_bytes = bytes;
-      const double want = ctx->l2_persist_frac * (double)ctx->l2_persist_set / (double)bytes;
-      cfg.hit_ratio = (float)(want > 1.0 ? 1.0 : want);
-      ctx->last_ls_hit_ratio = cfg.hit_ratio;
-      ctx->l2_persist_dirty = true;
-    }
-  }
   int workers = 0;
   SE_LAUNCH_T(ctx, SE_KF_EVAL, launch_gbm_linesearch_persist(lossid, a, ctx->sms, cfg, ctx->stream, &workers));
   ctx->last_ls_workers = workers;
@@ -1907,7 +1843,6 @@ int linesearch_persist(se_ctx* ctx, double lo, double hi, double start, double r
     ctx->last_fused_us[1] = ctx->h_scal[kScalRound + 21];  // fold + exchange + Brent step
     ctx->last_fused_us[2] = 0.0;
   }
-  release_l2_persist(ctx);
   if (rc != SE_OK) return rc;
   if (alpha) *alpha = res[0];
   if (loss) *loss = res[1];
@@ -1963,7 +1898,7 @@ int se_gbm_linesearch_brent(se_ctx* ctx, double lo, double hi, double start, dou
   // every one of Brent's 20-40 evaluations then reads 8 B/row instead of 12 — same values bit for bit
   // (multiplying by ±1 is exact and fma is sign-symmetric).
   const bool pack = (ctx->gbm.loss == SE_LOSS_BERNOULLI || ctx->gbm.loss == SE_LOSS_EXPONENTIAL) && max_eval >= 8 &&
-                    !ctx->gbm.use_bag && getenv("SE_NO_LS_PACK") == nullptr;
+                    !ctx->gbm.use_bag;
   if (pack) {
     SE_CUDA(ctx, cudaSetDevice(ctx->device));
     SE_TRY(ensure_ls_view(ctx));
@@ -1978,50 +1913,6 @@ int se_gbm_linesearch_brent(se_ctx* ctx, double lo, double hi, double start, dou
   if (rc != SE_OK) return fail(ctx, rc, "Brent exceeded MaxEval(%d)", max_eval);
   return SE_OK;
 }
-
-namespace {
-// Squared loss: statistics kernel -> Brent on the device over the exact parabola (se_brent.cu, same template and
-// rounding as the host line search) -> fused update reading alpha from device memory.  Three launches back to back,
-// one host synchronisation per round (for alpha, the evaluation count and the train loss) instead of two.  Opt-in
-// (SE_DEVICE_BRENT=1, see se_gbm_round).
-int round_squared_device_brent(se_ctx* ctx, double learning_rate, double tol, int max_iter, int flags, double* alpha,
-                               double* loss_sum, int* n_eval) {
-  SE_TRY(ensure_wsum(ctx));
-  SE_TRY(begin(ctx));
-  SE_TRY(settle_f(ctx));
-  GbmArgs a = gbm_args(ctx, false);
-  a.stats_from_r = ctx->gbm.r_current ? 1 : 0;
-  a.ws = red_ws(ctx, kScalRound);  // stats -> d_scal[kScalRound..+2], summed across GPUs
-  SE_LAUNCH_T(ctx, SE_KF_SQ_STATS, launch_gbm(SE_LOSS_SQUARED, GBM_SQ_STATS, a, ctx->ctas_per_sm, ctx->sms, ctx->stream));
-  SE_TRY(allreduce_dev(ctx, kScalRound, 3));
-  double* out_dev = ctx->d_scal + kScalRound + 4;
-  const bool mirror = ctx->use_mirror && ctx->h_mirror && (ctx->nranks <= 1 || ctx->p2p);
-  constexpr int kMirrorBrent = 32;  // mirror slots [32..34]: above what any reducing kernel writes before its ticket
-  SE_LAUNCH(ctx, launch_brent_parabola(ctx->d_scal + kScalRound, ctx->gbm.wsum, 0.0, 100.0, 1.0, tol, tol, max_iter,
-                                       out_dev, mirror ? ctx->d_mirror + kMirrorBrent : nullptr, ctx->stream));
-  GbmArgs u = gbm_args(ctx, false);
-  u.dev_alpha = out_dev;
-  u.lr64 = learning_rate;
-  const int mode = (flags & SE_UPD_RESIDUAL) ? GBM_UPDATE_RESID : GBM_UPDATE;
-  u.ws = red_ws(ctx);
-  SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm(SE_LOSS_SQUARED, mode, u, ctx->ctas_per_sm, ctx->sms, ctx->stream));
-  ctx->gbm.r_current = (mode != GBM_UPDATE);
-  double ls = 0.0;
-  SE_TRY(fetch_scalars(ctx, 0, 1, &ls));  // the line-search results were written before this kernel's ticket
-  double res[3];
-  if (mirror) {
-    for (int i = 0; i < 3; ++i) res[i] = ctx->h_mirror[kMirrorBrent + i];
-  } else {
-    SE_CUDA(ctx, cudaMemcpyAsync(res, out_dev, sizeof(res), cudaMemcpyDeviceToHost, ctx->stream));
-    SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  }
-  if (res[2] < 0.0) return fail(ctx, SE_ERR_OPT, "Brent exceeded MaxEval(%d)", max_iter);
-  if (alpha) *alpha = res[0];
-  if (loss_sum) *loss_sum = ls;
-  if (n_eval) *n_eval = (int)res[2];
-  return SE_OK;
-}
-}  // namespace
 
 namespace {
 // Squared loss, one cooperative launch per round (se_gbm_fused.cu): statistics -> cross-GPU sum -> Brent -> update +
@@ -2078,31 +1969,10 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   a.host_res = mirror ? ctx->d_mirror + kMirrorRound : nullptr;
   a.sync = ctx->d_fsync;
   a.epoch = ++ctx->fused_epoch;
-  {
-    // tiles of 16 KB per array; two arrays (r and h, or y and F) are prefetched: 32 KB per tile, over at most
-    // fused_ctas_per_sm * sms CTAs
-    const double per_cta = ctx->fused_prefetch_mb * 1e6 / (32768.0 * (double)(ctx->fused_ctas_per_sm * ctx->sms));
-    a.prefetch_tiles = per_cta < 0.0 ? 0 : (per_cta > 64.0 ? 64 : (int)(per_cta + 0.5));
-  }
   a.timing = ctx->fused_timing;
-  a.l2_mode = ctx->fused_l2_mode == 1 ? 1 : 0;
   int grid = 0, resident_slots = 0;
-  void* wbase = nullptr;
-  size_t wbytes = 0;
-  if (ctx->fused_l2_mode == 2 && ctx->l2_persist_max > 0 && ctx->l2_window_max > 0) {
-    wbytes = sizeof(float) * (size_t)g.n;
-    if (wbytes > ctx->l2_window_max) wbytes = ctx->l2_window_max;
-    if (wbytes > ctx->l2_persist_max) wbytes = ctx->l2_persist_max;
-    if (ctx->l2_persist_set != wbytes) {
-      if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, wbytes) == cudaSuccess) ctx->l2_persist_set = wbytes;
-      cudaGetLastError();
-    }
-    wbase = a.r;
-    ctx->l2_persist_dirty = true;
-  }
   SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->fused_resident, ctx->sms,
-                                                           ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots,
-                                                           wbase, wbytes));
+                                                           ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots));
   ctx->last_fused_grid = grid;
   ctx->last_fused_resident_tiles = resident_slots / 4.0;  // float4 groups per thread, U_SQ = 4 to a tile
   ctx->gbm.r_current = write_r != 0;
@@ -2152,15 +2022,11 @@ int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, i
     // With a communicator it needs the fused peer exchange (an NCCL all-reduce cannot run inside the kernel).
     const bool can = (ctx->nranks <= 1 || ctx->p2p);
     const bool want = ctx->fused_round > 0 || (ctx->fused_round < 0 && ctx->gbm.n <= ctx->fused_round_max_rows);
-    if (can && want && getenv("SE_DEVICE_BRENT") == nullptr) {
+    if (can && want) {
       ctx->last_round_fused = 1;
       return round_squared_fused(ctx, learning_rate, tol, max_iter, flags, alpha, loss_sum, n_eval);
     }
   }
-  // SE_DEVICE_BRENT=1: three launches (statistics, one-thread Brent, update) with one host synchronisation; kept as an
-  // experiment switch — the fused round above supersedes it.
-  if (sq_search && getenv("SE_DEVICE_BRENT") != nullptr)
-    return round_squared_device_brent(ctx, learning_rate, tol, max_iter, flags, alpha, loss_sum, n_eval);
   double a = 1.0, obj = 0.0;
   int ne = 0;
   if (optimized) SE_TRY(se_gbm_linesearch_brent(ctx, 0.0, 100.0, 1.0, tol, tol, max_iter, &a, &obj, &ne));
@@ -2358,7 +2224,6 @@ int se_boost_configure(se_ctx* ctx, int64_t n, int num_classes, int real) {
 }
 
 static BoostArgs boost_args(se_ctx* ctx, double sum_w) {
-  release_l2_persist(ctx);
   ensure_labels_checked(ctx, 0, ctx->boost.K, ctx->boost.n);  // SAMME / SAMME.R compare (and index with) the label
   BoostArgs a;
   a.y = ctx->slot[SE_SLOT_Y].d;
@@ -2422,7 +2287,6 @@ int se_boostreg_configure(se_ctx* ctx, int64_t n) {
 }
 
 static BoostRegArgs boostreg_args(se_ctx* ctx, double sum_w, int loss_type, double max_error, bool exchange = true) {
-  release_l2_persist(ctx);
   BoostRegArgs a;
   a.y = ctx->slot[SE_SLOT_Y].d;
   a.pred = ctx->slot[SE_SLOT_PRED].d;
@@ -2510,7 +2374,6 @@ int se_agg_run(se_ctx* ctx, const double* weights, const double* init) {
   SE_REQUIRE(ctx, ctx->agg.on, SE_ERR_STATE, "se_agg_configure first");
   const auto& g = ctx->agg;
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   AggArgs a;
   a.kind = g.kind; a.M = g.M; a.K = g.K; a.dim = g.dim; a.loss = g.loss; a.n = g.n;
   a.P = ctx->slot[SE_SLOT_P].d; a.ld = ctx->slot[SE_SLOT_P].rows > 1 ? ctx->slot[SE_SLOT_P].ld : ctx->slot[SE_SLOT_P].cols;
@@ -2719,7 +2582,6 @@ static int tree_predict_impl(se_ctx* ctx, int which, int n_nodes, const int32_t*
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
   SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row + n_out <= O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   int32_t* hf = reinterpret_cast<int32_t*>(ctx->h_small);
   float* ht = reinterpret_cast<float*>(hf + n_nodes);
@@ -2988,7 +2850,6 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
   SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
   const BinState& B = ctx->bins[which];
@@ -3044,7 +2905,6 @@ int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, in
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_PROB, out_c, n));
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_LABEL, 1, n));
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
   const BinState& B = ctx->bins[which];
@@ -3119,7 +2979,6 @@ int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets
   SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
   const BinState& B = ctx->bins[which];
@@ -3200,7 +3059,6 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
   SE_REQUIRE(ctx, O.d && out_row >= 0 && out_row < O.rows && O.cols == X.cols, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
   if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -3242,7 +3100,6 @@ int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const floa
     }
   }
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   BinState& B = ctx->bins[0];
   SE_REQUIRE(ctx, bins_ensure(B, X), SE_ERR_CUDA, "no device memory for the rank matrix (%lld x %lld bytes)",
              (long long)X.rows, (long long)X.cols);
@@ -3319,7 +3176,6 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   }
   const int nb = std::min(256, maxc + 2);  // ranks 0..maxc, then NaN (rank 255) in the last bin
   SE_TRY(begin(ctx));
-  release_l2_persist(ctx);
   if (label_slot == SE_SLOT_F || weight_slot == SE_SLOT_F || is_yfr(out_slot)) SE_TRY(settle_f(ctx));
   if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   SE_TRY(bins_rerank(ctx, B, X));  // X was rewritten since the candidates were set

@@ -1,8 +1,8 @@
 // se_brent.h — Brent's univariate minimiser, commons-math3 3.6.1 BrentOptimizer semantics (call site
 // regression/GBMRegressor.scala:311,413-421), as ONE host/device template so that the host line search
-// (se_gbm_linesearch_brent, se_brent_minimize) and the on-device line search of the squared-loss round
-// (se_brent.cu, compiled with -fmad=false so that no multiply-add is contracted) execute the same IEEE operations
-// in the same order and return the same iterates bit for bit.
+// (se_gbm_linesearch_brent, se_brent_minimize) and the on-device line searches of the one-launch squared-loss round
+// and the persistent line search (se_gbm_fused.cu, compiled with -fmad=false so that no multiply-add is contracted)
+// execute the same IEEE operations in the same order and return the same iterates bit for bit.
 // Golden-section fallback, parabolic interpolation when the fit lies inside the bracket and is shrinking, never
 // evaluates closer than tol1 = rel*|x| + abs to a previous abscissa, stops when |x - mid| <= 2*tol1 - (hi-lo)/2;
 // returns the best point evaluated.

@@ -63,11 +63,6 @@ __device__ __forceinline__ uint64_t l2_policy(bool evict_first) {
   else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 __device__ __forceinline__ float4 ld_stream4_p(const float* p, uint64_t pol) {
   float4 v;
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0,%1,%2,%3}, [%4], %5;"

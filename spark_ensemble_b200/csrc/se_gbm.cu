@@ -61,7 +61,6 @@ __global__ void __launch_bounds__(kBlock, LossTune<LOSS>::kMinCtas) gbm_scalar_k
   constexpr int U = LossTune<LOSS>::kU;
   float coef = a.coef[0];
   if (T::kWriteF && a.dev_stats != nullptr) coef = device_step(a);
-  if (T::kWriteF && a.dev_alpha != nullptr) coef = (float)(a.lr64 * *a.dev_alpha);  // same rounding as the host path
   const float param = a.param;
   const bool has_w = (a.w != nullptr);
   // bag multiplicities (row sub-sampling, GBMRegressor.scala:357-359): the line search and newton's Σh run on

@@ -19,9 +19,9 @@
 //  * gbm_linesearch_persist_kernel — Brent's <= MaxEval evaluations of the line-search objective
 //    (boosting/GBMLoss.scala:50-74 through RDDLossFunction; GBMRegressor.scala:408-421) for the non-squared scalar
 //    losses in ONE launch: worker CTAs own a fixed set of tiles, keep the first of them in SHARED MEMORY for the whole
-//    search (132 SMs x ~190 KB = 25 MB on an H100 that never touch HBM again) and stream the rest (the caller marks the packed
-//    view as L2-persisting); a coordinator warp folds the per-CTA partials in a fixed order, performs the cross-GPU
-//    sum, advances Brent and publishes the next abscissa.  The first evaluation of the binary losses also BUILDS the
+//    search (132 SMs x ~190 KB = 25 MB on an H100 that never touch HBM again) and stream the rest; a coordinator
+//    warp folds the per-CTA partials in a fixed order, performs the cross-GPU sum, advances Brent and publishes the
+//    next abscissa.  The first evaluation of the binary losses also BUILDS the
 //    signed view u = (2y-1)F, v = (2y-1)h (exact sign flips: later evaluations read 8 B/row and are bit-identical to
 //    evaluating on (y, F, h)).
 //
@@ -130,12 +130,8 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   // before it in shared memory: every group from p_res on is carried to phase B.
   const int64_t S = FROM_R ? min((int64_t)a.resident_slots, (cnt > 0 ? cnt - 1 : 0) * U) : 0;
   const int64_t p_res = (cnt - 1) * U - S;
-  // l2_mode 1: r and h are the arrays worth keeping between phases / rounds (r: written by the update, read by the
-  // next statistics pass; h: read by both phases) -> evict_last; y and F stream through -> evict_first
   const uint64_t pol_stream = l2_policy(a.l2_hints != 0);
-  const uint64_t pol_keep = (a.l2_mode == 1) ? l2_policy_evict_last() : l2_policy(false);
-  const uint64_t pol_r_in = (a.l2_mode == 1) ? pol_keep : pol_stream;
-  const uint64_t pol_h_b = (a.l2_mode == 1) ? pol_keep : pol_stream;
+  const uint64_t pol_keep = l2_policy(false);
   // carried groups are served from chip in phase B: their L2 lines go first, so that the L2 keeps the groups before
   // them, which phase B reads next
   const uint64_t pol_carried = l2_policy(true);
@@ -153,11 +149,11 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       if (ok[u]) {
         if constexpr (FROM_R) {
           const bool carried = i * U + u >= p_res;
-          vy[u] = ld_rw4_p(a.r + 4 * g, carried ? pol_carried : pol_r_in);
+          vy[u] = ld_rw4_p(a.r + 4 * g, carried ? pol_carried : pol_stream);
           vh[u] = ld_stream4_p(a.h + 4 * g, carried ? pol_carried : pol_keep);
         } else {
           if (stats_from_r) {
-            vy[u] = ld_rw4_p(a.r + 4 * g, pol_r_in);  // read again and rewritten by phase B
+            vy[u] = ld_rw4_p(a.r + 4 * g, pol_stream);  // read again and rewritten by phase B
           } else {
             vy[u] = ld_stream4_p(a.y + 4 * g, pol_keep);
             vF[u] = ld_rw4_p(a.F + 4 * g, pol_keep);
@@ -259,7 +255,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
           vy[u] = ld_stream4_p(a.y + 4 * g, pol_stream);
           vF[u] = ld_rw4_p(a.F + 4 * g, pol_stream);
         }
-        vh[u] = ld_stream4_p(a.h + 4 * g, pol_h_b);  // the update is h's last reader
+        vh[u] = ld_stream4_p(a.h + 4 * g, pol_stream);  // the update is h's last reader
       }
     }
   };
@@ -267,42 +263,21 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   // in flight while the last CTA reduces, exchanges and runs Brent (FROM_R: still in registers from phase A)
   if (!FROM_R && i >= 0) load_tile(i);
   if (threadIdx.x == 0) {
-    // The wait (partials fold + cross-GPU exchange + ~30 dependent fp64 Brent iterations) is turned into
-    // useful HBM time: every CTA pulls the ranges its next update tiles read (r and h, or y and F) into the L2 with
-    // bulk prefetches (one instruction per 16 KB), bounded so that the whole grid stays within a.prefetch_tiles tiles
-    // per CTA.
-    const float* pf0 = from_r ? a.r : a.y;
-    const float* pf1 = from_r ? a.h : a.F;
-    int64_t pf = i - 1;
     if constexpr (FROM_R) {
-      // nothing of the carried tail is loaded: the loads issued before the wait are those of the first tile phase B
-      // reads from global memory (its groups below p_res)
-      pf = p_res > 0 ? (p_res - 1) / U : -1;
+      // nothing of the carried tail is loaded: while the grid waits for the step, the first tile phase B reads from
+      // global memory (its groups below p_res) is pulled into the L2 with bulk prefetches of r and h
+      const int64_t pf = p_res > 0 ? (p_res - 1) / U : -1;
       if (pf >= 0) {
         const int64_t g0 = (blockIdx.x + pf * G) * tile;
         int64_t groups = (p_res - pf * U) * kBlock;
         if (groups > n4 - g0) groups = n4 - g0;
         if (groups > 0) {
-          prefetch_l2_bulk(pf0 + 4 * g0, (unsigned int)(groups * 16));
-          prefetch_l2_bulk(pf1 + 4 * g0, (unsigned int)(groups * 16));
+          prefetch_l2_bulk(a.r + 4 * g0, (unsigned int)(groups * 16));
+          prefetch_l2_bulk(a.h + 4 * g0, (unsigned int)(groups * 16));
         }
-        --pf;
       }
     }
-    int budget = a.prefetch_tiles;
-    while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {
-      if (budget > 0 && pf >= 0) {
-        const int64_t g0 = (blockIdx.x + pf * G) * tile;           // first float4 group of the tile
-        int64_t groups = n4 - g0;
-        if (groups > tile) groups = tile;
-        if (groups > 0) {
-          prefetch_l2_bulk(pf0 + 4 * g0, (unsigned int)(groups * 16));
-          prefetch_l2_bulk(pf1 + 4 * g0, (unsigned int)(groups * 16));
-        }
-        --pf;
-        --budget;
-      }
-    }
+    while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {}
     s_coef = (float)a.sync->x;  // same rounding as the host path: (float)(lr * alpha)
   }
   __syncthreads();
@@ -362,21 +337,6 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
 }
 
 // =================================================================================== persistent line search
-// 16-byte asynchronous global -> shared copies (LDGSTS).  Every thread copies, waits for and reads back ONLY its own
-// 16-byte slots, so the ring needs no block barrier: cp.async.wait_group orders the executing thread's own copies.
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void cp_async_wait_pending(int pending) {  // at most `pending` newest groups still in flight
-  switch (pending) {
-    case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
-    case 1: asm volatile("cp.async.wait_group 1;" ::: "memory"); break;
-    case 2: asm volatile("cp.async.wait_group 2;" ::: "memory"); break;
-    default: asm volatile("cp.async.wait_group 3;" ::: "memory"); break;
-  }
-}
-
 // Tiles hold U float4 groups per thread of NARR arrays: (u, v) for the binary losses, (y, F, h) otherwise.
 template <int LOSS>
 struct LsTraits {
@@ -410,7 +370,7 @@ __global__ void __launch_bounds__(kBlock, 4) gbm_linesearch_persist_kernel(const
   using T = LsTraits<LOSS>;
   constexpr int U = T::kU, NARR = T::kNarr;
   constexpr bool PACKED = T::kPacked;
-  extern __shared__ float4 s_dyn[];  // [ring stage][NARR][U][kBlock] then [resident][NARR][U][kBlock]
+  extern __shared__ float4 s_tiles[];  // [resident][NARR][U][kBlock]
   __shared__ double s_red[kBlock / 32];
   __shared__ double s_x;
   __shared__ int s_cmd;
@@ -487,9 +447,6 @@ __global__ void __launch_bounds__(kBlock, 4) gbm_linesearch_persist_kernel(const
   const int64_t R = cnt < a.resident_tiles ? cnt : a.resident_tiles;                           // kept in shared memory
   const float param = a.param;
   const uint64_t pol_keep = l2_policy(false);
-  const int S = a.ring_stages;
-  float4* const s_ring = s_dyn;
-  float4* const s_tiles = s_dyn + (size_t)S * NARR * U * kBlock;
 
   auto row_loss = [&](float c0, float c1, float c2, float coef) -> float {
     // PACKED: (u, v) hold the loss ARGUMENT directly (signed_scale folded in, exact): z = u + coef*v
@@ -531,36 +488,7 @@ __global__ void __launch_bounds__(kBlock, 4) gbm_linesearch_persist_kernel(const
         }
       }
     };
-    // ring: the streamed tiles of this pass travel global -> shared by cp.async, S stages ahead of the arithmetic.
-    // The first S of them are requested BEFORE the wait for the abscissa (they do not depend on it), so the
-    // coordinator's fold + exchange hides their latency.  The first evaluation of a packed loss converts (y, F, h)
-    // on the way and keeps the register path.
-    const bool ring = S > 0 && !(PACKED && first);
-    auto ring_issue = [&](int stage, int64_t i) {
-      const int64_t base = (blockIdx.x + i * (int64_t)W) * tile + tid;
-      float4* st = s_ring + (size_t)stage * NARR * U * kBlock;
-#pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const int64_t g = base + (int64_t)u * kBlock;
-        if (g >= n4) continue;
-        if constexpr (PACKED) {
-          cp_async16(&st[(0 * U + u) * kBlock + tid], a.u + 4 * g);
-          cp_async16(&st[(1 * U + u) * kBlock + tid], a.v + 4 * g);
-        } else {
-          cp_async16(&st[(0 * U + u) * kBlock + tid], a.y + 4 * g);
-          cp_async16(&st[(1 * U + u) * kBlock + tid], a.F + 4 * g);
-          cp_async16(&st[(2 * U + u) * kBlock + tid], a.h + 4 * g);
-        }
-      }
-    };
-    if (ring) {
-      for (int s = 0; s < S; ++s) {  // exactly S groups (empty ones past the end keep the wait_group count uniform)
-        if (s < nstream) ring_issue(s, stream_index(s));
-        cp_async_commit();
-      }
-    } else if (nstream > 0) {
-      load_tile(stream_index(0), first || !PACKED);
-    }
+    if (nstream > 0) load_tile(stream_index(0), first || !PACKED);
     double x;
     if (first) {
       x = a.start;
@@ -576,32 +504,8 @@ __global__ void __launch_bounds__(kBlock, 4) gbm_linesearch_persist_kernel(const
     }
     const float coef = (float)x;  // same narrowing as se_gbm_linesearch_eval
     double acc = 0.0;
-    if (ring) {
-      int stage = 0;
-      for (int64_t k = 0; k < nstream; ++k) {
-        cp_async_wait_pending(S - 1);  // group k (the oldest of the S outstanding) has landed
-        const int64_t base = (blockIdx.x + stream_index(k) * (int64_t)W) * tile + tid;
-        const float4* st = s_ring + (size_t)stage * NARR * U * kBlock;
-#pragma unroll
-        for (int u = 0; u < U; ++u) {
-          if (base + (int64_t)u * kBlock >= n4) continue;
-          float4 c[NARR];
-#pragma unroll
-          for (int q = 0; q < NARR; ++q) c[q] = st[(q * U + u) * kBlock + tid];
-          float l = 0.f;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) l += row_loss(f4at(c[0], q), f4at(c[1], q), f4at(c[NARR - 1], q), coef);
-          acc += (double)l;
-        }
-        // refill this stage only after its values were consumed (the thread's own reads precede its own new copy)
-        if (k + S < nstream) ring_issue(stage, stream_index(k + S));
-        cp_async_commit();
-        stage = (stage + 1 == S) ? 0 : stage + 1;
-      }
-      cp_async_wait_pending(0);
-    }
-    // streamed tiles, register path (the first one is already in registers)
-    for (int64_t k = 0; !ring && k < nstream; ++k) {
+    // streamed tiles (the first one is already in registers)
+    for (int64_t k = 0; k < nstream; ++k) {
       const int64_t i = stream_index(k);
       const int64_t base = (blockIdx.x + i * (int64_t)W) * tile + tid;
 #pragma unroll
@@ -726,23 +630,11 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
   int64_t budget = (int64_t)smem_cap / per_sm_ctas - 1024 - 256;
   if (budget > max_smem) budget = max_smem;
   const int64_t per_cta = (ntiles + workers - 1) / workers;
-  // ring stages for the tiles that do not stay resident: none when every tile of a worker fits in shared memory,
-  // else cfg.ring as far as the budget allows; what is left of the budget holds resident tiles.  Off by default:
-  // the ring costs resident tiles on small shards.
-  const int64_t tb = T::kTileBytes;
-  int ring = 0;
-  if (per_cta > (cfg.resident ? budget / tb : 0)) {
-    ring = cfg.ring < 0 ? 0 : (cfg.ring > 4 ? 4 : cfg.ring);
-    if (ring == 1) ring = 2;
-    if ((int64_t)ring * tb > budget) ring = (int)(budget / tb);
-    if (ring < 2) ring = 0;
-  }
-  int64_t resident = cfg.resident ? (budget - (int64_t)ring * tb) / tb : 0;
+  int64_t resident = cfg.resident ? budget / T::kTileBytes : 0;
   if (resident > per_cta) resident = per_cta;
   if (resident < 0) resident = 0;
   a.resident_tiles = (int)resident;
-  a.ring_stages = ring;
-  const size_t dyn = (size_t)(resident + ring) * T::kTileBytes;
+  const size_t dyn = (size_t)resident * T::kTileBytes;
   // the occupancy with this much dynamic shared memory must still cover the grid (cooperative launch would fail)
   int blocks = 0;
   cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, kBlock, dyn);
@@ -753,22 +645,11 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
   lc.blockDim = dim3(kBlock);
   lc.dynamicSmemBytes = dyn;
   lc.stream = st;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeCooperative;
-  attrs[na].val.cooperative = 1;
-  ++na;
-  if (cfg.window_bytes > 0 && cfg.window_base != nullptr) {
-    attrs[na].id = cudaLaunchAttributeAccessPolicyWindow;
-    attrs[na].val.accessPolicyWindow.base_ptr = cfg.window_base;
-    attrs[na].val.accessPolicyWindow.num_bytes = cfg.window_bytes;
-    attrs[na].val.accessPolicyWindow.hitRatio = cfg.hit_ratio;
-    attrs[na].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attrs[na].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    ++na;
-  }
-  lc.attrs = attrs;
-  lc.numAttrs = na;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeCooperative;
+  attr.val.cooperative = 1;
+  lc.attrs = &attr;
+  lc.numAttrs = 1;
   if (workers_out) *workers_out = (int)workers;
   return cudaLaunchKernelEx(&lc, kern, a);
 }
@@ -776,8 +657,7 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
 }  // namespace
 
 cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int loss_reduce, int resident, int sms,
-                                      int max_ctas_per_sm, cudaStream_t st, int* grid_out, int* resident_slots_out,
-                                      void* window_base, size_t window_bytes) {
+                                      int max_ctas_per_sm, cudaStream_t st, int* grid_out, int* resident_slots_out) {
   constexpr int kKerns = 6;
   void (*kerns[kKerns])(const SqRoundArgs) = {
       gbm_round_sq_fused_kernel<false, false, false>, gbm_round_sq_fused_kernel<false, true, false>,
@@ -854,21 +734,11 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
   lc.blockDim = dim3(kBlock);
   lc.dynamicSmemBytes = dyn;
   lc.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeCooperative;
-  attr[0].val.cooperative = 1;  // co-residency of all CTAs is what makes the in-kernel flag wait deadlock-free
-  int na = 1;
-  if (window_base != nullptr && window_bytes > 0) {
-    attr[na].id = cudaLaunchAttributeAccessPolicyWindow;
-    attr[na].val.accessPolicyWindow.base_ptr = window_base;
-    attr[na].val.accessPolicyWindow.num_bytes = window_bytes;
-    attr[na].val.accessPolicyWindow.hitRatio = 1.0f;
-    attr[na].val.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    attr[na].val.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    ++na;
-  }
-  lc.attrs = attr;
-  lc.numAttrs = na;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeCooperative;
+  attr.val.cooperative = 1;  // co-residency of all CTAs is what makes the in-kernel flag wait deadlock-free
+  lc.attrs = &attr;
+  lc.numAttrs = 1;
   if (grid_out) *grid_out = (int)grid;
   if (resident_slots_out) *resident_slots_out = (int)slots;
   return cudaLaunchKernelEx(&lc, kerns[which], a);

@@ -40,9 +40,6 @@ struct GbmArgs {
   // squared-loss device-resident step: step = lr * clip(stats[1]/stats[2], 0, 100) when non-null
   const double* dev_stats = nullptr;
   float lr = 1.f;
-  // step = (float)(lr64 * *dev_alpha) when non-null: alpha comes from the on-device line search (se_brent.cu)
-  const double* dev_alpha = nullptr;
-  double lr64 = 1.0;
   int stats_from_r = 0;  // squared-loss statistics read the current residual slot r = y - F (8 B/row) instead of y, F (12 B/row)
   int l2_hints = 0; // L2-sized shard: evict_first for the arrays the next pass does not re-read (se_common.cuh)
   int reverse = 0; // walk the tiles from the end: consecutive passes alternate direction so the tail of one
@@ -71,10 +68,6 @@ struct GenericArgs {
 cudaError_t launch_gbm_logloss_generic(int mode, const GbmArgs& a, const GenericArgs& ga, int grid, cudaStream_t stream);
 // LogLoss(K), wide K: 2-D TMA tiles of 256 rows x K classes, four rows per thread (se_gbm_tiled.cu)
 cudaError_t launch_gbm_logloss_tiled(int mode, const GbmArgs& a, int sms, cudaStream_t stream);
-// squared-loss line search on the device: Brent over the parabola of stats[0..2]; out[0] = alpha, out[1] = objective,
-// out[2] = evaluations (negative: MaxEval exceeded); out_host (mapped pinned memory) is optional
-cudaError_t launch_brent_parabola(const double* stats, double wsum, double lo, double hi, double start, double rel,
-                                  double abs_tol, int max_eval, double* out_dev, double* out_host, cudaStream_t stream);
 // squared-loss round result: out[0] = alpha*, computed on device from stats (for se_gbm_round_result)
 cudaError_t launch_sq_alpha(const double* stats, double* out_alpha, cudaStream_t stream);
 
@@ -102,9 +95,7 @@ struct SqRoundArgs {
   int64_t n = 0;
   int stats_from_r = 0;
   int l2_hints = 0;
-  int l2_mode = 0;         // 0: evict_normal / evict_first hints; 1: evict_last on r and h (experiment)
   int timing = 0;          // write %globaltimer stamps (us) to out[10..13]: start, statistics folded, step published, end
-  int prefetch_tiles = 0;  // update-phase tiles (r/h, or y/F) each CTA prefetches into L2 while it waits for the step
   int resident_slots = 0;  // set by the launcher: float4 groups of r and h per thread carried in shared memory
   double lr = 1.0, wsum = 1.0;                                   // learning rate, Σw (objective scale)
   double lo = 0.0, hi = 100.0, start = 1.0, rel = 1e-6, abs_tol = 1e-6;
@@ -121,8 +112,7 @@ struct SqRoundArgs {
   unsigned long long epoch = 0;
 };
 cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a, int write_r, int loss_reduce, int resident, int sms,
-                                      int max_ctas_per_sm, cudaStream_t stream, int* grid_out, int* resident_slots_out,
-                                      void* window_base = nullptr, size_t window_bytes = 0);
+                                      int max_ctas_per_sm, cudaStream_t stream, int* grid_out, int* resident_slots_out);
 
 // Brent's whole line search for a dim-1 scalar loss in one launch (persistent workers + coordinator warp).
 struct LsArgs {
@@ -140,7 +130,6 @@ struct LsArgs {
   int single = 0;        // evaluate the objective at `start` once (host-driven search over the same kernel)
   int first_parity = 0;  // tile direction of evaluation e is (first_parity + e) & 1
   int resident_tiles = 0;
-  int ring_stages = 0;   // > 0: streamed tiles go through a per-thread cp.async ring of this many stages in shared memory
   double* partials = nullptr;
   FusedSync* sync = nullptr;
   unsigned long long epoch0 = 0;
@@ -149,11 +138,7 @@ struct LsArgs {
 };
 struct LsLaunch {
   int max_ctas_per_sm = 4;
-  int resident = 1;             // keep each worker's first tiles in shared memory
-  int ring = 0;                 // cp.async ring stages for the streamed tiles: 0 off (register prefetch), 2..4
-  void* window_base = nullptr;  // L2 access-policy window (persisting) over the packed view
-  size_t window_bytes = 0;
-  float hit_ratio = 0.f;
+  int resident = 1;  // keep each worker's first tiles in shared memory
 };
 bool gbm_linesearch_persist_supported(int loss);
 bool gbm_linesearch_persist_packed(int loss);

@@ -827,51 +827,6 @@ def test_gbm_round_single_call(ctx, oracle, rng):
     ctx.set_option("fused_round", -1)
 
 
-def test_device_brent_matches_host_brent(oracle, rng, monkeypatch):
-    """Squared loss: with SE_DEVICE_BRENT=1 se_gbm_round runs Brent on the device over the parabola of the sufficient
-    statistics (se_brent.cu: the same template as the host line search, compiled without multiply-add contraction).
-    alpha, the evaluation count, the train loss and the updated F / R must equal the host line search bit for bit,
-    for interior minima, both interval ends and several tolerances."""
-    from spark_ensemble_b200 import _native as N
-    from spark_ensemble_b200.context import Context
-    monkeypatch.setenv("SE_ALTERNATE_PASSES", "0")  # one tile direction: sums do not depend on the call history
-    c = Context(0)
-    c.set_option("fused_round", 0)  # compare the three-launch device search with the two-launch host search
-    try:
-        n = 50021
-        for case, (scale, shift, tol) in enumerate([(1.0, 0.0, 1e-6), (0.01, 0.0, 1e-6), (-1.0, 0.0, 1e-6),
-                                                    (3.0, 0.5, 1e-9), (1e-3, 0.0, 1e-4), (0.3, -2.0, 1e-12)]):
-            y = f32(rng.standard_normal(n))
-            F = f32(0.3 * rng.standard_normal(n) + shift)
-            h = f32(scale * (y - F) + 0.1 * rng.standard_normal(n))
-            out = []
-            for host in (False, True):
-                c.gbm_configure(n, 0, 1, "squared", 0.0, False)
-                c.upload(N.SLOT_Y, y); c.upload(N.SLOT_F, F); c.upload(N.SLOT_H, h)
-                if host:
-                    monkeypatch.delenv("SE_DEVICE_BRENT", raising=False)
-                else:
-                    monkeypatch.setenv("SE_DEVICE_BRENT", "1")
-                a, l, ne = c.gbm_round(0.7, True, tol, 100, residual=True)
-                out.append((a, l, ne, c.download(N.SLOT_F).copy(), c.download(N.SLOT_R).copy()))
-            monkeypatch.delenv("SE_DEVICE_BRENT", raising=False)
-            (a1, l1, ne1, F1, r1), (a2, l2, ne2, F2, r2) = out
-            assert (a1, ne1, l1) == (a2, ne2, l2), (case, a1, a2, ne1, ne2, l1, l2)
-            np.testing.assert_array_equal(F1, F2)
-            np.testing.assert_array_equal(r1, r2)
-            assert ne1 >= 3
-        # MaxEval exceeded: both paths raise (commons-math: TooManyEvaluationsException)
-        for host in (False, True):
-            c.gbm_configure(n, 0, 1, "squared", 0.0, False)
-            c.upload(N.SLOT_Y, y); c.upload(N.SLOT_F, F); c.upload(N.SLOT_H, h)
-            if not host:
-                monkeypatch.setenv("SE_DEVICE_BRENT", "1")
-            with pytest.raises(N.NativeError):
-                c.gbm_round(0.7, True, 1e-12, 2, residual=True)
-        monkeypatch.delenv("SE_DEVICE_BRENT", raising=False)
-    finally:
-        c.close()
-
 def test_squared_stats_from_residual_slot(ctx, oracle, rng):
     """Squared loss: when R holds the current residual (after pseudo_residuals or a fused update) the line-search
     statistics are read from (r, h) — 8 B/row — and are bit-identical to the (y, F, h) pass; any write to
@@ -912,12 +867,12 @@ def test_brent_packed_line_search_view_is_bit_identical(oracle, rng, name, weigh
     ctx = Context(0)
     ctx.set_option("ls_mode", 0)  # the one-launch-per-evaluation path (the persistent search has its own test)
     try:
-        _packed_vs_plain(ctx, oracle, rng, name, weighted_bag, monkeypatch, N)
+        _packed_vs_plain(ctx, oracle, rng, name, weighted_bag, N)
     finally:
         ctx.close()
 
 
-def _packed_vs_plain(ctx, oracle, rng, name, weighted_bag, monkeypatch, N):
+def _packed_vs_plain(ctx, oracle, rng, name, weighted_bag, N):
     n = 40013
     dim, par, y, F, h, w = setup_gbm(ctx, rng, name, n, weighted_bag)
     r, _, _ = oracle.pseudo_residuals(O.LOSS_IDS[name], par, 1, y, None, F, False)
@@ -926,10 +881,10 @@ def _packed_vs_plain(ctx, oracle, rng, name, weighted_bag, monkeypatch, N):
     if weighted_bag:
         ctx.gbm_set_bag(rng.poisson(1.0, n).astype(np.float32))
     packed = ctx.gbm_linesearch_brent()
-    monkeypatch.setenv("SE_NO_LS_PACK", "1")
-    plain = ctx.gbm_linesearch_brent()
-    monkeypatch.delenv("SE_NO_LS_PACK")
-    assert packed == plain
+    # the same host Brent over plain (y, F, h) evaluations: se_gbm_linesearch_eval outside a search reads (y, F, h)
+    rc, *plain = _host_brent(lambda x: ctx.gbm_linesearch_eval([x], want_grad=False)[0])
+    assert rc == 0
+    assert packed == tuple(plain)
     assert packed[2] >= 8
 
 
@@ -1075,15 +1030,15 @@ LS_LOSSES = ["absolute", "huber", "quantile", "logcosh", "scaledlogcosh", "berno
 
 
 @pytest.mark.parametrize("name", LS_LOSSES)
-@pytest.mark.parametrize("n,ctas,resident,ring", [(3, 4, 1, 0), (2049, 4, 1, 0), (40013, 4, 1, 0), (700001, 1, 0, 3),
-                                                  (700001, 1, 0, 0), (700001, 1, 1, 0), (2000003, 2, 1, 0),
-                                                  (2000003, 4, 0, 2), (2000003, 4, 0, 4), (5000011, 4, 1, 3)])
-def test_device_line_search_matches_host_brent(ctx, oracle, rng, name, n, ctas, resident, ring):
+@pytest.mark.parametrize("n,ctas,resident", [(3, 4, 1), (2049, 4, 1), (40013, 4, 1), (700001, 1, 0), (700001, 1, 1),
+                                             (2000003, 2, 1), (2000003, 4, 0), (5000011, 4, 0), (5000011, 4, 1),
+                                             (9000011, 4, 1)])
+def test_device_line_search_matches_host_brent(ctx, oracle, rng, name, n, ctas, resident):
     """Brent's whole line search in ONE persistent launch (workers + coordinator warp, tiles resident in shared
     memory, the first evaluation builds the signed view of the binary losses).  ls_mode 2 runs the HOST Brent over
     single-evaluation launches of the same kernel: alpha, the objective and the evaluation count must be identical
-    bit for bit.  Tiles that do not stay resident stream through a per-thread cp.async ring (`ls_ring` stages; 0 = the
-    register prefetch).  Against the oracle: the objective value at the minimiser within 1e-5."""
+    bit for bit.  Tiles that do not stay resident are streamed through registers, one tile ahead; above 8 M rows the
+    default of 4 CTAs per SM applies (3 below).  Against the oracle: the objective value at the minimiser within 1e-5."""
     from spark_ensemble_b200 import _native as N
     dim, par, y, F, h, w = setup_gbm(ctx, rng, name, n, weighted=(n % 2 == 0))
     lid = O.LOSS_IDS[name]
@@ -1092,7 +1047,6 @@ def test_device_line_search_matches_host_brent(ctx, oracle, rng, name, n, ctas, 
     ctx.upload(N.SLOT_H, h)
     ctx.set_option("ls_ctas_per_sm", ctas)
     ctx.set_option("ls_resident", resident)
-    ctx.set_option("ls_ring", ring)
     try:
         ctx.set_option("ls_mode", 1)
         dev = ctx.gbm_linesearch_brent()
@@ -1125,12 +1079,13 @@ def test_device_line_search_matches_host_brent(ctx, oracle, rng, name, n, ctas, 
         ctx.set_option("ls_mode", 1)
         ctx.set_option("ls_ctas_per_sm", 4)
         ctx.set_option("ls_resident", 1)
-        ctx.set_option("ls_ring", 0)
 
 
-def test_options_roundtrip(ctx):
+def test_options_roundtrip_and_removed_keys(ctx):
+    """Settable keys read back what was set; read-only and unknown keys are refused, and so are the keys of the
+    experiment paths that no longer exist.  last_ls_hit_ratio stays readable for compatibility and is always 0."""
     from spark_ensemble_b200 import _native as N
-    for key, val in (("fused_round", 1), ("ls_mode", 2), ("peer_timeout_ms", 2500.0), ("l2_persist_frac", 0.5)):
+    for key, val in (("fused_round", 1), ("ls_mode", 2), ("peer_timeout_ms", 2500.0), ("ls_ctas_per_sm", 2)):
         old = ctx.get_option(key)
         ctx.set_option(key, val)
         assert ctx.get_option(key) == val
@@ -1139,7 +1094,13 @@ def test_options_roundtrip(ctx):
         ctx.set_option("no_such_option", 1)
     with pytest.raises(ValueError):
         ctx.set_option("last_round_fused", 1)  # read-only
-    assert ctx.get_option("l2_persist_max_bytes") >= 0
+    for key in ("fused_l2_mode", "fused_prefetch_mb", "ls_ring", "l2_persist", "l2_persist_frac",
+                "l2_persist_max_bytes", "l2_window_max_bytes"):
+        with pytest.raises(ValueError):
+            ctx.set_option(key, 0)
+        with pytest.raises(ValueError):
+            ctx.get_option(key)
+    assert ctx.get_option("last_ls_hit_ratio") == 0.0
 
 
 @pytest.mark.parametrize("bad", [-1.0, "K", 2.5, float("nan")])
