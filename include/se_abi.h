@@ -154,6 +154,11 @@ SE_API int se_comm_info(const se_ctx* ctx, int* nranks, int* rank);
 SE_API int se_comm_allreduce_host(se_ctx* ctx, double* values, int count);
 
 /* ---- slots ---------------------------------------------------------------------------------- */
+/* Any write to a slot through this ABI drops what the context derived from the slot's old contents: the current
+ * residual (Y, F, R), the line search's weight sum (W, BAG), the labels' class-index check (Y, VY), se_download's 1/S
+ * factor (WOUT) and the tree walks' rank matrix (X, VX).  An owed F (se_gbm_round) is rebuilt before Y, F or R change.
+ * Writes are: upload, fill, copy (destination), alloc, free, the device pointer of se_slot_info, and the rows the model
+ * calls (se_tree_predict*, se_forest_predict, se_forest_median, se_linear_predict) and the tree fits write. */
 SE_API int se_slot_alloc(se_ctx* ctx, int slot, int64_t count);               /* count fp32 elements */
 /* [rows][cols] slot; rows > 1 get a padded row stride `ld` (multiple of 32 floats = 128 B) so every
  * row starts 128-bit aligned.  se_upload/se_download offsets are LOGICAL (row*cols + col). */
@@ -209,7 +214,7 @@ SE_API int se_gbm_linesearch_eval(se_ctx* ctx, const double* alpha, double* loss
 /* squared loss only: the three sufficient statistics of the line-search parabola in one pass,
  * stats = {Σ(y-F)², Σh(y-F), Σh², weightSum}; objective(α) = (s0 - 2α s1 + α² s2) / (2 s3).
  * When SE_SLOT_R is current (after se_gbm_pseudo_residuals or a fused update) the pass reads r = y-F and h only
- * (8 B/row, bit-identical); any write to Y/F/R through this ABI reverts to reading y, F, h (12 B/row). */
+ * (8 B/row, bit-identical); otherwise it reads y, F, h (12 B/row). */
 SE_API int se_gbm_linesearch_stats(se_ctx* ctx, double* stats4);
 /* F_j += step_j·H_j (GBMRegressor.scala:437-441; GBMClassifier.scala:437-448), fused with what the
  * next round needs: flags select extra outputs computed from the NEW F in the same pass. */
@@ -232,9 +237,8 @@ SE_API int se_gbm_linesearch_brent(se_ctx* ctx, double lo, double hi, double sta
  * Same results as se_gbm_linesearch_brent + se_gbm_update, up to rounding; saves the host round-trips between them.
  * SE_SLOT_F after a squared-loss round in one launch (fused_round) with SE_UPD_RESIDUAL: the round writes only
  * R = r - weight·H and F is held as Y - R.  It is rebuilt (F = y - r, then R = y - F) the first time a call reads
- * SE_SLOT_F, writes SE_SLOT_Y, SE_SLOT_F or SE_SLOT_R, or hands out their device pointer (se_slot_info); reading R,
- * Y or H does not rebuild it.  The values are what the update computes, up to rounding: r - c·h and y - r instead of
- * F + c·h and y - F'.  A round that fails with SE_ERR_OPT (MaxEval) leaves F and R as they were. */
+ * SE_SLOT_F or writes SE_SLOT_Y, SE_SLOT_F or SE_SLOT_R (see the slots section); reading R, Y or H does not rebuild
+ * it.  The values are what the update computes, up to rounding: r - c·h and y - r instead of F + c·h and y - F'.  A round that fails with SE_ERR_OPT (MaxEval) leaves F and R as they were. */
 SE_API int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, int max_iter, int flags,
                         double* alpha, double* loss_sum, int* n_eval);
 /* Opt-in fast line search for dim == 1 losses with a hessian (squared, bernoulli, exponential, logcosh): each
@@ -415,7 +419,7 @@ enum se_tree_out { SE_TREE_OUT_LABEL = 0, SE_TREE_OUT_PROBA = 1 };
 /* Fits one classification tree: Spark's DecisionTreeClassifier (gini or entropy impurity, continuous features,
  * level-wise best split over the candidates of se_tree_fit_bins, prune = true), restated in DESIGN.md §3.  The
  * arguments are se_tree_fit's, plus: labels are class indices 0..num_classes-1 (clamped into that range on the device;
- * SE_SLOT_Y is validated once per upload and the call fails with SE_ERR_ARG on a bad label); 2 <= num_classes <= 64.
+ * SE_SLOT_Y is validated once per write and the call fails with SE_ERR_ARG on a bad label); 2 <= num_classes <= 64.
  * A node's statistics are fp64 rawCount Σ c and class weights n_k = Σ c·w over its rows of label k.  A weight row that
  * is a common multiple of the intended weights (e.g. SE_SLOT_BW, not divided by Σw) gives the same splits up to rounding.
  * Pruning merges two leaf children with equal labels into a leaf with that label and the PARENT's class weights.

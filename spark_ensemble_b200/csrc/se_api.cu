@@ -96,7 +96,7 @@ constexpr int kSmallBytes = 1 << 20;  // small device scratch: weights, init, tr
 
 struct SlotBuf {
   float* d = nullptr;
-  int64_t rows = 0, cols = 0, ld = 0;
+  int64_t rows = 0, cols = 0, ld = 0;  // ld: row stride in floats, cols itself when rows == 1
   size_t bytes = 0;
 };
 
@@ -179,7 +179,7 @@ struct se_ctx {
   int* h_p2p_err = nullptr;
   int* h_bad_label = nullptr;         // raised by kernels that met a label / vote outside [0, K) (mapped pinned memory)
   int* d_bad_label = nullptr;
-  // labels used as class indices are validated once per upload: 0 unknown, 1 validation launched (result not yet
+  // labels used as class indices are validated once per write: 0 unknown, 1 validation launched (result not yet
   // observed), 2 known good — per label slot (SE_SLOT_Y, SE_SLOT_VY) together with the K they were checked for
   int y_state[2] = {0, 0};
   int y_state_k[2] = {0, 0};
@@ -508,16 +508,26 @@ int settle_f(se_ctx* ctx) {
   return SE_OK;
 }
 
-bool is_yfr(int slot) { return slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R; }
-
-// any write to a feature-matrix slot makes its rank matrix stale
-void touch_slot(se_ctx* ctx, int slot) {
-  if (slot == SE_SLOT_Y) ctx->y_state[0] = 0;
-  if (slot == SE_SLOT_VY) ctx->y_state[1] = 0;
-  if (slot == SE_SLOT_WOUT) ctx->wout_scaled = false;
-  if (slot == SE_SLOT_X) ctx->bins[0].valid = false;
-  if (slot == SE_SLOT_VX) ctx->bins[1].valid = false;
+// Every entry point that writes a caller-chosen slot calls this once its own checks have passed, before the write is
+// enqueued: it drops what the context derived from the slot's old contents.  The owed F is rebuilt from Y and R first.
+// A call that derives something from the slot it writes (a walk over X into a row of X re-ranks X) calls it after that.
+int write_slot(se_ctx* ctx, int slot) {
+  switch (slot) {
+    case SE_SLOT_Y: case SE_SLOT_F: case SE_SLOT_R:
+      SE_TRY(settle_f(ctx));
+      ctx->gbm.r_current = false;
+      if (slot == SE_SLOT_Y) ctx->y_state[0] = 0;  // labels checked as class indices
+      break;
+    case SE_SLOT_VY: ctx->y_state[1] = 0; break;
+    case SE_SLOT_W: case SE_SLOT_BAG: ctx->gbm.wsum_valid = false; break;
+    case SE_SLOT_WOUT: ctx->wout_scaled = false; break;  // se_download's 1/S factor
+    case SE_SLOT_X: ctx->bins[0].valid = false; break;   // rank matrix
+    case SE_SLOT_VX: ctx->bins[1].valid = false; break;
+  }
+  return SE_OK;
 }
+
+int read_slot(se_ctx* ctx, int slot) { return slot == SE_SLOT_F ? settle_f(ctx) : SE_OK; }
 
 void free_bins(BinState& B) {
   if (B.d8) cudaFree(B.d8);
@@ -530,10 +540,9 @@ void free_bins(BinState& B) {
 
 int slot_alloc2d(se_ctx* ctx, int slot, int64_t rows, int64_t cols) {
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  touch_slot(ctx, slot);
   SE_REQUIRE(ctx, rows >= 1 && cols >= 0, SE_ERR_ARG, "bad slot shape %lld x %lld", (long long)rows,
              (long long)cols);
+  SE_TRY(write_slot(ctx, slot));
   SlotBuf& s = ctx->slot[slot];
   const int64_t ld = (rows > 1) ? ((cols + 31) / 32) * 32 : cols;
   const size_t bytes = sizeof(float) * (size_t)(rows * ld + 32);
@@ -553,6 +562,19 @@ int need_slot(se_ctx* ctx, int slot, int64_t rows, int64_t cols, const char* wha
   if (!s.d || s.rows != rows || s.cols != cols)
     return fail(ctx, SE_ERR_STATE, "%s: slot %d must hold [%lld][%lld] (has [%lld][%lld])", what,
                 slot, (long long)rows, (long long)cols, (long long)s.rows, (long long)s.cols);
+  return SE_OK;
+}
+
+// Rows [row, row + count) of a caller's output slot, n values each: records the write (write_slot) and hands out the
+// first row and the row stride (ld may be NULL).
+int out_rows(se_ctx* ctx, int slot, int row, int count, int64_t n, float** out, int64_t* ld) {
+  SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad output slot %d", slot);
+  const SlotBuf& s = ctx->slot[slot];
+  SE_REQUIRE(ctx, s.d && s.cols == n && row >= 0 && (int64_t)row + count <= s.rows, SE_ERR_STATE,
+             "output slot %d: no rows %d..%d of %lld values", slot, row, row + count - 1, (long long)n);
+  SE_TRY(write_slot(ctx, slot));
+  *out = s.d + (int64_t)row * s.ld;
+  if (ld) *ld = s.ld;
   return SE_OK;
 }
 
@@ -1204,7 +1226,7 @@ int se_slot_free(se_ctx* ctx, int slot) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
+  SE_TRY(write_slot(ctx, slot));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (ctx->slot[slot].d) SE_CUDA(ctx, cudaFree(ctx->slot[slot].d));
   ctx->slot[slot] = SlotBuf();
@@ -1217,17 +1239,13 @@ int se_slot_info(const se_ctx* ctx, int slot, void** device_ptr, int64_t* count)
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   if (slot < 0 || slot >= SE_NUM_SLOTS) return fail(nullptr, SE_ERR_ARG, "bad slot %d", slot);
   if (device_ptr) {
+    // the caller may read or write through the raw pointer
     se_ctx* mctx = const_cast<se_ctx*>(ctx);
-    // the caller may read or write through the raw pointer: F must hold its value, and everything cached about the
-    // slot's contents is dropped
-    if (is_yfr(slot) && ctx->gbm.f_owed) {
-      SE_TRY(settle_f(mctx));
-      SE_CUDA(mctx, cudaStreamSynchronize(ctx->stream));  // the caller's own stream may touch the slot next
-    }
+    const bool owed = ctx->gbm.f_owed;
+    SE_TRY(write_slot(mctx, slot));
+    // F was just rebuilt: the caller's own stream may touch the slot next
+    if (owed && !ctx->gbm.f_owed) SE_CUDA(mctx, cudaStreamSynchronize(ctx->stream));
     *device_ptr = ctx->slot[slot].d;
-    touch_slot(mctx, slot);
-    if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) mctx->gbm.r_current = false;
-    if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) mctx->gbm.wsum_valid = false;
   }
   if (count) *count = ctx->slot[slot].rows * ctx->slot[slot].cols;
   return SE_OK;
@@ -1245,11 +1263,8 @@ int se_slot_layout(const se_ctx* ctx, int slot, int64_t* rows, int64_t* cols, in
 int se_upload(se_ctx* ctx, int slot, const float* host, int64_t count, int64_t offset) {
   if (!ctx || !host) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
+  SE_TRY(write_slot(ctx, slot));
   SE_TRY(for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_CUDA(ctx, cudaMemcpyAsync(d, host + done, sizeof(float) * len, cudaMemcpyHostToDevice, ctx->stream));
     return SE_OK;
@@ -1262,11 +1277,8 @@ int se_upload(se_ctx* ctx, int slot, const float* host, int64_t count, int64_t o
 int se_upload_f64(se_ctx* ctx, int slot, const double* host, int64_t count, int64_t offset) {
   if (!ctx || !host) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
+  SE_TRY(write_slot(ctx, slot));
   // narrow on the host (halves PCIe bytes) through pinned staging, in chunks
   const int64_t chunk = 1 << 22;
   SE_TRY(ensure_stage(ctx, sizeof(float) * (size_t)chunk));
@@ -1285,7 +1297,6 @@ int se_upload_f64(se_ctx* ctx, int slot, const double* host, int64_t count, int6
 int se_upload_rowmajor(se_ctx* ctx, int slot, const float* host, int64_t n_rows, int d, int64_t row_offset) {
   if (!ctx || (!host && n_rows > 0)) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  touch_slot(ctx, slot);
   const SlotBuf& X = ctx->slot[slot];
   SE_REQUIRE(ctx, X.d && X.rows == d, SE_ERR_STATE, "slot %d must be allocated as [%d][n] (has [%lld][%lld])", slot, d,
              (long long)X.rows, (long long)X.cols);
@@ -1293,8 +1304,7 @@ int se_upload_rowmajor(se_ctx* ctx, int slot, const float* host, int64_t n_rows,
              "rows [%lld,+%lld) outside the slot's %lld rows", (long long)row_offset, (long long)n_rows, (long long)X.cols);
   if (n_rows == 0) return SE_OK;
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  const int64_t ld = X.rows > 1 ? X.ld : X.cols;
+  SE_TRY(write_slot(ctx, slot));
   // ~32 MB chunks, whole rows, multiple of 32 rows
   int64_t chunk_rows = (int64_t)(32u << 20) / ((int64_t)d * (int64_t)sizeof(float));
   chunk_rows = (chunk_rows / 32) * 32;
@@ -1349,7 +1359,7 @@ int se_upload_rowmajor(se_ctx* ctx, int slot, const float* host, int64_t n_rows,
     SE_ING(cudaMemcpyAsync(dstage[b], src, bytes, cudaMemcpyHostToDevice, copy_stream));
     SE_ING(cudaEventRecord(copied[b], copy_stream));
     SE_ING(cudaStreamWaitEvent(ctx->stream, copied[b], 0));
-    cudaError_t le = launch_transpose_rows(dstage[b], rows, d, X.d, ld, row_offset + done, ctx->stream);
+    cudaError_t le = launch_transpose_rows(dstage[b], rows, d, X.d, X.ld, row_offset + done, ctx->stream);
     ctx->launches++;
     if (le != cudaSuccess) SE_ING(le);
     SE_ING(cudaEventRecord(consumed[b], ctx->stream));
@@ -1364,7 +1374,7 @@ int se_download(se_ctx* ctx, int slot, float* host, int64_t count, int64_t offse
   if (!ctx || !host) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
+  SE_TRY(read_slot(ctx, slot));
   SE_TRY(for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_CUDA(ctx, cudaMemcpyAsync(host + done, d, sizeof(float) * len, cudaMemcpyDeviceToHost, ctx->stream));
     return SE_OK;
@@ -1392,11 +1402,8 @@ int se_download_scaled(se_ctx* ctx, int slot, double scale, float* host, int64_t
 int se_fill(se_ctx* ctx, int slot, float value, int64_t count, int64_t offset) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  touch_slot(ctx, slot);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
+  SE_TRY(write_slot(ctx, slot));
   return for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t, int64_t len) {
     SE_LAUNCH(ctx, launch_fill(d, value, len, ctx->sms, ctx->stream));
     return SE_OK;
@@ -1410,9 +1417,8 @@ int se_copy_slot(se_ctx* ctx, int dst_slot, int src_slot) {
   const SlotBuf &d = ctx->slot[dst_slot], &s = ctx->slot[src_slot];
   SE_REQUIRE(ctx, d.d && s.d && d.rows == s.rows && d.cols == s.cols, SE_ERR_STATE, "slot shapes differ");
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (is_yfr(dst_slot) || src_slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
-  touch_slot(ctx, dst_slot);
-  if (dst_slot == SE_SLOT_Y || dst_slot == SE_SLOT_F || dst_slot == SE_SLOT_R) ctx->gbm.r_current = false;
+  SE_TRY(read_slot(ctx, src_slot));
+  SE_TRY(write_slot(ctx, dst_slot));
   SE_CUDA(ctx, cudaMemcpyAsync(d.d, s.d, sizeof(float) * (size_t)(s.rows * s.ld), cudaMemcpyDeviceToDevice, ctx->stream));
   return SE_OK;
 }
@@ -1421,12 +1427,9 @@ int se_fill_synthetic(se_ctx* ctx, int slot, int kind, uint64_t seed, double a, 
                       int64_t offset) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
-  touch_slot(ctx, slot);
   SE_REQUIRE(ctx, kind >= 0 && kind <= 3, SE_ERR_ARG, "bad synthetic kind %d", kind);
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (slot == SE_SLOT_W || slot == SE_SLOT_BAG) ctx->gbm.wsum_valid = false;
-  if (is_yfr(slot)) SE_TRY(settle_f(ctx));
-  if (slot == SE_SLOT_Y || slot == SE_SLOT_F || slot == SE_SLOT_R) ctx->gbm.r_current = false;
+  SE_TRY(write_slot(ctx, slot));
   return for_segments(ctx, ctx->slot[slot], count, offset, [&](float* d, int64_t done, int64_t len) {
     SE_LAUNCH(ctx, launch_fill_synthetic(d, kind, seed, a, b, len, offset + done, ctx->sms, ctx->stream));
     return SE_OK;
@@ -1439,7 +1442,7 @@ int se_slot_sum(se_ctx* ctx, int slot, int64_t count, double* out) {
   const SlotBuf& s = ctx->slot[slot];
   SE_REQUIRE(ctx, s.d && s.rows == 1 && count <= s.cols, SE_ERR_STATE, "slot %d is not a [n] vector of >= %lld", slot, (long long)count);
   SE_TRY(begin(ctx));
-  if (slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
+  SE_TRY(read_slot(ctx, slot));
   SE_LAUNCH(ctx, launch_sum(s.d, count, red_ws(ctx), ctx->ctas_per_sm, ctx->sms, ctx->stream));
   return fetch_scalars(ctx, 0, 1, out);
 }
@@ -1461,7 +1464,7 @@ int se_quantile(se_ctx* ctx, int which, int slot, int64_t count, double q, doubl
     a = s.d;
   }
   SE_TRY(begin(ctx));
-  if (which == 1 || slot == SE_SLOT_F) SE_TRY(settle_f(ctx));
+  SE_TRY(read_slot(ctx, which == 1 ? SE_SLOT_F : slot));
   double total = (double)n;
   SE_TRY(se_comm_allreduce_host(ctx, &total, 1));
   SE_REQUIRE(ctx, total >= 1.0, SE_ERR_ARG, "quantile of an empty column");
@@ -1564,7 +1567,7 @@ int ensure_big(se_ctx* ctx, int dim) {
   return SE_OK;
 }
 
-// Labels as class indices: one validation pass per upload of the label slot (see validate_labels_kernel).
+// Labels as class indices: one validation pass per write of the label slot (see validate_labels_kernel).
 int ensure_labels_checked(se_ctx* ctx, int which /*0 train, 1 validation*/, int K, int64_t n) {
   if (ctx->y_state[which] == 2 && ctx->y_state_k[which] == K) return SE_OK;
   const SlotBuf& y = ctx->slot[which ? SE_SLOT_VY : SE_SLOT_Y];
@@ -2376,9 +2379,9 @@ int se_agg_run(se_ctx* ctx, const double* weights, const double* init) {
   SE_TRY(begin(ctx));
   AggArgs a;
   a.kind = g.kind; a.M = g.M; a.K = g.K; a.dim = g.dim; a.loss = g.loss; a.n = g.n;
-  a.P = ctx->slot[SE_SLOT_P].d; a.ld = ctx->slot[SE_SLOT_P].rows > 1 ? ctx->slot[SE_SLOT_P].ld : ctx->slot[SE_SLOT_P].cols;
+  a.P = ctx->slot[SE_SLOT_P].d; a.ld = ctx->slot[SE_SLOT_P].ld;
   a.raw = ctx->slot[SE_SLOT_RAW].d;
-  a.ld_out = ctx->slot[SE_SLOT_RAW].rows > 1 ? ctx->slot[SE_SLOT_RAW].ld : ctx->slot[SE_SLOT_RAW].cols;
+  a.ld_out = ctx->slot[SE_SLOT_RAW].ld;
   a.prob = ctx->slot[SE_SLOT_PROB].d;
   a.label = ctx->slot[SE_SLOT_LABEL].d;
   a.bad_label = ctx->d_bad_label;
@@ -2454,9 +2457,6 @@ int se_agg_run(se_ctx* ctx, const double* weights, const double* init) {
 
 // ---- on-device base models ---------------------------------------------------------------------
 namespace {
-// Walk the uint8 rank matrix instead of the fp32 features when every threshold of the tree fits the per-column edge
-// lists (<= 255 per column; Spark's trees draw theirs from the <= maxBins - 1 candidates of findSplits, the same on
-// every round).  Returns 1 when the binned kernel was launched, 0 when the caller must take the fp32 walk.
 // Makes the rank matrix of slot X cover every threshold of the given nodes (col[i] < 0: leaf): allocates it on first
 // use, inserts new thresholds into the per-column edge lists and re-ranks the columns that changed.  Returns 1 when the
 // matrix is ready, 0 when it cannot be used (disabled, no memory, NaN threshold, a column with more than 255 edges).
@@ -2501,7 +2501,7 @@ int bins_rerank(se_ctx* ctx, BinState& B, const SlotBuf& X) {
     SE_CUDA(ctx, cudaMemcpyAsync(B.d_cols, cols.data(), sizeof(int32_t) * cols.size(), cudaMemcpyHostToDevice, ctx->stream));
     SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the host vectors above go out of scope
     BinArgs b;
-    b.X = X.d; b.X8 = B.d8; b.n = X.cols; b.ld = X.rows > 1 ? X.ld : X.cols; b.ld8 = B.ld8;
+    b.X = X.d; b.X8 = B.d8; b.n = X.cols; b.ld = X.ld; b.ld8 = B.ld8;
     b.cols = B.d_cols; b.edges = B.d_edges; b.n_edges = B.d_nedges;
     SE_LAUNCH_T(ctx, SE_KF_OTHER, launch_bin_columns(b, (int)cols.size(), ctx->sms, ctx->stream));
     for (int32_t c : cols) B.dirty[c] = 0;
@@ -2533,10 +2533,12 @@ int bins_prepare(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const in
   return 1;
 }
 
-int tree_predict_binned(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const int32_t* col, const float* thr,
-                        const int32_t* left, const int32_t* right, const TreeArgs& t) {
-  ctx->last_tree_binned = 0;
-  ctx->last_tree_mask = 0;
+// Walk the uint8 rank matrix instead of the fp32 features when every threshold of the tree fits the per-column edge
+// lists (<= 255 per column; Spark's trees draw theirs from the <= maxBins - 1 candidates of findSplits, the same on
+// every round).  Returns 1 with the tree staged in bins[which].d_nodes and its internal node count in n_internal, 0
+// when the caller must take the fp32 walk.
+int tree_nodes_binned(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, const int32_t* col, const float* thr,
+                      const int32_t* left, const int32_t* right, int* n_internal) {
   if (n_nodes > 65535) return 0;
   {
     const int rc = bins_prepare(ctx, which, X, n_nodes, col, thr);
@@ -2550,10 +2552,10 @@ int tree_predict_binned(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, c
     B.nodes_cap = (size_t)n_nodes;
   }
   std::vector<uint4> nodes((size_t)n_nodes);
-  int n_internal = 0;
+  *n_internal = 0;
   for (int i = 0; i < n_nodes; ++i) {
     if (col[i] < 0) { nodes[i] = make_uint4(0u, 0u, 0x80000000u, 0u); continue; }
-    ++n_internal;
+    ++*n_internal;
     const std::vector<float>& E = B.edges[col[i]];
     const uint32_t j = (uint32_t)(std::lower_bound(E.begin(), E.end(), thr[i]) - E.begin());  // x <= t_j  <=>  rank(x) <= j
     const uint64_t off = (uint64_t)col[i] * (uint64_t)B.ld8;
@@ -2561,9 +2563,6 @@ int tree_predict_binned(se_ctx* ctx, int which, const SlotBuf& X, int n_nodes, c
   }
   SE_CUDA(ctx, cudaMemcpyAsync(B.d_nodes, nodes.data(), sizeof(uint4) * (size_t)n_nodes, cudaMemcpyHostToDevice, ctx->stream));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_predict_binned(t, B.d8, B.d_nodes, n_internal, ctx->tree_mask, ctx->sms, ctx->stream));
-  ctx->last_tree_binned = 1;
-  ctx->last_tree_mask = (ctx->tree_mask && n_internal <= 64 && n_nodes <= 256) ? 1 : 0;
   return 1;
 }
 }  // namespace
@@ -2576,11 +2575,8 @@ static int tree_predict_impl(se_ctx* ctx, int which, int n_nodes, const int32_t*
   const size_t bytes = (size_t)n_nodes * (16 + 4 * (size_t)n_out);
   SE_REQUIRE(ctx, n_nodes >= 1 && bytes <= (size_t)kSmallBytes && (size_t)n_nodes * 20 <= 200 * 1024,
              SE_ERR_ARG, "tree of %d nodes x %d outputs not supported", n_nodes, n_out);
-  SE_REQUIRE(ctx, out_slot >= 0 && out_slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad out slot");
   const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  const SlotBuf& O = ctx->slot[out_slot];
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row + n_out <= O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(begin(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   int32_t* hf = reinterpret_cast<int32_t*>(ctx->h_small);
@@ -2620,24 +2616,27 @@ static int tree_predict_impl(se_ctx* ctx, int which, int n_nodes, const int32_t*
   }
   memcpy(hv, value, sizeof(float) * (size_t)n_nodes * n_out);
   SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
-  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
+  int n_internal = 0;
+  const int binned = tree_nodes_binned(ctx, which, X, n_nodes, hf, ht, hl, hr, &n_internal);
+  if (binned < 0) return binned;
   TreeArgs t;
-  t.X = X.d; t.n = X.cols; t.ld = X.rows > 1 ? X.ld : X.cols; t.n_nodes = n_nodes;
+  // after the rank matrix is prepared: a walk over X into a row of X leaves it invalid
+  SE_TRY(out_rows(ctx, out_slot, out_row, n_out, X.cols, &t.out, &t.ld_out));
+  t.X = X.d; t.n = X.cols; t.ld = X.ld; t.n_nodes = n_nodes;
   t.feature = reinterpret_cast<const int32_t*>(ctx->d_small);
   t.threshold = reinterpret_cast<const float*>(t.feature + n_nodes);
   t.left = reinterpret_cast<const int32_t*>(t.threshold + n_nodes);
   t.right = t.left + n_nodes;
   t.value = reinterpret_cast<const float*>(t.right + n_nodes);
   t.n_out = n_out;
-  t.ld_out = O.rows > 1 ? O.ld : O.cols;
-  t.out = O.d + (int64_t)out_row * t.ld_out;
-  {
-    const int rc = tree_predict_binned(ctx, which, X, n_nodes, hf, ht, hl, hr, t);
-    if (rc < 0) return rc;
-    if (rc == 1) return end(ctx);
+  if (binned) {
+    const BinState& B = ctx->bins[which];
+    SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_predict_binned(t, B.d8, B.d_nodes, n_internal, ctx->tree_mask, ctx->sms, ctx->stream));
+  } else {
+    SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_predict(t, ctx->sms, ctx->stream));
   }
-  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_predict(t, ctx->sms, ctx->stream));
+  ctx->last_tree_binned = binned;
+  ctx->last_tree_mask = (binned && ctx->tree_mask && n_internal <= 64 && n_nodes <= 256) ? 1 : 0;
   return end(ctx);
 }
 
@@ -2843,11 +2842,8 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
                       const double* weights, double init, int out_slot, int out_row) {
   if (!ctx || !offsets || !feature || !threshold || !left || !right || !value) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= (1 << 20), SE_ERR_ARG, "bad tree count %d", n_trees);
-  SE_REQUIRE(ctx, out_slot >= 0 && out_slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad out slot");
   const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  const SlotBuf& O = ctx->slot[out_slot];
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
   SE_TRY(begin(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -2855,11 +2851,9 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
   const BinState& B = ctx->bins[which];
   std::vector<ForestChunk> chunks;
   SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, false, kForestTile, 0, chunks));
-  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
-  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
   ForestArgs a;
+  SE_TRY(out_rows(ctx, out_slot, out_row, 1, X.cols, &a.out, nullptr));  // after forest_bins, as in tree_predict_impl
   a.n = X.cols;
-  a.out = O.d + (int64_t)out_row * (O.rows > 1 ? O.ld : O.cols);
   a.init = init;
   for (size_t k = 0; k < chunks.size(); ++k) {
     SE_TRY(forest_upload_chunk(ctx, B, chunks[k], offsets, feature, threshold, left, right, value, weights, nullptr, a));
@@ -2945,7 +2939,7 @@ int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, in
   g.acc = ctx->d_forest_acc; g.ld_acc = ld_acc;
   const SlotBuf& R = ctx->slot[SE_SLOT_RAW];
   g.raw = R.d; g.prob = ctx->slot[SE_SLOT_PROB].d; g.label = ctx->slot[SE_SLOT_LABEL].d;
-  g.ld_out = R.rows > 1 ? R.ld : R.cols;
+  g.ld_out = R.ld;
   g.bad_label = ctx->d_bad_label;
   for (size_t k = 0; k < chunks.size(); ++k) {
     SE_TRY(forest_upload_chunk(ctx, B, chunks[k], offsets, feature, threshold, left, right, value, w.data(),
@@ -2972,11 +2966,8 @@ int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets
   SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= SE_FOREST_MEDIAN_MAX_TREES, SE_ERR_ARG,
              "se_forest_median serves 1..%d trees, got %d: evaluate the members with se_tree_predict + se_agg_run",
              SE_FOREST_MEDIAN_MAX_TREES, n_trees);
-  SE_REQUIRE(ctx, out_slot >= 0 && out_slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad out slot");
   const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  const SlotBuf& O = ctx->slot[out_slot];
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_REQUIRE(ctx, O.d && O.cols == X.cols && out_row >= 0 && out_row < O.rows, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
   SE_TRY(begin(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -2991,10 +2982,9 @@ int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets
   const size_t budget = std::min((size_t)(216 * 1024), (size_t)(228 * 1024) / (size_t)ctas - 1024 - 512 - 16);
   std::vector<ForestChunk> chunks;
   SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, false, kForestMedianTile, vals_bytes, chunks, budget));
-  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
-  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
-  // every chunk's packed trees in one buffer: the kernel walks them all for each tile
   ForestMedianArgs g;
+  SE_TRY(out_rows(ctx, out_slot, out_row, 1, X.cols, &g.out, nullptr));  // after forest_bins, as in tree_predict_impl
+  // every chunk's packed trees in one buffer: the kernel walks them all for each tile
   g.n = X.cols;
   g.X8 = B.d8; g.ld8 = B.ld8;
   g.M = n_trees;
@@ -3041,7 +3031,6 @@ int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets
     SE_CUDA(ctx, cudaMemsetAsync(ctx->d_wm, 0, sizeof(unsigned int), ctx->stream));
     g.deferred = ctx->d_wm;
   }
-  g.out = O.d + (int64_t)out_row * (O.rows > 1 ? O.ld : O.cols);
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_forest_median(g, (size_t)g.vals_off + vals_bytes, ctx->sms, ctx->stream));
   ctx->last_wm_mode = g.mode;
   ctx->last_forest_chunks = (int)chunks.size();
@@ -3053,14 +3042,11 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
                       const int32_t* subspace, int out_slot, int out_row) {
   if (!ctx || (!coef && n_coef > 0)) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, n_coef >= 0 && (size_t)n_coef * 8 <= (size_t)kSmallBytes, SE_ERR_ARG, "bad coefficient count");
-  SE_REQUIRE(ctx, out_slot >= 0 && out_slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad out slot");
   const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  const SlotBuf& O = ctx->slot[out_slot];
   SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_REQUIRE(ctx, O.d && out_row >= 0 && out_row < O.rows && O.cols == X.cols, SE_ERR_STATE, "output slot shape mismatch");
   SE_TRY(begin(ctx));
-  if (is_yfr(out_slot)) SE_TRY(settle_f(ctx));
-  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
+  float* out = nullptr;
+  SE_TRY(out_rows(ctx, out_slot, out_row, 1, X.cols, &out, nullptr));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   float* hc = reinterpret_cast<float*>(ctx->h_small);
   int32_t* hcol = reinterpret_cast<int32_t*>(hc + n_coef);
@@ -3074,8 +3060,8 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
     SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, (size_t)n_coef * 8, cudaMemcpyHostToDevice, ctx->stream));
   const float* dc = reinterpret_cast<const float*>(ctx->d_small);
   const int32_t* dcol = reinterpret_cast<const int32_t*>(dc + n_coef);
-  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_linear_predict(X.d, X.cols, X.rows > 1 ? X.ld : X.cols, n_coef, dc, dcol, intercept,
-                                       O.d + (int64_t)out_row * (O.rows > 1 ? O.ld : O.cols), ctx->sms, ctx->stream));
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_linear_predict(X.d, X.cols, X.ld, n_coef, dc, dcol, intercept, out, ctx->sms,
+                                                       ctx->stream));
   return end(ctx);
 }
 
@@ -3115,8 +3101,9 @@ int se_tree_fit_bins(se_ctx* ctx, int n_cols, const int32_t* offsets, const floa
 namespace {
 // What the local part of a fit (tree_fit_prepare) hands to its level loop.
 struct TreeFitPlan {
-  const float *r = nullptr, *w = nullptr, *bag = nullptr, *outc = nullptr;
-  int64_t n = 0, nw = 0;
+  const float *r = nullptr, *w = nullptr, *bag = nullptr;
+  float* out = nullptr;
+  int64_t n = 0, nw = 0, ld_out = 0;
   int nb = 0, sw = 0, top = 0;
   uint32_t hash = 0;  // 24 bits: the subspace, its columns' candidates and the validity rules
 };
@@ -3148,16 +3135,13 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
     const SlotBuf& s = ctx->slot[slot];
     SE_REQUIRE(ctx, s.d && s.cols == n && row >= 0 && row < s.rows, SE_ERR_STATE, "%s slot %d: no row %d of %lld values", what,
                slot, row, (long long)n);
-    *p = s.d + (int64_t)row * (s.rows > 1 ? s.ld : s.cols);
+    *p = s.d + (int64_t)row * s.ld;
     return SE_OK;
   };
-  const float *r = nullptr, *w = nullptr, *bag = nullptr, *outc = nullptr;
+  const float *r = nullptr, *w = nullptr, *bag = nullptr;
   SE_TRY(row_of(label_slot, label_row, "label", &r));
   if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &w));
   if (use_bag) SE_TRY(row_of(SE_SLOT_BAG, 0, "bag", &bag));
-  SE_TRY(row_of(out_slot, out_row, "output", &outc));
-  SE_REQUIRE(ctx, !out_proba || out_row + K <= ctx->slot[out_slot].rows, SE_ERR_STATE,
-             "output slot %d: no rows %d..%d for the class probabilities", out_slot, out_row, out_row + K - 1);
   SE_REQUIRE(ctx, n_subspace >= 1, SE_ERR_ARG, "empty subspace");
   BinState& B = ctx->bins[0];
   SE_REQUIRE(ctx, B.d8 && B.d == X.rows && B.n == X.cols, SE_ERR_STATE,
@@ -3176,8 +3160,8 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   }
   const int nb = std::min(256, maxc + 2);  // ranks 0..maxc, then NaN (rank 255) in the last bin
   SE_TRY(begin(ctx));
-  if (label_slot == SE_SLOT_F || weight_slot == SE_SLOT_F || is_yfr(out_slot)) SE_TRY(settle_f(ctx));
-  if (out_slot == SE_SLOT_F || out_slot == SE_SLOT_R || out_slot == SE_SLOT_Y) ctx->gbm.r_current = false;
+  SE_TRY(read_slot(ctx, label_slot));
+  SE_TRY(read_slot(ctx, weight_slot));
   SE_TRY(bins_rerank(ctx, B, X));  // X was rewritten since the candidates were set
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_small is reused below
   // ---- scratch
@@ -3231,7 +3215,9 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   const double frac[2] = {min_info_gain, min_weight_fraction};
   h = fnv_words(h, rules, 2);
   h = fnv_words(h, frac, sizeof(frac) / 4);
-  P.r = r; P.w = w; P.bag = bag; P.outc = outc;
+  // after the re-rank of X and the label check above: the output rows may be rows of X or Y themselves
+  SE_TRY(out_rows(ctx, out_slot, out_row, out_proba ? K : 1, n, &P.out, &P.ld_out));
+  P.r = r; P.w = w; P.bag = bag;
   P.n = n; P.nw = nw; P.nb = nb; P.sw = sw; P.top = top;
   P.hash = (h ^ (h >> 24)) & 0xFFFFFFu;
   return SE_OK;
@@ -3301,7 +3287,7 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
   BinState& B = ctx->bins[0];
   const int64_t n = P.n, nw = P.nw;
   const int nb = P.nb, sw = P.sw, top = P.top;
-  const float *r = P.r, *w = P.w, *bag = P.bag, *outc = P.outc;
+  const float *r = P.r, *w = P.w, *bag = P.bag;
   TreeFitArgs a;
   a.X8 = B.d8; a.ld8 = B.ld8; a.n = n;
   a.cols = T.d_cols; a.n_edges = B.d_nedges; a.edges = B.d_edges;
@@ -3350,11 +3336,8 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
   a.route = max_depth >= 1;
   a.nid_in = max_depth >= 2 ? nid[(max_depth - 1) & 1] : nullptr;
   a.nid_out = nullptr;
-  a.out = const_cast<float*>(outc);
-  {
-    const SlotBuf& O = ctx->slot[out_slot];
-    a.ld_out = O.rows > 1 ? O.ld : O.cols;
-  }
+  a.out = P.out;
+  a.ld_out = P.ld_out;
   if (K > 0) SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_prune(a, ctx->stream));
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_out(a, ctx->sms, ctx->stream));
   static_assert(sizeof(TreeFitNode) * kTreeFitHeap + (sizeof(double) + sizeof(float)) * kTreeFitHeap * kTreeFitMaxClasses +

@@ -10,13 +10,19 @@ pytestmark = pytest.mark.gpu
 
 LR = 0.7
 N_ROWS = 40961  # n % 4 == 1: the scalar tail of block 0 is covered
+D = 4
 
 
 @pytest.fixture(scope="module")
 def ctx():
+    from spark_ensemble_b200 import _native as N
     from spark_ensemble_b200.context import Context
     c = Context(0)
     c.set_option("fused_round", 1)
+    # resident features for the model writers, and a scratch row
+    c.alloc(N.SLOT_X, D, N_ROWS)
+    c.upload(N.SLOT_X, f32(np.random.default_rng(3).standard_normal((D, N_ROWS))))
+    c.alloc(N.SLOT_P, 1, N_ROWS)
     yield c
     c.close()
 
@@ -147,19 +153,48 @@ def test_gbm_reads_see_owed_F(ctx):
                                    err_msg=mode)
 
 
+TREE = {"feature": [1, -1, -1], "threshold": [0.25, 0.0, 0.0], "left": [1, 0, 0], "right": [2, 0, 0],
+        "value": [0.0, -1.25, 2.5]}
+TREE2 = {"feature": [0, 3, -1, -1, -1], "threshold": [-0.5, 0.75, 0.0, 0.0, 0.0], "left": [1, 2, 0, 0, 0],
+         "right": [4, 3, 0, 0, 0], "value": [0.0, 0.0, 1.5, -0.5, 0.75]}
+WHOLE_ROW = ("copy_slot", "linear_predict", "tree_predict", "forest_predict")
+
+
+def write(ctx, op, slot, lo, cnt):
+    """Writes elements [lo, lo + cnt) of the [1][n] slot through `op` (the whole-row writers: all of them)."""
+    from spark_ensemble_b200 import _native as N
+    vals = np.linspace(-3.0, 3.0, cnt)
+    if op == "upload":
+        ctx.upload(slot, f32(vals), offset=lo)
+    elif op == "upload_f64":
+        ctx.upload(slot, vals, offset=lo)
+    elif op == "upload_rowmajor":
+        ctx.upload_rowmajor(slot, f32(vals).reshape(-1, 1), row_offset=lo)
+    elif op == "fill":
+        ctx.fill(slot, 1.5, count=cnt, offset=lo)
+    elif op == "fill_synthetic":
+        ctx.fill_synthetic(slot, "normal", 7, 0.5, 2.0, count=cnt, offset=lo)
+    elif op == "copy_slot":
+        ctx.copy_slot(slot, N.SLOT_P)
+    elif op == "linear_predict":
+        ctx.linear_predict([0.5, -2.0], 0.25, slot, subspace=[0, 2])
+    elif op == "tree_predict":
+        ctx.tree_predict(TREE, slot)
+    else:
+        ctx.forest_predict([TREE, TREE2], slot, weights=[0.5, 1.5], init=0.125)
+
+
 @pytest.mark.parametrize("slot_name", ["SLOT_Y", "SLOT_R", "SLOT_F"])
-@pytest.mark.parametrize("op", ["upload", "fill"])
+@pytest.mark.parametrize("op", ["upload", "fill", "upload_f64", "upload_rowmajor", "fill_synthetic"] + list(WHOLE_ROW))
 def test_partial_write_keeps_owed_rows(ctx, slot_name, op):
     from spark_ensemble_b200 import _native as N
     slot = getattr(N, slot_name)
+    lo, cnt = (0, N_ROWS) if op in WHOLE_ROW else (1001, 500)
+    # what the call writes, from the same call into a slot nothing is derived from (copy_slot copies that slot)
+    write(ctx, "upload" if op == "copy_slot" else op, N.SLOT_P, lo, cnt)
+    vals = ctx.download(N.SLOT_P, count=cnt, offset=lo).copy()
     y, h, r, Fe = lazy_state(ctx, 41)
-    lo, cnt = 1001, 500
-    vals = f32(np.linspace(-3.0, 3.0, cnt))
-    if op == "upload":
-        ctx.upload(slot, vals, offset=lo)
-    else:
-        ctx.fill(slot, 1.5, count=cnt, offset=lo)
-        vals = np.full(cnt, 1.5, dtype=np.float32)
+    write(ctx, op, slot, lo, cnt)
     want = Fe.copy()
     if slot == N.SLOT_F:
         want[lo:lo + cnt] = vals
