@@ -223,12 +223,12 @@ def tau(m, scale) -> float:
     return TAU_C * EPS * (1.0 + np.sqrt(m)) * abs(scale)
 
 
-def _column_gains(rk, c, cw, r, ncand, p, w_root):
-    """Gain of every candidate of one column over a node's in-bag rows (-inf where not valid, and where no row ranks
-    j > 0: candidate j then repeats candidate j - 1's partition, which the fit takes first)."""
+def _gains(per, ncand, p, w_root):
+    """Gain of every candidate of one column from the node's per-rank sums per [256][4] (c, c·w, c·w·r, c·w·r²):
+    -inf where not valid, and where no row ranks j > 0 (candidate j then repeats candidate j - 1's partition, which
+    the fit takes first)."""
     if ncand == 0:
         return np.full(0, -np.inf)
-    per = np.stack([np.bincount(rk, weights=v, minlength=256) for v in (c, cw, cw * r, cw * r * r)], axis=1)
     cum = np.cumsum(per, axis=0)
     tot = cum[-1]
     ls = cum[:ncand]
@@ -244,11 +244,24 @@ def _column_gains(rk, c, cw, r, ncand, p, w_root):
     return np.where(ok, g, -np.inf)
 
 
+def _column_gains(rk, c, cw, r, ncand, p, w_root):
+    """_gains over a node's in-bag rows (rk their ranks in the column)."""
+    per = np.stack([np.bincount(rk, weights=v, minlength=256) for v in (c, cw, cw * r, cw * r * r)], axis=1)
+    return _gains(per, ncand, p, w_root)
+
+
 def _node_search(R, ncand, ib, c, cw, r, p, w_root):
-    """(gain, column, candidate) of every valid split of a node, sorted by gain descending, then column, candidate."""
+    """search() over a node's in-bag rows ib."""
+    return search([np.stack([np.bincount(R[k][ib], weights=v[ib], minlength=256) for v in (c, cw, cw * r, cw * r * r)],
+                            axis=1) for k in range(len(R))], ncand, p, w_root)
+
+
+def search(hist, ncand, p, w_root, gains=_gains):
+    """(gain, column, candidate) of every valid split of a node (hist: its [S][256][stats] sums per column and rank),
+    sorted by gain descending, then column, candidate."""
     out = []
-    for k in range(len(R)):
-        g = _column_gains(R[k][ib], c[ib], cw[ib], r[ib], ncand[k], p, w_root)
+    for k in range(len(ncand)):
+        g = gains(hist[k], ncand[k], p, w_root)
         for j in np.flatnonzero(np.isfinite(g)):
             out.append((float(g[j]), k, int(j)))
     out.sort(key=lambda t: (-t[0], t[1], t[2]))
@@ -261,13 +274,19 @@ def route(tree, X, cands, sub):
     sub = np.asarray(sub).reshape(-1)
     R = [ranks(X[:, col], cands[col]) for col in sub]
     ncand = [np.asarray(cands[col]).size for col in sub]
+    return R, ncand, bins_of(tree, [cands[col] for col in sub])
+
+
+def bins_of(tree, cands):
+    """Per node, the candidate index of its threshold, which must be a candidate of its column (cands[k]: the
+    candidates of subspace column k)."""
     bins = np.zeros(tree["feature"].size, np.int64)
     for i in np.flatnonzero(tree["feature"] >= 0):
-        cc = np.asarray(cands[sub[tree["feature"][i]]], np.float32)
+        cc = np.asarray(cands[tree["feature"][i]], np.float32)
         b = int(np.searchsorted(cc, np.float32(tree["threshold"][i])))
         assert b < cc.size and cc[b] == np.float32(tree["threshold"][i]), f"node {i}: threshold is not a candidate"
         bins[i] = b
-    return R, ncand, bins
+    return bins
 
 
 def walk(tree, n):
@@ -283,6 +302,137 @@ def walk(tree, n):
             stack.append((int(tree["right"][i]), rows[~go], depth + 1))
             stack.append((int(tree["left"][i]), rows[go], depth + 1))
     assert seen.all(), f"nodes {np.flatnonzero(~seen).tolist()} are not reached from the root"
+
+
+# ---- per-node statistics of a tree's rows ----------------------------------------------------------------------
+class Nodes:
+    """A list of row sets: node 0 holds every row, node v > 0 the rows of parent[v] whose rank in subspace column
+    col[v] is <= bin[v] (left[v]) or > bin[v].  A tree's nodes are one such list; the classifier's audit adds the
+    children of the splits a pruned node may have grown."""
+
+    def __init__(self):
+        self.parent, self.col, self.bin, self.left, self.depth = [-1], [0], [0], [1], [0]
+        self._key = {}
+
+    def __len__(self):
+        return len(self.parent)
+
+    def child(self, v, k, b, left) -> int:
+        key = (int(v), int(k), int(b), int(bool(left)))
+        if key not in self._key:
+            self._key[key] = len(self.parent)
+            self.parent.append(key[0]); self.col.append(key[1]); self.bin.append(key[2]); self.left.append(key[3])
+            self.depth.append(self.depth[key[0]] + 1)
+        return self._key[key]
+
+    @classmethod
+    def of_tree(cls, tree, bins):
+        """The nodes of a tree, after checking that every node is reached from the root once.  Returns (nodes,
+        order): node v here is node order[v] of the tree, parents before children."""
+        f = tree["feature"]
+        nodes, seen, order = cls(), np.zeros(f.size, bool), [0]
+        seen[0] = True
+        for v, i in enumerate(order):
+            if f[i] < 0:
+                continue
+            for side, j in ((1, int(tree["left"][i])), (0, int(tree["right"][i]))):
+                assert 0 <= j < f.size and not seen[j], f"node {j} is reached twice"
+                seen[j] = True
+                nodes.child(v, f[i], bins[i], side)
+                order.append(j)
+        assert seen.all(), f"nodes {np.flatnonzero(~seen).tolist()} are not reached from the root"
+        return nodes, order
+
+
+def row_stats(R, K, labels, w=None, counts=None):
+    """Statistics of Nodes over rows held in memory (R[k]: the ranks of subspace column k), as
+    oracle.Oracle.tree_hist sums them over chunks: a function (nodes, want) -> (totals, hists), totals[v] the node's
+    sums (c, c·w, c·w·r, c·w·r²) or (c, c·w per class), then Σ c·w·|r| and its in-bag row count; hists[v] for v in
+    want its [S][256][stats] sums per column and rank.  K == 0: regression labels, else class indices."""
+    y = np.asarray(labels, dtype=np.float32).astype(np.float64)
+    n = y.size
+    w = np.ones(n) if w is None else np.asarray(w, dtype=np.float32).astype(np.float64)
+    c = np.ones(n) if counts is None else np.asarray(counts, dtype=np.float32).astype(np.float64)
+    cw = c * w
+    if K:
+        per_row = np.zeros((n, K + 1))
+        per_row[:, 0] = c
+        per_row[np.arange(n), 1 + y.astype(np.int64)] = cw
+    else:
+        per_row = np.stack([c, cw, cw * y, cw * y * y], axis=1)
+    rows = {}
+
+    def stats(nodes, want):
+        tot, hists = np.zeros((len(nodes), per_row.shape[1] + 2)), {}
+        for v in range(len(nodes)):
+            if v not in rows:
+                p = nodes.parent[v]
+                rows[v] = np.flatnonzero(c > 0) if p < 0 else \
+                    rows[p][(R[nodes.col[v]][rows[p]] <= nodes.bin[v]) == bool(nodes.left[v])]
+            ib = rows[v]
+            tot[v, :-2] = per_row[ib].sum(axis=0)
+            tot[v, -2] = 0.0 if K else (cw[ib] * np.abs(y[ib])).sum()
+            tot[v, -1] = ib.size
+            if v in want:
+                hists[v] = np.stack([np.stack([np.bincount(R[k][ib], weights=per_row[ib, s], minlength=256)
+                                               for s in range(per_row.shape[1])], axis=1) for k in range(len(R))])
+        return tot, hists
+    return stats
+
+
+def check(tree, bins, ncand, stats, params=None, exact=False) -> int:
+    """The checks of audit() on a regression tree from the statistics of its nodes (stats: as row_stats returns);
+    bins[i] is node i's candidate index (bins_of), ncand[k] the candidate count of subspace column k.  Returns the
+    number of nodes checked (every node)."""
+    p = {"max_depth": 5, "min_instances": 1, "min_info_gain": 0.0, "min_weight_fraction": 0.0}
+    p.update(params or {})
+    f, value, gain = tree["feature"], tree["value"], tree["gain"]
+    nodes, order = Nodes.of_tree(tree, bins)
+    want = {v for v, i in enumerate(order) if f[i] >= 0 or nodes.depth[v] < p["max_depth"]}
+    tot, hist = stats(nodes, want)
+    w_root = tot[0, 1]
+    parent = {}  # per node: its parent's (relative rounding bound, Σ c·w·|r|, W)
+    for v, i in enumerate(order):
+        depth = nodes.depth[v]
+        st, a_abs, m_rows = tot[v, :4], tot[v, 4], tot[v, 5]
+        W = st[1]
+        t = tau(m_rows, st[3] / W) if W != 0 else 0.0
+        if i == 0:
+            parent[0] = (tau(m_rows, 1.0), a_abs, W)
+        if W == 0:
+            assert np.isnan(value[i]), f"node {i}: no in-bag weight, value {value[i]} (S/W is NaN)"
+        else:
+            m = st[2] / W
+            d = ulps32(value[i], np.float32(m))
+            if exact:
+                assert d == 0, f"node {i}: value {value[i]!r} is not fp32(S/W) = {m!r}"
+            elif d > 1:  # a right child's S and W are the parent's minus the left's: the parent's rounding
+                rel, a_p, w_p = parent[i]
+                assert abs(float(value[i]) - m) <= float(np.spacing(np.float32(m))) + rel * (a_p + abs(m) * w_p) / W, \
+                    f"node {i}: value {value[i]!r} is {d} ulps from fp32(S/W) = {m!r}, beyond the sums' rounding"
+        if f[i] < 0:
+            if depth < p["max_depth"] and not abs(_impurity(st)) < EPS + t:
+                cand = search(hist[v], ncand, p, w_root)
+                assert not cand or not cand[0][0] > t, f"node {i}: a leaf, but split {cand[0]} has gain > τ = {t:.3g}"
+            continue
+        assert depth < p["max_depth"], f"node {i}: a split at depth {depth}"
+        k, b = int(f[i]), int(bins[i])
+        per = hist[v][k]
+        assert b == 0 or per[b, 0] > 0, f"node {i}: candidate {b} repeats candidate {b - 1}'s partition"
+        ls = per[:b + 1].sum(axis=0)
+        rs = st - ls
+        slack = 1e-12 * w_root
+        assert ls[0] >= p["min_instances"] and rs[0] >= p["min_instances"], f"node {i}: rawCount {ls[0]}, {rs[0]}"
+        assert min(ls[1], rs[1]) >= p["min_weight_fraction"] * w_root - slack, f"node {i}: weights {ls[1]}, {rs[1]}"
+        assert gain[i] >= p["min_info_gain"] and gain[i] > 0, f"node {i}: gain {gain[i]}"
+        g = _impurity(st) - ls[1] / W * _impurity(ls) - rs[1] / W * _impurity(rs)
+        assert abs(g - gain[i]) <= t, f"node {i}: gain {gain[i]!r}, recomputed {g!r}, τ = {t:.3g}"
+        cand = search(hist[v], ncand, p, w_root)
+        assert cand and cand[0][0] <= g + t, f"node {i}: split {cand[0]} beats gain {g!r} by more than τ = {t:.3g}"
+        if len(cand) == 1 or cand[0][0] - cand[1][0] > t:
+            assert (k, b) == cand[0][1:], f"node {i}: the clear winner is {cand[0]}, the fit took ({k}, {b})"
+        parent[int(tree["left"][i])] = parent[int(tree["right"][i])] = (tau(m_rows, 1.0), a_abs, W)
+    return len(nodes)
 
 
 def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=None, exact=False) -> int:
@@ -301,72 +451,30 @@ def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=Non
                   split has children of equal means: gain 0 up to rounding);
       output      out (when given) is every row's leaf value, bit for bit.
     cands are the candidates of every column of X, sub the subspace; params holds max_depth, min_instances,
-    min_info_gain and min_weight_fraction."""
-    p = {"max_depth": 5, "min_instances": 1, "min_info_gain": 0.0, "min_weight_fraction": 0.0}
-    p.update(params or {})
+    min_info_gain and min_weight_fraction.  The checks run on per-node sums (check); oracle/tree_audit.py takes the
+    same sums over row chunks."""
     R, ncand, bins = route(tree, X, cands, sub)
-    r = np.asarray(labels, dtype=np.float32).astype(np.float64)
-    n = r.size
-    w = np.ones(n) if w is None else np.asarray(w, dtype=np.float32).astype(np.float64)
-    c = np.ones(n) if counts is None else np.asarray(counts, dtype=np.float32).astype(np.float64)
-    cw = c * w
-    inbag = c > 0
-    w_root = cw[inbag].sum()
-    f, value, gain = tree["feature"], tree["value"], tree["gain"]
-    leaf_of = np.zeros(n, np.int64)
-    parent = {}  # per node: its parent's (relative rounding bound, Σ c·w·|r|, W)
-    it = walk(tree, n)
-    step = next(it)
-    audited = 0
-    while step is not None:
-        i, rows, depth = step
-        audited += 1
-        ib = rows[inbag[rows]]
-        st = _stats(r[ib], w[ib], c[ib])
-        W = st[1]
-        t = tau(ib.size, st[3] / W) if W != 0 else 0.0
-        if i == 0:
-            parent[0] = (tau(ib.size, 1.0), (cw[ib] * np.abs(r[ib])).sum(), W)
-        if W == 0:
-            assert np.isnan(value[i]), f"node {i}: no in-bag weight, value {value[i]} (S/W is NaN)"
-        else:
-            m = st[2] / W
-            d = ulps32(value[i], np.float32(m))
-            if exact:
-                assert d == 0, f"node {i}: value {value[i]!r} is not fp32(S/W) = {m!r}"
-            elif d > 1:  # a right child's S and W are the parent's minus the left's: the parent's rounding
-                rel, a_p, w_p = parent[i]
-                assert abs(float(value[i]) - m) <= float(np.spacing(np.float32(m))) + rel * (a_p + abs(m) * w_p) / W, \
-                    f"node {i}: value {value[i]!r} is {d} ulps from fp32(S/W) = {m!r}, beyond the sums' rounding"
-        if f[i] < 0:
-            leaf_of[rows] = i
-            if depth < p["max_depth"] and not abs(_impurity(st)) < EPS + t:
-                cand = _node_search(R, ncand, ib, c, cw, r, p, w_root)
-                assert not cand or not cand[0][0] > t, f"node {i}: a leaf, but split {cand[0]} has gain > τ = {t:.3g}"
-            step = next(it, None)
-            continue
-        assert depth < p["max_depth"], f"node {i}: a split at depth {depth}"
-        k, b = int(f[i]), int(bins[i])
-        go_ib = R[k][ib] <= b
-        assert b == 0 or np.any(R[k][ib] == b), f"node {i}: candidate {b} repeats candidate {b - 1}'s partition"
-        ls = _stats(r[ib[go_ib]], w[ib[go_ib]], c[ib[go_ib]])
-        rs = st - ls
-        slack = 1e-12 * w_root
-        assert ls[0] >= p["min_instances"] and rs[0] >= p["min_instances"], f"node {i}: rawCount {ls[0]}, {rs[0]}"
-        assert min(ls[1], rs[1]) >= p["min_weight_fraction"] * w_root - slack, f"node {i}: weights {ls[1]}, {rs[1]}"
-        assert gain[i] >= p["min_info_gain"] and gain[i] > 0, f"node {i}: gain {gain[i]}"
-        g = _impurity(st) - ls[1] / W * _impurity(ls) - rs[1] / W * _impurity(rs)
-        assert abs(g - gain[i]) <= t, f"node {i}: gain {gain[i]!r}, recomputed {g!r}, τ = {t:.3g}"
-        cand = _node_search(R, ncand, ib, c, cw, r, p, w_root)
-        assert cand and cand[0][0] <= g + t, f"node {i}: split {cand[0]} beats gain {g!r} by more than τ = {t:.3g}"
-        if len(cand) == 1 or cand[0][0] - cand[1][0] > t:
-            assert (k, b) == cand[0][1:], f"node {i}: the clear winner is {cand[0]}, the fit took ({k}, {b})"
-        parent[int(tree["left"][i])] = parent[int(tree["right"][i])] = \
-            (tau(ib.size, 1.0), (cw[ib] * np.abs(r[ib])).sum(), W)
-        step = send(it, R[k][rows] <= b)
+    audited = check(tree, bins, ncand, row_stats(R, 0, labels, w, counts), params, exact)
     if out is not None:
-        np.testing.assert_array_equal(np.asarray(out, np.float32), value[leaf_of].astype(np.float32))
+        np.testing.assert_array_equal(np.asarray(out, np.float32),
+                                      tree["value"][leaf_of(tree, R, bins)].astype(np.float32))
     return audited
+
+
+def leaf_of(tree, rank_cols, bins) -> np.ndarray:
+    """Index of every row's leaf in an array-form tree (bins: its candidate indices), walking the ranks."""
+    Rk = np.stack([np.asarray(a, dtype=np.int64) for a in rank_cols])
+    n = Rk.shape[1]
+    node = np.zeros(n, dtype=np.int64)
+    for _ in range(64):
+        f = tree["feature"][node]
+        live = f >= 0
+        if not live.any():
+            break
+        rk = Rk[np.maximum(f, 0), np.arange(n)]
+        go = np.where(rk <= bins[node], tree["left"][node], tree["right"][node])
+        node = np.where(live, go, node)
+    return node
 
 
 def send(it, go):

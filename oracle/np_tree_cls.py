@@ -9,7 +9,8 @@ import math
 import numpy as np
 
 from .np_tree import EPS, candidates, ranks  # noqa: F401  (the candidates and ranks are the regressor's)
-from .np_tree import route, send, tau, ulps32, walk
+from .np_tree import Nodes, route, row_stats, send, tau, ulps32, walk  # noqa: F401
+from .np_tree import leaf_of as np_leaf_of
 
 
 def impurity(n, kind: str) -> float:
@@ -193,12 +194,13 @@ def _impurity_rows(nm, kind):
     return np.where(W == 0, 0.0, v)
 
 
-def _column_gains(rk, yk, c, cw, K, ncand, kind, p, w_root):
+def _gains(per, ncand, kind, p, w_root):
+    """Gain of every candidate of one column from the node's per-rank sums per [256][K + 1] (c, then c·w per class):
+    -inf where not valid, and where no row ranks j > 0."""
     if ncand == 0:
         return np.full(0, -np.inf)
-    per = np.bincount(rk * K + yk, weights=cw, minlength=256 * K).reshape(256, K)
-    cnt = np.bincount(rk, weights=c, minlength=256)
-    cum, cc = np.cumsum(per, axis=0), np.cumsum(cnt)
+    cnt = per[:, 0]
+    cum, cc = np.cumsum(per[:, 1:], axis=0), np.cumsum(cnt)
     tot = cum[-1]
     ls, lc = cum[:ncand], cc[:ncand]
     rs, rc = tot - ls, cc[-1] - lc
@@ -211,6 +213,12 @@ def _column_gains(rk, yk, c, cw, K, ncand, kind, p, w_root):
         ok &= g >= p["min_info_gain"]
     ok &= (np.arange(ncand) == 0) | (cnt[:ncand] > 0)
     return np.where(ok, g, -np.inf)
+
+
+def _column_gains(rk, yk, c, cw, K, ncand, kind, p, w_root):
+    per = np.concatenate([np.bincount(rk, weights=c, minlength=256)[:, None],
+                          np.bincount(rk * K + yk, weights=cw, minlength=256 * K).reshape(256, K)], axis=1)
+    return _gains(per, ncand, kind, p, w_root)
 
 
 def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=None, out_proba=None,
@@ -231,71 +239,88 @@ def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=Non
                   tie, one of the tied choices must lead there, not merely any choice;
       output      out / out_proba (when given, out_proba [K, n]) are every row's leaf label / values, bit for bit.
     τ = TAU_C · 2⁻⁵² · (1 + √m), times log₂K for entropy (np_tree.TAU_C).  params holds num_classes, impurity,
-    max_depth, min_instances, min_info_gain and min_weight_fraction."""
+    max_depth, min_instances, min_info_gain and min_weight_fraction.  The checks run on per-node sums (check);
+    oracle/tree_audit.py takes the same sums over row chunks."""
+    K = int(params["num_classes"])
+    R, ncand, bins = route(tree, X, cands, sub)
+    audited = check(tree, bins, ncand, row_stats(R, K, labels, w, counts), params, exact)
+    leaf = np_leaf_of(tree, R, bins)
+    if out is not None:
+        np.testing.assert_array_equal(np.asarray(out, np.float32), tree["value"][leaf].astype(np.float32))
+    if out_proba is not None:
+        np.testing.assert_array_equal(np.asarray(out_proba, np.float32).reshape(K, leaf.size),
+                                      np.asarray(tree["values"], np.float32)[leaf].T)
+    return audited
+
+
+def check(tree, bins, ncand, stats, params, exact=False) -> int:
+    """The checks of audit() on a classification tree from the statistics of its nodes (stats: as np_tree.row_stats
+    returns), asked again for the children of the splits a pruned leaf may have grown.  Returns the number of nodes
+    checked (every node)."""
     p = {"impurity": "gini", "max_depth": 5, "min_instances": 1, "min_info_gain": 0.0, "min_weight_fraction": 0.0}
     p.update(params or {})
     K, kind = int(p["num_classes"]), p["impurity"]
-    R, ncand, bins = route(tree, X, cands, sub)
-    y = np.asarray(labels, dtype=np.float32).astype(np.int64)
-    n = y.size
-    w = np.ones(n) if w is None else np.asarray(w, dtype=np.float32).astype(np.float64)
-    c = np.ones(n) if counts is None else np.asarray(counts, dtype=np.float32).astype(np.float64)
-    cw = c * w
-    inbag = c > 0
-    w_root = cw[inbag].sum()
     f, gain = tree["feature"], tree["gain"]
     scale = 1.0 if kind == "gini" else math.log2(K)
+    nodes, order = Nodes.of_tree(tree, bins)
+    tot, hist = stats(nodes, {v for v, i in enumerate(order) if f[i] >= 0 or nodes.depth[v] < p["max_depth"]})
+    tot = {v: tot[v] for v in range(len(order))}
+    w_root = tot[0][1:K + 1].sum()
     parent_w = {0: w_root}
 
-    def splits(ib):
+    def splits(v):
         out = []
-        for kk in range(len(R)):
-            gk = _column_gains(R[kk][ib], y[ib], c[ib], cw[ib], K, ncand[kk], kind, p, w_root)
+        for kk in range(len(ncand)):
+            gk = _gains(hist[v][kk], ncand[kk], kind, p, w_root)
             out += [(float(gk[j]), kk, int(j)) for j in np.flatnonzero(np.isfinite(gk))]
         out.sort(key=lambda x: (-x[0], x[1], x[2]))
         return out
 
-    def collapses(ib, depth, label, pw):
-        """Whether the fit, growing a subtree on the in-bag rows ib at `depth` (pw: the parent's weight), can end
-        with every leaf of it labelled `label`, so that pruning merges it into one leaf.  Where rounding may decide
-        (gains within τ or 1e-7 of the best, impurity within τ of the purity rule, a gain within τ of 0), every
-        choice the fit may make is tried; anywhere else there is one."""
-        nk = np.bincount(y[ib], weights=cw[ib], minlength=K)
+    need = set()
+
+    def collapses(v, label, pw):
+        """Whether the fit, growing a subtree on node v's in-bag rows (pw: the parent's weight), can end with every
+        leaf of it labelled `label`, so that pruning merges it into one leaf; None while the statistics of a node it
+        depends on are not known yet (they are then in `need`).  Where rounding may decide (gains within τ or 1e-7 of
+        the best, impurity within τ of the purity rule, a gain within τ of 0), every choice the fit may make is tried;
+        anywhere else there is one."""
+        depth = nodes.depth[v]
+        if v not in tot or (depth < p["max_depth"] and v not in hist):
+            need.add(v)
+            return None
+        nk = tot[v][1:K + 1]
         labelled = labels_like(nk, label, CW_RTOL * pw)
-        t = tau(ib.size, scale)
+        t = tau(tot[v][-1], scale)
         imp = abs(impurity(nk, kind))
         if depth >= p["max_depth"] or imp < EPS - t:
             return labelled
-        cand = splits(ib)
+        cand = splits(v)
         best = cand[0][0] if cand else -np.inf
         if labelled and (imp < EPS + t or not best > t):
             return True  # the fit may stop here: pure within rounding, or no split clearly above 0
-        seen = set()
+        seen, unknown = set(), False
         for g, k, j in cand:
             if g < best - max(t, 1e-7 * abs(best)) or not g > -t:
                 break
-            m = R[k][ib] <= j
-            key = m.tobytes()
+            key = tuple(hist[v][k][:j + 1].sum(axis=0))  # the partition, by the sums of its left side
             if key in seen:
                 continue
             seen.add(key)
             W = nk.sum()
-            if collapses(ib[m], depth + 1, label, W) and collapses(ib[~m], depth + 1, label, W):
+            a = collapses(nodes.child(v, k, j, 1), label, W)
+            b = collapses(nodes.child(v, k, j, 0), label, W) if a is not False else False
+            if a and b:
                 return True
-        return False
+            unknown |= a is None or b is None
+        return None if unknown else False
 
-    leaf_of = np.zeros(n, np.int64)
-    it = walk(tree, n)
-    step = next(it)
-    audited = 0
-    while step is not None:
-        i, rows, depth = step
-        audited += 1
-        ib = rows[inbag[rows]]
-        nk = np.bincount(y[ib], weights=cw[ib], minlength=K)
+    pending = []
+    for v, i in enumerate(order):
+        depth = nodes.depth[v]
+        nk = tot[v][1:K + 1]
         W = nk.sum()
-        t = tau(ib.size, scale)
-        tol = 0.0 if exact else CW_RTOL * parent_w[i]
+        t = tau(tot[v][-1], scale)
+        tol = 0.0 if exact else CW_RTOL * parent_w[v]
         dev_cw = np.asarray(tree["class_weights"][i], np.float64)
         assert np.all(np.abs(dev_cw - nk) <= tol), f"node {i}: class weights {dev_cw} against {nk}"
         want = np.zeros(K, np.float32) if W == 0 else (nk / W).astype(np.float32)
@@ -314,23 +339,21 @@ def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=Non
             assert labels_like(nk, label, tol), f"node {i}: label {label} is not the first arg-max of {nk}"
         imp = impurity(nk, kind)
         if f[i] < 0:
-            leaf_of[rows] = i
             if depth < p["max_depth"] and not abs(imp) < EPS + t:
-                best = max((g.max() for k in range(len(R)) if ncand[k] > 0 for g in
-                            [_column_gains(R[k][ib], y[ib], c[ib], cw[ib], K, ncand[k], kind, p, w_root)]),
-                           default=-np.inf)
+                cand = splits(v)
+                best = cand[0][0] if cand else -np.inf
                 if best > t:  # only a pruned node: its subtree's leaves all carry one label
-                    assert collapses(ib, depth, label, parent_w[i]), \
-                        f"node {i}: a leaf, but a split of gain {best!r} > τ = {t:.3g} leads to other labels"
-            step = next(it, None)
+                    pending.append((i, v, label, parent_w[v], best, t))
             continue
         assert depth < p["max_depth"], f"node {i}: a split at depth {depth}"
         k, b = int(f[i]), int(bins[i])
-        go_ib = R[k][ib] <= b
-        assert b == 0 or np.any(R[k][ib] == b), f"node {i}: candidate {b} repeats candidate {b - 1}'s partition"
-        lk = np.bincount(y[ib[go_ib]], weights=cw[ib[go_ib]], minlength=K)
-        rk = nk - lk
-        lc, rc = c[ib[go_ib]].sum(), c[ib[~go_ib]].sum()
+        per = hist[v][k]
+        assert b == 0 or per[b, 0] > 0, f"node {i}: candidate {b} repeats candidate {b - 1}'s partition"
+        # each side summed over its own ranks: a class absent from a side weighs exactly 0 there (the parent's sum
+        # minus the other side's, summed in another order, may leave -1e-16, outside the impurities' domain)
+        left, right = per[:b + 1].sum(axis=0), per[b + 1:].sum(axis=0)
+        lk, rk = left[1:], right[1:]
+        lc, rc = left[0], right[0]
         slack = 1e-12 * w_root
         assert lc >= p["min_instances"] and rc >= p["min_instances"], f"node {i}: rawCount {lc}, {rc}"
         assert min(lk.sum(), rk.sum()) >= p["min_weight_fraction"] * w_root - slack, f"node {i}: weights"
@@ -338,18 +361,26 @@ def audit(tree, X, cands, sub, labels, w=None, counts=None, params=None, out=Non
         lw, rw = lk.sum(), rk.sum()
         g = imp - lw / (lw + rw) * impurity(lk, kind) - rw / (lw + rw) * impurity(rk, kind)
         assert abs(g - gain[i]) <= t, f"node {i}: gain {gain[i]!r}, recomputed {g!r}, τ = {t:.3g}"
-        cand = splits(ib)
+        cand = splits(v)
         assert cand and cand[0][0] <= g + t, f"node {i}: split {cand[0]} beats gain {g!r} by more than τ = {t:.3g}"
         if len(cand) == 1 or cand[0][0] - cand[1][0] > t:
             assert (k, b) == cand[0][1:], f"node {i}: the clear winner is {cand[0]}, the fit took ({k}, {b})"
-        parent_w[int(tree["left"][i])] = parent_w[int(tree["right"][i])] = W
-        step = send(it, R[k][rows] <= b)
-    if out is not None:
-        np.testing.assert_array_equal(np.asarray(out, np.float32), tree["value"][leaf_of].astype(np.float32))
-    if out_proba is not None:
-        np.testing.assert_array_equal(np.asarray(out_proba, np.float32).reshape(K, n),
-                                      np.asarray(tree["values"], np.float32)[leaf_of].T)
-    return audited
+        parent_w[order.index(int(tree["left"][i]))] = parent_w[order.index(int(tree["right"][i]))] = W
+    # pruned leaves: grow what the fit may have grown below them, one level of statistics per round
+    while pending:
+        need.clear()
+        left_over = []
+        for i, v, label, pw, best, t in pending:
+            ok = collapses(v, label, pw)
+            assert ok is not False, f"node {i}: a leaf, but a split of gain {best!r} > τ = {t:.3g} leads to other labels"
+            if ok is None:
+                left_over.append((i, v, label, pw, best, t))
+        pending = left_over
+        if pending:
+            more_tot, more_hist = stats(nodes, {u for u in need if nodes.depth[u] < p["max_depth"]})
+            tot.update({u: more_tot[u] for u in need})
+            hist.update(more_hist)
+    return len(order)
 
 
 def leaf_of(tree, rank_cols) -> np.ndarray:

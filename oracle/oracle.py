@@ -96,6 +96,11 @@ class Oracle:
         L.orc_r2_update.argtypes = [i32, i64, _dp, _dp, _dp, d, d, d, _dp, _dp]
         L.orc_agg_weighted_median.restype = None; L.orc_agg_weighted_median.argtypes = [i32, i64, _dp, _dp, _dp]
         L.orc_agg_weighted_mean.restype = None; L.orc_agg_weighted_mean.argtypes = [i32, i64, _dp, _dp, _dp]
+        _u8, _i32p = C.POINTER(C.c_uint8), C.POINTER(C.c_int32)
+        L.orc_ranks.restype = None; L.orc_ranks.argtypes = [i64, C.POINTER(C.c_float), i32, C.POINTER(C.c_float), _u8]
+        L.orc_tree_walk.restype = None; L.orc_tree_walk.argtypes = [i64, _u8, _i32p, _i32p, _i32p, _i32p, _i32p]
+        L.orc_tree_hist.restype = None
+        L.orc_tree_hist.argtypes = [i64, i32, _u8, i32, _dp, _dp, _dp, i32, _i32p, _i32p, _i32p, _i32p, _i32p, _dp, _dp]
         L.orc_num_threads.restype = i32
         L.orc_set_num_threads.argtypes = [i32]
 
@@ -287,3 +292,34 @@ class Oracle:
         out = np.zeros(n)
         self.lib.orc_argmax(Cn, n, _p(raw), _p(out))
         return out
+
+    # ---- audit of a fitted tree over row chunks (oracle/tree_audit.py)
+    def ranks(self, x, cands) -> np.ndarray:
+        """uint8 rank of every fp32 x among the sorted fp32 candidates (#{cand < x}; 255 for NaN)."""
+        x = np.ascontiguousarray(x, dtype=np.float32).reshape(-1)
+        c = np.ascontiguousarray(cands, dtype=np.float32).reshape(-1)
+        out = np.empty(x.size, np.uint8)
+        self.lib.orc_ranks(x.size, x.ctypes.data_as(C.POINTER(C.c_float)), c.size,
+                           c.ctypes.data_as(C.POINTER(C.c_float)), out.ctypes.data_as(C.POINTER(C.c_uint8)))
+        return out
+
+    def tree_walk(self, R, feature, bins, left, right) -> np.ndarray:
+        """Leaf index of every row of R ([S][m] uint8 ranks) in a tree (bins: rank thresholds)."""
+        R = np.ascontiguousarray(R, dtype=np.uint8)
+        a = [np.ascontiguousarray(v, dtype=np.int32) for v in (feature, bins, left, right)]
+        out = np.empty(R.shape[1], np.int32)
+        self.lib.orc_tree_walk(R.shape[1], R.ctypes.data_as(C.POINTER(C.c_uint8)),
+                               *[v.ctypes.data_as(C.POINTER(C.c_int32)) for v in a],
+                               out.ctypes.data_as(C.POINTER(C.c_int32)))
+        return out
+
+    def tree_hist(self, R, K, lab, w, c, parent, col, bins, left, hist_of, totals, hist):
+        """Adds one chunk of rows (R [S][m] uint8 ranks, fp64 labels, weights and counts, None: 1) to the statistics
+        of a node list (se_oracle.h orc_tree_hist): totals [n_nodes][stats + 2] and hist [h][S][256][stats]."""
+        R = np.ascontiguousarray(R, dtype=np.uint8)
+        lab, w, c = _f64(lab), _f64(w), _f64(c)
+        a = [np.ascontiguousarray(v, dtype=np.int32) for v in (parent, col, bins, left, hist_of)]
+        assert totals.dtype == np.float64 and totals.flags["C_CONTIGUOUS"] and hist.flags["C_CONTIGUOUS"]
+        self.lib.orc_tree_hist(R.shape[1], R.shape[0], R.ctypes.data_as(C.POINTER(C.c_uint8)), int(K), _p(lab),
+                               _p(w), _p(c), a[0].size, *[v.ctypes.data_as(C.POINTER(C.c_int32)) for v in a],
+                               _p(totals), _p(hist))

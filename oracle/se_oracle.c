@@ -734,3 +734,125 @@ void orc_argmax(int C, int64_t n, const double* raw, double* pred) {
     pred[i] = (double)am;
   }
 }
+
+/* ---- audit of a fitted tree over row chunks (oracle/tree_audit.py) ---- */
+
+void orc_ranks(int64_t m, const float* x, int ncand, const float* cand, uint8_t* out) {
+#ifdef _OPENMP
+#pragma omp parallel for schedule(static)
+#endif
+  for (int64_t i = 0; i < m; ++i) {
+    const float v = x[i];
+    if (isnan(v)) { out[i] = 255; continue; }
+    int lo = 0, hi = ncand; /* first candidate >= v */
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (cand[mid] < v) lo = mid + 1; else hi = mid;
+    }
+    out[i] = (uint8_t)lo;
+  }
+}
+
+void orc_tree_walk(int64_t m, const uint8_t* R, const int32_t* feature, const int32_t* bin, const int32_t* left,
+                   const int32_t* right, int32_t* leaf) {
+#ifdef _OPENMP
+#pragma omp parallel for schedule(static)
+#endif
+  for (int64_t i = 0; i < m; ++i) {
+    int v = 0;
+    while (feature[v] >= 0) v = (int)R[(int64_t)feature[v] * m + i] <= bin[v] ? left[v] : right[v];
+    leaf[i] = v;
+  }
+}
+
+/* The rows of node v are the rows of parent[v] whose rank in column col[v] is <= bin[v] (left[v] != 0) or > bin[v].
+ * Each row is routed depth first from node 0 through every node it belongs to; a row may belong to several children of
+ * one node (alternative splits).  Rows are visited in order and each column is one task, so the sums do not depend on
+ * the thread count. */
+void orc_tree_hist(int64_t m, int S, const uint8_t* R, int K, const double* lab, const double* w, const double* c,
+                   int n_nodes, const int32_t* parent, const int32_t* col, const int32_t* bin, const int32_t* left,
+                   const int32_t* hist_of, double* totals, double* hist) {
+  const int ns = K > 0 ? K + 1 : 4, nt = ns + 2;
+  int32_t* first = (int32_t*)malloc(sizeof(int32_t) * (size_t)n_nodes);
+  int32_t* next = (int32_t*)malloc(sizeof(int32_t) * (size_t)n_nodes);
+  for (int v = 0; v < n_nodes; ++v) first[v] = next[v] = -1;
+  for (int v = n_nodes - 1; v >= 1; --v) { next[v] = first[parent[v]]; first[parent[v]] = v; }
+  int64_t* start = (int64_t*)calloc((size_t)m + 1, sizeof(int64_t));
+  /* pass 1 counts the nodes of each row, pass 2 lists them (CSR) */
+  for (int pass = 0; pass < 2; ++pass) {
+    int32_t* vis = NULL;
+    if (pass == 1) {
+      for (int64_t i = 0; i < m; ++i) start[i + 1] += start[i];
+      vis = (int32_t*)malloc(sizeof(int32_t) * (size_t)(start[m] > 0 ? start[m] : 1));
+    }
+#ifdef _OPENMP
+#pragma omp parallel
+#endif
+    {
+      int32_t* stack = (int32_t*)malloc(sizeof(int32_t) * (size_t)n_nodes);
+#ifdef _OPENMP
+#pragma omp for schedule(static)
+#endif
+      for (int64_t i = 0; i < m; ++i) {
+        int64_t k = 0;
+        if (c && !(c[i] > 0.0)) { if (pass == 0) start[i + 1] = 0; continue; }
+        int sp = 0;
+        stack[sp++] = 0;
+        while (sp) {
+          const int v = stack[--sp];
+          if (pass == 1) vis[start[i] + k] = v;
+          ++k;
+          for (int u = first[v]; u >= 0; u = next[u]) {
+            const int go = (int)R[(int64_t)col[u] * m + i] <= bin[u];
+            if (go == (left[u] != 0)) stack[sp++] = u;
+          }
+        }
+        if (pass == 0) start[i + 1] = k;
+      }
+      free(stack);
+    }
+    if (pass == 1) {
+      /* task S: the node totals; task k < S: column k of every histogram */
+#ifdef _OPENMP
+#pragma omp parallel for schedule(dynamic, 1)
+#endif
+      for (int k = 0; k <= S; ++k) {
+        double s[4];
+        for (int64_t i = 0; i < m; ++i) {
+          if (start[i + 1] == start[i]) continue;
+          const double ci = c ? c[i] : 1.0, cw = ci * (w ? w[i] : 1.0);
+          int y = 0;
+          if (K > 0) {
+            y = (int)lab[i];
+            s[0] = ci;
+          } else {
+            const double cwr = cw * lab[i];
+            s[0] = ci; s[1] = cw; s[2] = cwr; s[3] = cwr * lab[i];
+          }
+          for (int64_t q = start[i]; q < start[i + 1]; ++q) {
+            const int v = vis[q];
+            double* o;
+            if (k == S) {
+              o = totals + (int64_t)v * nt;
+              o[ns] += K > 0 ? 0.0 : cw * fabs(lab[i]);
+              o[ns + 1] += 1.0;
+            } else {
+              if (hist_of[v] < 0) continue;
+              o = hist + (((int64_t)hist_of[v] * S + k) * 256 + R[(int64_t)k * m + i]) * ns;
+            }
+            if (K > 0) {
+              o[0] += s[0];
+              o[1 + y] += cw;
+            } else {
+              o[0] += s[0]; o[1] += s[1]; o[2] += s[2]; o[3] += s[3];
+            }
+          }
+        }
+      }
+      free(vis);
+    }
+  }
+  free(start);
+  free(first);
+  free(next);
+}

@@ -124,6 +124,22 @@ void orc_agg_weighted_mean(int M, int64_t n, const double* P, const double* a, d
 /* Spark ClassificationModel.raw2prediction = argmax (first maximum). raw[C][n] -> pred[n] */
 void orc_argmax(int C, int64_t n, const double* raw, double* pred);
 
+/* ---- audit of a fitted tree over row chunks (oracle/tree_audit.py) ----
+ * orc_ranks: out[i] = #{cand < x[i]} (the rank of x[i] among ncand sorted fp32 candidates), 255 for NaN.
+ * orc_tree_walk: leaf[i] = the node where row i stops walking a tree over the ranks R[S][m] (left when rank <= bin).
+ * orc_tree_hist: adds the rows [0, m) of a chunk to the fp64 statistics of every node of a node list (node 0 the
+ * root; node v > 0 holds the rows of parent[v] < v whose rank in column col[v] is <= bin[v] when left[v], > bin[v]
+ * otherwise; a row may reach several children of one node).  Only rows with c > 0 count (c NULL: all, as 1).  Per
+ * row, K == 0 (regression, lab = label): (c, c·w, c·w·lab, c·w·lab²); K >= 2 (lab = class index): (c, c·w in class
+ * lab), ns = 4 or K + 1 values.  totals[n_nodes][ns + 2] gets the node's sums, then Σ c·w·|lab| (regression) and its
+ * row count; hist[h][S][256][ns] (h = hist_of[v] >= 0) the sums per column and rank. */
+void orc_ranks(int64_t m, const float* x, int ncand, const float* cand, uint8_t* out);
+void orc_tree_walk(int64_t m, const uint8_t* R, const int32_t* feature, const int32_t* bin, const int32_t* left,
+                   const int32_t* right, int32_t* leaf);
+void orc_tree_hist(int64_t m, int S, const uint8_t* R, int K, const double* lab, const double* w, const double* c,
+                   int n_nodes, const int32_t* parent, const int32_t* col, const int32_t* bin, const int32_t* left,
+                   const int32_t* hist_of, double* totals, double* hist);
+
 /* number of OpenMP threads the library will use (1 when built without -fopenmp) */
 int orc_num_threads(void);
 void orc_set_num_threads(int t);

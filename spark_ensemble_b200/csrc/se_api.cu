@@ -252,6 +252,9 @@ struct se_ctx {
   int tree_mask = 1;                  // shallow trees (<= 64 internal nodes): all-nodes comparison kernel over the rank matrix
   int last_tree_mask = 0;
   int last_tree_binned = 0, last_tree_rebinned_cols = 0;
+  // the last tree fit's histogram path per level L, in octal digit L: 0 several columns per CTA in shared memory, 1 one
+  // column per CTA, 2 one column with opt-in shared memory at 2 CTAs/SM, 3 the same at 1 CTA/SM, 4 global fp64 atomics
+  int64_t last_tree_fit_hist = 0;
   // regression-tree fit (se_tree_fit): scratch kept across the rounds of a fit
   struct {
     uint16_t* d_nid = nullptr;        // two [nid_cap] node-index buffers (levels alternate)
@@ -901,7 +904,7 @@ int se_ctx_kernel_time_reset(se_ctx* ctx) {
 
 namespace {
 struct OptKey { const char* name; int id; };
-enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS,
+enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_LAST_TREE_FIT_HIST, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS,
        OPT_PEER_TIMEOUT_MS, OPT_ALTERNATE, OPT_L2_HINTS, OPT_CTAS_PER_SM, OPT_HOST_MIRROR,
        // read-only diagnostics
        OPT_LAST_ROUND_FUSED, OPT_LAST_LS_WORKERS, OPT_LAST_LS_PASSES, OPT_LAST_LS_HIT_RATIO, OPT_LAST_FUSED_GRID,
@@ -909,6 +912,7 @@ enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, O
 const OptKey kOpts[] = {
   {"last_forest_chunks", OPT_LAST_FOREST_CHUNKS}, {"wm_fast", OPT_WM_FAST}, {"wm_list_cap", OPT_WM_LIST_CAP}, {"last_wm_mode", OPT_LAST_WM_MODE}, {"last_wm_deferred", OPT_LAST_WM_DEFERRED},
   {"tree_bins", OPT_TREE_BINS}, {"tree_mask", OPT_TREE_MASK}, {"last_tree_mask", OPT_LAST_TREE_MASK}, {"last_tree_binned", OPT_LAST_TREE_BINNED}, {"last_tree_rebinned_cols", OPT_LAST_TREE_REBINNED},
+  {"last_tree_fit_hist", OPT_LAST_TREE_FIT_HIST},
   {"fused_loss_reduce", OPT_FUSED_LOSS_REDUCE}, {"fused_timing", OPT_FUSED_TIMING}, {"last_fused_stats_us", OPT_LAST_FUSED_US0}, {"last_fused_brent_us", OPT_LAST_FUSED_US1},
   {"last_fused_update_us", OPT_LAST_FUSED_US2}, {"fused_round", OPT_FUSED_ROUND}, {"fused_round_max_rows", OPT_FUSED_MAX_ROWS}, {"fused_ctas_per_sm", OPT_FUSED_CTAS},
   {"fused_resident", OPT_FUSED_RESIDENT},
@@ -983,6 +987,7 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_TREE_MASK: *value = ctx->last_tree_mask; break;
     case OPT_LAST_TREE_BINNED: *value = ctx->last_tree_binned; break;
     case OPT_LAST_TREE_REBINNED: *value = ctx->last_tree_rebinned_cols; break;
+    case OPT_LAST_TREE_FIT_HIST: *value = (double)ctx->last_tree_fit_hist; break;
     case OPT_LAST_FUSED_US0: *value = ctx->last_fused_us[0]; break;
     case OPT_LAST_FUSED_US1: *value = ctx->last_fused_us[1]; break;
     case OPT_LAST_FUSED_US2: *value = ctx->last_fused_us[2]; break;
@@ -3299,6 +3304,7 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
   a.cw = T.d_cw; a.prob = T.d_prob; a.prn = T.d_prn;
   uint16_t* nid[2] = {T.d_nid, T.d_nid + T.nid_cap};
   SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, ctx->stream));
+  ctx->last_tree_fit_hist = 0;
   for (int L = 0; L <= top; ++L) {
     a.L = L;
     a.route = L >= 1;
@@ -3319,6 +3325,8 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
       per_sm = 8;
     }
     if (smem_mode) smem = per_col * (size_t)a.cb;
+    const int path = !smem_mode ? 4 : per_col > (size_t)kTreeFitSmemBudget ? (per_sm == 2 ? 2 : 3) : (a.cb > 1 ? 0 : 1);
+    ctx->last_tree_fit_hist |= (int64_t)path << (3 * L);
     const int gx = smem_mode ? (n_subspace + a.cb - 1) / a.cb : 1;
     int64_t gy = ((int64_t)ctx->sms * per_sm + gx - 1) / gx;
     gy = std::min<int64_t>(gy, (nw + 255) / 256);
