@@ -435,6 +435,26 @@ SE_API int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, in
                                   int out_kind, int out_slot, int out_row, int max_nodes, int32_t* feature,
                                   float* threshold, int32_t* left, int32_t* right, float* value, float* proba,
                                   double* class_weights, double* gain, int* n_nodes);
+/* ---- several trees at once (DESIGN.md §3 "Device forest fit") --------------------------------------------------- */
+/* Fits n_trees trees that share the labels (row label_row of label_slot), the weights (row weight_row of weight_slot,
+ * or none when weight_slot < 0), the bag (SE_SLOT_BAG when use_bag), the candidates of se_tree_fit_bins and max_depth,
+ * min_instances, min_info_gain, min_weight_fraction; tree t searches its own subspace
+ * sub_cols[sub_offsets[t] .. sub_offsets[t + 1]) (sub_offsets[0] == 0, every subspace non-empty).  num_classes == 0:
+ * regression trees (se_tree_fit); 2..64: classification trees with impurity gini or entropy (se_tree_fit_classifier).
+ * Tree t comes back at entry t · max_nodes of every array (proba and class_weights at t · max_nodes · K) in the form
+ * the one-tree call returns (BFS order, subspace-local features), with its node count in n_nodes[t]; it equals that
+ * call's tree for subspace t up to the order of fp64 atomic additions.  No per-row output is written.  The trees are
+ * fitted in batches of at most 64 whose node ids (4 B/row per tree) and deepest histograms fit half of the free device
+ * memory: one launch sequence and one download of the records per batch (read-only option last_forest_fit_batches).
+ * Bounds as se_tree_fit's; an empty subspace, a bad column or a tree of more than max_nodes nodes fails with
+ * SE_ERR_ARG / SE_ERR_STATE naming the tree.  The batches' node-id and histogram scratch is freed when the call returns.
+ * Not collective: with a communicator of two or more ranks attached it fails with SE_ERR_STATE.  gain, proba (for
+ * regression) and class_weights may be NULL. */
+SE_API int se_forest_fit(se_ctx* ctx, int n_trees, const int32_t* sub_offsets, const int32_t* sub_cols, int label_slot,
+                         int label_row, int weight_slot, int weight_row, int use_bag, int num_classes, int impurity,
+                         int max_depth, int min_instances, double min_info_gain, double min_weight_fraction,
+                         int max_nodes, int32_t* feature, float* threshold, int32_t* left, int32_t* right, float* value,
+                         float* proba, double* class_weights, double* gain, int* n_nodes);
 /* linear model: out = intercept + Σ_j coef[j]·X[subspace[j]] */
 SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,
                       const int32_t* subspace, int out_slot, int out_row);

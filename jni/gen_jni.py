@@ -152,6 +152,7 @@ NOT_BOUND = {
     "se_tree_fit_bins": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
     "se_tree_fit": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
     "se_tree_fit_classifier": "the JVM train() keeps Spark's own trees; a Scala learner over the device tree fit is a follow-up",
+    "se_forest_fit": "the JVM bagging train() keeps Spark's own trees; a Scala binding of the forest fit is a follow-up",
 }
 
 HAND_CPP = r'''

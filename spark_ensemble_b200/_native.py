@@ -123,6 +123,8 @@ PROTOTYPES = {
                     _ip, _fp, _ip, _ip, _fp, _dp, C.POINTER(_i32)],
     "se_tree_fit_classifier": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _i32, _i32, _d, _d, _i32,
                                _i32, _i32, _i32, _ip, _fp, _ip, _ip, _fp, _fp, _dp, _dp, C.POINTER(_i32)],
+    "se_forest_fit": [_vp, _i32, _ip, _ip, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _d, _d, _i32,
+                      _ip, _fp, _ip, _ip, _fp, _fp, _dp, _dp, _ip],
 }
 _RESTYPES = {"se_last_error": C.c_char_p}
 

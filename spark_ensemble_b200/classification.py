@@ -16,8 +16,8 @@ from .ensemble import DataFrame, fit_dummy_classifier, java_string_hash, subspac
 from .gbm_engine import GBMEngine
 from .params import (Param, Params, ParamValidators, boosting_params, gbm_params, random_uid,
                      shared_classifier_params, shared_predictor_params, subbag_params)
-from .regression import (_check_device_learner, _device_trees, _extract_instances, _rank_matrix_full,
-                         _resident_context, _split_validation, bag_counts)
+from .regression import (_bagging_forest_fit, _check_device_learner, _device_trees, _extract_instances,
+                         _rank_matrix_full, _resident_context, _split_validation, bag_counts)
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -400,7 +400,9 @@ BoostingClassificationModel._declare(_p + _pc + _pb + _pboost + [Param("seed", "
 
 # ================================================================================ BaggingClassifier
 class BaggingClassifier(Params):
-    """classification/BaggingClassifier.scala:106-207. Only the model's predictRaw is on the hot path."""
+    """classification/BaggingClassifier.scala:106-207.  With residentFeatures and a device tree learner every member's
+    tree grows in one forest fit over the device-resident features (regression._bagging_forest_fit); otherwise
+    train is one learner.fit per member."""
 
     def __init__(self, uid: str | None = None, device: int = 0):
         super().__init__(uid or random_uid("BaggingClassifier"))
@@ -417,7 +419,11 @@ class BaggingClassifier(Params):
                   else (rng.random(n) < self("subsampleRatio"))).astype(np.float64)
         bw = counts if w is None else counts * w
         keep = bw > 0
-        models = [self("baseLearner").fit(X[keep][:, subs[i]], y[keep], bw[keep], num_classes=K) for i in range(M)]
+        learner = self("baseLearner")
+        if bool(self("residentFeatures")) and getattr(learner, "device_learner", False):
+            models = _bagging_forest_fit(self.device, learner, X, y, bw, subs, num_classes=K)
+        else:
+            models = [learner.fit(X[keep][:, subs[i]], y[keep], bw[keep], num_classes=K) for i in range(M)]
         m = BaggingClassificationModel(K, subs, models, device=self.device)
         self._copyValues(m)
         m.parent = self

@@ -522,3 +522,47 @@ class Context:
         k = nn.value
         return {"feature": f[:k].copy(), "threshold": t[:k].copy(), "left": l[:k].copy(), "right": r[:k].copy(),
                 "value": v[:k].copy(), "values": p[:k].copy(), "class_weights": cw[:k].copy(), "gain": g[:k].copy()}
+
+    def forest_fit(self, subspaces, label_slot: int, label_row: int = 0, weight_slot: int = -1, weight_row: int = 0,
+                   use_bag: bool = False, num_classes: int = 0, impurity: str = "gini", max_depth: int = 5,
+                   min_instances: int = 1, min_info_gain: float = 0.0, min_weight_fraction: float = 0.0) -> list:
+        """Fits one tree per subspace over the same labels, weights and bag (se_forest_fit): regression trees when
+        num_classes is 0, classification trees for 2..64 classes.  Returns one dict per tree, in the form tree_fit
+        (regression) or tree_fit_classifier returns; no per-row output is written."""
+        imp = {"gini": 0, "entropy": 1}.get(str(impurity).lower())
+        if imp is None:
+            raise ValueError(f"impurity must be gini or entropy, got {impurity!r}")
+        subs = [np.ascontiguousarray(s, dtype=np.int32).reshape(-1) for s in subspaces]
+        T = len(subs)
+        offs = np.zeros(T + 1, dtype=np.int32)
+        offs[1:] = np.cumsum([s.size for s in subs])
+        cols = np.ascontiguousarray(np.concatenate(subs) if T else np.zeros(0), dtype=np.int32)
+        K = int(num_classes)
+        cap = (1 << (int(max_depth) + 1)) - 1 if 0 <= int(max_depth) <= 8 else 1
+        kk = K if 0 < K <= 64 else 1
+        tt = max(T, 1)
+        f = np.zeros((tt, cap), dtype=np.int32)
+        t = np.zeros((tt, cap), dtype=np.float32)
+        l = np.zeros((tt, cap), dtype=np.int32)
+        r = np.zeros((tt, cap), dtype=np.int32)
+        v = np.zeros((tt, cap), dtype=np.float32)
+        p = np.zeros((tt, cap, kk), dtype=np.float32)
+        cw = np.zeros((tt, cap, kk), dtype=np.float64)
+        g = np.zeros((tt, cap), dtype=np.float64)
+        nn = np.zeros(tt, dtype=np.int32)
+        self._ck(self._lib.se_forest_fit(
+            self._h, T, N.iptr(offs), N.iptr(cols) if cols.size else None, int(label_slot), int(label_row),
+            int(weight_slot), int(weight_row), int(bool(use_bag)), K, imp, int(max_depth), int(min_instances),
+            float(min_info_gain), float(min_weight_fraction), cap, N.iptr(f), N.fptr(t), N.iptr(l), N.iptr(r),
+            N.fptr(v), N.fptr(p) if K else None, N.dptr(cw) if K else None, N.dptr(g), N.iptr(nn)))
+        out = []
+        for i in range(T):
+            k = int(nn[i])
+            d = {"feature": f[i, :k].copy(), "threshold": t[i, :k].copy(), "left": l[i, :k].copy(),
+                 "right": r[i, :k].copy(), "value": v[i, :k].copy()}
+            if K:
+                d["values"] = p[i, :k].copy()
+                d["class_weights"] = cw[i, :k].copy()
+            d["gain"] = g[i, :k].copy()
+            out.append(d)
+        return out

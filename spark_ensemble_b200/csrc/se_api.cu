@@ -255,20 +255,24 @@ struct se_ctx {
   // the last tree fit's histogram path per level L, in octal digit L: 0 several columns per CTA in shared memory, 1 one
   // column per CTA, 2 one column with opt-in shared memory at 2 CTAs/SM, 3 the same at 1 CTA/SM, 4 global fp64 atomics
   int64_t last_tree_fit_hist = 0;
-  // regression-tree fit (se_tree_fit): scratch kept across the rounds of a fit
+  int last_forest_fit_batches = 0;    // launch sequences of the last se_forest_fit
+  // tree fits (se_tree_fit, se_forest_fit): scratch kept across the rounds of a fit, for up to *_trees trees at once
   struct {
-    uint16_t* d_nid = nullptr;        // two [nid_cap] node-index buffers (levels alternate)
+    uint16_t* d_nid = nullptr;        // per tree two [nid_cap] node-index buffers (levels alternate)
     int64_t nid_cap = 0;
+    int nid_trees = 0;
     double* d_hist = nullptr;
     size_t hist_bytes = 0;
-    TreeFitNode* d_nodes = nullptr;   // [kTreeFitHeap]
-    uint2* d_dec = nullptr;           // [kTreeFitHeap]
-    int32_t* d_cols = nullptr;
+    TreeFitNode* d_nodes = nullptr;   // [rec_trees][kTreeFitHeap]
+    uint2* d_dec = nullptr;           // [rec_trees][kTreeFitHeap]
+    int rec_trees = 0;
+    int32_t* d_cols = nullptr;        // the trees' subspace columns, then their T + 1 offsets
     int cols_cap = 0;
     int smem_optin = 0;
-    double* d_cw = nullptr;           // classification: [kTreeFitHeap][kTreeFitMaxClasses]
-    float* d_prob = nullptr;          // [kTreeFitHeap][kTreeFitMaxClasses]
-    int4* d_prn = nullptr;            // [kTreeFitHeap]
+    double* d_cw = nullptr;           // classification: [cls_trees][kTreeFitHeap][kTreeFitMaxClasses]
+    float* d_prob = nullptr;          // [cls_trees][kTreeFitHeap][kTreeFitMaxClasses]
+    int4* d_prn = nullptr;            // [cls_trees][kTreeFitHeap]
+    int cls_trees = 0;
   } tf;
   std::string err;
   // stopwatch + per-kernel-family timing
@@ -904,7 +908,7 @@ int se_ctx_kernel_time_reset(se_ctx* ctx) {
 
 namespace {
 struct OptKey { const char* name; int id; };
-enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_LAST_TREE_FIT_HIST, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS,
+enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, OPT_LAST_WM_DEFERRED, OPT_TREE_MASK, OPT_LAST_TREE_MASK, OPT_TREE_BINS, OPT_LAST_TREE_BINNED, OPT_LAST_TREE_REBINNED, OPT_LAST_TREE_FIT_HIST, OPT_LAST_FOREST_FIT_BATCHES, OPT_FUSED_LOSS_REDUCE, OPT_FUSED_TIMING, OPT_LAST_FUSED_US0, OPT_LAST_FUSED_US1, OPT_LAST_FUSED_US2, OPT_FUSED_ROUND, OPT_FUSED_MAX_ROWS, OPT_FUSED_CTAS, OPT_FUSED_RESIDENT, OPT_LS_MODE, OPT_LS_RESIDENT, OPT_LS_CTAS,
        OPT_PEER_TIMEOUT_MS, OPT_ALTERNATE, OPT_L2_HINTS, OPT_CTAS_PER_SM, OPT_HOST_MIRROR,
        // read-only diagnostics
        OPT_LAST_ROUND_FUSED, OPT_LAST_LS_WORKERS, OPT_LAST_LS_PASSES, OPT_LAST_LS_HIT_RATIO, OPT_LAST_FUSED_GRID,
@@ -912,7 +916,7 @@ enum { OPT_LAST_FOREST_CHUNKS, OPT_WM_FAST, OPT_WM_LIST_CAP, OPT_LAST_WM_MODE, O
 const OptKey kOpts[] = {
   {"last_forest_chunks", OPT_LAST_FOREST_CHUNKS}, {"wm_fast", OPT_WM_FAST}, {"wm_list_cap", OPT_WM_LIST_CAP}, {"last_wm_mode", OPT_LAST_WM_MODE}, {"last_wm_deferred", OPT_LAST_WM_DEFERRED},
   {"tree_bins", OPT_TREE_BINS}, {"tree_mask", OPT_TREE_MASK}, {"last_tree_mask", OPT_LAST_TREE_MASK}, {"last_tree_binned", OPT_LAST_TREE_BINNED}, {"last_tree_rebinned_cols", OPT_LAST_TREE_REBINNED},
-  {"last_tree_fit_hist", OPT_LAST_TREE_FIT_HIST},
+  {"last_tree_fit_hist", OPT_LAST_TREE_FIT_HIST}, {"last_forest_fit_batches", OPT_LAST_FOREST_FIT_BATCHES},
   {"fused_loss_reduce", OPT_FUSED_LOSS_REDUCE}, {"fused_timing", OPT_FUSED_TIMING}, {"last_fused_stats_us", OPT_LAST_FUSED_US0}, {"last_fused_brent_us", OPT_LAST_FUSED_US1},
   {"last_fused_update_us", OPT_LAST_FUSED_US2}, {"fused_round", OPT_FUSED_ROUND}, {"fused_round_max_rows", OPT_FUSED_MAX_ROWS}, {"fused_ctas_per_sm", OPT_FUSED_CTAS},
   {"fused_resident", OPT_FUSED_RESIDENT},
@@ -988,6 +992,7 @@ int se_ctx_get_option(const se_ctx* ctx, const char* key, double* value) {
     case OPT_LAST_TREE_BINNED: *value = ctx->last_tree_binned; break;
     case OPT_LAST_TREE_REBINNED: *value = ctx->last_tree_rebinned_cols; break;
     case OPT_LAST_TREE_FIT_HIST: *value = (double)ctx->last_tree_fit_hist; break;
+    case OPT_LAST_FOREST_FIT_BATCHES: *value = ctx->last_forest_fit_batches; break;
     case OPT_LAST_FUSED_US0: *value = ctx->last_fused_us[0]; break;
     case OPT_LAST_FUSED_US1: *value = ctx->last_fused_us[1]; break;
     case OPT_LAST_FUSED_US2: *value = ctx->last_fused_us[2]; break;
@@ -3110,8 +3115,37 @@ struct TreeFitPlan {
   float* out = nullptr;
   int64_t n = 0, nw = 0, ld_out = 0;
   int nb = 0, sw = 0, top = 0;
+  int n_trees = 0, total_cols = 0, max_cols = 0;  // the trees' subspaces: summed and largest size
   uint32_t hash = 0;  // 24 bits: the subspace, its columns' candidates and the validity rules
 };
+
+// The rank matrix holds the split candidates of a fit for the feature matrix as it is now.
+int tree_fit_bins_ready(se_ctx* ctx) {
+  const SlotBuf& X = ctx->slot[SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
+  const BinState& B = ctx->bins[0];
+  SE_REQUIRE(ctx, B.d8 && B.d == X.rows && B.n == X.cols, SE_ERR_STATE,
+             "no split candidates for this feature matrix: call se_tree_fit_bins first");
+  return SE_OK;
+}
+
+// One tree's subspace (cols null: columns 0 .. S - 1); tree >= 0 names the tree of a forest fit in the messages.
+int tree_fit_check_subspace(se_ctx* ctx, const int32_t* cols, int S, int tree) {
+  char who[32] = "";
+  if (tree >= 0) snprintf(who, sizeof(who), "tree %d: ", tree);
+  SE_REQUIRE(ctx, S >= 1, SE_ERR_ARG, "%sempty subspace", who);
+  const SlotBuf& X = ctx->slot[SE_SLOT_X];
+  const BinState& B = ctx->bins[0];
+  for (int k = 0; k < S; ++k) {
+    const int32_t c = cols ? cols[k] : k;
+    SE_REQUIRE(ctx, c >= 0 && c < X.rows, SE_ERR_ARG, "%ssubspace entry %d: column %d outside X with %lld columns", who,
+               k, c, (long long)X.rows);
+    SE_REQUIRE(ctx, B.fit[c], SE_ERR_STATE,
+               "%scolumn %d does not hold the fit's split candidates (never set, or a tree walk added a threshold to "
+               "it): call se_tree_fit_bins again", who, c);
+  }
+  return SE_OK;
+}
 
 // FNV-1a over 32-bit words
 inline uint32_t fnv_words(uint32_t h, const void* p, size_t words) {
@@ -3121,12 +3155,15 @@ inline uint32_t fnv_words(uint32_t h, const void* p, size_t words) {
   return h;
 }
 
-// The checks, the scratch and the uploads of a fit: everything that depends on this rank alone.  Under a communicator
-// its failure is not returned to the caller straight away: tree_fit_agree tells every rank first.
+// The checks, the scratch and the uploads of a fit of n_trees trees, tree t over sub_cols[sub_off[t] .. sub_off[t + 1])
+// (sub_cols null: columns 0 .. S - 1 of the one tree): everything that depends on this rank alone.  Under a
+// communicator its failure is not returned to the caller straight away: tree_fit_agree tells every rank first.
+// with_out: the fit writes every row's output into out_slot (the forest fit writes none).  first_tree: the index of
+// tree 0 in a forest fit's messages (-1: a one-tree fit, whose messages name no tree).
 int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_slot, int label_row, int weight_slot,
-                     int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth,
-                     int min_instances, double min_info_gain, double min_weight_fraction, int out_slot, int out_row,
-                     TreeFitPlan& P) {
+                     int weight_row, int use_bag, int n_trees, int first_tree, const int32_t* sub_off,
+                     const int32_t* sub_cols, int max_depth, int min_instances, double min_info_gain,
+                     double min_weight_fraction, bool with_out, int out_slot, int out_row, TreeFitPlan& P) {
   SE_REQUIRE(ctx, max_depth >= 0 && max_depth <= 8, SE_ERR_ARG, "maxDepth %d outside [0, 8]", max_depth);
   SE_REQUIRE(ctx, min_instances >= 1, SE_ERR_ARG, "minInstancesPerNode %d < 1", min_instances);
   SE_REQUIRE(ctx, min_weight_fraction >= 0.0 && min_weight_fraction < 0.5, SE_ERR_ARG,
@@ -3147,22 +3184,23 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   SE_TRY(row_of(label_slot, label_row, "label", &r));
   if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &w));
   if (use_bag) SE_TRY(row_of(SE_SLOT_BAG, 0, "bag", &bag));
-  SE_REQUIRE(ctx, n_subspace >= 1, SE_ERR_ARG, "empty subspace");
+  SE_REQUIRE(ctx, sub_off[0] == 0 && sub_off[n_trees] - sub_off[0] >= 1, SE_ERR_ARG, "empty subspace");
+  SE_TRY(tree_fit_bins_ready(ctx));
   BinState& B = ctx->bins[0];
-  SE_REQUIRE(ctx, B.d8 && B.d == X.rows && B.n == X.cols, SE_ERR_STATE,
-             "no split candidates for this feature matrix: call se_tree_fit_bins first");
-  std::vector<int32_t> cols((size_t)n_subspace);
-  int maxc = 0;
-  for (int k = 0; k < n_subspace; ++k) {
-    const int32_t c = subspace ? subspace[k] : k;
-    SE_REQUIRE(ctx, c >= 0 && c < X.rows, SE_ERR_ARG, "subspace entry %d: column %d outside X with %lld columns", k, c,
-               (long long)X.rows);
-    SE_REQUIRE(ctx, B.fit[c], SE_ERR_STATE,
-               "column %d does not hold the fit's split candidates (never set, or a tree walk added a threshold to it): "
-               "call se_tree_fit_bins again", c);
-    cols[k] = c;
-    maxc = std::max(maxc, (int)B.edges[c].size());
+  const int total = sub_off[n_trees];
+  std::vector<int32_t> cols((size_t)total + (size_t)n_trees + 1);  // the columns, then the offsets: one upload
+  int maxc = 0, maxS = 0;
+  for (int t = 0; t < n_trees; ++t) {
+    const int S = sub_off[t + 1] - sub_off[t];
+    SE_TRY(tree_fit_check_subspace(ctx, sub_cols ? sub_cols + sub_off[t] : nullptr, S, first_tree >= 0 ? first_tree + t : -1));
+    maxS = std::max(maxS, S);
+    for (int k = sub_off[t]; k < sub_off[t + 1]; ++k) {
+      const int32_t c = sub_cols ? sub_cols[k] : k;
+      cols[k] = c;
+      maxc = std::max(maxc, (int)B.edges[c].size());
+    }
   }
+  for (int t = 0; t <= n_trees; ++t) cols[(size_t)total + t] = sub_off[t];
   const int nb = std::min(256, maxc + 2);  // ranks 0..maxc, then NaN (rank 255) in the last bin
   SE_TRY(begin(ctx));
   SE_TRY(read_slot(ctx, label_slot));
@@ -3172,43 +3210,55 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   // ---- scratch
   auto& T = ctx->tf;
   const int64_t nw = (n + 3) >> 2;
-  if (T.nid_cap < 4 * nw) {
+  if (T.nid_cap < 4 * nw || T.nid_trees < n_trees) {
     if (T.d_nid) cudaFree(T.d_nid);
-    T.d_nid = nullptr; T.nid_cap = 0;
-    SE_CUDA(ctx, cudaMalloc(&T.d_nid, sizeof(uint16_t) * 2 * 4 * (size_t)nw));
+    T.d_nid = nullptr; T.nid_cap = 0; T.nid_trees = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_nid, sizeof(uint16_t) * 2 * 4 * (size_t)nw * (size_t)n_trees));
     T.nid_cap = 4 * nw;
+    T.nid_trees = n_trees;
   }
   const int top = max_depth > 0 ? max_depth - 1 : 0;  // deepest level that is searched (or, at depth 0, only summed)
   const int sw = K > 0 ? K + (w ? 1 : 0) : 4;  // doubles per histogram bin
-  const size_t hist_bytes = ((size_t)1 << top) * (size_t)n_subspace * (size_t)nb * (size_t)sw * sizeof(double);
+  const size_t hist_bytes = ((size_t)1 << top) * (size_t)total * (size_t)nb * (size_t)sw * sizeof(double);
   if (T.hist_bytes < hist_bytes) {
     if (T.d_hist) cudaFree(T.d_hist);
     T.d_hist = nullptr; T.hist_bytes = 0;
     SE_CUDA(ctx, cudaMalloc(&T.d_hist, hist_bytes));
     T.hist_bytes = hist_bytes;
   }
-  if (!T.d_nodes) {
-    SE_CUDA(ctx, cudaMalloc(&T.d_nodes, sizeof(TreeFitNode) * kTreeFitHeap));
-    SE_CUDA(ctx, cudaMalloc(&T.d_dec, sizeof(uint2) * kTreeFitHeap));
+  if (T.rec_trees < n_trees) {
+    if (T.d_nodes) cudaFree(T.d_nodes);
+    if (T.d_dec) cudaFree(T.d_dec);
+    T.d_nodes = nullptr; T.d_dec = nullptr; T.rec_trees = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_nodes, sizeof(TreeFitNode) * kTreeFitHeap * (size_t)n_trees));
+    SE_CUDA(ctx, cudaMalloc(&T.d_dec, sizeof(uint2) * kTreeFitHeap * (size_t)n_trees));
+    T.rec_trees = n_trees;
     int optin = 0;
     SE_CUDA(ctx, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     T.smem_optin = optin;
   }
-  if (K > 0 && !T.d_cw) {
-    SE_CUDA(ctx, cudaMalloc(&T.d_cw, sizeof(double) * kTreeFitHeap * kTreeFitMaxClasses));
-    SE_CUDA(ctx, cudaMalloc(&T.d_prob, sizeof(float) * kTreeFitHeap * kTreeFitMaxClasses));
-    SE_CUDA(ctx, cudaMalloc(&T.d_prn, sizeof(int4) * kTreeFitHeap));
+  if (K > 0 && T.cls_trees < n_trees) {
+    if (T.d_cw) cudaFree(T.d_cw);
+    if (T.d_prob) cudaFree(T.d_prob);
+    if (T.d_prn) cudaFree(T.d_prn);
+    T.d_cw = nullptr; T.d_prob = nullptr; T.d_prn = nullptr; T.cls_trees = 0;
+    SE_CUDA(ctx, cudaMalloc(&T.d_cw, sizeof(double) * kTreeFitHeap * kTreeFitMaxClasses * (size_t)n_trees));
+    SE_CUDA(ctx, cudaMalloc(&T.d_prob, sizeof(float) * kTreeFitHeap * kTreeFitMaxClasses * (size_t)n_trees));
+    SE_CUDA(ctx, cudaMalloc(&T.d_prn, sizeof(int4) * kTreeFitHeap * (size_t)n_trees));
+    T.cls_trees = n_trees;
   }
-  if (T.cols_cap < n_subspace) {
+  const int ncols = (int)cols.size();
+  if (T.cols_cap < ncols) {
     if (T.d_cols) cudaFree(T.d_cols);
     T.d_cols = nullptr; T.cols_cap = 0;
-    SE_CUDA(ctx, cudaMalloc(&T.d_cols, sizeof(int32_t) * (size_t)n_subspace));
-    T.cols_cap = n_subspace;
+    SE_CUDA(ctx, cudaMalloc(&T.d_cols, sizeof(int32_t) * (size_t)ncols));
+    T.cols_cap = ncols;
   }
-  SE_REQUIRE(ctx, sizeof(int32_t) * (size_t)n_subspace <= (size_t)kSmallBytes, SE_ERR_ARG, "subspace too large");
-  memcpy(ctx->h_small, cols.data(), sizeof(int32_t) * (size_t)n_subspace);
-  SE_CUDA(ctx, cudaMemcpyAsync(T.d_cols, ctx->h_small, sizeof(int32_t) * (size_t)n_subspace, cudaMemcpyHostToDevice, ctx->stream));
+  SE_REQUIRE(ctx, sizeof(int32_t) * (size_t)ncols <= (size_t)kSmallBytes, SE_ERR_ARG, "subspace too large");
+  memcpy(ctx->h_small, cols.data(), sizeof(int32_t) * (size_t)ncols);
+  SE_CUDA(ctx, cudaMemcpyAsync(T.d_cols, ctx->h_small, sizeof(int32_t) * (size_t)ncols, cudaMemcpyHostToDevice, ctx->stream));
   if (K > 0 && label_slot == SE_SLOT_Y) SE_TRY(ensure_labels_checked(ctx, 0, K, n));  // class indices, checked per upload
+  cols.resize((size_t)total);
   uint32_t h = 2166136261u;
   h = fnv_words(h, cols.data(), cols.size());
   for (int32_t c : cols) {
@@ -3221,9 +3271,10 @@ int tree_fit_prepare(se_ctx* ctx, int K, int entropy, int out_proba, int label_s
   h = fnv_words(h, rules, 2);
   h = fnv_words(h, frac, sizeof(frac) / 4);
   // after the re-rank of X and the label check above: the output rows may be rows of X or Y themselves
-  SE_TRY(out_rows(ctx, out_slot, out_row, out_proba ? K : 1, n, &P.out, &P.ld_out));
+  if (with_out) SE_TRY(out_rows(ctx, out_slot, out_row, out_proba ? K : 1, n, &P.out, &P.ld_out));
   P.r = r; P.w = w; P.bag = bag;
   P.n = n; P.nw = nw; P.nb = nb; P.sw = sw; P.top = top;
+  P.n_trees = n_trees; P.total_cols = total; P.max_cols = maxS;
   P.hash = (h ^ (h >> 24)) & 0xFFFFFFu;
   return SE_OK;
 }
@@ -3263,27 +3314,38 @@ int tree_fit_agree(se_ctx* ctx, int rc, const double* shape, int count) {
   return SE_OK;
 }
 
-// The part of a fit that se_tree_fit and se_tree_fit_classifier share: argument checks, scratch, the level loop with
-// its shared-memory / global-atomics choice, the classifier's pruning, the out kernel and the download of the node
-// records into h_small: [kTreeFitHeap] TreeFitNode, then for K >= 2 the class weights ([kTreeFitHeap][K] double), the
-// probabilities ([kTreeFitHeap][K] float) and the pruning table ([kTreeFitHeap] int4).  K == 0: regression.  rc0 is
-// the caller's own checks.
+// Bytes of one tree's node records as tree_fit_run downloads them (K == 0: regression).
+size_t tree_fit_record_bytes(int K) {
+  return sizeof(TreeFitNode) * kTreeFitHeap +
+         (K > 0 ? (sizeof(double) + sizeof(float)) * kTreeFitHeap * (size_t)K + sizeof(int4) * kTreeFitHeap : 0);
+}
+
+// The part of a fit that se_tree_fit, se_tree_fit_classifier and se_forest_fit share: argument checks, scratch, the
+// level loop with its shared-memory / global-atomics choice, the classifier's pruning, the out kernel (with_out) and
+// the download of the n_trees trees' node records into the pinned `records`: [T][kTreeFitHeap] TreeFitNode, then for
+// K >= 2 the class weights ([T][kTreeFitHeap][K] double), the probabilities ([T][kTreeFitHeap][K] float) and the
+// pruning tables ([T][kTreeFitHeap] int4).  K == 0: regression.  rc0 is the caller's own checks.
 //
-// Under a communicator the fit is collective: each level's histogram is summed over the ranks (one fp64 NCCL
-// all-reduce between the histogram and the split kernels), so every rank splits on the histogram of the union of the
-// shards and writes its own rows' output.  The collective sequence is fixed by the shape tree_fit_agree checks.
+// The trees grow together: every kernel of the level loop covers all of them, so T trees cost one launch sequence.
+// The shared-memory / global-atomics choice depends on the level's 2^L · nb · sw alone, so it is the same for all.
+//
+// Under a communicator the fit is collective (one tree only): each level's histogram is summed over the ranks (one
+// fp64 NCCL all-reduce between the histogram and the split kernels), so every rank splits on the histogram of the
+// union of the shards and writes its own rows' output.  The collective sequence is fixed by the shape tree_fit_agree
+// checks.
 int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int label_slot, int label_row,
-                 int weight_slot, int weight_row, int use_bag, const int32_t* subspace, int n_subspace, int max_depth,
-                 int min_instances, double min_info_gain, double min_weight_fraction, int out_slot, int out_row) {
+                 int weight_slot, int weight_row, int use_bag, int n_trees, int first_tree, const int32_t* sub_off,
+                 const int32_t* sub_cols, int max_depth, int min_instances, double min_info_gain,
+                 double min_weight_fraction, bool with_out, int out_slot, int out_row, unsigned char* records) {
   TreeFitPlan P;
   int rc = rc0 != SE_OK ? rc0
                         : tree_fit_prepare(ctx, K, entropy, out_proba, label_slot, label_row, weight_slot, weight_row,
-                                           use_bag, subspace, n_subspace, max_depth, min_instances, min_info_gain,
-                                           min_weight_fraction, out_slot, out_row, P);
+                                           use_bag, n_trees, first_tree, sub_off, sub_cols, max_depth, min_instances,
+                                           min_info_gain, min_weight_fraction, with_out, out_slot, out_row, P);
   const bool collective = ctx->comm && ctx->nranks > 1;
   if (collective) {
-    const double shape[] = {0.0, (double)max_depth, (double)n_subspace, (double)P.nb, (double)P.sw, (double)K,
-                            P.w ? 1.0 : 0.0, P.bag ? 1.0 : 0.0, (double)P.hash};
+    const double shape[] = {0.0, (double)max_depth, (double)(sub_off[1] - sub_off[0]), (double)P.nb, (double)P.sw,
+                            (double)K, P.w ? 1.0 : 0.0, P.bag ? 1.0 : 0.0, (double)P.hash};
     rc = tree_fit_agree(ctx, rc, shape, (int)(sizeof(shape) / sizeof(shape[0])));
   }
   if (rc != SE_OK) return rc;
@@ -3291,19 +3353,20 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
   auto& T = ctx->tf;
   BinState& B = ctx->bins[0];
   const int64_t n = P.n, nw = P.nw;
-  const int nb = P.nb, sw = P.sw, top = P.top;
+  const int nb = P.nb, sw = P.sw, top = P.top, nt = P.n_trees, total = P.total_cols, maxS = P.max_cols;
   const float *r = P.r, *w = P.w, *bag = P.bag;
   TreeFitArgs a;
   a.X8 = B.d8; a.ld8 = B.ld8; a.n = n;
   a.cols = T.d_cols; a.n_edges = B.d_nedges; a.edges = B.d_edges;
-  a.S = n_subspace; a.nb = nb; a.max_depth = max_depth; a.search = max_depth > 0 ? 1 : 0;
+  a.S = maxS; a.nb = nb; a.max_depth = max_depth; a.search = max_depth > 0 ? 1 : 0;
   a.has_w = w ? 1 : 0; a.r = r; a.w = w; a.bag = bag;
   a.dec = T.d_dec; a.nodes = T.d_nodes; a.hist = T.d_hist;
   a.min_instances = min_instances; a.min_info_gain = min_info_gain; a.min_weight_fraction = min_weight_fraction;
   a.K = K; a.sw = sw; a.entropy = entropy; a.out_proba = out_proba;
   a.cw = T.d_cw; a.prob = T.d_prob; a.prn = T.d_prn;
+  a.T = nt; a.sub_off = T.d_cols + total; a.nid_stride = 2 * T.nid_cap;
   uint16_t* nid[2] = {T.d_nid, T.d_nid + T.nid_cap};
-  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, ctx->stream));
+  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_init(T.d_nodes, T.d_dec, nt, ctx->stream));
   ctx->last_tree_fit_hist = 0;
   for (int L = 0; L <= top; ++L) {
     a.L = L;
@@ -3311,31 +3374,34 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
     a.nid_in = L >= 2 ? nid[(L - 1) & 1] : nullptr;
     a.nid_out = L >= 1 ? nid[L & 1] : nullptr;
     const size_t per_col = ((size_t)1 << L) * (size_t)nb * (size_t)sw * sizeof(double);
-    SE_CUDA(ctx, cudaMemsetAsync(T.d_hist, 0, per_col * (size_t)n_subspace, ctx->stream));
+    SE_CUDA(ctx, cudaMemsetAsync(T.d_hist, 0, per_col * (size_t)total, ctx->stream));
     int smem_mode = 1, per_sm = 4;
     size_t smem = 0;
     if (per_col <= (size_t)kTreeFitSmemBudget) {
-      a.cb = (int)std::min<size_t>((size_t)n_subspace, kTreeFitSmemBudget / per_col);
+      a.cb = (int)std::min<size_t>((size_t)maxS, kTreeFitSmemBudget / per_col);
     } else if (per_col <= (size_t)T.smem_optin) {
       a.cb = 1;
       per_sm = per_col <= (size_t)T.smem_optin / 2 ? 2 : 1;
     } else {  // one column's histogram of every node of the level does not fit: global fp64 atomics
       smem_mode = 0;
-      a.cb = n_subspace;
+      a.cb = maxS;
       per_sm = 8;
     }
     if (smem_mode) smem = per_col * (size_t)a.cb;
     const int path = !smem_mode ? 4 : per_col > (size_t)kTreeFitSmemBudget ? (per_sm == 2 ? 2 : 3) : (a.cb > 1 ? 0 : 1);
     ctx->last_tree_fit_hist |= (int64_t)path << (3 * L);
-    const int gx = smem_mode ? (n_subspace + a.cb - 1) / a.cb : 1;
+    const int gx = smem_mode ? (maxS + a.cb - 1) / a.cb : 1;
     int64_t gy = ((int64_t)ctx->sms * per_sm + gx - 1) / gx;
+    // T trees share the grid one tree would use, rounded down: rounding up would leave a few CTAs in a second wave,
+    // each with a whole CTA's rows to do alone
+    gy = std::max<int64_t>(gy / nt, 1);
     gy = std::min<int64_t>(gy, (nw + 255) / 256);
     gy = std::max<int64_t>(std::min<int64_t>(gy, 65535), 1);
     a.words_per_cta = (nw + gy - 1) / gy;
     SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_hist(a, smem_mode, (int)gy, smem, ctx->stream));
     if (collective) {  // the level's histogram over the union of the shards, bit-identical on every rank
       NcclApi& api = nccl();
-      const int nr = api.AllReduce(T.d_hist, T.d_hist, per_col / sizeof(double) * (size_t)n_subspace, kNcclFloat64,
+      const int nr = api.AllReduce(T.d_hist, T.d_hist, per_col / sizeof(double) * (size_t)total, kNcclFloat64,
                                    kNcclSum, ctx->comm, ctx->stream);
       if (nr != 0) return fail(ctx, SE_ERR_NCCL, "ncclAllReduce: %s", api.GetErrorString(nr));
     }
@@ -3347,37 +3413,27 @@ int tree_fit_run(se_ctx* ctx, int rc0, int K, int entropy, int out_proba, int la
   a.out = P.out;
   a.ld_out = P.ld_out;
   if (K > 0) SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_prune(a, ctx->stream));
-  SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_out(a, ctx->sms, ctx->stream));
-  static_assert(sizeof(TreeFitNode) * kTreeFitHeap + (sizeof(double) + sizeof(float)) * kTreeFitHeap * kTreeFitMaxClasses +
-                        sizeof(int4) * kTreeFitHeap <= (size_t)kSmallBytes,
-                "node records fit the staging buffer");
-  char* hs = reinterpret_cast<char*>(ctx->h_small);
-  size_t off = sizeof(TreeFitNode) * kTreeFitHeap;
+  if (with_out) SE_LAUNCH_T(ctx, SE_KF_TREE, launch_tree_fit_out(a, ctx->sms, ctx->stream));
+  char* hs = reinterpret_cast<char*>(records);
+  size_t off = sizeof(TreeFitNode) * kTreeFitHeap * (size_t)nt;
   SE_CUDA(ctx, cudaMemcpyAsync(hs, T.d_nodes, off, cudaMemcpyDeviceToHost, ctx->stream));
   if (K > 0) {
-    const size_t cwb = sizeof(double) * kTreeFitHeap * (size_t)K, pb = sizeof(float) * kTreeFitHeap * (size_t)K;
+    const size_t cwb = sizeof(double) * kTreeFitHeap * (size_t)K * nt, pb = sizeof(float) * kTreeFitHeap * (size_t)K * nt;
     SE_CUDA(ctx, cudaMemcpyAsync(hs + off, T.d_cw, cwb, cudaMemcpyDeviceToHost, ctx->stream));
     SE_CUDA(ctx, cudaMemcpyAsync(hs + off + cwb, T.d_prob, pb, cudaMemcpyDeviceToHost, ctx->stream));
-    SE_CUDA(ctx, cudaMemcpyAsync(hs + off + cwb + pb, T.d_prn, sizeof(int4) * kTreeFitHeap, cudaMemcpyDeviceToHost, ctx->stream));
+    SE_CUDA(ctx, cudaMemcpyAsync(hs + off + cwb + pb, T.d_prn, sizeof(int4) * kTreeFitHeap * nt, cudaMemcpyDeviceToHost,
+                                 ctx->stream));
   }
   SE_TRY(end(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (K > 0) SE_TRY(check_labels(ctx));  // a label outside [0, K) was clamped: the fit is invalid
   return SE_OK;
 }
-}  // namespace
 
-int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
-                const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
-                double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
-                float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
-  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
-  const int rc0 = (!feature || !threshold || !left || !right || !value || !n_nodes) ? fail(ctx, SE_ERR_ARG, "null argument")
-                                                                                    : SE_OK;
-  SE_TRY(tree_fit_run(ctx, rc0, 0, 0, 0, label_slot, label_row, weight_slot, weight_row, use_bag, subspace, n_subspace,
-                      max_depth, min_instances, min_info_gain, min_weight_fraction, out_slot, out_row));
-  // ---- prune (bottom-up: two leaf children with equal fp64 predictions) and number the nodes in BFS order
-  const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(ctx->h_small);
+// One regression tree's records R in the array form of se_tree_predict: pruned bottom-up (two leaf children with
+// equal fp64 predictions), numbered in BFS order.
+int tree_fit_arrays(se_ctx* ctx, const TreeFitNode* R, int max_nodes, int32_t* feature, float* threshold,
+                    int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
   std::vector<char> leaf(kTreeFitHeap, 1);
   std::vector<double> pred(kTreeFitHeap, 0.0);
   std::vector<float> val(kTreeFitHeap, 0.f);
@@ -3414,32 +3470,11 @@ int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int
   return SE_OK;
 }
 
-// ---- classification-tree fit over the rank matrix (se_tree_fit.cu) -------------------------------
-int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
-                           const int32_t* subspace, int n_subspace, int num_classes, int impurity, int max_depth,
-                           int min_instances, double min_info_gain, double min_weight_fraction, int out_kind,
-                           int out_slot, int out_row, int max_nodes, int32_t* feature, float* threshold, int32_t* left,
-                           int32_t* right, float* value, float* proba, double* class_weights, double* gain,
-                           int* n_nodes) {
-  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
-  auto checks = [&]() -> int {  // this rank's own: under a communicator tree_fit_run tells the other ranks
-    SE_REQUIRE(ctx, feature && threshold && left && right && value && proba && n_nodes, SE_ERR_ARG, "null argument");
-    SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= kTreeFitMaxClasses, SE_ERR_ARG, "numClasses %d outside [2, %d]",
-               num_classes, kTreeFitMaxClasses);
-    SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
-    SE_REQUIRE(ctx, out_kind == SE_TREE_OUT_LABEL || out_kind == SE_TREE_OUT_PROBA, SE_ERR_ARG, "bad output kind %d", out_kind);
-    return SE_OK;
-  };
-  const int K = num_classes;
-  SE_TRY(tree_fit_run(ctx, checks(), K, impurity == SE_IMPURITY_ENTROPY, out_kind == SE_TREE_OUT_PROBA, label_slot,
-                      label_row, weight_slot, weight_row, use_bag, subspace, n_subspace, max_depth, min_instances,
-                      min_info_gain, min_weight_fraction, out_slot, out_row));
-  // the device pruned the tree (tree_prune_cls_kernel): number what is left in BFS order
-  const char* hs = reinterpret_cast<const char*>(ctx->h_small);
-  const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(hs);
-  const double* CW = reinterpret_cast<const double*>(hs + sizeof(TreeFitNode) * kTreeFitHeap);
-  const float* PR = reinterpret_cast<const float*>(CW + (size_t)kTreeFitHeap * K);
-  const int4* PN = reinterpret_cast<const int4*>(PR + (size_t)kTreeFitHeap * K);
+// One classification tree's records (pruned on the device by tree_prune_cls_kernel) in the array form of
+// se_tree_predict_multi, numbered in BFS order.
+int tree_fit_arrays_cls(se_ctx* ctx, const TreeFitNode* R, const double* CW, const float* PR, const int4* PN, int K,
+                        int max_nodes, int32_t* feature, float* threshold, int32_t* left, int32_t* right, float* value,
+                        float* proba, double* class_weights, double* gain, int* n_nodes) {
   std::vector<int> order;
   order.push_back(1);
   for (size_t q = 0; q < order.size(); ++q)
@@ -3463,5 +3498,150 @@ int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weigh
     if (gain) gain[q] = lf ? 0.0 : R[h].gain;
   }
   *n_nodes = (int)order.size();
+  return SE_OK;
+}
+}  // namespace
+
+int se_tree_fit(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                const int32_t* subspace, int n_subspace, int max_depth, int min_instances, double min_info_gain,
+                double min_weight_fraction, int out_slot, int out_row, int max_nodes, int32_t* feature,
+                float* threshold, int32_t* left, int32_t* right, float* value, double* gain, int* n_nodes) {
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  const int rc0 = (!feature || !threshold || !left || !right || !value || !n_nodes) ? fail(ctx, SE_ERR_ARG, "null argument")
+                                                                                    : SE_OK;
+  const int32_t sub_off[2] = {0, n_subspace};
+  SE_TRY(tree_fit_run(ctx, rc0, 0, 0, 0, label_slot, label_row, weight_slot, weight_row, use_bag, 1, -1, sub_off,
+                      subspace, max_depth, min_instances, min_info_gain, min_weight_fraction, true, out_slot, out_row,
+                      ctx->h_small));
+  return tree_fit_arrays(ctx, reinterpret_cast<const TreeFitNode*>(ctx->h_small), max_nodes, feature, threshold, left,
+                         right, value, gain, n_nodes);
+}
+
+// ---- classification-tree fit over the rank matrix (se_tree_fit.cu) -------------------------------
+int se_tree_fit_classifier(se_ctx* ctx, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                           const int32_t* subspace, int n_subspace, int num_classes, int impurity, int max_depth,
+                           int min_instances, double min_info_gain, double min_weight_fraction, int out_kind,
+                           int out_slot, int out_row, int max_nodes, int32_t* feature, float* threshold, int32_t* left,
+                           int32_t* right, float* value, float* proba, double* class_weights, double* gain,
+                           int* n_nodes) {
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  auto checks = [&]() -> int {  // this rank's own: under a communicator tree_fit_run tells the other ranks
+    SE_REQUIRE(ctx, feature && threshold && left && right && value && proba && n_nodes, SE_ERR_ARG, "null argument");
+    SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= kTreeFitMaxClasses, SE_ERR_ARG, "numClasses %d outside [2, %d]",
+               num_classes, kTreeFitMaxClasses);
+    SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
+    SE_REQUIRE(ctx, out_kind == SE_TREE_OUT_LABEL || out_kind == SE_TREE_OUT_PROBA, SE_ERR_ARG, "bad output kind %d", out_kind);
+    return SE_OK;
+  };
+  const int K = num_classes;
+  static_assert(sizeof(TreeFitNode) * kTreeFitHeap + (sizeof(double) + sizeof(float)) * kTreeFitHeap * kTreeFitMaxClasses +
+                        sizeof(int4) * kTreeFitHeap <= (size_t)kSmallBytes,
+                "one tree's node records fit the staging buffer");
+  const int32_t sub_off[2] = {0, n_subspace};
+  SE_TRY(tree_fit_run(ctx, checks(), K, impurity == SE_IMPURITY_ENTROPY, out_kind == SE_TREE_OUT_PROBA, label_slot,
+                      label_row, weight_slot, weight_row, use_bag, 1, -1, sub_off, subspace, max_depth, min_instances,
+                      min_info_gain, min_weight_fraction, true, out_slot, out_row, ctx->h_small));
+  const char* hs = reinterpret_cast<const char*>(ctx->h_small);
+  const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(hs);
+  const double* CW = reinterpret_cast<const double*>(hs + sizeof(TreeFitNode) * kTreeFitHeap);
+  const float* PR = reinterpret_cast<const float*>(CW + (size_t)kTreeFitHeap * K);
+  const int4* PN = reinterpret_cast<const int4*>(PR + (size_t)kTreeFitHeap * K);
+  return tree_fit_arrays_cls(ctx, R, CW, PR, PN, K, max_nodes, feature, threshold, left, right, value, proba,
+                             class_weights, gain, n_nodes);
+}
+
+// ---- several trees over the same rows, labels, weights and bag, one subspace each (se_tree_fit.cu) ----------------
+int se_forest_fit(se_ctx* ctx, int n_trees, const int32_t* sub_offsets, const int32_t* sub_cols, int label_slot,
+                  int label_row, int weight_slot, int weight_row, int use_bag, int num_classes, int impurity,
+                  int max_depth, int min_instances, double min_info_gain, double min_weight_fraction, int max_nodes,
+                  int32_t* feature, float* threshold, int32_t* left, int32_t* right, float* value, float* proba,
+                  double* class_weights, double* gain, int* n_nodes) {
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  SE_REQUIRE(ctx, !(ctx->comm && ctx->nranks > 1), SE_ERR_STATE,
+             "se_forest_fit does not fit over row-sharded GPUs: call it without a communicator");
+  SE_REQUIRE(ctx, n_trees >= 1 && sub_offsets && sub_cols, SE_ERR_ARG, "null argument or no tree");
+  SE_REQUIRE(ctx, feature && threshold && left && right && value && n_nodes, SE_ERR_ARG, "null argument");
+  const int K = num_classes;
+  SE_REQUIRE(ctx, K == 0 || (K >= 2 && K <= kTreeFitMaxClasses), SE_ERR_ARG,
+             "numClasses %d: 0 (regression) or [2, %d]", K, kTreeFitMaxClasses);
+  if (K > 0) {
+    SE_REQUIRE(ctx, proba, SE_ERR_ARG, "null argument");
+    SE_REQUIRE(ctx, impurity == SE_IMPURITY_GINI || impurity == SE_IMPURITY_ENTROPY, SE_ERR_ARG, "bad impurity %d", impurity);
+  }
+  SE_REQUIRE(ctx, max_nodes >= 1, SE_ERR_ARG, "max_nodes %d < 1", max_nodes);
+  SE_REQUIRE(ctx, sub_offsets[0] == 0, SE_ERR_ARG, "sub_offsets[0] must be 0");
+  SE_TRY(tree_fit_bins_ready(ctx));
+  const BinState& B = ctx->bins[0];
+  int maxc = 0;
+  for (int t = 0; t < n_trees; ++t) {
+    const int S = sub_offsets[t + 1] - sub_offsets[t];
+    SE_TRY(tree_fit_check_subspace(ctx, sub_cols + sub_offsets[t], S, t));
+    for (int k = sub_offsets[t]; k < sub_offsets[t + 1]; ++k) maxc = std::max(maxc, (int)B.edges[sub_cols[k]].size());
+  }
+  // ---- batches: at most kBatch trees whose node ids (4 B/row) and deepest histograms take at most half of the free
+  // device memory (plus the fit scratch this context already holds, which the batch reuses)
+  constexpr int kBatch = 64;
+  const int64_t n = ctx->slot[SE_SLOT_X].cols;
+  const int64_t nw = (n + 3) >> 2;
+  const int top = max_depth > 0 && max_depth <= 8 ? max_depth - 1 : 0;
+  const int sw = K > 0 ? K + (weight_slot >= 0 ? 1 : 0) : 4;
+  const int nb_all = std::min(256, maxc + 2);
+  SE_TRY(begin(ctx));
+  size_t free_b = 0, total_b = 0;
+  SE_CUDA(ctx, cudaMemGetInfo(&free_b, &total_b));
+  auto& T = ctx->tf;
+  const double budget = 0.5 * (double)free_b + (double)T.hist_bytes +
+                        (T.d_nid ? (double)sizeof(uint16_t) * 2.0 * (double)T.nid_cap * T.nid_trees : 0.0);
+  const size_t rec = tree_fit_record_bytes(K);
+  ctx->last_forest_fit_batches = 0;
+  std::vector<int32_t> off;
+  for (int t0 = 0; t0 < n_trees;) {
+    double bytes = 0.0;
+    int t1 = t0;
+    while (t1 < n_trees && t1 - t0 < kBatch) {
+      const int S = sub_offsets[t1 + 1] - sub_offsets[t1];
+      const double tree_b = 4.0 * 4.0 * (double)nw + (double)((size_t)1 << top) * S * nb_all * sw * sizeof(double);
+      const int cols = sub_offsets[t1 + 1] - sub_offsets[t0] + (t1 + 1 - t0) + 1;  // one upload through h_small
+      if (t1 > t0 && (bytes + tree_b > budget || (size_t)cols * sizeof(int32_t) > (size_t)kSmallBytes)) break;
+      bytes += tree_b;
+      ++t1;
+    }
+    const int nt = t1 - t0;
+    off.assign(sub_offsets + t0, sub_offsets + t1 + 1);
+    for (int32_t& o : off) o -= sub_offsets[t0];
+    SE_TRY(ensure_stage(ctx, rec * nt));
+    unsigned char* hs = reinterpret_cast<unsigned char*>(ctx->h_stage);
+    SE_TRY(tree_fit_run(ctx, SE_OK, K, impurity == SE_IMPURITY_ENTROPY, 0, label_slot, label_row, weight_slot,
+                        weight_row, use_bag, nt, t0, off.data(), sub_cols + sub_offsets[t0], max_depth, min_instances,
+                        min_info_gain, min_weight_fraction, false, -1, 0, hs));
+    ++ctx->last_forest_fit_batches;
+    const TreeFitNode* R = reinterpret_cast<const TreeFitNode*>(hs);
+    const double* CW = reinterpret_cast<const double*>(R + (size_t)kTreeFitHeap * nt);
+    const float* PR = reinterpret_cast<const float*>(CW + (size_t)kTreeFitHeap * K * nt);
+    const int4* PN = reinterpret_cast<const int4*>(PR + (size_t)kTreeFitHeap * K * nt);
+    for (int i = 0; i < nt; ++i) {
+      const size_t t = (size_t)(t0 + i), o = t * (size_t)max_nodes;
+      int rc;
+      if (K == 0) {
+        rc = (tree_fit_arrays(ctx, R + (size_t)kTreeFitHeap * i, max_nodes, feature + o, threshold + o, left + o,
+                               right + o, value + o, gain ? gain + o : nullptr, n_nodes + t));
+      } else {
+        rc = (tree_fit_arrays_cls(ctx, R + (size_t)kTreeFitHeap * i, CW + (size_t)kTreeFitHeap * K * i,
+                                   PR + (size_t)kTreeFitHeap * K * i, PN + (size_t)kTreeFitHeap * i, K, max_nodes,
+                                   feature + o, threshold + o, left + o, right + o, value + o, proba + o * K,
+                                   class_weights ? class_weights + o * K : nullptr, gain ? gain + o : nullptr,
+                                   n_nodes + t));
+      }
+      if (rc != SE_OK) {
+        const std::string msg = ctx->err;
+        return fail(ctx, rc, "tree %d: %s", (int)t, msg.c_str());
+      }
+    }
+    t0 = t1;
+  }
+  // the batch's node ids and histograms were sized for up to 64 trees: give them back rather than hold them for the
+  // life of the context (the next fit allocates what it needs)
+  cudaFree(T.d_nid); T.d_nid = nullptr; T.nid_cap = 0; T.nid_trees = 0;
+  cudaFree(T.d_hist); T.d_hist = nullptr; T.hist_bytes = 0;
   return SE_OK;
 }

@@ -363,13 +363,21 @@ struct TreeFitArgs {
   float* prob = nullptr;             // [kTreeFitHeap][K] fp32 of cw / W (all 0 when W == 0)
   int4* prn = nullptr;               // [kTreeFitHeap] after pruning: x the node whose statistics a row at h outputs,
                                      // y its label, z 1 when h is a leaf of the pruned tree
+  // T trees over the same rows, labels, weights and bag (se_forest_fit; the one-tree fits are T = 1).  Tree t searches
+  // the columns cols[sub_off[t] .. sub_off[t + 1]); S above is the largest of them.  Its dec / nodes / prn records start
+  // at t·kTreeFitHeap, its cw / prob at t·kTreeFitHeap·K, its level histogram at 2^L·nb·sw·sub_off[t] doubles and its
+  // node ids at t·nid_stride.  Every such offset is 64-bit.
+  int T = 1;
+  const int32_t* sub_off = nullptr;  // device [T + 1]
+  int64_t nid_stride = 0;
 };
-cudaError_t launch_tree_fit_init(TreeFitNode* nodes, uint2* dec, cudaStream_t s);
+// one CTA per tree: the T trees' records of a fit
+cudaError_t launch_tree_fit_init(TreeFitNode* nodes, uint2* dec, int T, cudaStream_t s);
 // smem_mode 1: shared-memory histograms of a.cb columns per CTA (smem bytes), folded into a.hist; 0: global atomics
 cudaError_t launch_tree_fit_hist(const TreeFitArgs& a, int smem_mode, int grid_y, size_t smem, cudaStream_t s);
 cudaError_t launch_tree_fit_split(const TreeFitArgs& a, cudaStream_t s);
 cudaError_t launch_tree_fit_prune(const TreeFitArgs& a, cudaStream_t s);  // classification only
-cudaError_t launch_tree_fit_out(const TreeFitArgs& a, int sms, cudaStream_t s);
+cudaError_t launch_tree_fit_out(const TreeFitArgs& a, int sms, cudaStream_t s);  // tree 0 only
 
 cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_coef,
                                   const float* coef, const int32_t* cols, float intercept,

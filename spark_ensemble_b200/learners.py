@@ -159,20 +159,40 @@ class _DeviceTreeLearner:
         N.check(N.load().se_spark_bernoulli_sample(ctypes.c_int64(s64), required / n, n, 0, N.fptr(c)))
         return np.flatnonzero(c > 0)
 
-    def split_candidates(self, X) -> list:
-        """Split candidates of every column of X, computed once per fit from the feature values only."""
+    def split_candidates(self, X, rows=None) -> list:
+        """Split candidates of every column of X, computed once per fit from the feature values only.  With `rows`
+        (row indices), exactly those of X[rows], without copying X[rows]: the candidate sample of len(rows) rows is
+        taken through `rows`, so only the sampled rows are gathered."""
         self._check()
-        X = np.asarray(X, dtype=np.float32)
-        rows = self.sample_rows(X.shape[0])
-        S = X if rows is None else X[rows]
-        return [continuous_split_candidates(S[:, j], self.maxBins) for j in range(X.shape[1])]
+        if rows is None:
+            X = np.asarray(X, dtype=np.float32)
+            sample = self.sample_rows(X.shape[0])
+            S = X if sample is None else X[sample]
+        else:
+            rows = np.asarray(rows, dtype=np.int64).reshape(-1)
+            sample = self.sample_rows(rows.size)
+            S = np.asarray(X[rows if sample is None else rows[sample]], dtype=np.float32)
+        return [continuous_split_candidates(S[:, j], self.maxBins) for j in range(S.shape[1])]
+
+    def _forest_subspaces(self, subspaces):
+        """The distinct subspaces (each fitted once) and, per member, the index of its distinct subspace."""
+        keys, first, index = {}, [], []
+        for s in subspaces:
+            s = np.asarray(s, dtype=np.int32).reshape(-1)
+            key = s.tobytes()
+            if key not in keys:
+                keys[key] = len(first)
+                first.append(s)
+            index.append(keys[key])
+        return first, index
 
 
 class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
     """org.apache.spark.ml.regression.DecisionTreeRegressor fitted on the GPU: variance impurity, continuous features,
     level-wise best split over at most maxBins - 1 candidates per column (se_tree_fit).  Params keep Spark's names and
-    defaults.  Inside GBMRegressor / GBMClassifier (residentFeatures=True) it fits on the device-resident residuals;
-    `fit` alone opens a context on `device`, uploads X, fits and closes it."""
+    defaults.  Inside GBMRegressor / GBMClassifier (residentFeatures=True) it fits on the device-resident residuals,
+    inside BaggingRegressor (residentFeatures=True) every member's tree grows in one forest fit
+    (fit_forest_resident); `fit` alone opens a context on `device`, uploads X, fits and closes it."""
 
     def __init__(self, maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1, minInfoGain: float = 0.0,
                  minWeightFractionPerNode: float = 0.0, seed: int | None = None, device: int = 0):
@@ -201,6 +221,18 @@ class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
                          min_info_gain=self.minInfoGain, min_weight_fraction=self.minWeightFractionPerNode,
                          out_slot=out_slot, out_row=out_row)
         return DeviceDecisionTreeRegressionModel(t)
+
+    def fit_forest_resident(self, ctx, label_slot: int, label_row: int, weight_slot: int, weight_row: int,
+                            use_bag: bool, subspaces) -> list:
+        """One tree per subspace over the same labels, weights and bag of a context whose SLOT_X holds this learner's
+        candidates, fitted together (Context.forest_fit).  Equal subspaces are fitted once: their trees would be
+        fits of the same data.  Returns one model per subspace, with subspace-local features."""
+        self._check()
+        distinct, index = self._forest_subspaces(subspaces)
+        trees = ctx.forest_fit(distinct, label_slot, label_row, weight_slot, weight_row, use_bag,
+                               max_depth=self.maxDepth, min_instances=self.minInstancesPerNode,
+                               min_info_gain=self.minInfoGain, min_weight_fraction=self.minWeightFractionPerNode)
+        return [DeviceDecisionTreeRegressionModel(trees[i]) for i in index]
 
     def fit(self, X, y, w=None) -> DeviceDecisionTreeRegressionModel:
         from . import _native as N
@@ -316,8 +348,9 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
     """org.apache.spark.ml.classification.DecisionTreeClassifier fitted on the GPU: gini or entropy impurity,
     continuous features, level-wise best split over at most maxBins - 1 candidates per column, Spark's pruning
     (se_tree_fit_classifier).  Params keep Spark's names and defaults; 2..64 classes.  Inside BoostingClassifier
-    (residentFeatures=True) it fits on the device-resident labels and boosting weights; `fit` alone opens a context on
-    `device`, uploads X, fits and closes it (BaggingClassifier uses it that way)."""
+    (residentFeatures=True) it fits on the device-resident labels and boosting weights, and inside BaggingClassifier
+    (residentFeatures=True) every member's tree grows in one forest fit (fit_forest_resident); `fit` alone opens a
+    context on `device`, uploads X, fits and closes it (BaggingClassifier without residentFeatures uses it that way)."""
 
     def __init__(self, maxDepth: int = 5, maxBins: int = 32, impurity: str = "gini", minInstancesPerNode: int = 1,
                  minInfoGain: float = 0.0, minWeightFractionPerNode: float = 0.0, seed: int | None = None,
@@ -362,6 +395,20 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
                                     min_weight_fraction=self.minWeightFractionPerNode, proba=proba,
                                     out_slot=out_slot, out_row=out_row)
         return DeviceDecisionTreeClassificationModel(t, num_classes)
+
+    def fit_forest_resident(self, ctx, num_classes: int, label_slot: int, label_row: int, weight_slot: int,
+                            weight_row: int, use_bag: bool, subspaces) -> list:
+        """One tree per subspace over the same labels, weights and bag of a context whose SLOT_X holds this learner's
+        candidates, fitted together (Context.forest_fit).  Equal subspaces are fitted once: their trees would be
+        fits of the same data.  Returns one model per subspace, with subspace-local features."""
+        self._check()
+        self._check_classes(int(num_classes))
+        distinct, index = self._forest_subspaces(subspaces)
+        trees = ctx.forest_fit(distinct, label_slot, label_row, weight_slot, weight_row, use_bag,
+                               num_classes=int(num_classes), impurity=self.impurity.lower(), max_depth=self.maxDepth,
+                               min_instances=self.minInstancesPerNode, min_info_gain=self.minInfoGain,
+                               min_weight_fraction=self.minWeightFractionPerNode)
+        return [DeviceDecisionTreeClassificationModel(trees[i], num_classes) for i in index]
 
     def fit(self, X, y, w=None, num_classes: int | None = None) -> DeviceDecisionTreeClassificationModel:
         from . import _native as N

@@ -334,10 +334,44 @@ class GBMRegressionModel(Params):
 GBMRegressionModel._declare(_p + _ps + _pb + _pg + _preg, _GBM_REG_DEFAULTS)
 
 
-# ---- Bagging (train is out of the hot path: embarrassingly parallel base-learner fits) ---------------
+# ---- Bagging: every member sees the same bag (reference quirk 3) and differs only in its subspace -----------------
+def _bagging_forest_fit(device: int, learner, X, y, bw, subs, num_classes: int | None = None) -> list:
+    """Bagging's members fitted together on the device: X is uploaded once, the candidates come from the in-bag rows,
+    and one forest fit grows every member's tree.  The labels sit in SLOT_Y, the weights bw in SLOT_W and the in-bag
+    indicator in SLOT_BAG, so a node's rawCount counts distinct in-bag rows and its weight is Σ bw: the statistics
+    learner.fit(X[keep][:, sub], y[keep], bw[keep]) sees, hence the same trees.  Raises the ValueError that route
+    raises for no in-bag row, an empty subspace, bad labels or Params."""
+    keep = bw > 0
+    rows = np.flatnonzero(keep)
+    if rows.size == 0 or any(len(s) == 0 for s in subs):
+        raise ValueError(f"{type(learner).__name__}.fit needs at least one row and one column")
+    n, d = X.shape
+    if num_classes is not None:
+        K = int(num_classes)
+        yk = np.asarray(y, dtype=np.float64).reshape(-1)[rows]
+        if np.any(yk < 0) or np.any(yk != np.floor(yk)) or np.any(yk >= K):
+            raise ValueError(f"labels must be integer class indices in [0, {K}) and one per row")
+        learner._check_classes(K)
+    cands = learner.split_candidates(X, rows=rows)
+    with Context(device) as ctx:
+        ctx.alloc(N.SLOT_X, d, n)
+        ctx.upload_rowmajor(N.SLOT_X, X)
+        ctx.alloc(N.SLOT_Y, n)
+        ctx.upload(N.SLOT_Y, np.asarray(y, dtype=np.float32))
+        ctx.alloc(N.SLOT_W, n)
+        ctx.upload(N.SLOT_W, np.asarray(bw, dtype=np.float32))
+        ctx.alloc(N.SLOT_BAG, n)
+        ctx.upload(N.SLOT_BAG, keep.astype(np.float32))
+        ctx.tree_fit_bins(cands)
+        if num_classes is None:
+            return learner.fit_forest_resident(ctx, N.SLOT_Y, 0, N.SLOT_W, 0, True, subs)
+        return learner.fit_forest_resident(ctx, int(num_classes), N.SLOT_Y, 0, N.SLOT_W, 0, True, subs)
+
+
 class BaggingRegressor(Params):
-    """regression/BaggingRegressor.scala:77-172.  Only the model's predict is on the hot path; train
-    here is the minimal host loop (one base learner per bootstrap bag)."""
+    """regression/BaggingRegressor.scala:77-172.  With residentFeatures and a device tree learner every member's
+    tree grows in one forest fit over the device-resident features (_bagging_forest_fit); otherwise train is the
+    minimal host loop (one learner.fit per member)."""
 
     def __init__(self, uid: str | None = None, device: int = 0):
         super().__init__(uid or random_uid("BaggingRegressor"))
@@ -348,6 +382,7 @@ class BaggingRegressor(Params):
         n, d = X.shape
         seed = self("seed")
         M = self("numBaseLearners")
+        learner = self("baseLearner")
         subs = [subspace(self("subspaceRatio"), d, seed + i) for i in range(M)]
         models = []
         rng = np.random.default_rng(seed & 0xFFFFFFFF)  # same sample for every bag: reference quirk 3
@@ -357,8 +392,11 @@ class BaggingRegressor(Params):
             counts = (rng.random(n) < self("subsampleRatio")).astype(np.float64)
         bw = counts if w is None else counts * w
         keep = bw > 0
-        for i in range(M):
-            models.append(self("baseLearner").fit(X[keep][:, subs[i]], y[keep], bw[keep]))
+        if bool(self("residentFeatures")) and getattr(learner, "device_learner", False):
+            models = _bagging_forest_fit(self.device, learner, X, y, bw, subs)
+        else:
+            for i in range(M):
+                models.append(learner.fit(X[keep][:, subs[i]], y[keep], bw[keep]))
         m = BaggingRegressionModel(subs, models, device=self.device)
         self._copyValues(m)
         m.parent = self
