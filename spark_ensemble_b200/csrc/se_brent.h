@@ -10,7 +10,7 @@
 
 #include <math.h>
 
-#if defined(__CUDACC__) && !defined(SE_BRENT_HOST_ONLY)  // se_api.cu instantiates it with host callbacks only
+#if defined(__CUDACC__) && !defined(SE_BRENT_HOST_ONLY)  // se_api_gbm.cu instantiates it with host callbacks only
 #define SE_HD __host__ __device__
 #else
 #define SE_HD

@@ -56,7 +56,7 @@ __device__ __forceinline__ void st_stream1(float* p, float v) {
 //    every access while read-only passes use the plain instructions — so POL is a template flag set per mode;
 //  * on shards whose four arrays are of the order of the L2, marking what the next pass does not re-read as
 //    evict_first keeps r and h resident between the statistics pass and the update; on shards much larger than the
-//    L2 the hints buy nothing, so they are enabled by size (se_api.cu gbm_args, l2_hint_rows from the device's L2).
+//    L2 the hints buy nothing, so they are enabled by size (se_api_gbm.cu gbm_args, l2_hint_rows from the device's L2).
 __device__ __forceinline__ uint64_t l2_policy(bool evict_first) {
   uint64_t p;
   if (evict_first) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));

@@ -12,7 +12,7 @@
 //    last tile in registers and the groups before it in shared memory; otherwise the tail is in the L2) -> loss
 //    reduction + second exchange + host mirror.  1 launch, 0 host round trips inside the round.
 //    The round (residual mode) does not read or write F: nothing reads it between rounds, and for the squared loss
-//    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api.cu settle_f).
+//    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api_ctx.cu settle_f).
 //    A round whose residual slot is not current (Y, F or R were just written) reads (y, F, h) instead of (r, h):
 //    r' = (y - F) - c h, 16 B/row.  Without residual mode the update is F' = F + c h (F, y, h read; F written).
 //

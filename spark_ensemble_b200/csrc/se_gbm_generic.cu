@@ -43,7 +43,7 @@ __global__ void __launch_bounds__(32) gbm_logloss_generic_kernel(const GbmArgs a
     const bool in = i < a.n;
     const int64_t ii = in ? i : a.n - 1;  // out-of-range lanes shadow the last row (they never store or count)
     const float yf = a.y[ii];
-    const int yi = min(max((int)yf, 0), K - 1);  // validity is checked once per label upload (se_api.cu)
+    const int yi = min(max((int)yf, 0), K - 1);  // validity is checked once per label upload (se_api_gbm.cu)
     const float c = has_bag ? a.bag[ii] : 1.0f;
     const float w = (T::kNewton && has_w) ? a.w[ii] : 1.0f;
     // sweep 1: p_k = F_k + coef_k h_k (GBMLoss.scala:56-59), running max (first maximum), F update

@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(kBlock) tree_predict_kernel(const TreeArgs a) 
 // candidates `findSplits` computes once per fit: so X can be replaced, for the walk, by the RANK of each value among the
 // thresholds seen so far — bin(x) = #{t : t < x} in a uint8 — and `x <= t_j` becomes `bin(x) <= j`, EXACTLY (no
 // rounding involved: it is the same comparison, pre-evaluated).  A gather then costs 1 byte and a sector holds 32 rows:
-// 3.5x fewer DRAM bytes for the same walk.  The host side (se_api.cu tree_predict_impl) keeps the per-column threshold
+// 3.5x fewer DRAM bytes for the same walk.  The host side (se_api_trees.cu tree_predict_impl) keeps the per-column threshold
 // lists, re-bins the columns a new tree adds thresholds to, and falls back to the fp32 walk when a column would need
 // more than 255 thresholds.
 
