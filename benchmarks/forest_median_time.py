@@ -23,7 +23,8 @@ from spark_ensemble_b200 import DataFrame  # noqa: E402
 from spark_ensemble_b200 import _native as N  # noqa: E402
 from spark_ensemble_b200.context import Context  # noqa: E402
 from spark_ensemble_b200.learners import DeviceDecisionTreeRegressionModel, DeviceDecisionTreeRegressor  # noqa: E402
-from spark_ensemble_b200.regression import BoostingRegressionModel, BoostingRegressor, _resident_context  # noqa: E402
+from spark_ensemble_b200.regression import BoostingRegressionModel, BoostingRegressor  # noqa: E402
+from spark_ensemble_b200.routes import resident_context  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--reps", type=int, default=3)
@@ -76,7 +77,7 @@ def member_route(ctx, trees, w, n):
 
 def member_transform(X, trees, w):
     """The member route end to end, as BoostingRegressionModel took it before the one-pass kernel."""
-    with _resident_context(0, X) as ctx:
+    with resident_context(0, X) as ctx:
         member_route(ctx, trees, w, X.shape[0])
         return ctx.download(N.SLOT_RAW).astype(np.float64)
 

@@ -5,7 +5,11 @@ classification/DummyClassifier.scala:90-123).  Nothing here touches per-row nume
 """
 from __future__ import annotations
 
+import ctypes as C
+
 import numpy as np
+
+from . import _native as N
 
 
 # ---- a minimal columnar stand-in for a Spark DataFrame ----------------------------------------------
@@ -126,6 +130,17 @@ def subspace(subspace_ratio: float, num_features: int, seed: int) -> np.ndarray:
     """ensemble/HasSubBag.scala:73-79: keep feature j iff rng.nextDouble() < subspaceRatio."""
     rng = XORShiftRandom(seed)
     return np.array([j for j in range(num_features) if rng.next_double() < subspace_ratio], dtype=np.int32)
+
+
+def spark_bernoulli_sample(n: int, fraction: float, seed: int) -> np.ndarray:
+    """Multiplicity (0 or 1, fp32) of each of n rows in `RDD.sample(false, fraction, seed)` over ONE partition: Spark's
+    own algorithm (java.util.Random -> per-partition seed -> XORShiftRandom -> BernoulliSampler with gap sampling below
+    0.4), restated in the native library (se_spark_bernoulli_sample, host only)."""
+    c = np.zeros(n, dtype=np.float32)
+    s64 = int(seed) & 0xFFFFFFFFFFFFFFFF  # the Scala Long seed
+    s64 = s64 - (1 << 64) if s64 >= (1 << 63) else s64
+    N.check(N.load().se_spark_bernoulli_sample(C.c_int64(s64), float(fraction), n, 0, N.fptr(c)))
+    return c
 
 
 def slice_features(indices: np.ndarray, X: np.ndarray) -> np.ndarray:

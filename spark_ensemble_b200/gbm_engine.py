@@ -1,5 +1,5 @@
 """Host-side driver of one GBM fit on one GPU shard: the glue between the estimator mirrors
-(regression.GBMRegressor, classification.GBMClassifier) and the C ABI.
+(regression.GBMRegressor, classification.GBMClassifier) and the C ABI, and the round loop both run (fit_rounds).
 
 It mirrors the data flow of the reference's train() loop (regression/GBMRegressor.scala:340-469,
 classification/GBMClassifier.scala:325-483) with the RDD closures replaced by native calls:
@@ -12,6 +12,9 @@ import numpy as np
 
 from . import _native as N
 from .context import Context
+from .ensemble import subspace
+from .routes import bag_counts
+from .sharded import make_context
 
 
 class GBMEngine:
@@ -152,3 +155,72 @@ class GBMEngine:
         alpha, loss_sum, _ = self.ctx.gbm_round(learning_rate, True, tol, max_iter, residual=True)
         self.ctx.download(N.SLOT_R, out=r_out)
         return alpha, loss_sum
+
+
+def fit_rounds(est, X, y, w, Xv, yv, dim: int, loss: str, param: float, F0, vF0, learner, device_fit: bool,
+               newton: bool, line_search):
+    """The round loop of GBMRegressor.train (regression/GBMRegressor.scala:340-474) and GBMClassifier.train
+    (classification/GBMClassifier.scala:325-494) over the Params of `est`, on one context or, with Param `devices`
+    naming two or more GPUs, on rows sharded over one context per GPU (sharded.ShardedContext: the per-round scalars
+    are summed across GPUs inside the kernels).  F0 / vF0 are the init model's outputs (a constant per dimension is
+    broadcast on the device); line_search(eng) returns the round's step per dimension.  Returns the kept rounds'
+    (models [round][dim], weights [round] of [dim], subspaces) and every round's history entry."""
+    validation = yv is not None
+    n, nv = y.shape[0], (yv.shape[0] if validation else 0)
+    seed, num_learners = est("seed"), est("numBaseLearners")
+    counts = bag_counts(n, est("subsampleRatio"), est("replacement"), seed)  # same bag every round (quirk 3)
+    subspaces = [subspace(est("subspaceRatio"), X.shape[1], seed + i) for i in range(num_learners)]
+    ctx = make_context(est.device, est("devices"))
+    try:
+        eng = GBMEngine(ctx, n, nv, dim, loss, param, has_weights=w is not None)
+        eng.load(y, w, F0, yv, vF0)
+        if bool(est("residentFeatures")):
+            eng.load_features(X, Xv)
+        if counts is not None:
+            ctx.gbm_set_bag(counts)
+            in_bag = counts > 0
+        best = ctx.gbm_mean_loss(validation=True) if validation else 0.0
+        models, weights, history = [], [], []
+        eng.residuals(newton)  # residuals of F0; later rounds get them fused with the update
+        i = v = 0
+        while i < num_learners and v < est("numRounds"):
+            if loss == "huber":  # δ = α-quantile of |y − F| every round (approxQuantile -> exact radix select)
+                ctx.gbm_set_loss_param(ctx.gbm_abs_residual_quantile(est("alpha")))
+                eng.residuals(False)
+            sub = subspaces[i]
+            if device_fit:  # each dimension's tree is fitted where the residuals live: only the tree comes back
+                imodels = [eng.fit_direction(j, learner, sub, newton=newton, bag=counts is not None)
+                           for j in range(dim)]
+            else:
+                r, wout = eng.fetch_residuals(newton)
+                imodels = []
+                for j in range(dim):  # one regressor per dimension (Futures in the reference)
+                    fit_w = wout[j] if newton else w
+                    if counts is None:
+                        imodels.append(learner.fit(X[:, sub], r[j], fit_w))
+                    else:  # the base learner sees the bag: row i with multiplicity c_i (== weight c_i·w_i)
+                        bw = counts[in_bag] if fit_w is None else counts[in_bag] * fit_w[in_bag]
+                        imodels.append(learner.fit(X[in_bag][:, sub], r[j][in_bag], bw))
+                for j in range(dim):
+                    eng.set_direction_from_model(j, imodels[j], sub, X)
+            alpha = np.atleast_1d(line_search(eng)) if est("optimizedWeights") else np.ones(dim)
+            iweights = alpha * est("learningRate")
+            loss_sum, _ = eng.update(iweights, residual=(not newton and loss != "huber"), newton=newton)
+            models.append(imodels)
+            weights.append(iweights)
+            history.append({"alpha": alpha.copy(), "trainLoss": loss_sum / n if n else float("nan")})
+            if validation:
+                for j in range(dim):
+                    eng.set_direction_from_model(j, imodels[j], sub, Xv, validation=True)
+                err = eng.update_validation(iweights)
+                history[-1]["validationLoss"] = err
+                if best - err < est("validationTol") * max(err, 0.01):
+                    v += 1
+                elif err < best:
+                    best = err
+                    v = 0
+            i += 1
+        keep = i - v  # the rounds after the best validation loss are dropped
+        return models[:keep], weights[:keep], subspaces[:keep], history
+    finally:
+        ctx.close()

@@ -10,6 +10,10 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import _native as N
+from .context import Context
+from .ensemble import java_string_hash, spark_bernoulli_sample
+
 
 def _floor_f32(t64: np.ndarray) -> np.ndarray:
     """Largest fp32 <= each fp64 value, so `x <= t32` equals `x <= t64` for every fp32 x."""
@@ -98,25 +102,28 @@ def continuous_split_candidates(values, max_bins: int) -> np.ndarray:
     return np.unique(out)  # sorted; clamping can only merge two candidates at the extremes
 
 
-class DeviceDecisionTreeRegressionModel(_Model):
-    """A regression tree fitted on the device, in the array form of se_tree_predict."""
+def check_class_labels(y: np.ndarray, num_classes: int, n: int):
+    """The device classification tree's labels: n of them, each an integer class index in [0, num_classes)."""
+    if y.size != n or np.any(y < 0) or np.any(y != np.floor(y)) or np.any(y >= num_classes):
+        raise ValueError(f"labels must be integer class indices in [0, {num_classes}) and one per row")
+
+
+class _DeviceTreeModel(_Model):
+    """A tree fitted on the device, in the array form of se_tree_predict, with the gain of every node."""
 
     def __init__(self, arrays: dict):
         self._arrays = {k: np.asarray(v).copy() for k, v in arrays.items()}
         self.numNodes = int(self._arrays["feature"].size)
 
-    def tree_arrays(self):
-        return {k: self._arrays[k] for k in ("feature", "threshold", "left", "right", "value")}
-
     @property
     def gains(self) -> np.ndarray:
         return self._arrays["gain"]
 
-    def predict(self, X) -> np.ndarray:
-        """Host walk of the same arrays: left when x <= threshold (NaN goes right), fp32 features and values."""
+    def _leaf(self, X) -> np.ndarray:
+        """Host walk of the arrays: the leaf of every row, left when x <= threshold (NaN goes right), fp32 features."""
         X = np.asarray(X, dtype=np.float32)
         f, t = self._arrays["feature"], self._arrays["threshold"]
-        l, r, v = self._arrays["left"], self._arrays["right"], self._arrays["value"]
+        l, r = self._arrays["left"], self._arrays["right"]
         node = np.zeros(X.shape[0], dtype=np.int64)
         rows = np.arange(X.shape[0])
         while True:
@@ -127,7 +134,17 @@ class DeviceDecisionTreeRegressionModel(_Model):
             nd = node[idx]
             go_left = X[idx, f[nd]] <= t[nd]
             node[idx] = np.where(go_left, l[nd], r[nd])
-        return v[node].astype(np.float64)
+        return node
+
+
+class DeviceDecisionTreeRegressionModel(_DeviceTreeModel):
+    """A regression tree fitted on the device, in the array form of se_tree_predict."""
+
+    def tree_arrays(self):
+        return {k: self._arrays[k] for k in ("feature", "threshold", "left", "right", "value")}
+
+    def predict(self, X) -> np.ndarray:
+        return self._arrays["value"][self._leaf(X)].astype(np.float64)
 
 
 class _DeviceTreeLearner:
@@ -151,13 +168,7 @@ class _DeviceTreeLearner:
         required = max(self.maxBins * self.maxBins, 10000)
         if n <= required:
             return None
-        import ctypes
-        from . import _native as N
-        c = np.zeros(n, dtype=np.float32)
-        s64 = int(self.seed) & 0xFFFFFFFFFFFFFFFF
-        s64 = s64 - (1 << 64) if s64 >= (1 << 63) else s64
-        N.check(N.load().se_spark_bernoulli_sample(ctypes.c_int64(s64), required / n, n, 0, N.fptr(c)))
-        return np.flatnonzero(c > 0)
+        return np.flatnonzero(spark_bernoulli_sample(n, required / n, self.seed) > 0)
 
     def split_candidates(self, X, rows=None) -> list:
         """Split candidates of every column of X, computed once per fit from the feature values only.  With `rows`
@@ -173,6 +184,35 @@ class _DeviceTreeLearner:
             sample = self.sample_rows(rows.size)
             S = np.asarray(X[rows if sample is None else rows[sample]], dtype=np.float32)
         return [continuous_split_candidates(S[:, j], self.maxBins) for j in range(S.shape[1])]
+
+    def _tree_params(self) -> dict:
+        """This learner's Params as the keyword arguments of Context.tree_fit / forest_fit."""
+        return {"max_depth": self.maxDepth, "min_instances": self.minInstancesPerNode, "min_info_gain": self.minInfoGain,
+                "min_weight_fraction": self.minWeightFractionPerNode}
+
+    def _fit_alone(self, X, y, w, out_slot: int, fit):
+        """`fit` alone: a context of its own on `device` holding X (fp32, checked by _rows), the labels y (fp32) in
+        SLOT_Y, the weights w (if any) in SLOT_W, out_slot for every row's output and this learner's candidates;
+        fit(ctx, weight_slot, columns) fits over it, and the context is closed."""
+        n, d = X.shape
+        cands = self.split_candidates(X)
+        with Context(self.device) as ctx:
+            ctx.alloc(N.SLOT_X, d, n)
+            ctx.upload_rowmajor(N.SLOT_X, X)
+            ctx.alloc(N.SLOT_Y, n)
+            ctx.upload(N.SLOT_Y, y)
+            if w is not None:
+                ctx.alloc(N.SLOT_W, n)
+                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
+            ctx.alloc(out_slot, n)
+            ctx.tree_fit_bins(cands)
+            return fit(ctx, N.SLOT_W if w is not None else -1, np.arange(d, dtype=np.int32))
+
+    def _rows(self, X) -> np.ndarray:
+        X = np.asarray(X, dtype=np.float32)
+        if X.shape[0] == 0 or X.shape[1] == 0:
+            raise ValueError(f"{type(self).__name__}.fit needs at least one row and one column")
+        return X
 
     def _forest_subspaces(self, subspaces):
         """The distinct subspaces (each fitted once) and, per member, the index of its distinct subspace."""
@@ -196,7 +236,6 @@ class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
 
     def __init__(self, maxDepth: int = 5, maxBins: int = 32, minInstancesPerNode: int = 1, minInfoGain: float = 0.0,
                  minWeightFractionPerNode: float = 0.0, seed: int | None = None, device: int = 0):
-        from .ensemble import java_string_hash
         self.maxDepth, self.maxBins = int(maxDepth), int(maxBins)
         self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
         self.minWeightFractionPerNode = float(minWeightFractionPerNode)
@@ -217,9 +256,7 @@ class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
         """Fit over a context whose SLOT_X already holds this learner's candidates (Context.tree_fit_bins)."""
         self._check()
         t = ctx.tree_fit(label_slot, label_row, weight_slot, weight_row, use_bag, subspace=subspace,
-                         max_depth=self.maxDepth, min_instances=self.minInstancesPerNode,
-                         min_info_gain=self.minInfoGain, min_weight_fraction=self.minWeightFractionPerNode,
-                         out_slot=out_slot, out_row=out_row)
+                         out_slot=out_slot, out_row=out_row, **self._tree_params())
         return DeviceDecisionTreeRegressionModel(t)
 
     def fit_forest_resident(self, ctx, label_slot: int, label_row: int, weight_slot: int, weight_row: int,
@@ -229,31 +266,13 @@ class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
         fits of the same data.  Returns one model per subspace, with subspace-local features."""
         self._check()
         distinct, index = self._forest_subspaces(subspaces)
-        trees = ctx.forest_fit(distinct, label_slot, label_row, weight_slot, weight_row, use_bag,
-                               max_depth=self.maxDepth, min_instances=self.minInstancesPerNode,
-                               min_info_gain=self.minInfoGain, min_weight_fraction=self.minWeightFractionPerNode)
+        trees = ctx.forest_fit(distinct, label_slot, label_row, weight_slot, weight_row, use_bag, **self._tree_params())
         return [DeviceDecisionTreeRegressionModel(trees[i]) for i in index]
 
     def fit(self, X, y, w=None) -> DeviceDecisionTreeRegressionModel:
-        from . import _native as N
-        from .context import Context
-        X = np.asarray(X, dtype=np.float32)
-        n, d = X.shape
-        if n == 0 or d == 0:
-            raise ValueError("DeviceDecisionTreeRegressor.fit needs at least one row and one column")
-        cands = self.split_candidates(X)
-        with Context(self.device) as ctx:
-            ctx.alloc(N.SLOT_X, d, n)
-            ctx.upload_rowmajor(N.SLOT_X, X)
-            ctx.alloc(N.SLOT_Y, n)
-            ctx.upload(N.SLOT_Y, np.asarray(y, dtype=np.float32))
-            if w is not None:
-                ctx.alloc(N.SLOT_W, n)
-                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
-            ctx.alloc(N.SLOT_H, n)
-            ctx.tree_fit_bins(cands)
-            return self.fit_resident(ctx, N.SLOT_Y, 0, N.SLOT_W if w is not None else -1, 0, False,
-                                     np.arange(d, dtype=np.int32), N.SLOT_H, 0)
+        return self._fit_alone(self._rows(X), np.asarray(y, dtype=np.float32), w, N.SLOT_H,
+                               lambda ctx, wslot, cols: self.fit_resident(ctx, N.SLOT_Y, 0, wslot, 0, False, cols,
+                                                                          N.SLOT_H, 0))
 
 
 class DecisionTreeClassificationModel(_Model):
@@ -300,42 +319,20 @@ class DecisionTreeClassifier:
         return DecisionTreeClassificationModel(sk, int(num_classes or (yi.max() + 1)))
 
 
-class DeviceDecisionTreeClassificationModel(_Model):
+class DeviceDecisionTreeClassificationModel(_DeviceTreeModel):
     """A classification tree fitted on the device, in the array form of se_tree_predict ("value": the label) and
     se_tree_predict_multi ("values": [n_nodes, K] class probabilities), as DecisionTreeClassificationModel gives."""
 
     def __init__(self, arrays: dict, num_classes: int):
-        self._arrays = {k: np.asarray(v).copy() for k, v in arrays.items()}
+        super().__init__(arrays)
         self.numClasses = int(num_classes)
-        self.numNodes = int(self._arrays["feature"].size)
 
     def tree_arrays(self):
         return {k: self._arrays[k] for k in ("feature", "threshold", "left", "right", "value", "values")}
 
     @property
-    def gains(self) -> np.ndarray:
-        return self._arrays["gain"]
-
-    @property
     def class_weights(self) -> np.ndarray:
         return self._arrays["class_weights"]
-
-    def _leaf(self, X) -> np.ndarray:
-        """Host walk of the arrays: left when x <= threshold (NaN goes right), fp32 features."""
-        X = np.asarray(X, dtype=np.float32)
-        f, t = self._arrays["feature"], self._arrays["threshold"]
-        l, r = self._arrays["left"], self._arrays["right"]
-        node = np.zeros(X.shape[0], dtype=np.int64)
-        rows = np.arange(X.shape[0])
-        while True:
-            live = f[node] >= 0
-            if not live.any():
-                break
-            idx = rows[live]
-            nd = node[idx]
-            go_left = X[idx, f[nd]] <= t[nd]
-            node[idx] = np.where(go_left, l[nd], r[nd])
-        return node
 
     def predict(self, X) -> np.ndarray:
         return self._arrays["value"][self._leaf(X)].astype(np.float64)
@@ -355,7 +352,6 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
     def __init__(self, maxDepth: int = 5, maxBins: int = 32, impurity: str = "gini", minInstancesPerNode: int = 1,
                  minInfoGain: float = 0.0, minWeightFractionPerNode: float = 0.0, seed: int | None = None,
                  device: int = 0):
-        from .ensemble import java_string_hash
         self.maxDepth, self.maxBins, self.impurity = int(maxDepth), int(maxBins), str(impurity)
         self.minInstancesPerNode, self.minInfoGain = int(minInstancesPerNode), float(minInfoGain)
         self.minWeightFractionPerNode = float(minWeightFractionPerNode)
@@ -368,6 +364,9 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
         super()._check()
         if self.impurity.lower() not in ("gini", "entropy"):
             raise ValueError(f"impurity must be gini or entropy, got {self.impurity!r}")
+
+    def _tree_params(self) -> dict:
+        return {**super()._tree_params(), "impurity": self.impurity.lower()}
 
     def copy(self, extra=None):
         c = DeviceDecisionTreeClassifier(self.maxDepth, self.maxBins, self.impurity, self.minInstancesPerNode,
@@ -390,10 +389,8 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
         self._check()
         self._check_classes(int(num_classes))
         t = ctx.tree_fit_classifier(label_slot, num_classes, label_row, weight_slot, weight_row, use_bag,
-                                    subspace=subspace, impurity=self.impurity.lower(), max_depth=self.maxDepth,
-                                    min_instances=self.minInstancesPerNode, min_info_gain=self.minInfoGain,
-                                    min_weight_fraction=self.minWeightFractionPerNode, proba=proba,
-                                    out_slot=out_slot, out_row=out_row)
+                                    subspace=subspace, proba=proba, out_slot=out_slot, out_row=out_row,
+                                    **self._tree_params())
         return DeviceDecisionTreeClassificationModel(t, num_classes)
 
     def fit_forest_resident(self, ctx, num_classes: int, label_slot: int, label_row: int, weight_slot: int,
@@ -405,36 +402,18 @@ class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
         self._check_classes(int(num_classes))
         distinct, index = self._forest_subspaces(subspaces)
         trees = ctx.forest_fit(distinct, label_slot, label_row, weight_slot, weight_row, use_bag,
-                               num_classes=int(num_classes), impurity=self.impurity.lower(), max_depth=self.maxDepth,
-                               min_instances=self.minInstancesPerNode, min_info_gain=self.minInfoGain,
-                               min_weight_fraction=self.minWeightFractionPerNode)
+                               num_classes=int(num_classes), **self._tree_params())
         return [DeviceDecisionTreeClassificationModel(trees[i], num_classes) for i in index]
 
     def fit(self, X, y, w=None, num_classes: int | None = None) -> DeviceDecisionTreeClassificationModel:
-        from . import _native as N
-        from .context import Context
-        X = np.asarray(X, dtype=np.float32)
-        n, d = X.shape
-        if n == 0 or d == 0:
-            raise ValueError("DeviceDecisionTreeClassifier.fit needs at least one row and one column")
+        X = self._rows(X)
         y = np.asarray(y, dtype=np.float64).reshape(-1)
         K = int(num_classes) if num_classes is not None else int(y.max()) + 1
-        if y.size != n or np.any(y < 0) or np.any(y != np.floor(y)) or np.any(y >= K):
-            raise ValueError(f"labels must be integer class indices in [0, {K}) and one per row")
+        check_class_labels(y, K, X.shape[0])
         self._check_classes(K)
-        cands = self.split_candidates(X)
-        with Context(self.device) as ctx:
-            ctx.alloc(N.SLOT_X, d, n)
-            ctx.upload_rowmajor(N.SLOT_X, X)
-            ctx.alloc(N.SLOT_Y, n)
-            ctx.upload(N.SLOT_Y, y.astype(np.float32))
-            if w is not None:
-                ctx.alloc(N.SLOT_W, n)
-                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
-            ctx.alloc(N.SLOT_PRED, n)
-            ctx.tree_fit_bins(cands)
-            return self.fit_resident(ctx, K, N.SLOT_Y, 0, N.SLOT_W if w is not None else -1, 0, False,
-                                     np.arange(d, dtype=np.int32), N.SLOT_PRED, 0)
+        return self._fit_alone(X, y.astype(np.float32), w, N.SLOT_PRED,
+                               lambda ctx, wslot, cols: self.fit_resident(ctx, K, N.SLOT_Y, 0, wslot, 0, False, cols,
+                                                                          N.SLOT_PRED, 0))
 
 
 class LinearRegressionModel(_Model):

@@ -172,6 +172,20 @@ def boosting_params():
     ], {"numBaseLearners": 10, "checkpointInterval": 10, "aggregationDepth": 2}
 
 
+# ---- the expert Params this project adds to the reference's surface --------------------------------------------------
+# SURVEY.md §5: keep the column-major feature matrix in HBM and evaluate fitted trees / linear models on device instead
+# of model.predict on the host; with a device tree learner, fit the trees there too
+RESIDENT_FEATURES = Param("residentFeatures", "evaluate base models on device over the HBM-resident feature matrix",
+                          convert=bool)
+# "brent" = the reference's optimiser (default); "newton" = curvature-based line search on the same objective (dim 1,
+# losses with a hessian): same minimiser within tol, ~6x fewer data passes
+LINE_SEARCH = Param("lineSearch", "line-search optimiser for dim 1: brent (reference) or newton",
+                    lambda v: v in ("brent", "newton"), str)
+# GPUs to shard the rows of a GBM fit over (one context per GPU, contiguous row blocks); [] = the estimator's `device`
+DEVICES = Param("devices", "CUDA device ordinals to shard the training rows over", lambda v: all(int(d) >= 0 for d in v),
+                lambda v: [int(d) for d in v])
+
+
 def gbm_params():
     """boosting/GBMParams.scala:29-131 (defaults :121-129)."""
     return [

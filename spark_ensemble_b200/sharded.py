@@ -6,7 +6,7 @@ exactly where the reference calls treeAggregate/treeReduce — and rank 0's valu
 
 ShardedContext exposes the subset of Context that gbm_engine.GBMEngine and the estimator mirrors use for a fit, with
 the same signatures: host arrays are passed / returned WHOLE (the [dim][n_total] layout of the single-GPU path) and
-are split / concatenated here, so the estimator code is unchanged (Param `devices`, regression.GBMRegressor).
+are split / concatenated here, so the estimator code is unchanged (Param `devices`, gbm_engine.fit_rounds).
 """
 from __future__ import annotations
 

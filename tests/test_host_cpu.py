@@ -101,7 +101,7 @@ def test_dummy_init_models():
 
 def test_bag_counts_same_every_round():
     """Reference quirk 3: RDD.sample gets the same seed every round => one bag per fit."""
-    from spark_ensemble_b200.regression import bag_counts
+    from spark_ensemble_b200.routes import bag_counts
     assert bag_counts(100, 1.0, False, 7) is None
     a, b = bag_counts(10000, 0.6, False, 7), bag_counts(10000, 0.6, False, 7)
     np.testing.assert_array_equal(a, b)

@@ -53,23 +53,24 @@ def test_gbm_device_learner_accepts_several_devices_that_exist(monkeypatch):
     from spark_ensemble_b200 import _native as N
     from spark_ensemble_b200.classification import GBMClassifier
     from spark_ensemble_b200.learners import DeviceDecisionTreeRegressor
-    from spark_ensemble_b200.regression import GBMRegressor, _check_device_learner
+    from spark_ensemble_b200.regression import GBMRegressor
+    from spark_ensemble_b200.routes import device_fit
     learner = DeviceDecisionTreeRegressor(maxDepth=2)
     monkeypatch.setattr(N, "device_count", lambda: 4)
     for est in (GBMRegressor(), GBMClassifier()):
         est.set("residentFeatures", True)
         for devices in ([], [2], [0, 1], [3, 1, 2]):
             est.set("devices", devices)
-            assert _check_device_learner(est, learner) is True
+            assert device_fit(est, learner, require_resident=True) is True
         est.set("devices", [0, 1, 0])
         with pytest.raises(ValueError, match="distinct"):
-            _check_device_learner(est, learner)
+            device_fit(est, learner, require_resident=True)
         est.set("devices", [0, 4])
         with pytest.raises(ValueError, match="GPU 4 is not one of the 4 visible"):
-            _check_device_learner(est, learner)
+            device_fit(est, learner, require_resident=True)
         est.set("residentFeatures", False)
         with pytest.raises(ValueError, match="residentFeatures"):
-            _check_device_learner(est, learner)
+            device_fit(est, learner, require_resident=True)
 
 
 @pytest.mark.parametrize("key", ["feature", "threshold", "value", "gain"])
