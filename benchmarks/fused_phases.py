@@ -4,7 +4,12 @@ exchange + Brent, update phase), the kernel's CUDA-event duration and the host w
 
 The update phase re-reads r and h (8 B/row) and writes r' (4 B/row).  Each CTA carries its statistics pass's last tile
 in registers and, with `fused_resident`, the groups before it in shared memory (`last_fused_resident_tiles` per CTA);
-`phase_b_offchip_read_bytes` is what the update phase then still reads from the L2 or HBM."""
+`phase_b_offchip_read_bytes` is what the update phase then still reads from the L2 or HBM.
+
+Consecutive rounds over one direction are carried (`last_round_stats_carried`): the previous update phase summed their
+statistics, so the statistics phase is only the cross-GPU exchange and the "statistics" stamp measures the time to
+it.  `carry: 0` drops the carried statistics before every round (handing out H's device pointer, which launches
+nothing), so that every round runs its statistics pass."""
 import json
 import math
 import os
@@ -43,37 +48,44 @@ for n in (100_000_000, 50_000_000, 25_000_000, 12_500_000, 6_250_000):
     ctx.copy_slot(N.SLOT_H, N.SLOT_F)   # h = 0.5 y + N(0, 0.5)
     ctx.fill(N.SLOT_F, 0.0)
     ctx.gbm_pseudo_residuals(False)
-    for fused, res in ((1, 1), (1, 0), (0, 1)):
+    for fused, res, carry in ((1, 1, 1), (1, 1, 0), (1, 0, 1), (1, 0, 0), (0, 1, 0)):
         ctx.set_option("fused_round", fused)
         ctx.set_option("fused_resident", res)
         ctx.set_option("fused_timing", 0)
+
+        def round_():
+            if not carry:
+                ctx.device_ptr(N.SLOT_H)
+            return ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
         for _ in range(5):
-            ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
+            round_()
         ctx.sync()
         t0 = time.perf_counter()
         R = 200
         for _ in range(R):
-            ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
+            round_()
         ctx.sync()
         wall = 1e6 * (time.perf_counter() - t0) / R
         ctx.kernel_timing(True); ctx.kernel_times_reset()
         for _ in range(50):
-            ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
+            round_()
         kt = ctx.kernel_times(); ctx.kernel_timing(False)
-        out = {"rows": n, "fused": fused, "fused_resident": res, "wall_us_per_round": wall,
+        out = {"rows": n, "fused": fused, "fused_resident": res, "carry": carry,
+               "last_round_stats_carried": int(ctx.get_option("last_round_stats_carried")), "wall_us_per_round": wall,
                "kernel_event_us": {k: 1e3 * v["ms"] / v["launches"] for k, v in kt.items()}}
         if fused:
             ctx.set_option("fused_timing", 1)
             ph = []
             for _ in range(100):
-                _, _, ne = ctx.gbm_round(0.01, True, 1e-6, 100, residual=True)
+                _, _, ne = round_()
                 ph.append([ctx.get_option("last_fused_stats_us"), ctx.get_option("last_fused_brent_us"),
                            ctx.get_option("last_fused_update_us")])
             ph.sort(key=lambda p: sum(p))
             out["phases_us_median"] = ph[len(ph) // 2]
             out["brent_evals"] = ne
             grid, tiles = int(ctx.get_option("last_fused_grid")), ctx.get_option("last_fused_resident_tiles")
-            carried = carried_float4s(n, grid, int(round(tiles * U)))
+            # a carried round's shared-memory groups are loaded while the step is computed: still read off chip
+            carried = 0 if carry else carried_float4s(n, grid, int(round(tiles * U)))
             out.update({"grid": grid, "last_fused_resident_tiles": tiles, "phase_b_carried_bytes": 32 * carried,
                         "phase_b_offchip_read_bytes": 8 * n - 32 * carried, "phase_b_write_bytes": 4 * n})
             ctx.set_option("fused_timing", 0)

@@ -126,6 +126,7 @@ SE_API int se_ctx_kernel_time_reset(se_ctx* ctx);
  * weights >= 0: keys-only sort + margin-checked model-order sums, exact kernel for the deferred rows), "wm_list_cap"
  * (deferred-row list capacity, 0 = rows / 4).  Read-only: "last_tree_binned", "last_tree_mask", "last_wm_mode" (0 exact,
  * 1 fast with margin, 2 equal weights), "last_wm_deferred" (synchronises), "last_round_fused",
+ * "last_round_stats_carried" (1: the last one-launch round took its statistics from the previous round's update pass),
  * "last_ls_workers", "last_ls_passes", "last_ls_hit_ratio" (kept for compatibility, always 0), "last_fused_grid",
  * "last_fused_resident_tiles" (tiles per CTA the last one-launch round carried in shared memory).  Unknown keys fail
  * with SE_ERR_ARG. */

@@ -230,6 +230,7 @@ int settle_f(se_ctx* ctx) {
   SE_LAUNCH_T(ctx, SE_KF_OTHER, launch_gbm_settle_f(ctx->slot[SE_SLOT_Y].d, ctx->slot[SE_SLOT_R].d, ctx->slot[SE_SLOT_F].d,
                                                     ctx->gbm.n, ctx->sms, ctx->stream));
   ctx->gbm.f_owed = false;
+  ctx->gbm.sq_stats_current = false;  // y - (y - r) need not equal r bit for bit
   return SE_OK;
 }
 
@@ -241,8 +242,10 @@ int write_slot(se_ctx* ctx, int slot) {
     case SE_SLOT_Y: case SE_SLOT_F: case SE_SLOT_R:
       SE_TRY(settle_f(ctx));
       ctx->gbm.r_current = false;
+      ctx->gbm.sq_stats_current = false;
       if (slot == SE_SLOT_Y) ctx->y_state[0] = 0;  // labels checked as class indices
       break;
+    case SE_SLOT_H: ctx->gbm.sq_stats_current = false; break;  // the squared round's carried statistics
     case SE_SLOT_VY: ctx->y_state[1] = 0; break;
     case SE_SLOT_W: case SE_SLOT_BAG: ctx->gbm.wsum_valid = false; break;
     case SE_SLOT_WOUT: ctx->wout_scaled = false; break;  // se_download's 1/S factor
@@ -516,6 +519,7 @@ const Option kOptions[] = {
   {"last_fused_brent_us", SE_GET(c->last_fused_us[1])},
   {"last_fused_update_us", SE_GET(c->last_fused_us[2])},
   {"last_round_fused", SE_GET(c->last_round_fused)},
+  {"last_round_stats_carried", SE_GET(c->last_round_carried)},
   {"last_ls_workers", SE_GET(c->last_ls_workers)},
   {"last_ls_passes", SE_GET(c->last_ls_passes)},
   {"last_ls_hit_ratio", SE_GET(0.0)},  // kept for compatibility: no L2 window is ever requested

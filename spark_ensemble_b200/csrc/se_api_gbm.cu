@@ -101,6 +101,7 @@ int se_gbm_configure(se_ctx* ctx, int64_t n_train, int64_t n_valid, int dim, int
   g.has_w = has_weights != 0;
   g.use_bag = false;
   g.r_current = false;
+  g.sq_stats_current = false;
   g.wsum_valid = false; g.counts_valid = false;
   ctx->y_state[0] = ctx->y_state[1] = 0;
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_Y, 1, n_train));
@@ -122,6 +123,7 @@ int se_gbm_set_loss_param(se_ctx* ctx, double param) {
   SE_TRY(settle_f(ctx));
   ctx->gbm.param = param;
   ctx->gbm.r_current = false;
+  ctx->gbm.sq_stats_current = false;
   return SE_OK;
 }
 
@@ -132,6 +134,7 @@ int se_gbm_set_bag(se_ctx* ctx, int on) {
   if (on) SE_TRY(slot_alloc2d(ctx, SE_SLOT_BAG, 1, ctx->gbm.n));
   ctx->gbm.use_bag = on != 0;
   ctx->gbm.wsum_valid = false;
+  ctx->gbm.sq_stats_current = false;
   return SE_OK;
 }
 
@@ -238,6 +241,7 @@ int se_gbm_pseudo_residuals(se_ctx* ctx, int newton, double* sum_hess) {
   SE_REQUIRE(ctx, !newton || loss_has_hessian(ctx->gbm.loss), SE_ERR_ARG, "loss %d has no hessian (updates=newton)", ctx->gbm.loss);
   SE_TRY(begin(ctx));
   SE_TRY(settle_f(ctx));
+  ctx->gbm.sq_stats_current = false;  // R is rewritten
   if (newton) SE_TRY(slot_alloc2d(ctx, SE_SLOT_WOUT, ctx->gbm.dim, ctx->gbm.n));
   GbmArgs a = gbm_args(ctx, false);
   ctx->wout_scaled = false;
@@ -296,6 +300,7 @@ int se_gbm_update(se_ctx* ctx, const double* step, int flags, double* loss_sum, 
   SE_REQUIRE(ctx, !newton || loss_has_hessian(ctx->gbm.loss), SE_ERR_ARG, "loss %d has no hessian", ctx->gbm.loss);
   SE_TRY(begin(ctx));
   SE_TRY(settle_f(ctx));
+  ctx->gbm.sq_stats_current = false;  // F or R is rewritten
   if (newton) SE_TRY(slot_alloc2d(ctx, SE_SLOT_WOUT, ctx->gbm.dim, ctx->gbm.n));
   GbmArgs a = gbm_args(ctx, false);
   const int mode = newton ? GBM_UPDATE_NEWTON : ((flags & SE_UPD_RESIDUAL) ? GBM_UPDATE_RESID : GBM_UPDATE);
@@ -523,6 +528,17 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   // second cross-GPU exchange, and the host is served before the update phase ends.  With a bag the statistics run
   // over the bag while the loss runs over all rows: then the loss is reduced over the rows as in the two-launch path.
   const bool loss_reduce = g.use_bag || ctx->fused_loss_reduce;
+  // Such a residual round's update pass also sums the statistics of what it writes, (r', h), into d_scal[kScalCarry]:
+  // the next round over the same direction takes them from there and skips its statistics pass (12 B/row, not 20).
+  // The update then walks its tiles opposite to the previous one, so that it starts on what is still in the L2.
+  const bool stats_out = write_r && !loss_reduce;
+  const bool carried = stats_out && g.r_current && g.sq_stats_current;
+  a.carried = carried ? 1 : 0;
+  a.forward = (carried && !g.sq_last_up) ? 1 : 0;
+  a.ws_next.partials = ctx->d_partials + (size_t)(kMaxGridPartials / 2) * 4;  // ws_b's, unused without a row-reduced loss
+  a.ws_next.counter = &ctx->d_fsync->counter_b;
+  a.ws_next.out = ctx->d_scal + kScalCarry;
+  ctx->gbm.sq_stats_current = false;           // until the round has succeeded
   a.ws_a = red_ws(ctx, kScalRound);            // sequence number s (statistics)
   a.ws_a.host_out = nullptr;                   // the mirror ticket is written after Brent / the second reduction
   a.ws_a.host_flag = nullptr;
@@ -554,6 +570,7 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->fused_resident, ctx->sms,
                                                            ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots));
   ctx->last_fused_grid = grid;
+  ctx->last_round_carried = carried ? 1 : 0;
   ctx->last_fused_resident_tiles = resident_slots / 4.0;  // float4 groups per thread, U_SQ = 4 to a tile
   ctx->gbm.r_current = write_r != 0;
   const bool owed_before = ctx->gbm.f_owed;
@@ -585,6 +602,10 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
     ctx->gbm.f_owed = owed_before;
     return fail(ctx, SE_ERR_OPT, "Brent exceeded MaxEval(%d)", max_iter);
   }
+  if (stats_out) {
+    ctx->gbm.sq_stats_current = true;
+    ctx->gbm.sq_last_up = a.forward != 0;
+  }
   return SE_OK;
 }
 }  // namespace
@@ -594,6 +615,7 @@ int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, i
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.dim == 1, SE_ERR_STATE, "se_gbm_round needs dim == 1");
   ctx->last_round_fused = 0;
+  ctx->last_round_carried = 0;
   const bool sq_search = optimized && ctx->gbm.loss == SE_LOSS_SQUARED && !(flags & SE_UPD_NEWTON) && max_iter >= 1;
   if (sq_search) {
     // commons-math3 BrentOptimizer constructor checks (the host path performs them in brent_impl's caller)
@@ -672,6 +694,7 @@ int se_gbm_round_squared_async(se_ctx* ctx, double learning_rate) {
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.loss == SE_LOSS_SQUARED, SE_ERR_STATE, "squared loss only");
   SE_TRY(begin(ctx));
   SE_TRY(settle_f(ctx));
+  ctx->gbm.sq_stats_current = false;  // R is rewritten
   GbmArgs a = gbm_args(ctx, false);
   a.stats_from_r = ctx->gbm.r_current ? 1 : 0;
   a.ws = red_ws(ctx, kScalRound);  // stats -> d_scal[kScalRound..+2]

@@ -42,6 +42,7 @@ extern thread_local std::string g_last_error;
 constexpr int kScal = 1024;         // doubles in the device/host scalar blocks ([0, 160): generic reductions)
 constexpr int kScalHist = 704;      // 256-bin radix-select histogram
 constexpr int kScalRound = 160;     // offset of the squared-round results (statistics, alpha, loss)
+constexpr int kScalCarry = 184;     // the squared round's carried statistics (3 values, gbm.sq_stats_current)
 constexpr int kScalHost = 192;      // offset used by se_comm_allreduce_host (up to kScalHist - kScalHost values)
 constexpr int kSmallBytes = 1 << 20;  // small device scratch: weights, init, tree arrays, factors
 
@@ -179,6 +180,10 @@ struct se_ctx {
     bool r_current = false;  // SE_SLOT_R holds -g(y, F) of the CURRENT F (squared loss: y - F)
     bool f_owed = false;     // SE_SLOT_F is stale: its value is y - r (residual-mode fused squared round); settle_f
                              // rebuilds it.  Implies r_current.
+    // d_scal[kScalCarry..+2] holds this GPU's Σr², Σhr, Σh² over the current R and H: the update pass of the last
+    // residual fused round summed them over what it wrote.  Dropped by every write of Y, F, R or H.
+    bool sq_stats_current = false;
+    bool sq_last_up = false;  // the last fused round's update pass walked its tiles upwards (ended on the highest)
     double wsum = 0.0;
     bool wsum_valid = false;
     double n_global = 0.0, nv_global = 0.0;
@@ -250,7 +255,7 @@ struct se_ctx {
   int clock_khz = 1965000;
   double peer_timeout_ms = 120000.0;  // spin bound of the fused peer exchange (0 = wait forever)
   // diagnostics of the last call (se_ctx_get_option)
-  int last_round_fused = 0, last_ls_workers = 0, last_ls_resident = 0, last_ls_passes = 0, last_fused_grid = 0;
+  int last_round_fused = 0, last_round_carried = 0, last_ls_workers = 0, last_ls_resident = 0, last_ls_passes = 0, last_fused_grid = 0;
   double last_round_stats[3] = {0.0, 0.0, 0.0};
   // newton updates: SE_SLOT_WOUT holds 1/2 hc w; the 1/S_j of each dimension is applied on download
   std::vector<float> wout_scale;

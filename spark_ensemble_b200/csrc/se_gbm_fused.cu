@@ -15,6 +15,8 @@
 //    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api_ctx.cu settle_f).
 //    A round whose residual slot is not current (Y, F or R were just written) reads (y, F, h) instead of (r, h):
 //    r' = (y - F) - c h, 16 B/row.  Without residual mode the update is F' = F + c h (F, y, h read; F written).
+//    A residual round without a bag also sums the statistics of (r', h) in its update pass; while R and H stay as
+//    it left them, the next round takes those sums and skips the statistics pass (12 B/row).
 //
 //  * gbm_linesearch_persist_kernel — Brent's <= MaxEval evaluations of the line-search objective
 //    (boosting/GBMLoss.scala:50-74 through RDDLossFunction; GBMRegressor.scala:408-421) for the non-squared scalar
@@ -110,26 +112,45 @@ __device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
   }
 }
 
-// FROM_R (the path a fit and the benchmark take: residual mode, the residual slot current, no bag) is a compile-time
+__device__ __forceinline__ void cp_async16(float4* smem, const float* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem)
+               : "memory");
+}
+
+// FROM_R (a fit's round after a new direction: residual mode, the residual slot current, no bag) is a compile-time
 // specialisation: it carries phase A's tail into phase B on chip (kSqSlotBytes) and has no y / F / bag arrays live.
-template <bool WRITE_R, bool LOSS_REDUCE, bool FROM_R>
+// CARRIED (the rounds after it over the same direction) has no phase A at all: the previous round's update pass left
+// the statistics of (r, h) in a.ws_next.out.  One CTA sums them across GPUs and runs Brent while every CTA has its
+// first update tile in registers and, with resident slots, the groups after it in flight to shared memory.
+// Residual rounds whose loss comes from the statistics (STATS_OUT) sum the next round's statistics in phase B.
+template <bool WRITE_R, bool LOSS_REDUCE, bool FROM_R, bool CARRIED>
 __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqRoundArgs a) {
   static_assert(WRITE_R || !FROM_R, "FROM_R is a residual-mode round");
+  static_assert(!CARRIED || (WRITE_R && !LOSS_REDUCE && !FROM_R), "CARRIED is a residual round without a bag");
+  constexpr bool STATS_OUT = WRITE_R && !LOSS_REDUCE;
   constexpr int U = U_SQ;
-  extern __shared__ float4 s_res[];  // FROM_R: [slot][r, h][kBlock]
+  extern __shared__ float4 s_res[];  // FROM_R, CARRIED: [slot][r, h][kBlock]
   __shared__ float s_coef;
-  __shared__ float4 s_brent_regs[2 * U];  // FROM_R: the Brent thread's carried groups while it runs Brent
+  __shared__ float4 s_brent_regs[2 * U];  // FROM_R, CARRIED: the Brent thread's tile registers while it runs Brent
   const int64_t n4 = a.n >> 2;
   constexpr int64_t tile = (int64_t)kBlock * U;
   const int64_t ntiles = (n4 + tile - 1) / tile;
   const int64_t G = gridDim.x;
   const int64_t cnt = (ntiles > (int64_t)blockIdx.x) ? (ntiles - 1 - blockIdx.x) / G + 1 : 0;  // tiles b, b+G, ...
-  const bool has_bag = !FROM_R && (a.bag != nullptr);
-  const bool stats_from_r = FROM_R || a.stats_from_r;
-  // FROM_R: group u of tile i has the flat index i*U + u.  The last tile (cnt-1) stays in registers, the S groups
-  // before it in shared memory: every group from p_res on is carried to phase B.
-  const int64_t S = FROM_R ? min((int64_t)a.resident_slots, (cnt > 0 ? cnt - 1 : 0) * U) : 0;
+  const bool has_bag = !FROM_R && !CARRIED && (a.bag != nullptr);
+  const bool stats_from_r = FROM_R || CARRIED || a.stats_from_r;
+  // Phase B's k-th tile is i = cnt-1-k (downwards, from where phase A ended), or i = k on a carried round that walks
+  // upwards.  FROM_R: group u of tile i has the flat index i*U + u.  The last tile (cnt-1) stays in registers, the S
+  // groups before it in shared memory: every group from p_res on is carried to phase B.  CARRIED: the first tile is
+  // in registers and the S groups after it, in phase B's order, in shared memory.
+  const bool up = CARRIED && a.forward;
+  const int64_t S = (FROM_R || CARRIED) ? min((int64_t)a.resident_slots, (cnt > 0 ? cnt - 1 : 0) * U) : 0;
   const int64_t p_res = (cnt - 1) * U - S;
+  auto slot_of = [&](int64_t k, int64_t i, int u) -> int64_t {  // shared-memory slot of a phase-B group, or -1
+    if constexpr (FROM_R) return i * U + u - p_res;
+    if constexpr (CARRIED) return (k >= 1 && (k - 1) * U + u < S) ? (k - 1) * U + u : -1;
+    return -1;
+  };
   const uint64_t pol_stream = l2_policy(a.l2_hints != 0);
   const uint64_t pol_keep = l2_policy(false);
   // carried groups are served from chip in phase B: their L2 lines go first, so that the L2 keeps the groups before
@@ -137,6 +158,67 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   const uint64_t pol_carried = l2_policy(true);
 
   if (a.timing && blockIdx.x == 0 && threadIdx.x == 0) a.out[10] = global_timer_us();
+  // phase B's tile registers.  FROM_R: phase A loads into them, so that its last tile is where phase B starts; the
+  // other rounds keep phase A's tiles local, so that nothing is live across the wait but what phase B loads.
+  float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
+  bool ok[U];
+  // the Brent thread parks the tile registers in shared memory meanwhile: Brent needs more registers than are left
+  // beside them, and local memory would be the alternative
+  auto run_brent = [&]() {
+    if constexpr (FROM_R || CARRIED) {
+#pragma unroll
+      for (int u = 0; u < U; ++u) s_brent_regs[u] = vy[u], s_brent_regs[U + u] = vh[u];
+    }
+    fused_round_brent<LOSS_REDUCE>(a);
+    if constexpr (FROM_R || CARRIED) {
+#pragma unroll
+      for (int u = 0; u < U; ++u) vy[u] = s_brent_regs[u], vh[u] = s_brent_regs[U + u];
+    }
+  };
+  const bool from_r = WRITE_R && stats_from_r;
+  auto load_tile = [&](int64_t k) {
+    const int64_t i = up ? k : cnt - 1 - k;
+    const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int64_t g = base + (int64_t)u * kBlock;
+      ok[u] = g < n4;
+      if (ok[u]) {
+        const int64_t s = slot_of(k, i, u);
+        if ((FROM_R || CARRIED) && s >= 0) {
+          vy[u] = s_res[(2 * s) * kBlock + threadIdx.x];
+          vh[u] = s_res[(2 * s + 1) * kBlock + threadIdx.x];
+          continue;
+        }
+        if (from_r) {
+          vy[u] = ld_rw4_p(a.r + 4 * g, pol_stream);
+        } else {
+          vy[u] = ld_stream4_p(a.y + 4 * g, pol_stream);
+          vF[u] = ld_rw4_p(a.F + 4 * g, pol_stream);
+        }
+        vh[u] = ld_stream4_p(a.h + 4 * g, pol_stream);  // the update is h's last reader
+      }
+    }
+  };
+
+  if constexpr (CARRIED) {
+    // the first tile into registers, the S groups after it into shared memory (each thread copies, and in phase B
+    // reads back, only its own slots: no barrier)
+    if (cnt > 0) load_tile(0);
+    for (int64_t s = 0; s < S; ++s) {
+      const int64_t k = 1 + s / U, i = up ? k : cnt - 1 - k;
+      const int64_t g = (blockIdx.x + i * G) * tile + threadIdx.x + (s % U) * (int64_t)kBlock;
+      if (g < n4) {
+        cp_async16(&s_res[(2 * s) * kBlock + threadIdx.x], a.r + 4 * g);
+        cp_async16(&s_res[(2 * s + 1) * kBlock + threadIdx.x], a.h + 4 * g);
+      }
+    }
+    if (blockIdx.x == 0) {
+      peer_exchange(a.ws_next.out, 3, a.ws_a);  // this GPU's statistics -> a.out[0..2], summed across GPUs
+      __syncthreads();
+      if (threadIdx.x == 0) run_brent();
+    }
+  } else {
   // ---- phase A: Σ(y-F)², Σh(y-F), Σh² (from the current residual slot when it is valid: 8 B/row)
   double acc[3] = {0.0, 0.0, 0.0};
   auto stats_tile = [&](int64_t i, float4 (&vy)[U], float4 (&vF)[U], float4 (&vh)[U], bool (&ok)[U]) {
@@ -192,10 +274,6 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       }
     }
   };
-  // phase B's tile registers.  FROM_R: phase A loads into them, so that its last tile is where phase B starts; the
-  // other rounds keep phase A's tiles local, so that nothing is live across the wait but what phase B loads.
-  float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
-  bool ok[U];
   for (int64_t i = 0; i < cnt; ++i) {
     if constexpr (FROM_R) {
       stats_tile(i, vy, vF, vh, ok);
@@ -216,52 +294,16 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   const bool last = block_reduce_publish<3>(acc, a.ws_a);  // the last CTA also sums across GPUs (peer_exchange)
   if (last) {
     __syncthreads();  // a.out[0..2] were written by other threads of this CTA
-    if (threadIdx.x == 0) {
-      // FROM_R: Brent needs more registers than are left beside the carried tile; its thread parks that tile in
-      // shared memory meanwhile instead of spilling to local memory
-      if constexpr (FROM_R) {
-#pragma unroll
-        for (int u = 0; u < U; ++u) s_brent_regs[u] = vy[u], s_brent_regs[U + u] = vh[u];
-      }
-      fused_round_brent<LOSS_REDUCE>(a);
-      if constexpr (FROM_R) {
-#pragma unroll
-        for (int u = 0; u < U; ++u) vy[u] = s_brent_regs[u], vh[u] = s_brent_regs[U + u];
-      }
-    }
+    if (threadIdx.x == 0) run_brent();
   }
+  // in flight while the last CTA reduces, exchanges and runs Brent (FROM_R: still in registers from phase A)
+  if (!FROM_R && cnt > 0) load_tile(0);
+  }  // phase A
 
   // ---- phase B, tiles in the opposite direction.  WRITE_R (residual mode): r' = r - step*h, Σ r'²/2; F is not
   // touched (the host rebuilds it as y - r' when it is next accessed), or r' = (y - F) - step*h on a round whose
   // residual slot is not current.  Otherwise: F' = F + step*h, Σ (y-F')²/2.  The order of the tiles, and so of the
   // loss sum, is the same whether a tile comes from registers, shared memory or global memory.
-  const bool from_r = WRITE_R && stats_from_r;
-  auto load_tile = [&](int64_t i) {
-    const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t g = base + (int64_t)u * kBlock;
-      ok[u] = g < n4;
-      if (ok[u]) {
-        const int64_t s = i * U + u - p_res;
-        if (FROM_R && s >= 0) {
-          vy[u] = s_res[(2 * s) * kBlock + threadIdx.x];
-          vh[u] = s_res[(2 * s + 1) * kBlock + threadIdx.x];
-          continue;
-        }
-        if (from_r) {
-          vy[u] = ld_rw4_p(a.r + 4 * g, pol_stream);
-        } else {
-          vy[u] = ld_stream4_p(a.y + 4 * g, pol_stream);
-          vF[u] = ld_rw4_p(a.F + 4 * g, pol_stream);
-        }
-        vh[u] = ld_stream4_p(a.h + 4 * g, pol_stream);  // the update is h's last reader
-      }
-    }
-  };
-  int64_t i = cnt - 1;
-  // in flight while the last CTA reduces, exchanges and runs Brent (FROM_R: still in registers from phase A)
-  if (!FROM_R && i >= 0) load_tile(i);
   if (threadIdx.x == 0) {
     if constexpr (FROM_R) {
       // nothing of the carried tail is loaded: while the grid waits for the step, the first tile phase B reads from
@@ -280,17 +322,20 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {}
     s_coef = (float)a.sync->x;  // same rounding as the host path: (float)(lr * alpha)
   }
+  if constexpr (CARRIED) asm volatile("cp.async.wait_all;" ::: "memory");  // this thread's slots have landed
   __syncthreads();
   const float coef = s_coef;
   double accb[1] = {0.0};
-  while (i >= 0) {
+  double accn[3] = {0.0, 0.0, 0.0};  // STATS_OUT: Σr'², Σhr', Σh² over what this pass writes, as phase A sums them
+  for (int64_t k = 0; k < cnt; ++k) {
+    const int64_t i = up ? k : cnt - 1 - k;
     const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (!ok[u]) continue;
       const int64_t g = base + (int64_t)u * kBlock;
       float4 o;
-      float l_acc = 0.f;
+      float l_acc = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f;
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         float d;
@@ -305,13 +350,19 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
           f4at(o, e) = p;
         }
         if (LOSS_REDUCE) l_acc = fmaf(0.5f * d, d, l_acc);           // GBMLoss.scala:129-137
+        if (STATS_OUT) {
+          const float h = f4at(vh[u], e);
+          s0 = fmaf(d, d, s0);
+          s1 = fmaf(h, d, s1);
+          s2 = fmaf(h, h, s2);
+        }
       }
       if (WRITE_R) st_stream4_p(a.r + 4 * g, o, pol_keep);  // the next statistics pass starts where this one ends
       else st_stream4_p(a.F + 4 * g, o, pol_stream);
       if (LOSS_REDUCE) accb[0] += (double)l_acc;
+      if (STATS_OUT) accn[0] += (double)s0, accn[1] += (double)s1, accn[2] += (double)s2;
     }
-    --i;
-    if (i >= 0) load_tile(i);
+    if (k + 1 < cnt) load_tile(k + 1);
   }
   if (blockIdx.x == 0 && threadIdx.x < (a.n & 3)) {
     const int64_t j = (n4 << 2) + threadIdx.x;
@@ -325,14 +376,22 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       a.F[j] = p;
     }
     accb[0] += (double)(0.5f * d * d);
+    if (STATS_OUT) {
+      const float h = a.h[j];
+      accn[0] += (double)(d * d), accn[1] += (double)(h * d), accn[2] += (double)(h * h);
+    }
   }
   if constexpr (LOSS_REDUCE) {
     const bool last_b = block_reduce_publish<1>(accb, a.ws_b);  // Σloss -> a.ws_b.out (+ cross-GPU sum, host mirror + ticket)
     if (a.timing && last_b && threadIdx.x == 0) a.out[13] = global_timer_us();
-  } else if (a.timing) {
-    // no reduction (the loss came from the statistics): the latest stamp of any CTA marks the end of the update
-    __syncthreads();
-    if (threadIdx.x == 0) atomicMax(reinterpret_cast<unsigned long long*>(&a.out[13]), (unsigned long long)__double_as_longlong(global_timer_us()));
+  } else {
+    // the next round's statistics, this GPU's: a carried round reads them before any CTA of it arrives here
+    if constexpr (STATS_OUT) block_reduce_publish<3>(accn, a.ws_next);
+    if (a.timing) {
+      // the loss came from the statistics: the latest stamp of any CTA marks the end of the update
+      __syncthreads();
+      if (threadIdx.x == 0) atomicMax(reinterpret_cast<unsigned long long*>(&a.out[13]), (unsigned long long)__double_as_longlong(global_timer_us()));
+    }
   }
 }
 
@@ -658,13 +717,16 @@ cudaError_t launch_ls(const LsArgs& a0, int sms, const LsLaunch& cfg, cudaStream
 
 cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int loss_reduce, int resident, int sms,
                                       int max_ctas_per_sm, cudaStream_t st, int* grid_out, int* resident_slots_out) {
-  constexpr int kKerns = 6;
+  constexpr int kKerns = 7;
   void (*kerns[kKerns])(const SqRoundArgs) = {
-      gbm_round_sq_fused_kernel<false, false, false>, gbm_round_sq_fused_kernel<false, true, false>,
-      gbm_round_sq_fused_kernel<true, false, false>,  gbm_round_sq_fused_kernel<true, true, false>,
-      gbm_round_sq_fused_kernel<true, false, true>,   gbm_round_sq_fused_kernel<true, true, true>};
-  const bool from_r = write_r && a0.stats_from_r && a0.bag == nullptr;
-  const int which = from_r ? 4 + (loss_reduce ? 1 : 0) : (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
+      gbm_round_sq_fused_kernel<false, false, false, false>, gbm_round_sq_fused_kernel<false, true, false, false>,
+      gbm_round_sq_fused_kernel<true, false, false, false>,  gbm_round_sq_fused_kernel<true, true, false, false>,
+      gbm_round_sq_fused_kernel<true, false, true, false>,   gbm_round_sq_fused_kernel<true, true, true, false>,
+      gbm_round_sq_fused_kernel<true, false, false, true>};
+  const bool carried = a0.carried != 0;
+  if (carried && !(write_r && !loss_reduce && a0.bag == nullptr)) return cudaErrorInvalidValue;
+  const bool from_r = !carried && write_r && a0.stats_from_r && a0.bag == nullptr;
+  const int which = carried ? 6 : from_r ? 4 + (loss_reduce ? 1 : 0) : (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
   // function attributes and occupancy are per DEVICE (a process may drive several GPUs, as in launch_ls)
   constexpr int kMaxDev = 64;
   struct KernInfo {
@@ -687,7 +749,7 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
     if (e != cudaSuccess) return e;
     info.static_smem = (int)fa.sharedSizeBytes;
     info.max_dyn = 0;
-    if (which >= 4) {  // the carry-over sizes its dynamic shared memory past the default 48 KB
+    if (which >= 4) {  // the shared-memory carry sizes its dynamic shared memory past the default 48 KB
       int optin = 0;
       cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
       info.max_dyn = optin - info.static_smem;
@@ -708,9 +770,9 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
   if (grid < 1) grid = 1;
   if (grid > kMaxGridPartials / 2) grid = kMaxGridPartials / 2;
   // carried slots per CTA: the SM's shared memory split between its co-resident CTAs (1 KB per CTA is reserved by
-  // the system), and no more than the busiest CTA has groups before its last tile
+  // the system), and no more than the busiest CTA has groups besides the tile it keeps in registers
   int64_t slots = 0;
-  if (from_r && resident) {
+  if ((from_r || carried) && resident) {
     int64_t budget = (int64_t)smem_per_sm_dev[dev] / per_sm - 1024 - info.static_smem;
     if (budget > info.max_dyn) budget = info.max_dyn;
     slots = budget / kSqSlotBytes;

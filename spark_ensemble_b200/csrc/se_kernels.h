@@ -86,6 +86,8 @@ struct FusedSync {
 // write_r (residual mode): the update writes r' = r - c h only and leaves F for the host to rebuild as y - r'.
 // A residual-mode round that reads r (no bag) carries its statistics pass's last tile in registers and, with
 // `resident`, the groups before it in shared memory into the update pass; *resident_slots_out = groups per thread.
+// A carried round (a.carried) has no statistics pass: it loads its first update tile into registers and, with
+// `resident`, the groups after it into shared memory while the step is computed.
 struct SqRoundArgs {
   const float* y = nullptr;
   float* F = nullptr;
@@ -102,6 +104,11 @@ struct SqRoundArgs {
   int max_eval = 100;
   RedWs ws_a{};  // statistics: out = `out`, no host mirror
   RedWs ws_b{};  // loss (only when it is reduced over the rows: bags): out = out + 8, host mirror + ticket
+  // Residual rounds without a bag and with the loss from the statistics: the update pass also sums Σr'², Σhr', Σh²
+  // over what it writes, i.e. the next round's statistics, into ws_next.out (this GPU's sums: no exchange, no mirror).
+  RedWs ws_next{};
+  int carried = 0;  // 1: ws_next.out holds the statistics of (r, h): skip the statistics pass
+  int forward = 0;  // carried round: walk the update's tiles upwards (the previous update ended on the lowest ones)
   double* out = nullptr;       // [0..2] statistics, [4] alpha, [5] objective, [6] +-evaluations, [8] Σloss
   double* host_res = nullptr;  // mapped host copy of out[0..6] (nullable)
   // loss-from-statistics mode: the Brent thread also serves the host (final value + ticket) before the update phase ends
