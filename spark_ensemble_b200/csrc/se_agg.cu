@@ -15,6 +15,7 @@
 #include "se_loss.cuh"
 #include "se_tma.cuh"
 #include "se_sortnet.h"
+#include <type_traits>
 #include "../../include/se_abi.h"
 
 namespace se {
@@ -873,6 +874,51 @@ __device__ __forceinline__ uint32_t wm_candidate(const uint32_t (&s)[MP], uint32
   return v;
 }
 
+// The fast path's pick for a row of keys key[0..MP) in model order (padding keys ~0u carry weight 0): the smallest key
+// whose model-order cumulative weight reaches half the total.  safe: the crossing clears the margin tau on both sides,
+// so the reference's sorted-order sums pick the same key.  w is a __grid_constant__ parameter: the DFMAs of the
+// bisection read the weights as constant-bank operands.
+template <int MP>
+__device__ __forceinline__ uint32_t wm_fast_pick(const uint32_t (&key)[MP], const double (&w)[64], double total,
+                                                 double tau, bool& safe) {
+  constexpr int LOG = (MP == 1) ? 0 : (MP == 2) ? 1 : (MP == 4) ? 2 : (MP == 8) ? 3 : (MP == 16) ? 4 : (MP == 32) ? 5 : 6;
+  uint32_t s[MP];
+#pragma unroll
+  for (int m = 0; m < MP; ++m) s[m] = key[m];
+  sortnet_oddeven<MP>(s, [](uint32_t& x, uint32_t& y) {
+    const uint32_t lo = min(x, y), hi = max(x, y);
+    x = lo;
+    y = hi;
+  });
+  const double half = 0.5 * total;
+  // invariant: P(lo) false, P(hi) true with P(k) := Ĉ(s[k]) >= ĥ; lo = t - 1, hi = t after LOG probes
+  uint32_t t = 0, v_hi = s[MP - 1];
+  double c_lo = 0.0, c_hi = total;
+  auto probe = [&](uint32_t v) {
+    double c = 0.0;
+#pragma unroll
+    for (int m = 0; m < MP; ++m) {
+      // model order; padding (and m >= M) weights are 0.  fma(w, 1.0 or 0.0, c) is c + w rounded once, or c: one
+      // select of the high word of the 0/1 factor instead of the two selects `if (...) c += w` compiles to
+      const double b = __hiloint2double((key[m] <= v) ? 0x3ff00000 : 0, 0);
+      c = fma(w[m], b, c);
+    }
+    const bool right = !(c >= half);
+    c_lo = right ? c : c_lo;
+    c_hi = right ? c_hi : c;
+    v_hi = right ? v_hi : v;
+    t = 2u * t + (right ? 1u : 0u);
+  };
+  if constexpr (LOG > 0) probe(wm_candidate<MP, 0>(s, t));
+  if constexpr (LOG > 1) probe(wm_candidate<MP, 1>(s, t));
+  if constexpr (LOG > 2) probe(wm_candidate<MP, 2>(s, t));
+  if constexpr (LOG > 3) probe(wm_candidate<MP, 3>(s, t));
+  if constexpr (LOG > 4) probe(wm_candidate<MP, 4>(s, t));
+  if constexpr (LOG > 5) probe(wm_candidate<MP, 5>(s, t));
+  safe = (c_hi - half > tau) && (half - c_lo > tau);
+  return v_hi;
+}
+
 template <int MP>
 __global__ void __launch_bounds__(128) agg_wmedian_fast_kernel(const __grid_constant__ CUtensorMap mapP, int64_t n, int M,
                                                                const __grid_constant__ WmWeights wts, double total,
@@ -895,8 +941,6 @@ __global__ void __launch_bounds__(128) agg_wmedian_fast_kernel(const __grid_cons
     tma_load_tile(stage0 + (size_t)st * stage_floats, &mapP, (int)(tile * 128), &full[st]);
   };
   if (threadIdx.x == 0 && blockIdx.x < ntiles) issue(blockIdx.x, 0);
-  const double half = 0.5 * total;
-  constexpr int LOG = (MP == 1) ? 0 : (MP == 2) ? 1 : (MP == 4) ? 2 : (MP == 8) ? 3 : (MP == 16) ? 4 : (MP == 32) ? 5 : 6;
   uint32_t it = 0;
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
     const int st = it & 1;
@@ -905,45 +949,16 @@ __global__ void __launch_bounds__(128) agg_wmedian_fast_kernel(const __grid_cons
     const bool in = row < n;
     mbar_wait(&full[st], (it >> 1) & 1);
     const float* src = stage0 + (size_t)st * stage_floats + threadIdx.x;
-    uint32_t key[MP], s[MP];
+    uint32_t key[MP];
 #pragma unroll
     for (int m = 0; m < MP; ++m) {
       key[m] = 0xFFFFFFFFu;  // padding sorts last and carries weight 0
       if (m < M) key[m] = wm_key(src[m * 128]);
-      s[m] = key[m];
     }
     __syncthreads();  // the tile is in registers: its stage may be refilled
-    sortnet_oddeven<MP>(s, [](uint32_t& x, uint32_t& y) {
-      const uint32_t lo = min(x, y), hi = max(x, y);
-      x = lo;
-      y = hi;
-    });
-    // invariant: P(lo) false, P(hi) true with P(k) := Ĉ(s[k]) >= ĥ; lo = t - 1, hi = t after LOG probes
-    uint32_t t = 0, v_hi = s[MP - 1];
-    double c_lo = 0.0, c_hi = total;
-    auto probe = [&](uint32_t v) {
-      double c = 0.0;
-#pragma unroll
-      for (int m = 0; m < MP; ++m) {
-        // model order; padding (and m >= M) weights are 0.  fma(w, 1.0 or 0.0, c) is c + w rounded once, or c: one
-        // select of the high word of the 0/1 factor instead of the two selects `if (...) c += w` compiles to
-        const double b = __hiloint2double((key[m] <= v) ? 0x3ff00000 : 0, 0);
-        c = fma(wts.w[m], b, c);
-      }
-      const bool right = !(c >= half);
-      c_lo = right ? c : c_lo;
-      c_hi = right ? c_hi : c;
-      v_hi = right ? v_hi : v;
-      t = 2u * t + (right ? 1u : 0u);
-    };
-    if constexpr (LOG > 0) probe(wm_candidate<MP, 0>(s, t));
-    if constexpr (LOG > 1) probe(wm_candidate<MP, 1>(s, t));
-    if constexpr (LOG > 2) probe(wm_candidate<MP, 2>(s, t));
-    if constexpr (LOG > 3) probe(wm_candidate<MP, 3>(s, t));
-    if constexpr (LOG > 4) probe(wm_candidate<MP, 4>(s, t));
-    if constexpr (LOG > 5) probe(wm_candidate<MP, 5>(s, t));
-    const bool safe = (c_hi - half > tau) && (half - c_lo > tau);
-    if (in) out[row] = wm_unkey(v_hi);
+    bool safe;
+    const uint32_t pick = wm_fast_pick<MP>(key, wts.w, total, tau, safe);
+    if (in) out[row] = wm_unkey(pick);
     // rows whose decision could depend on the order of summation go to the exact kernel (warp-aggregated append)
     const bool defer = in && list != nullptr && !safe;
     const unsigned mask = __ballot_sync(0xffffffffu, defer);
@@ -985,13 +1000,6 @@ __global__ void __launch_bounds__(128) agg_wmedian_list_kernel(const float* __re
   }
 }
 
-inline int grid_rows(int64_t items, int64_t per_cta, int ctas_per_sm, int sms) {
-  int64_t need = (items + per_cta - 1) / per_cta;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)ctas_per_sm * sms;
-  return (int)(need < cap ? need : cap);
-}
-
 // class-wide sum kinds through the tile kernel (2 <= C <= 32 classes, the tile fits in shared memory)
 cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int sms, cudaStream_t st, bool* launched) {
   *launched = false;
@@ -1026,21 +1034,37 @@ cudaError_t try_launch_agg_class_tile(const AggArgs& a, const FinArgs& f0, int s
   int per_sm = (int)((228 * 1024) / (smem + 1280));
   if (per_sm > 16) per_sm = 16;
   if (per_sm < 1) return cudaSuccess;
-  const int64_t ntiles = (a.n + kAR - 1) / kAR;
-  const int64_t cap = (int64_t)per_sm * sms;
-  const int grid = (int)(ntiles < cap ? ntiles : cap);
-#define SE_CT(CM, LG)                                                                                    \
-  {                                                                                                      \
-    auto kern = agg_class_tile_kernel<CM, LG>;                                                           \
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);              \
-    if (e != cudaSuccess) return e;                                                                      \
-    kern<<<grid, 32, smem, st>>>(ta, f, mapP);                                                           \
+  const int grid = grid_rows(a.n, kAR, per_sm, sms);
+  auto launch = [&](auto kern) {
+    const cudaError_t e = allow_dynamic_smem(kern, smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, 32, smem, st>>>(ta, f, mapP);
+    *launched = true;
+    return cudaGetLastError();
+  };
+  if (ta.logp) return launch(agg_class_tile_kernel<32, true>);  // no register batch: CMAX is unused
+  if (C <= 4) return launch(agg_class_tile_kernel<4, false>);
+  if (C <= 8) return launch(agg_class_tile_kernel<8, false>);
+  if (C <= 16) return launch(agg_class_tile_kernel<16, false>);
+  return launch(agg_class_tile_kernel<32, false>);
+}
+
+// Calls f(std::integral_constant<int, MP>()) for the power of two MP >= M that the kernels for M <= 64 models are
+// instantiated for.
+template <class F>
+cudaError_t with_mp(int M, F f) {
+  int Mp = 1;
+  while (Mp < M) Mp <<= 1;
+  switch (Mp) {
+    case 1: return f(std::integral_constant<int, 1>());
+    case 2: return f(std::integral_constant<int, 2>());
+    case 4: return f(std::integral_constant<int, 4>());
+    case 8: return f(std::integral_constant<int, 8>());
+    case 16: return f(std::integral_constant<int, 16>());
+    case 32: return f(std::integral_constant<int, 32>());
+    case 64: return f(std::integral_constant<int, 64>());
+    default: return cudaErrorInvalidValue;
   }
-  if (ta.logp) SE_CT(32, true)  // no register batch: CMAX is unused
-  else if (C <= 4) SE_CT(4, false) else if (C <= 8) SE_CT(8, false) else if (C <= 16) SE_CT(16, false) else SE_CT(32, false)
-#undef SE_CT
-  *launched = true;
-  return cudaGetLastError();
 }
 
 // ---- a classifier forest in one pass (se_forest_agg) -------------------------------------------------------------
@@ -1075,6 +1099,8 @@ __global__ void __launch_bounds__(kForestAggTile) forest_agg_kernel(const Forest
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     __syncthreads();  // the packed trees are staged (first tile) / the previous tile's walks are over
     const int64_t row0 = tile * TILE;
+    // forest_stage_ranks written out: through the helper, nvcc 12.9 allocates the kFaSoft instantiation 32 instead of
+    // 40 registers and it runs 21 % slower (2 M rows, K = 26, H100)
     for (int i = threadIdx.x; i < a.C * (TILE / 4); i += TILE) {
       const int c = i / (TILE / 4), q = i % (TILE / 4);
       const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
@@ -1106,26 +1132,7 @@ __global__ void __launch_bounds__(kForestAggTile) forest_agg_kernel(const Forest
         }
       }
     };
-    int t = 0;
-    for (; t + 1 < a.T; t += 2) {  // two independent walks in flight, terms added in model order
-      const uint2* n0 = s_nodes + s_toff[t];
-      const uint2* n1 = s_nodes + s_toff[t + 1];
-      int d0 = 0, d1 = 0;
-      bool l0 = true, l1 = true;
-      while (l0 || l1) {
-        if (l0) forest_step<TILE>(n0, myr, d0, l0);
-        if (l1) forest_step<TILE>(n1, myr, d1, l1);
-      }
-      add(t, d0);
-      add(t + 1, d1);
-    }
-    if (t < a.T) {
-      const uint2* n0 = s_nodes + s_toff[t];
-      int d0 = 0;
-      bool l0 = true;
-      while (l0) forest_step<TILE>(n0, myr, d0, l0);
-      add(t, d0);
-    }
+    forest_walk<TILE>(s_nodes, s_toff, a.T, myr, add);
     if (!g.last) {
       for (int c = 0; c < C; ++c) g.acc[c * g.ld_acc + row] = tot[c * TILE];
     } else if (MODE == kFaTreeClass && g.dim == 1 && g.K == 2) {
@@ -1153,14 +1160,12 @@ static_assert(kForestMedianMaxTrees == SE_FOREST_MEDIAN_MAX_TREES, "the kernel's
 template <int MP>
 __global__ void __launch_bounds__(kForestMedianTile, 1) forest_median_kernel(const __grid_constant__ ForestMedianArgs g) {
   constexpr int TILE = kForestMedianTile;
-  constexpr int LOG = (MP == 1) ? 0 : (MP == 2) ? 1 : (MP == 4) ? 2 : (MP == 8) ? 3 : (MP == 16) ? 4 : (MP == 32) ? 5 : 6;
   extern __shared__ __align__(16) unsigned char fsm[];
   __shared__ double s_a[kForestMedianMaxTrees];
   for (int m = threadIdx.x; m < kForestMedianMaxTrees; m += TILE) s_a[m] = (m < g.M) ? g.w[m] : 0.0;
   const int M = g.M;
   float* vals = reinterpret_cast<float*>(fsm + g.vals_off) + threadIdx.x;  // this row's leaf values: own column
   const unsigned char* myr = fsm + threadIdx.x;  // + the chunk's blob_bytes: this row's ranks
-  const double half = 0.5 * g.total;
   const int64_t ntiles = (g.n + TILE - 1) / TILE;
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int64_t row0 = tile * TILE, row = row0 + threadIdx.x;
@@ -1174,83 +1179,32 @@ __global__ void __launch_bounds__(kForestMedianTile, 1) forest_median_kernel(con
           reinterpret_cast<uint4*>(fsm)[i] = __ldg(reinterpret_cast<const uint4*>(blob) + i);
       const unsigned long long* coloff = reinterpret_cast<const unsigned long long*>(blob + ch.off_coloff);
       unsigned char* s_rank = fsm + ch.blob_bytes;
-      for (int i = threadIdx.x; i < ch.C * (TILE / 4); i += TILE) {
-        const int c = i / (TILE / 4), q = i % (TILE / 4);
-        const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
-        uint32_t v = 0;
-        if (r < g.ld8) v = __ldg(reinterpret_cast<const uint32_t*>(g.X8 + __ldg(coloff + c) + r));
-        *reinterpret_cast<uint32_t*>(s_rank + c * TILE + 4 * q) = v;
-      }
+      // the offsets are read from the global blob: no barrier orders the blob's staging above before this read
+      forest_stage_ranks<TILE>(s_rank, g.X8, g.ld8, ch.C, row0, [&](int c) { return __ldg(coloff + c); });
       __syncthreads();
       if (!in) continue;
       const uint2* s_nodes = reinterpret_cast<const uint2*>(fsm + ch.off_nodes);
       const int* s_toff = reinterpret_cast<const int*>(fsm + ch.off_treeoff);
       const float* s_val = reinterpret_cast<const float*>(fsm + ch.off_values);
-      const unsigned char* r8 = myr + ch.blob_bytes;
       float* v = vals + (size_t)ch.t0 * TILE;
-      int t = 0;
-      for (; t + 1 < ch.T; t += 2) {  // two independent walks in flight
-        const uint2* n0 = s_nodes + s_toff[t];
-        const uint2* n1 = s_nodes + s_toff[t + 1];
-        int d0 = 0, d1 = 0;
-        bool l0 = true, l1 = true;
-        while (l0 || l1) {
-          if (l0) forest_step<TILE>(n0, r8, d0, l0);
-          if (l1) forest_step<TILE>(n1, r8, d1, l1);
-        }
-        v[t * TILE] = s_val[s_toff[t] + d0];
-        v[(t + 1) * TILE] = s_val[s_toff[t + 1] + d1];
-      }
-      if (t < ch.T) {
-        const uint2* n0 = s_nodes + s_toff[t];
-        int d0 = 0;
-        bool l0 = true;
-        while (l0) forest_step<TILE>(n0, r8, d0, l0);
-        v[t * TILE] = s_val[s_toff[t] + d0];
-      }
+      forest_walk<TILE>(s_nodes, s_toff, ch.T, myr + ch.blob_bytes,
+                        [&](int t, int leaf) { v[t * TILE] = s_val[s_toff[t] + leaf]; });
     }
-    // agg_wmedian_fast_kernel on the row's values (modes 1 and 2)
+    // agg_wmedian_fast_kernel's pick (wm_fast_pick) on the row's values (modes 1 and 2)
     uint32_t pick = 0;
     bool exact = (g.mode == 0);
     if constexpr (MP == 1) {  // one tree: both routes return its value (one weight is always "all equal": no margin)
       pick = wm_key(vals[0]);
       exact = false;
     } else if (in && g.mode != 0) {
-      uint32_t key[MP], s[MP];
+      uint32_t key[MP];
 #pragma unroll
       for (int m = 0; m < MP; ++m) {
         key[m] = 0xFFFFFFFFu;  // padding sorts last and carries weight 0
         if (m < M) key[m] = wm_key(vals[m * TILE]);
-        s[m] = key[m];
       }
-      sortnet_oddeven<MP>(s, [](uint32_t& x, uint32_t& y) {
-        const uint32_t lo = min(x, y), hi = max(x, y);
-        x = lo;
-        y = hi;
-      });
-      uint32_t t = 0, v_hi = s[MP - 1];
-      double c_lo = 0.0, c_hi = g.total;
-      auto probe = [&](uint32_t v) {
-        double c = 0.0;
-#pragma unroll
-        for (int m = 0; m < MP; ++m) {
-          const double b = __hiloint2double((key[m] <= v) ? 0x3ff00000 : 0, 0);
-          c = fma(g.w[m], b, c);
-        }
-        const bool right = !(c >= half);
-        c_lo = right ? c : c_lo;
-        c_hi = right ? c_hi : c;
-        v_hi = right ? v_hi : v;
-        t = 2u * t + (right ? 1u : 0u);
-      };
-      if constexpr (LOG > 0) probe(wm_candidate<MP, 0>(s, t));
-      if constexpr (LOG > 1) probe(wm_candidate<MP, 1>(s, t));
-      if constexpr (LOG > 2) probe(wm_candidate<MP, 2>(s, t));
-      if constexpr (LOG > 3) probe(wm_candidate<MP, 3>(s, t));
-      if constexpr (LOG > 4) probe(wm_candidate<MP, 4>(s, t));
-      if constexpr (LOG > 5) probe(wm_candidate<MP, 5>(s, t));
-      const bool safe = (c_hi - half > g.tau) && (half - c_lo > g.tau);
-      pick = v_hi;
+      bool safe;
+      pick = wm_fast_pick<MP>(key, g.w, g.total, g.tau, safe);
       exact = (g.mode == 1) && !safe;
     }
     // the exact (key, model) sort and sorted-order sums, as agg_wmedian_list_kernel / agg_wmedian_reg_kernel
@@ -1325,48 +1279,34 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
             e = cudaMemsetAsync(a.wm_count, 0, sizeof(unsigned int), st);
             if (e != cudaSuccess) return e;
           }
-          switch (Mp) {
-#define SE_WMF(MPV)                                                                                             \
-  case MPV: {                                                                                                   \
-    auto kern = agg_wmedian_fast_kernel<MPV>;                                                                   \
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);                   \
-    if (e != cudaSuccess) return e;                                                                             \
-    kern<<<grid, 128, fsmem, st>>>(mapP, a.n, a.M, wts, total, tau, margin ? a.wm_list : nullptr, a.wm_count,   \
-                                   a.wm_cap, a.raw);                                                            \
-    if (margin) agg_wmedian_list_kernel<MPV><<<sms * 4, 128, 0, st>>>(a.P, a.n, a.ld, a.M, a.weights64, a.wm_list, \
-                                                                     a.wm_count, a.wm_cap, a.raw);              \
-    break;                                                                                                      \
-  }
-            SE_WMF(1) SE_WMF(2) SE_WMF(4) SE_WMF(8) SE_WMF(16) SE_WMF(32) SE_WMF(64)
-#undef SE_WMF
-            default: return cudaErrorInvalidValue;
-          }
+          return with_mp(a.M, [&](auto mp) {
+            constexpr int MP = decltype(mp)::value;
+            const cudaError_t e = allow_dynamic_smem(agg_wmedian_fast_kernel<MP>, fsmem);
+            if (e != cudaSuccess) return e;
+            agg_wmedian_fast_kernel<MP><<<grid, 128, fsmem, st>>>(mapP, a.n, a.M, wts, total, tau,
+                                                                   margin ? a.wm_list : nullptr, a.wm_count, a.wm_cap,
+                                                                   a.raw);
+            if (margin)
+              agg_wmedian_list_kernel<MP><<<sms * 4, 128, 0, st>>>(a.P, a.n, a.ld, a.M, a.weights64, a.wm_list,
+                                                                    a.wm_count, a.wm_cap, a.raw);
+            return cudaGetLastError();
+          });
+        }
+        return with_mp(a.M, [&](auto mp) {
+          constexpr int MP = decltype(mp)::value;
+          const cudaError_t e = allow_dynamic_smem(agg_wmedian_reg_kernel<MP>, smem);
+          if (e != cudaSuccess) return e;
+          agg_wmedian_reg_kernel<MP><<<grid, 128, smem, st>>>(mapP, a.n, a.M, a.weights64, a.raw);
           return cudaGetLastError();
-        }
-        switch (Mp) {
-#define SE_WM(MPV)                                                                                              \
-  case MPV: {                                                                                                   \
-    auto kern = agg_wmedian_reg_kernel<MPV>;                                                                    \
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                    \
-    if (e != cudaSuccess) return e;                                                                             \
-    kern<<<grid, 128, smem, st>>>(mapP, a.n, a.M, a.weights64, a.raw);                                          \
-    break;                                                                                                      \
-  }
-          SE_WM(1) SE_WM(2) SE_WM(4) SE_WM(8) SE_WM(16) SE_WM(32) SE_WM(64)
-#undef SE_WM
-          default: return cudaErrorInvalidValue;
-        }
-        return cudaGetLastError();
+        });
       }
       const int T = 64;
       const size_t smem = (size_t)a.M * sizeof(double) + (size_t)Mp * T * sizeof(unsigned long long);
       if (smem > 200 * 1024) {  // M > 256: one warp per row
         const size_t wsmem = (size_t)a.M * sizeof(double) + (size_t)kWmWarps * Mp * sizeof(unsigned long long);
         if (wsmem > 200 * 1024) return cudaErrorInvalidValue;  // M > 8192
-        if (wsmem > 48 * 1024) {
-          cudaError_t e = cudaFuncSetAttribute(agg_wmedian_warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wsmem);
-          if (e != cudaSuccess) return e;
-        }
+        cudaError_t e = allow_dynamic_smem(agg_wmedian_warp_kernel, wsmem);
+        if (e != cudaSuccess) return e;
         int per_sm_w = (int)((220 * 1024) / (wsmem + 1024));
         if (per_sm_w < 1) per_sm_w = 1;
         if (per_sm_w > 16) per_sm_w = 16;
@@ -1375,10 +1315,8 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
         return cudaGetLastError();
       }
       auto kern = agg_wmedian_kernel<64>;
-      if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-      }
+      const cudaError_t e = allow_dynamic_smem(kern, smem);
+      if (e != cudaSuccess) return e;
       int per_sm = (int)((220 * 1024) / (smem + 1024));
       if (per_sm < 1) per_sm = 1;
       const int grid = grid_rows(a.n, T, per_sm, sms);
@@ -1405,10 +1343,8 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
       const bool weighted = (a.kind == SE_AGG_BOOSTING_DISCRETE);
       if (!weighted && a.M <= 255 && (size_t)((a.K + 3) / 4) * kVR * kBlock * 4 <= 160 * 1024) {
         const size_t psmem = (size_t)((a.K + 3) / 4) * kVR * kBlock * sizeof(uint32_t);
-        if (psmem > 48 * 1024) {
-          cudaError_t e = cudaFuncSetAttribute(agg_hard_votes_packed_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem);
-          if (e != cudaSuccess) return e;
-        }
+        const cudaError_t e = allow_dynamic_smem(agg_hard_votes_packed_kernel, psmem);
+        if (e != cudaSuccess) return e;
         f.C = a.K;
         const int gridp = grid_rows((a.n + kVR - 1) / kVR, kBlock, ctas_per_sm, sms);
         agg_hard_votes_packed_kernel<<<gridp, kBlock, psmem, st>>>(a.P, a.ld, a.M, f);
@@ -1423,10 +1359,8 @@ cudaError_t launch_agg(const AggArgs& a, int ctas_per_sm, int sms, cudaStream_t 
         return cudaGetLastError();
       }
       auto kern = weighted ? agg_votes_kernel<double> : agg_votes_kernel<float>;
-      if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-      }
+      const cudaError_t e = allow_dynamic_smem(kern, smem);
+      if (e != cudaSuccess) return e;
       kern<<<grid1, kBlock, smem, st>>>(a.P, a.ld, a.M, weighted ? a.weights : nullptr, f);
       return cudaGetLastError();  // epilogue fused: no separate finalize launch
     }
@@ -1456,42 +1390,27 @@ cudaError_t launch_forest_agg(const ForestAggArgs& g, int sms, cudaStream_t st) 
   int per_sm = (int)((220 * 1024) / (smem + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 16) per_sm = 16;
-  int64_t need = (a.n + kForestAggTile - 1) / kForestAggTile;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * per_sm;
-  const int grid = (int)(need < cap ? need : cap);
-#define SE_FA(MODE)                                                                                              \
-  {                                                                                                              \
-    auto kern = forest_agg_kernel<MODE>;                                                                         \
-    if (smem > 48 * 1024) {                                                                                      \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
-      if (e != cudaSuccess) return e;                                                                            \
-    }                                                                                                            \
-    kern<<<grid, kForestAggTile, smem, st>>>(g, f);                                                              \
-  }
+  const int grid = grid_rows(a.n, kForestAggTile, per_sm, sms);
+  auto launch = [&](auto kern) {
+    const cudaError_t e = allow_dynamic_smem(kern, smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, kForestAggTile, smem, st>>>(g, f);
+    return cudaGetLastError();
+  };
   switch (g.kind) {
-    case SE_AGG_GBM_CLASSIFIER: SE_FA(kFaTreeClass) break;
+    case SE_AGG_GBM_CLASSIFIER: return launch(forest_agg_kernel<kFaTreeClass>);
     case SE_AGG_BAGGING_HARD:
-    case SE_AGG_BOOSTING_DISCRETE: SE_FA(kFaVote) break;
-    case SE_AGG_BAGGING_SOFT: SE_FA(kFaSoft) break;
-    case SE_AGG_BOOSTING_REAL: SE_FA(kFaReal) break;
+    case SE_AGG_BOOSTING_DISCRETE: return launch(forest_agg_kernel<kFaVote>);
+    case SE_AGG_BAGGING_SOFT: return launch(forest_agg_kernel<kFaSoft>);
+    case SE_AGG_BOOSTING_REAL: return launch(forest_agg_kernel<kFaReal>);
     default: return cudaErrorInvalidValue;
   }
-#undef SE_FA
-  return cudaGetLastError();
 }
 
 cudaError_t forest_median_ctas_per_sm(int M, int* ctas) {
-  int Mp = 1;
-  while (Mp < M) Mp <<= 1;
   cudaFuncAttributes fa{};
-  cudaError_t e = cudaErrorInvalidValue;
-  switch (Mp) {
-#define SE_FM(MPV) case MPV: e = cudaFuncGetAttributes(&fa, forest_median_kernel<MPV>); break;
-    SE_FM(1) SE_FM(2) SE_FM(4) SE_FM(8) SE_FM(16) SE_FM(32) SE_FM(64)
-#undef SE_FM
-    default: break;
-  }
+  const cudaError_t e =
+      with_mp(M, [&](auto mp) { return cudaFuncGetAttributes(&fa, forest_median_kernel<decltype(mp)::value>); });
   if (e != cudaSuccess) return e;
   const int regs = (fa.numRegs + 7) / 8 * 8;  // allocated per thread in units of 8
   *ctas = regs > 0 ? 65536 / (regs * kForestMedianTile) : 16;
@@ -1505,28 +1424,14 @@ cudaError_t launch_forest_median(const ForestMedianArgs& g, size_t smem, int sms
   int per_sm = (int)((228 * 1024) / (smem + sizeof(double) * kForestMedianMaxTrees + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 16) per_sm = 16;
-  int64_t need = (g.n + kForestMedianTile - 1) / kForestMedianTile;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * per_sm;
-  const int grid = (int)(need < cap ? need : cap);
-  int Mp = 1;
-  while (Mp < g.M) Mp <<= 1;
-  switch (Mp) {
-#define SE_FM(MPV)                                                                                               \
-  case MPV: {                                                                                                    \
-    auto kern = forest_median_kernel<MPV>;                                                                       \
-    if (smem > 48 * 1024) {                                                                                      \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);       \
-      if (e != cudaSuccess) return e;                                                                            \
-    }                                                                                                            \
-    kern<<<grid, kForestMedianTile, smem, st>>>(g);                                                              \
-    break;                                                                                                       \
-  }
-    SE_FM(1) SE_FM(2) SE_FM(4) SE_FM(8) SE_FM(16) SE_FM(32) SE_FM(64)
-#undef SE_FM
-    default: return cudaErrorInvalidValue;
-  }
-  return cudaGetLastError();
+  const int grid = grid_rows(g.n, kForestMedianTile, per_sm, sms);
+  return with_mp(g.M, [&](auto mp) {
+    auto kern = forest_median_kernel<decltype(mp)::value>;
+    const cudaError_t e = allow_dynamic_smem(kern, smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, kForestMedianTile, smem, st>>>(g);
+    return cudaGetLastError();
+  });
 }
 
 }  // namespace se

@@ -246,6 +246,22 @@ int forest_bins(se_ctx* ctx, int which, const SlotBuf& X, int n_trees, const int
   return SE_OK;
 }
 
+// The prologue of the one-pass entry points: the X slot `which` names, checked against the forest, and its rank matrix
+// made to cover every threshold of the forest.  *X and *B point into the context.
+int forest_prepare(se_ctx* ctx, int which, int n_trees, const int32_t* offsets, const int32_t* feature,
+                   const float* threshold, const int32_t* left, const int32_t* right, const SlotBuf** X,
+                   const BinState** B) {
+  const SlotBuf& x = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
+  SE_REQUIRE(ctx, x.d, SE_ERR_STATE, "feature matrix slot not allocated");
+  SE_TRY(forest_check(ctx, x.rows, n_trees, offsets, feature, left, right));
+  SE_TRY(begin(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  SE_TRY(forest_bins(ctx, which, x, n_trees, offsets, feature, threshold));
+  *X = &x;
+  *B = &ctx->bins[which];
+  return SE_OK;
+}
+
 // Trees [t0, t1) run as one launch; cols are the global columns they use (local column c = cols[c]).
 struct ForestChunk {
   int t0 = 0, t1 = 0;
@@ -378,13 +394,11 @@ int se_forest_predict(se_ctx* ctx, int which, int n_trees, const int32_t* offset
                       const double* weights, double init, int out_slot, int out_row) {
   if (!ctx || !offsets || !feature || !threshold || !left || !right || !value) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= (1 << 20), SE_ERR_ARG, "bad tree count %d", n_trees);
-  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
-  SE_TRY(begin(ctx));
-  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
-  const BinState& B = ctx->bins[which];
+  const SlotBuf* xs;
+  const BinState* bs;
+  SE_TRY(forest_prepare(ctx, which, n_trees, offsets, feature, threshold, left, right, &xs, &bs));
+  const SlotBuf& X = *xs;
+  const BinState& B = *bs;
   std::vector<ForestChunk> chunks;
   SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, false, kForestTile, 0, chunks));
   ForestArgs a;
@@ -425,19 +439,17 @@ int se_forest_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, in
   }
   SE_REQUIRE(ctx, !vec || probs, SE_ERR_ARG, "bagging soft / boosting real need the leaf probabilities");
   SE_REQUIRE(ctx, kind != SE_AGG_BOOSTING_DISCRETE || weights, SE_ERR_ARG, "boosting discrete needs the weights");
-  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
+  const SlotBuf* xs;
+  const BinState* bs;
+  SE_TRY(forest_prepare(ctx, which, n_trees, offsets, feature, threshold, left, right, &xs, &bs));
+  const SlotBuf& X = *xs;
+  const BinState& B = *bs;
   const int C = gbm ? dim : num_classes;               // totals per row
   const int out_c = (gbm && dim == 1) ? 2 : C;         // classes of RAW / PROB
   const int64_t n = X.cols;
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_RAW, out_c, n));
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_PROB, out_c, n));
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_LABEL, 1, n));
-  SE_TRY(begin(ctx));
-  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
-  const BinState& B = ctx->bins[which];
   std::vector<ForestChunk> chunks;
   SE_TRY(forest_plan(ctx, X.rows, n_trees, offsets, feature, gbm, kForestAggTile,
                      (size_t)C * kForestAggTile * sizeof(double), chunks));
@@ -492,13 +504,11 @@ int se_forest_median(se_ctx* ctx, int which, int n_trees, const int32_t* offsets
   SE_REQUIRE(ctx, n_trees >= 1 && n_trees <= SE_FOREST_MEDIAN_MAX_TREES, SE_ERR_ARG,
              "se_forest_median serves 1..%d trees, got %d: evaluate the members with se_tree_predict + se_agg_run",
              SE_FOREST_MEDIAN_MAX_TREES, n_trees);
-  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
-  SE_REQUIRE(ctx, X.d, SE_ERR_STATE, "feature matrix slot not allocated");
-  SE_TRY(forest_check(ctx, X.rows, n_trees, offsets, feature, left, right));
-  SE_TRY(begin(ctx));
-  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  SE_TRY(forest_bins(ctx, which, X, n_trees, offsets, feature, threshold));
-  const BinState& B = ctx->bins[which];
+  const SlotBuf* xs;
+  const BinState* bs;
+  SE_TRY(forest_prepare(ctx, which, n_trees, offsets, feature, threshold, left, right, &xs, &bs));
+  const SlotBuf& X = *xs;
+  const BinState& B = *bs;
   const size_t vals_bytes = (size_t)n_trees * kForestMedianTile * sizeof(float);
   // chunks as large as the CTAs its registers let an SM hold can use: every chunk beyond the first re-stages its trees
   // for each tile, and the median's registers (up to 252 at 64 trees) cap the CTAs per SM below four already

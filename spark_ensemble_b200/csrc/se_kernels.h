@@ -278,6 +278,48 @@ __device__ __forceinline__ void forest_step(const uint2* __restrict__ nodes, con
   }
 }
 
+// Stages the ranks of rows [row0, row0 + TILE) of the chunk's C local columns into s_rank ([C][TILE] bytes, one row
+// per thread of a TILE-thread CTA); coloff(c) is the byte offset of local column c in X8.
+template <int TILE, class ColOff>
+__device__ __forceinline__ void forest_stage_ranks(unsigned char* s_rank, const uint8_t* X8, int64_t ld8, int C,
+                                                   int64_t row0, ColOff coloff) {
+  for (int i = threadIdx.x; i < C * (TILE / 4); i += TILE) {
+    const int c = i / (TILE / 4), q = i % (TILE / 4);
+    const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
+    uint32_t v = 0;
+    if (r < ld8) v = __ldg(reinterpret_cast<const uint32_t*>(X8 + coloff(c) + r));
+    *reinterpret_cast<uint32_t*>(s_rank + c * TILE + 4 * q) = v;
+  }
+}
+
+// Walks the chunk's T trees for the row whose ranks start at myr, two walks in flight, and calls visit(t, leaf) with
+// each tree's tree-local leaf in model order: t before t + 1, once both walks have ended.  The model order keeps the
+// fp64 totals of the one-pass kernels equal term for term to the member route's.
+template <int TILE, class Visit>
+__device__ __forceinline__ void forest_walk(const uint2* s_nodes, const int* s_toff, int T, const unsigned char* myr,
+                                            Visit visit) {
+  int t = 0;
+  for (; t + 1 < T; t += 2) {
+    const uint2* n0 = s_nodes + s_toff[t];
+    const uint2* n1 = s_nodes + s_toff[t + 1];
+    int d0 = 0, d1 = 0;
+    bool l0 = true, l1 = true;
+    while (l0 || l1) {
+      if (l0) forest_step<TILE>(n0, myr, d0, l0);
+      if (l1) forest_step<TILE>(n1, myr, d1, l1);
+    }
+    visit(t, d0);
+    visit(t + 1, d1);
+  }
+  if (t < T) {
+    const uint2* n0 = s_nodes + s_toff[t];
+    int d0 = 0;
+    bool l0 = true;
+    while (l0) forest_step<TILE>(n0, myr, d0, l0);
+    visit(t, d0);
+  }
+}
+
 // A classifier forest in ONE pass with the aggregation's epilogue (se_forest_agg, se_agg.cu): the chunk's trees are
 // staged as for forest_predict_kernel, each row's C class totals are fp64 in shared memory ([C][kForestAggTile] after
 // the ranks), carried between chunks in `acc` ([C][ld_acc] fp64) and finished by finalize_row / finalize_real_row.
@@ -385,6 +427,21 @@ cudaError_t launch_tree_fit_hist(const TreeFitArgs& a, int smem_mode, int grid_y
 cudaError_t launch_tree_fit_split(const TreeFitArgs& a, cudaStream_t s);
 cudaError_t launch_tree_fit_prune(const TreeFitArgs& a, cudaStream_t s);  // classification only
 cudaError_t launch_tree_fit_out(const TreeFitArgs& a, int sms, cudaStream_t s);  // tree 0 only
+
+// ---- launch arithmetic shared by the launchers ------------------------------------------------
+// CTAs for `items` work items, per_cta per CTA, at most ctas_per_sm per SM (at least one CTA)
+inline int grid_rows(int64_t items, int64_t per_cta, int ctas_per_sm, int sms) {
+  int64_t need = (items + per_cta - 1) / per_cta;
+  if (need < 1) need = 1;
+  const int64_t cap = (int64_t)ctas_per_sm * sms;
+  return (int)(need < cap ? need : cap);
+}
+// A kernel launched with more than 48 KB of dynamic shared memory has to opt in first (per device and kernel).
+template <class Kernel>
+cudaError_t allow_dynamic_smem(Kernel* kern, size_t smem) {
+  if (smem <= 48 * 1024) return cudaSuccess;
+  return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
 
 cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_coef,
                                   const float* coef, const int32_t* cols, float intercept,

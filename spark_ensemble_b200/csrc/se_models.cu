@@ -333,38 +333,14 @@ __global__ void __launch_bounds__(kForestTile) forest_predict_kernel(const Fores
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     __syncthreads();  // the packed trees are staged (first tile) / the previous tile's walks are over
     const int64_t row0 = tile * kForestTile;
-    for (int i = threadIdx.x; i < a.C * (kForestTile / 4); i += kForestTile) {
-      const int c = i / (kForestTile / 4), q = i % (kForestTile / 4);
-      const int64_t r = row0 + 4 * q;  // columns are padded to 128 rows: a word at r < ld8 stays inside its column
-      uint32_t v = 0;
-      if (r < a.ld8) v = __ldg(reinterpret_cast<const uint32_t*>(a.X8 + s_coloff[c] + r));
-      *reinterpret_cast<uint32_t*>(s_rank + c * kForestTile + 4 * q) = v;
-    }
+    forest_stage_ranks<kForestTile>(s_rank, a.X8, a.ld8, a.C, row0, [&](int c) { return s_coloff[c]; });
     __syncthreads();
     const int64_t row = row0 + threadIdx.x;
     if (row < a.n) {
       double acc = a.accumulate ? (double)a.out[row] : a.init;
-      const unsigned char* myr = s_rank + threadIdx.x;
-      int t = 0;
-      for (; t + 1 < a.T; t += 2) {  // two independent walks in flight
-        const uint2* n0 = s_nodes + s_toff[t];
-        const uint2* n1 = s_nodes + s_toff[t + 1];
-        int d0 = 0, d1 = 0;
-        bool l0 = true, l1 = true;
-        while (l0 || l1) {
-          if (l0) forest_step<kForestTile>(n0, myr, d0, l0);
-          if (l1) forest_step<kForestTile>(n1, myr, d1, l1);
-        }
-        acc += s_w[t] * (double)s_val[s_toff[t] + d0];  // model order (GBMRegressor.scala:534-537)
-        acc += s_w[t + 1] * (double)s_val[s_toff[t + 1] + d1];
-      }
-      if (t < a.T) {
-        const uint2* n0 = s_nodes + s_toff[t];
-        int d0 = 0;
-        bool l0 = true;
-        while (l0) forest_step<kForestTile>(n0, myr, d0, l0);
-        acc += s_w[t] * (double)s_val[s_toff[t] + d0];
-      }
+      forest_walk<kForestTile>(s_nodes, s_toff, a.T, s_rank + threadIdx.x, [&](int t, int leaf) {
+        acc += s_w[t] * (double)s_val[s_toff[t] + leaf];  // model order (GBMRegressor.scala:534-537)
+      });
       a.out[row] = (float)acc;
     }
   }
@@ -418,16 +394,9 @@ __global__ void __launch_bounds__(kBlock) linear_predict_kernel(const float* __r
 cudaError_t launch_tree_predict(const TreeArgs& a, int sms, cudaStream_t st) {
   const size_t smem = (size_t)a.n_nodes * 5 * sizeof(float);
   if (smem > 200 * 1024) return cudaErrorInvalidValue;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(tree_predict_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
-  const int64_t ngroups = (a.n + TV - 1) / TV;
-  int64_t need = (ngroups + kBlock - 1) / kBlock;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * 8;
-  tree_predict_kernel<<<(int)(need < cap ? need : cap), kBlock, smem, st>>>(a);
+  const cudaError_t e = allow_dynamic_smem(tree_predict_kernel, smem);
+  if (e != cudaSuccess) return e;
+  tree_predict_kernel<<<grid_rows((a.n + TV - 1) / TV, kBlock, 8, sms), kBlock, smem, st>>>(a);
   return cudaGetLastError();
 }
 
@@ -450,19 +419,14 @@ cudaError_t launch_tree_predict_binned(const TreeArgs& a, const uint8_t* X8, con
   // deeper ones walk the rank matrix level by level (tree_predict_binned_kernel)
   const bool all_nodes = mask_mode && n_internal <= 64 && a.n_nodes <= 256;
   const int64_t rows_per_thread = all_nodes ? 4 * RW : TV;
-  int64_t need = ((a.n + rows_per_thread - 1) / rows_per_thread + kBlock - 1) / kBlock;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * 16;
-  const int grid = (int)(need < cap ? need : cap);
+  const int grid = grid_rows((a.n + rows_per_thread - 1) / rows_per_thread, kBlock, 16, sms);
   if (all_nodes) {
     tree_predict_mask_kernel<<<grid, kBlock, 0, st>>>(a, X8, nodes);
     return cudaGetLastError();
   }
   auto kern = tree_predict_binned_kernel<1, 4>;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(kern, smem);
+  if (e != cudaSuccess) return e;
   kern<<<grid, kBlock, smem, st>>>(a, X8, nodes);
   return cudaGetLastError();
 }
@@ -470,28 +434,20 @@ cudaError_t launch_tree_predict_binned(const TreeArgs& a, const uint8_t* X8, con
 cudaError_t launch_forest_predict(const ForestArgs& a, int sms, cudaStream_t st) {
   const size_t smem = (size_t)a.off_ranks + (size_t)a.C * kForestTile;
   if (a.T < 1 || a.C < 0 || smem > 220 * 1024 || (a.blob_bytes & 15) != 0) return cudaErrorInvalidValue;
-  if (smem > 48 * 1024) {  // per device and per launch (a handful of launches per transform)
-    cudaError_t e = cudaFuncSetAttribute(forest_predict_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-  }
+  const cudaError_t e = allow_dynamic_smem(forest_predict_kernel, smem);  // a handful of launches per transform
+  if (e != cudaSuccess) return e;
   int per_sm = (int)((220 * 1024) / (smem + 1024));
   if (per_sm < 1) per_sm = 1;
   if (per_sm > 8) per_sm = 8;
-  int64_t need = (a.n + kForestTile - 1) / kForestTile;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * per_sm;
-  forest_predict_kernel<<<(int)(need < cap ? need : cap), kForestTile, smem, st>>>(a);
+  forest_predict_kernel<<<grid_rows(a.n, kForestTile, per_sm, sms), kForestTile, smem, st>>>(a);
   return cudaGetLastError();
 }
 
 cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_coef,
                                   const float* coef, const int32_t* cols, float intercept,
                                   float* out, int sms, cudaStream_t st) {
-  int64_t need = ((n >> 2) + kBlock - 1) / kBlock;
-  if (need < 1) need = 1;
-  const int64_t cap = (int64_t)sms * 8;
-  linear_predict_kernel<<<(int)(need < cap ? need : cap), kBlock, 0, st>>>(X, n, ld, n_coef, coef, cols,
-                                                                        intercept, out);
+  linear_predict_kernel<<<grid_rows(n >> 2, kBlock, 8, sms), kBlock, 0, st>>>(X, n, ld, n_coef, coef, cols, intercept,
+                                                                             out);
   return cudaGetLastError();
 }
 
