@@ -180,6 +180,9 @@ SE_API int se_download(se_ctx* ctx, int slot, float* host, int64_t count, int64_
 SE_API int se_download_scaled(se_ctx* ctx, int slot, double scale, float* host, int64_t count, int64_t offset);
 SE_API int se_fill(se_ctx* ctx, int slot, float value, int64_t count, int64_t offset);
 SE_API int se_copy_slot(se_ctx* ctx, int dst_slot, int src_slot);
+/* rows [src_row, src_row + count) of src_slot into rows [dst_row, ...) of dst_slot: both slots hold rows of the same
+ * length, the ranges lie inside them and do not overlap (SE_ERR_ARG otherwise) */
+SE_API int se_copy_rows(se_ctx* ctx, int dst_slot, int dst_row, int src_slot, int src_row, int count);
 /* deterministic counter-based synthetic fill (bench/tests): kind 0 uniform[a,b), 1 normal(a,b),
  * 2 integer uniform in [a,b) stored as float, 3 bernoulli(p=a) 0/1 */
 SE_API int se_fill_synthetic(se_ctx* ctx, int slot, int kind, uint64_t seed, double a, double b,
@@ -459,6 +462,17 @@ SE_API int se_forest_fit(se_ctx* ctx, int n_trees, const int32_t* sub_offsets, c
 /* linear model: out = intercept + Σ_j coef[j]·X[subspace[j]] */
 SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, float intercept,
                       const int32_t* subspace, int out_slot, int out_row);
+/* ---- weighted moment matrix of resident columns (DESIGN.md §3 "Device linear fit") ------------------------------- */
+/* For the p = n_cols columns cols[0 .. p) of src_slot (SE_SLOT_X or SE_SLOT_P, [cols][n]; any order, repeats allowed)
+ * and every row i: z = (x[cols[0]] − shift[0], ..., x[cols[p−1]] − shift[p−1], 1, y − label_shift), with y row
+ * label_row of label_slot, and c = w·bag, with w row weight_row of weight_slot (1 when weight_slot < 0) and bag
+ * SE_SLOT_BAG's multiplicity (1 unless use_bag).  Writes out[(p+2)·(p+2)], row-major and symmetric, = Σ_i c·z zᵀ in fp64:
+ * XᵀWX, XᵀWy, the weighted column sums, Σ c and yᵀWy of the shifted values (shift NULL: 0).  Every fp32 product is exact
+ * in fp64, every sum is fp64, and the per-CTA partials are folded in a fixed order: identical calls give identical bits.
+ * 0 <= p <= 254; a label, weight or bag row that does not exist, or a column outside the slot, fails with SE_ERR_ARG. */
+SE_API int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
+                             double label_shift, int label_slot, int label_row, int weight_slot, int weight_row,
+                             int use_bag, double* out);
 
 #ifdef __cplusplus
 }

@@ -57,6 +57,8 @@ TABLE = [
     ("slotFree", "se_slot_free", [("ctx", "ctx"), ("slot", "i32")], ""),
     ("fill", "se_fill", [("ctx", "ctx"), ("slot", "i32"), ("value", "f32"), ("count", "i64"), ("offset", "i64")], ""),
     ("copySlot", "se_copy_slot", [("ctx", "ctx"), ("dstSlot", "i32"), ("srcSlot", "i32")], ""),
+    ("copyRows", "se_copy_rows", [("ctx", "ctx"), ("dstSlot", "i32"), ("dstRow", "i32"), ("srcSlot", "i32"), ("srcRow", "i32"),
+                                  ("count", "i32")], ""),
     ("fillSynthetic", "se_fill_synthetic", [("ctx", "ctx"), ("slot", "i32"), ("kind", "i32"), ("seed", "u64"), ("a", "f64"),
                                             ("b", "f64"), ("count", "i64"), ("offset", "i64")], ""),
     ("quantile", "se_quantile", [("ctx", "ctx"), ("which", "i32"), ("slot", "i32"), ("count", "i64"), ("q", "f64"), ("out", "o_f64")],
@@ -122,6 +124,10 @@ TABLE = [
      "BoostingRegressionModel.predict (median) for 1..64 tree members: the weighted median in one pass, without member outputs"),
     ("linearPredict", "se_linear_predict", [("ctx", "ctx"), ("which", "i32"), ("nCoef", "i32"), ("coef", "in_f32"), ("intercept", "f32"),
                                             ("subspace", "in_i32"), ("outSlot", "i32"), ("outRow", "i32")], ""),
+    ("linearMoments", "se_linear_moments", [("ctx", "ctx"), ("srcSlot", "i32"), ("nCols", "i32"), ("cols", "in_i32"),
+                                            ("shift", "in_f64"), ("labelShift", "f64"), ("labelSlot", "i32"), ("labelRow", "i32"),
+                                            ("weightSlot", "i32"), ("weightRow", "i32"), ("useBag", "bool"), ("out", "out_f64")],
+     "fp64 (nCols+2)^2 moment matrix of (x_cols - shift, 1, y - labelShift), weighted, into out"),
 ]
 
 # hand-written natives (bulk transfers, handles, byte arrays): scala signature + which ABI functions they cover

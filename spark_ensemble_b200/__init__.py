@@ -5,8 +5,10 @@ pierrenodet/spark-ensemble behind the reference's Estimator/Model surface.
     _native.py       ctypes binding of the C ABI (no fallback: raises when the library/GPU is missing)
     context.py       one GPU == one row shard (thin wrapper over se_ctx)
     gbm_engine.py    host driver of a GBM fit on a shard
-    regression.py    GBMRegressor, GBMRegressionModel, BaggingRegressor(Model)
-    classification.py GBMClassifier(Model), BoostingClassifier(Model), BaggingClassifier(Model)
+    regression.py    GBMRegressor, GBMRegressionModel, BaggingRegressor(Model), BoostingRegressor(Model),
+                     StackingRegressor(Model)
+    classification.py GBMClassifier(Model), BoostingClassifier(Model), BaggingClassifier(Model),
+                     StackingClassifier(Model)
     ensemble.py      DataFrame stand-in, HasSubBag.subspace, row partitioner, Dummy init models
     learners.py      base learners (third party in the reference; scikit-learn stand-ins here)
 """

@@ -31,6 +31,7 @@ UPD_RESIDUAL, UPD_NEWTON, UPD_LOSS = 1, 2, 4
 R2_LOSS = {"exponential": 0, "linear": 1, "squared": 2}
 FOREST_AGG_MAX_CLASSES = 32  # SE_FOREST_AGG_MAX_CLASSES: se_forest_agg's class limit
 FOREST_MEDIAN_MAX_TREES = 64  # SE_FOREST_MEDIAN_MAX_TREES: se_forest_median's tree limit
+LINEAR_MOMENTS_MAX_COLS = 254  # se_linear_moments: p + 2 <= 256
 
 # enum se_kernel_family
 KERNEL_FAMILIES = ["sq_stats", "eval", "update", "resid", "mean_loss", "boost_real", "boost_err",
@@ -82,6 +83,7 @@ PROTOTYPES = {
     "se_download_scaled": [_vp, _i32, _d, _fp, _i64, _i64],
     "se_fill": [_vp, _i32, _f, _i64, _i64],
     "se_copy_slot": [_vp, _i32, _i32],
+    "se_copy_rows": [_vp, _i32, _i32, _i32, _i32, _i32],
     "se_fill_synthetic": [_vp, _i32, _i32, _u64, _d, _d, _i64, _i64],
     "se_slot_sum": [_vp, _i32, _i64, _dp],
     "se_quantile": [_vp, _i32, _i32, _i64, _d, _dp],
@@ -118,6 +120,7 @@ PROTOTYPES = {
     "se_forest_agg": [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _fp, _ip, _dp, _dp],
     "se_forest_median": [_vp, _i32, _i32, _ip, _ip, _fp, _ip, _ip, _fp, _dp, _i32, _i32],
     "se_linear_predict": [_vp, _i32, _i32, _fp, _f, _ip, _i32, _i32],
+    "se_linear_moments": [_vp, _i32, _i32, _ip, _dp, _d, _i32, _i32, _i32, _i32, _i32, _dp],
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,
                     _ip, _fp, _ip, _ip, _fp, _dp, C.POINTER(_i32)],

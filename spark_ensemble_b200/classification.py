@@ -16,8 +16,8 @@ from .ensemble import DataFrame, fit_dummy_classifier, java_string_hash
 from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_classifier_params, shared_predictor_params, subbag_params)
-from .routes import (bagging_fit, device_fit, device_trees, extract_instances, load_boosting, member_route, one_pass,
-                     split_validation)
+from .routes import (STACK_METHODS, bagging_fit, device_fit, device_trees, extract_instances, load_boosting,
+                     member_route, one_pass, split_validation, stacking_fit, stacking_predict, tree_list)
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -78,6 +78,23 @@ class _ClassifierModelBase(Params):
             return None
         return one_pass(self.device, X, trees, lambda ctx, t: ctx.forest_agg(kind, self.numClasses, t, **kw),
                         self._fetch)
+
+    def _forest_agg_args(self):  # -> (kind, the members in forest order, keyword arguments of forest_agg)
+        raise NotImplementedError
+
+    def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
+        """A stacking member's meta-features over ctx's SLOT_X, on the device, when every member is a tree: one
+        se_forest_agg pass, then its probability (proba), raw (raw) or label rows are copied into out_slot from
+        out_row on.  False when the forest is outside se_forest_agg's reach."""
+        kind, members, kw = self._forest_agg_args()
+        trees = tree_list(members) if members else None
+        if trees is None or self.numClasses > N.FOREST_AGG_MAX_CLASSES:
+            return False
+        ctx.forest_agg(kind, self.numClasses, trees, **kw)
+        src, count = {"proba": (N.SLOT_PROB, self._out_classes), "raw": (N.SLOT_RAW, self._out_classes)}.get(
+            method, (N.SLOT_LABEL, 1))
+        ctx.copy_rows(out_slot, out_row, src, 0, count)
+        return True
 
 
 # ================================================================================ GBMClassifier
@@ -166,13 +183,17 @@ class GBMClassificationModel(_ClassifierModelBase):
         self.parent = None
         self._out_classes = 2 if (self.dim == 1 and self.numClasses == 2) else self.dim
 
-    def _raw_prob_label(self, X):
-        n, M, dim = X.shape[0], self.numModels, self.dim
-        out = self._forest_agg_resident(
-            X, N.AGG_GBM_CLASSIFIER, device_trees(self, [m for ms in self.models for m in ms]),
+    def _forest_agg_args(self):
+        M, dim = self.numModels, self.dim
+        return N.AGG_GBM_CLASSIFIER, [m for ms in self.models for m in ms], dict(
             weights=np.concatenate([np.asarray(wt, dtype=np.float64).reshape(dim) for wt in self.weights]) if M else None,
             init=self.init, tree_class=np.tile(np.arange(dim, dtype=np.int32), M), dim=dim, loss=self("loss").lower(),
             subspaces=[s for s in self.subspaces[:M] for _ in range(dim)])
+
+    def _raw_prob_label(self, X):
+        n, M, dim = X.shape[0], self.numModels, self.dim
+        kind, members, kw = self._forest_agg_args()
+        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
         if out is not None:
             return out
         P = np.zeros((max(M, 1), dim, n), dtype=np.float32)
@@ -282,11 +303,16 @@ class BoostingClassificationModel(_ClassifierModelBase):
         self.parent = None
         self._out_classes = self.numClasses
 
+    def _forest_agg_args(self):
+        real = self("algorithm").lower() == "real"
+        kind = N.AGG_BOOSTING_REAL if real else N.AGG_BOOSTING_DISCRETE
+        return kind, self.models, dict(weights=None if real else self.weights)
+
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         real = self("algorithm").lower() == "real"
-        kind = N.AGG_BOOSTING_REAL if real else N.AGG_BOOSTING_DISCRETE
-        out = self._forest_agg_resident(X, kind, device_trees(self, self.models), weights=None if real else self.weights)
+        kind, members, kw = self._forest_agg_args()
+        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
         if out is not None:
             return out
         if real:
@@ -349,11 +375,16 @@ class BaggingClassificationModel(_ClassifierModelBase):
         self.parent = None
         self._out_classes = self.numClasses
 
+    def _forest_agg_args(self):
+        soft = self("votingStrategy").lower() == "soft"
+        kind = N.AGG_BAGGING_SOFT if soft else N.AGG_BAGGING_HARD
+        return kind, self.models, dict(subspaces=self.subspaces)
+
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         soft = self("votingStrategy").lower() == "soft"
-        kind = N.AGG_BAGGING_SOFT if soft else N.AGG_BAGGING_HARD
-        out = self._forest_agg_resident(X, kind, device_trees(self, self.models), subspaces=self.subspaces)
+        kind, members, kw = self._forest_agg_args()
+        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
         if out is not None:
             return out
         P = np.zeros((M, K, n) if soft else (M, n), dtype=np.float32)
@@ -364,3 +395,73 @@ class BaggingClassificationModel(_ClassifierModelBase):
 
 
 BaggingClassificationModel._declare(_p + _pc + _ps + _pbagc, _BAG_CLS_DEFAULTS)
+
+
+# ================================================================================ StackingClassifier
+class StackingClassifier(Params):
+    """classification/StackingClassifier.scala: every base learner fits on the dataset, its outputs become the
+    meta-features of each row (stackMethod: the members' labels, raw vectors or probabilities, member-major) and the
+    stacker fits on them.  residentFeatures keeps X and the meta-features on the device (routes.stacking_fit)."""
+
+    def __init__(self, uid: str | None = None, device: int = 0):
+        super().__init__(uid or random_uid("StackingClassifier"))
+        self.device = device
+
+    def copy(self, extra=None):
+        c = super().copy(extra)
+        if c.isDefined("baseLearners"):
+            c.set("baseLearners", [m.copy(extra) for m in c("baseLearners")])
+        if c.isDefined("stacker"):
+            c.set("stacker", c("stacker").copy(extra))
+        return c
+
+    def fit(self, dataset: DataFrame) -> "StackingClassificationModel":
+        y = np.asarray(dataset[self("labelCol")], dtype=np.float64)
+        K = _num_classes(y)
+        _validate_labels(y, K)
+        models, stack, widths = stacking_fit(self, dataset, num_classes=K)
+        m = StackingClassificationModel(models, stack, K, widths, device=self.device)
+        self._copyValues(m)
+        m.parent = self
+        return m
+
+
+_pstack = [Param("baseLearners", "base learners that will be used by the ensemble learner", convert=list),
+           Param("stacker", "stacker that will be used by the ensemble learner to aggregate results of base learner(s)"),
+           Param("parallelism", "the number of threads to use when running parallel algorithms (>= 1)",
+                 ParamValidators.gtEq(1), int),
+           RESIDENT_FEATURES]
+_pstackc = [Param("stackMethod", "stackMethod, (case-insensitive). Supported options:" + ",".join(STACK_METHODS),
+                  lambda v: v.lower() in STACK_METHODS, str)]
+_STACK_CLS_DEFAULTS = {**_d, **_dc, "parallelism": 1, "residentFeatures": False, "stackMethod": "class"}
+StackingClassifier._declare(_p + _pc + _pstack + _pstackc, _STACK_CLS_DEFAULTS)
+
+
+class StackingClassificationModel(Params):
+    """classification/StackingClassifier.scala StackingClassificationModel: predict = stack.predict(the members'
+    meta-features); transform writes the prediction column only (PredictionModel)."""
+
+    def __init__(self, models, stack, numClasses, widths, uid=None, device: int = 0):
+        super().__init__(uid or random_uid("StackingClassificationModel"))
+        self.models, self.stack = list(models), stack
+        self.numClasses = int(numClasses)
+        self.widths = [int(k) for k in widths]
+        self.device = device
+        self.parent = None
+
+    def copy(self, extra=None):
+        c = super().copy(extra)
+        c.parent = self.parent
+        return c
+
+    def _predict(self, X) -> np.ndarray:
+        return stacking_predict(self, X)
+
+    def transform(self, dataset: DataFrame) -> DataFrame:
+        return dataset.withColumn(self("predictionCol"), self._predict(np.asarray(dataset[self("featuresCol")])))
+
+    def predict(self, features) -> float:
+        return float(self._predict(np.asarray(features).reshape(1, -1))[0])
+
+
+StackingClassificationModel._declare(_p + _pc + _pstack + _pstackc, _STACK_CLS_DEFAULTS)

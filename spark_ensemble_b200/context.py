@@ -215,6 +215,10 @@ class Context:
     def copy_slot(self, dst: int, src: int):
         self._ck(self._lib.se_copy_slot(self._h, dst, src))
 
+    def copy_rows(self, dst: int, dst_row: int, src: int, src_row: int = 0, count: int = 1):
+        """Rows src_row .. src_row + count - 1 of slot src into rows dst_row .. of slot dst (se_copy_rows)."""
+        self._ck(self._lib.se_copy_rows(self._h, int(dst), int(dst_row), int(src), int(src_row), int(count)))
+
     def slot_sum(self, slot: int, count: int | None = None) -> float:
         if count is None:
             _, count, _ = self.layout(slot)
@@ -453,6 +457,23 @@ class Context:
         sub = None if subspace is None else np.ascontiguousarray(subspace, dtype=np.int32)
         self._ck(self._lib.se_linear_predict(self._h, int(validation), c.size, N.fptr(c), float(intercept),
                                              None if sub is None else N.iptr(sub), out_slot, out_row))
+
+    def linear_moments(self, src_slot: int, cols, label_slot: int, label_row: int = 0, weight_slot: int = -1,
+                       weight_row: int = 0, use_bag: bool = False, shift=None, label_shift: float = 0.0) -> np.ndarray:
+        """The fp64 (p+2)×(p+2) matrix Σ_rows c·w·z zᵀ with z = (x[cols] − shift, 1, y − label_shift) over columns
+        `cols` of src_slot (SLOT_X or SLOT_P), labels row label_row of label_slot, weights row weight_row of weight_slot
+        (none when < 0) and the bag of SLOT_BAG when use_bag (se_linear_moments)."""
+        c = np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+        s = None if shift is None else np.ascontiguousarray(shift, dtype=np.float64).reshape(-1)
+        if s is not None and s.size != c.size:
+            raise ValueError("one shift per column")
+        m = c.size + 2
+        out = np.zeros((m, m)) if c.size <= N.LINEAR_MOMENTS_MAX_COLS else np.zeros(1)
+        self._ck(self._lib.se_linear_moments(self._h, int(src_slot), c.size, N.iptr(c) if c.size else None,
+                                             None if s is None else N.dptr(s), float(label_shift), int(label_slot),
+                                             int(label_row), int(weight_slot), int(weight_row), int(bool(use_bag)),
+                                             N.dptr(out)))
+        return out
 
     # ---- regression-tree fit on the device
     def tree_fit_bins(self, candidates):

@@ -227,6 +227,28 @@ int se_copy_slot(se_ctx* ctx, int dst_slot, int src_slot) {
   return SE_OK;
 }
 
+int se_copy_rows(se_ctx* ctx, int dst_slot, int dst_row, int src_slot, int src_row, int count) {
+  if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");
+  SE_REQUIRE(ctx, dst_slot >= 0 && dst_slot < SE_NUM_SLOTS && src_slot >= 0 && src_slot < SE_NUM_SLOTS,
+             SE_ERR_ARG, "bad slot");
+  const SlotBuf &d = ctx->slot[dst_slot], &s = ctx->slot[src_slot];
+  SE_REQUIRE(ctx, d.d && s.d && d.cols == s.cols, SE_ERR_STATE, "slots %d and %d do not hold rows of the same length",
+             dst_slot, src_slot);
+  SE_REQUIRE(ctx, count >= 0 && src_row >= 0 && dst_row >= 0 && (int64_t)src_row + count <= s.rows &&
+             (int64_t)dst_row + count <= d.rows, SE_ERR_ARG, "rows %d..%d of slot %d into rows %d.. of slot %d: out of range",
+             src_row, src_row + count - 1, src_slot, dst_row, dst_slot);
+  SE_REQUIRE(ctx, dst_slot != src_slot || count == 0 || src_row + count <= dst_row || dst_row + count <= src_row,
+             SE_ERR_ARG, "overlapping rows");
+  if (count == 0 || s.cols == 0) return SE_OK;
+  SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  SE_TRY(read_slot(ctx, src_slot));
+  SE_TRY(write_slot(ctx, dst_slot));
+  SE_CUDA(ctx, cudaMemcpy2DAsync(d.d + (int64_t)dst_row * d.ld, sizeof(float) * (size_t)d.ld, s.d + (int64_t)src_row * s.ld,
+                                 sizeof(float) * (size_t)s.ld, sizeof(float) * (size_t)s.cols, (size_t)count,
+                                 cudaMemcpyDeviceToDevice, ctx->stream));
+  return SE_OK;
+}
+
 int se_fill_synthetic(se_ctx* ctx, int slot, int kind, uint64_t seed, double a, double b, int64_t count,
                       int64_t offset) {
   if (!ctx) return fail(nullptr, SE_ERR_ARG, "null context");

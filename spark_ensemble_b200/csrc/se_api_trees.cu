@@ -587,3 +587,65 @@ int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* coef, flo
                                                        ctx->stream));
   return end(ctx);
 }
+
+int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
+                      double label_shift, int label_slot, int label_row, int weight_slot, int weight_row, int use_bag,
+                      double* out) {
+  if (!ctx || !out || (n_cols > 0 && !cols)) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, src_slot == SE_SLOT_X || src_slot == SE_SLOT_P, SE_ERR_ARG,
+             "source slot %d: only SE_SLOT_X or SE_SLOT_P", src_slot);
+  SE_REQUIRE(ctx, n_cols >= 0 && n_cols <= kLinearMomentsMaxCols, SE_ERR_ARG, "%d columns (0..%d supported)", n_cols,
+             kLinearMomentsMaxCols);
+  const SlotBuf& X = ctx->slot[src_slot];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "source slot %d not allocated", src_slot);
+  const int64_t n = X.cols;
+  for (int k = 0; k < n_cols; ++k)
+    SE_REQUIRE(ctx, cols[k] >= 0 && cols[k] < X.rows, SE_ERR_ARG, "column list entry %d: column %d outside slot %d "
+               "with %lld columns", k, cols[k], src_slot, (long long)X.rows);
+  auto row_of = [&](int slot, int row, const char* what, const float** p) -> int {
+    SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad %s slot %d", what, slot);
+    const SlotBuf& s = ctx->slot[slot];
+    SE_REQUIRE(ctx, s.d && s.cols == n && row >= 0 && row < s.rows, SE_ERR_ARG, "%s slot %d: no row %d of %lld values",
+               what, slot, row, (long long)n);
+    *p = s.d + (int64_t)row * s.ld;
+    return SE_OK;
+  };
+  LinearMomentsArgs a;
+  SE_TRY(row_of(label_slot, label_row, "label", &a.y));
+  if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &a.w));
+  if (use_bag) SE_TRY(row_of(SE_SLOT_BAG, 0, "bag", &a.bag));
+  SE_TRY(begin(ctx));
+  SE_TRY(read_slot(ctx, src_slot));
+  SE_TRY(read_slot(ctx, label_slot));
+  SE_TRY(read_slot(ctx, weight_slot));
+  const int m = n_cols + 2;
+  size_t n_part = 0;
+  int n_cnt = 0;
+  linear_moments_scratch(n_cols, n, ctx->sms, &n_part, &n_cnt);
+  auto& L = ctx->lm;
+  SE_CUDA(ctx, L.d_part.grow(n_part));
+  SE_CUDA(ctx, L.d_cnt.grow((size_t)n_cnt));
+  SE_CUDA(ctx, L.d_out.grow((size_t)m * m));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_small is reused below
+  int32_t* hcol = reinterpret_cast<int32_t*>(ctx->h_small.get());
+  double* hs = reinterpret_cast<double*>(ctx->h_small.get() + 1024);  // 254 columns fit below it
+  for (int k = 0; k < n_cols; ++k) {
+    hcol[k] = cols[k];
+    hs[k] = shift ? shift[k] : 0.0;
+  }
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, 1024 + sizeof(double) * (size_t)n_cols, cudaMemcpyHostToDevice,
+                               ctx->stream));
+  SE_CUDA(ctx, cudaMemsetAsync(L.d_cnt, 0, sizeof(unsigned int) * (size_t)n_cnt, ctx->stream));
+  a.X = X.d; a.ld = X.ld; a.n = n; a.p = n_cols;
+  a.cols = reinterpret_cast<const int32_t*>(ctx->d_small.get());
+  a.shift = reinterpret_cast<const double*>(ctx->d_small.get() + 1024);
+  a.y_shift = label_shift;
+  a.partials = L.d_part; a.counters = L.d_cnt; a.out = L.d_out;
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_linear_moments(a, ctx->sms, ctx->stream));
+  double* hout = reinterpret_cast<double*>(ctx->h_small.get());
+  SE_CUDA(ctx, cudaMemcpyAsync(hout, L.d_out, sizeof(double) * (size_t)m * m, cudaMemcpyDeviceToHost, ctx->stream));
+  SE_TRY(end(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  memcpy(out, hout, sizeof(double) * (size_t)m * m);
+  return SE_OK;
+}

@@ -300,6 +300,11 @@ struct se_ctx {
     se_host::DevBuf<float> d_prob;    // [trees][kTreeFitHeap][kTreeFitMaxClasses]
     se_host::DevBuf<int4> d_prn;      // [trees][kTreeFitHeap]
   } tf;
+  struct {  // se_linear_moments: CTA partials, tile tickets and the matrix, kept across calls
+    se_host::DevBuf<double> d_part;
+    se_host::DevBuf<unsigned int> d_cnt;
+    se_host::DevBuf<double> d_out;
+  } lm;
   std::string err;
   // stopwatch + per-kernel-family timing
   se_host::Event tm0, tm1;

@@ -447,6 +447,26 @@ cudaError_t launch_linear_predict(const float* X, int64_t n, int64_t ld, int n_c
                                   const float* coef, const int32_t* cols, float intercept,
                                   float* out, int sms, cudaStream_t s);
 
+// ---- weighted moment matrix of resident columns (se_linear_fit.cu) -----------------------------
+constexpr int kLinearMomentsMaxCols = 254;  // p + 2 <= 256
+struct LinearMomentsArgs {
+  const float* X = nullptr;          // [cols][ld] source slot
+  int64_t ld = 0, n = 0;
+  int p = 0;
+  const int32_t* cols = nullptr;     // device [p]
+  const double* shift = nullptr;     // device [p]
+  double y_shift = 0.0;
+  const float* y = nullptr;          // label row
+  const float* w = nullptr;          // weight row or nullptr (1)
+  const float* bag = nullptr;        // multiplicities or nullptr (1)
+  double* partials = nullptr;        // linear_moments_scratch's doubles
+  unsigned int* counters = nullptr;  // linear_moments_scratch's tickets, zero before the launch
+  double* out = nullptr;             // [p + 2][p + 2], row-major, both triangles
+};
+// the scratch one launch over n rows needs: fp64 partials and ticket counters
+void linear_moments_scratch(int p, int64_t n, int sms, size_t* partials, int* counters);
+cudaError_t launch_linear_moments(const LinearMomentsArgs& a, int sms, cudaStream_t s);
+
 // ---- exact quantile by radix select (se_util.cu) ---------------------------------------------
 // One pass: histogram (256 bins, fp64 counts in `hist`) of byte `shift/8` of the order-preserving key of each
 // value whose higher bytes equal `prefix` (mask = bits above the byte).  value = a[i], or |a[i] - b[i]| when b.

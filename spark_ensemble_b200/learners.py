@@ -288,6 +288,18 @@ class DecisionTreeClassificationModel(_Model):
     def predict(self, X) -> np.ndarray:
         return np.argmax(self.predictProbability(X), axis=1).astype(np.float64)
 
+    def node_raw(self) -> np.ndarray:
+        """[n_nodes, numClasses] weighted class counts of every node: Spark's rawPrediction of a leaf."""
+        t = self.sk.tree_
+        v = t.value[:, 0, :].astype(np.float64)
+        v = v / np.maximum(v.sum(axis=1, keepdims=True), 1e-300) * t.weighted_n_node_samples[:, None]
+        full = np.zeros((v.shape[0], self.numClasses))
+        full[:, self.sk.classes_.astype(int)] = v
+        return full
+
+    def predictRaw(self, X) -> np.ndarray:
+        return self.node_raw()[self.sk.apply(np.asarray(X, dtype=np.float32))]
+
     def tree_arrays(self):
         """Array form with per-node class-probability vectors ("values" [n_nodes, K]) and the predicted label
         ("value" [n_nodes]) so both predictProbability and predict can be evaluated on device."""
@@ -339,6 +351,13 @@ class DeviceDecisionTreeClassificationModel(_DeviceTreeModel):
 
     def predictProbability(self, X) -> np.ndarray:
         return self._arrays["values"][self._leaf(X)].astype(np.float64)
+
+    def node_raw(self) -> np.ndarray:
+        """[n_nodes, numClasses] class weights of every node: Spark's rawPrediction of a leaf."""
+        return self.class_weights
+
+    def predictRaw(self, X) -> np.ndarray:
+        return self.class_weights[self._leaf(X)]
 
 
 class DeviceDecisionTreeClassifier(_DeviceTreeLearner):
@@ -426,6 +445,89 @@ class LinearRegressionModel(_Model):
 
     def linear_arrays(self):
         return {"coef": self.coefficients.astype(np.float32), "intercept": np.float32(self.intercept)}
+
+
+def solve_linear_moments(M, shift, label_shift: float, reg_param: float = 0.0):
+    """(coefficients, intercept) minimising Σ w·(y − xβ − b)² + α‖β‖², α = max(reg_param, 1e-12), b unpenalised, from the
+    moment matrix M of se_linear_moments (z = (x − shift, 1, y − label_shift)): the centred normal equations in fp64,
+    by Cholesky, or by a least-squares solve when they are singular to working precision (collinear columns)."""
+    from scipy.linalg import LinAlgError, cho_factor, cho_solve
+    M = np.asarray(M, dtype=np.float64)
+    p = M.shape[0] - 2
+    sw = M[p, p]
+    if not sw > 0:
+        raise ValueError("the linear fit needs a positive total weight")
+    sx, sy = M[:p, p], M[p + 1, p]
+    A = M[:p, :p] - np.outer(sx, sx) / sw
+    b = M[:p, p + 1] - sx * (sy / sw)
+    A[np.diag_indices(p)] += max(float(reg_param), 1e-12)
+    try:
+        beta = cho_solve(cho_factor(A, lower=True, check_finite=True), b) if p else np.zeros(0)
+    except LinAlgError:
+        beta = np.linalg.lstsq(A, b, rcond=None)[0]
+    shift = np.zeros(p) if shift is None else np.asarray(shift, dtype=np.float64)
+    intercept = (label_shift + sy / sw) - float((shift + sx / sw) @ beta)
+    return beta, intercept
+
+
+class DeviceLinearRegression:
+    """org.apache.spark.ml.regression.LinearRegression fitted on the GPU, with the objective of the host stand-in
+    LinearRegression:
+
+        minimise Σ w·(y − xβ − b)² + α‖β‖², with α = max(regParam, 1e-12) and b unpenalised
+
+    which, with the default regParam = 0, is Spark's default (least squares with an intercept) on full-rank data.  One
+    pass over the resident columns forms the fp64 moment matrix of (x − s, 1, y − s_y) (se_linear_moments); the host
+    solves its (p+1)-sized centred normal equations (solve_linear_moments).  Its model is LinearRegressionModel, scored
+    on the device by se_linear_predict.  It is not a resident learner of the GBM, Bagging or Boosting loops: they call
+    its `fit`, which opens a context on `device`."""
+
+    def __init__(self, regParam: float = 0.0, device: int = 0):
+        self.regParam, self.device = float(regParam), int(device)
+        if self.regParam < 0:
+            raise ValueError(f"regParam must be >= 0, got {self.regParam}")
+
+    def copy(self, extra=None):
+        return DeviceLinearRegression(self.regParam, self.device)
+
+    def fit_resident(self, ctx, src_slot: int, cols, label_slot: int, label_row: int, weight_slot: int,
+                     weight_row: int, use_bag: bool, out_slot: int | None, out_row: int = 0,
+                     shift=None) -> LinearRegressionModel:
+        """Fit over columns `cols` of src_slot in ctx: one se_linear_moments call, then the host solve.  The shifts
+        default to the values of row 0 (a few downloads), which keeps the centring well away from cancellation.  With
+        out_slot, every row's prediction goes to its row out_row (src_slot must then be SLOT_X)."""
+        cols = np.asarray(cols, dtype=np.int32).reshape(-1)
+        n = ctx.layout(src_slot)[1]
+        if shift is None:
+            shift = np.array([ctx.download(src_slot, count=1, offset=int(c) * n)[0] for c in cols], dtype=np.float64)
+        label_shift = float(ctx.download(label_slot, count=1, offset=int(label_row) * n)[0])
+        M = ctx.linear_moments(src_slot, cols, label_slot, label_row, weight_slot, weight_row, use_bag, shift,
+                               label_shift)
+        coef, intercept = solve_linear_moments(M, shift, label_shift, self.regParam)
+        model = LinearRegressionModel(coef, intercept)
+        if out_slot is not None:
+            if src_slot != N.SLOT_X:
+                raise ValueError("predictions are written from SLOT_X only")
+            a = model.linear_arrays()
+            ctx.linear_predict(a["coef"], float(a["intercept"]), out_slot, out_row, subspace=cols)
+        return model
+
+    def fit(self, X, y, w=None) -> LinearRegressionModel:
+        X = np.asarray(X, dtype=np.float32)
+        n, d = X.shape
+        if n == 0:
+            raise ValueError("DeviceLinearRegression.fit needs at least one row")
+        with Context(self.device) as ctx:
+            ctx.alloc(N.SLOT_X, d, n)
+            ctx.upload_rowmajor(N.SLOT_X, X)
+            ctx.alloc(N.SLOT_Y, n)
+            ctx.upload(N.SLOT_Y, np.asarray(y, dtype=np.float32))
+            if w is not None:
+                ctx.alloc(N.SLOT_W, n)
+                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
+            return self.fit_resident(ctx, N.SLOT_X, np.arange(d, dtype=np.int32), N.SLOT_Y, 0,
+                                     N.SLOT_W if w is not None else -1, 0, False, None,
+                                     shift=X.mean(axis=0, dtype=np.float64))
 
 
 class LinearRegression:

@@ -16,7 +16,8 @@ from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_predictor_params, subbag_params)
 from .routes import (bagging_fit, device_fit, device_trees, download_raw, extract_instances, forest_sum, load_boosting,
-                     member_route, one_pass, resident_context, split_validation, stack_outputs)
+                     member_route, one_pass, resident_context, split_validation, stack_outputs, stacking_fit,
+                     stacking_predict, tree_list)
 
 _REG_LOSSES = ("squared", "absolute", "huber", "quantile")  # GBMRegressor.scala:119-120
 _REG_INIT = ("constant", "zero", "base")                     # :121-123
@@ -112,12 +113,27 @@ class GBMRegressionModel(Params):
         self.device = device
         self.parent = None
 
-    def _aggregate(self, X) -> np.ndarray:
+    def _forest(self):  # -> (members, subspaces, weights, init) of the one-pass sum
         const_init = hasattr(self.init, "prediction")  # else a tree init scores as one more member of weight 1
         members = self.models if const_init else [self.init] + self.models
         subs = list(self.subspaces) if const_init else [None] + list(self.subspaces)
         a = self.weights if const_init else np.concatenate([[1.0], self.weights])
         init = self.init.prediction if const_init else 0.0
+        return members, subs, a, init
+
+    def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
+        """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
+        (a stacking member's meta-feature)."""
+        members, subs, a, init = self._forest()
+        trees = tree_list(members) if members else None
+        if trees is None:
+            return False
+        ctx.forest_predict(trees, out_slot, weights=a, init=init, out_row=out_row, subspaces=subs)
+        return True
+
+    def _aggregate(self, X) -> np.ndarray:
+        const_init = hasattr(self.init, "prediction")
+        members, subs, a, init = self._forest()
         out = forest_sum(self.device, X, device_trees(self, members), subs, a, init)
         if out is not None:
             return out
@@ -173,6 +189,16 @@ class BaggingRegressionModel(Params):
         self.numModels = len(self.models)
         self.device = device
         self.parent = None
+
+    def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
+        """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
+        (a stacking member's meta-feature): Σ_t tree_t(x) / M as weights 1/M."""
+        trees = tree_list(self.models) if self.models else None
+        if trees is None:
+            return False
+        ctx.forest_predict(trees, out_slot, weights=np.full(len(trees), 1.0 / len(trees)), out_row=out_row,
+                           subspaces=self.subspaces)
+        return True
 
     def _aggregate(self, X) -> np.ndarray:
         s = forest_sum(self.device, X, device_trees(self, self.models), self.subspaces, None, 0.0)
@@ -267,6 +293,20 @@ class BoostingRegressionModel(Params):
         self.device = device
         self.parent = None
 
+    def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
+        """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
+        (a stacking member's meta-feature): the weighted median of at most 64 trees, or the weighted mean."""
+        trees = tree_list(self.models) if self.models else None
+        if trees is None:
+            return False
+        if self("votingStrategy").lower() == "median":
+            if len(trees) > N.FOREST_MEDIAN_MAX_TREES:
+                return False
+            ctx.forest_median(trees, out_slot, self.weights, out_row=out_row)
+        else:
+            ctx.forest_predict(trees, out_slot, weights=self.weights / float(np.sum(self.weights)), out_row=out_row)
+        return True
+
     def _aggregate_resident(self, X, median: bool) -> np.ndarray | None:
         """Members evaluated over the device-resident features when every one is a tree: the weighted mean in one
         forest pass, and the median of at most 64 trees too (se_forest_median).  Above 64 trees, or when the rank
@@ -309,3 +349,66 @@ class BoostingRegressionModel(Params):
 
 
 BoostingRegressionModel._declare(_p + _pb + _pbr, _BOOST_REG_DEFAULTS)
+
+
+# ---- Stacking ------------------------------------------------------------------------------------------------------
+class StackingRegressor(Params):
+    """regression/StackingRegressor.scala: every base learner fits on the dataset, its predictions become the
+    meta-features of each row and the stacker fits on them.  residentFeatures keeps X and the meta-features on the
+    device (routes.stacking_fit)."""
+
+    def __init__(self, uid: str | None = None, device: int = 0):
+        super().__init__(uid or random_uid("StackingRegressor"))
+        self.device = device
+
+    def copy(self, extra=None):
+        c = super().copy(extra)
+        if c.isDefined("baseLearners"):
+            c.set("baseLearners", [m.copy(extra) for m in c("baseLearners")])
+        if c.isDefined("stacker"):
+            c.set("stacker", c("stacker").copy(extra))
+        return c
+
+    def fit(self, dataset: DataFrame) -> "StackingRegressionModel":
+        models, stack, widths = stacking_fit(self, dataset)
+        m = StackingRegressionModel(models, stack, device=self.device)
+        self._copyValues(m)
+        m.parent = self
+        return m
+
+
+_pstack = [Param("baseLearners", "base learners that will be used by the ensemble learner", convert=list),
+           Param("stacker", "stacker that will be used by the ensemble learner to aggregate results of base learner(s)"),
+           Param("parallelism", "the number of threads to use when running parallel algorithms (>= 1)",
+                 ParamValidators.gtEq(1), int),
+           RESIDENT_FEATURES]
+_STACK_REG_DEFAULTS = {**_d, "parallelism": 1, "residentFeatures": False}
+StackingRegressor._declare(_p + _pstack, _STACK_REG_DEFAULTS)
+
+
+class StackingRegressionModel(Params):
+    """regression/StackingRegressor.scala StackingRegressionModel: predict = stack.predict(every member's prediction)."""
+
+    def __init__(self, models, stack, uid: str | None = None, device: int = 0):
+        super().__init__(uid or random_uid("StackingRegressionModel"))
+        self.models, self.stack = list(models), stack
+        self.widths = [1] * len(self.models)
+        self.device = device
+        self.parent = None
+
+    def copy(self, extra=None):
+        c = super().copy(extra)
+        c.parent = self.parent
+        return c
+
+    def _aggregate(self, X) -> np.ndarray:
+        return stacking_predict(self, X)
+
+    def transform(self, dataset: DataFrame) -> DataFrame:
+        return dataset.withColumn(self("predictionCol"), self._aggregate(np.asarray(dataset[self("featuresCol")])))
+
+    def predict(self, features) -> float:
+        return float(self._aggregate(np.asarray(features).reshape(1, -1))[0])
+
+
+StackingRegressionModel._declare(_p + _pstack, _STACK_REG_DEFAULTS)

@@ -10,6 +10,8 @@ Each decision lives here once, so the estimators that make it differently make t
 """
 from __future__ import annotations
 
+import inspect
+
 import numpy as np
 
 from . import _native as N
@@ -226,3 +228,240 @@ def member_route(device: int, kind: int, P, num_classes: int = 0, dim: int = 1, 
             ctx.upload(N.SLOT_P, P)
         ctx.agg_run(weights, init)
         return fetch(ctx)
+
+
+# ---- Stacking ----------------------------------------------------------------------------------------------------------
+STACK_METHODS = ("class", "raw", "proba")  # classification/StackingClassifier.scala supportedStackMethod
+
+
+def is_classifier(member) -> bool:
+    """A classification estimator mirror (it has rawPredictionCol) or a learner whose fit takes num_classes."""
+    if isinstance(member, Params):
+        return member.hasParam("rawPredictionCol")
+    return "num_classes" in inspect.signature(member.fit).parameters
+
+
+def takes_weights(member) -> bool:
+    """HasWeightCol: an estimator mirror with weightCol, or a learner whose fit takes w."""
+    if isinstance(member, Params):
+        return member.hasParam("weightCol")
+    return "w" in inspect.signature(member.fit).parameters
+
+
+def member_width(member, method: str, num_classes: int | None) -> int:
+    """Meta-features a member contributes (the reference's models.flatMap): its K probabilities (proba) or its K-wide
+    raw vector (raw) for a classifier, else its one prediction."""
+    if num_classes is not None and method in ("raw", "proba") and is_classifier(member):
+        return int(num_classes)
+    return 1
+
+
+def fit_member(est: Params, member, dataset: DataFrame, X, y, w, num_classes: int | None, weight_col: str = ""):
+    """fitBaseLearner: an estimator mirror fits on the frame with the stacking estimator's label, features and
+    prediction columns (and weight_col when w is given); a learner fits on (X, y, w)."""
+    if isinstance(member, Params):
+        m = member.copy()
+        for name in ("labelCol", "featuresCol", "predictionCol"):
+            m.set(name, est(name))
+        if w is not None:
+            m.set("weightCol", weight_col)
+        return m.fit(dataset)
+    kw = {"num_classes": num_classes} if (num_classes is not None and is_classifier(member)) else {}
+    return member.fit(X, y, w, **kw) if takes_weights(member) else member.fit(X, y, **kw)
+
+
+def model_outputs(model, X, method: str, width: int) -> np.ndarray:
+    """[width][n] fp64 meta-features of one member model on the host."""
+    if hasattr(model, "_raw_prob_label"):  # a classification estimator model
+        raw, prob, label = model._raw_prob_label(X)
+        out = prob.T if (width > 1 and method == "proba") else raw.T if width > 1 else label[None]
+    elif hasattr(model, "_aggregate"):  # a regression estimator model
+        out = model._aggregate(X)[None]
+    elif width > 1 and method == "proba":
+        out = model.predictProbability(X).T
+    elif width > 1:
+        out = model.predictRaw(X).T
+    else:
+        out = np.asarray(model.predict(X))[None]
+    out = np.asarray(out, dtype=np.float64)
+    if out.shape[0] != width:
+        raise ValueError(f"{type(model).__name__} gives {out.shape[0]} meta-features where {width} are expected")
+    return out
+
+
+def model_predict(model, F) -> np.ndarray:
+    """The stack's predict over meta-features F [n, W]."""
+    return model_outputs(model, F, "class", 1)[0]
+
+
+def write_member_rows(ctx: Context, model, method: str, row: int, width: int) -> bool:
+    """A fitted member's meta-features into rows row .. row + width - 1 of SLOT_P over the context's SLOT_X, on the
+    device: single trees (se_tree_predict / se_tree_predict_multi), linear models (se_linear_predict) and the estimator
+    models of trees (their write_rows).  False when the model has no device form, or when its thresholds do not fit
+    the rank matrix (SE_ERR_STATE): the caller predicts it on the host then."""
+    try:
+        t = model.tree_arrays() if hasattr(model, "tree_arrays") else None
+        if t is not None:
+            if width == 1:
+                ctx.tree_predict(t, N.SLOT_P, row)
+                return True
+            vals = t["values"] if method == "proba" else model.node_raw()
+            ctx.alloc(N.SLOT_PROBA, width, ctx.layout(N.SLOT_P)[1])
+            ctx.tree_predict_multi({**t, "values": np.asarray(vals, dtype=np.float32)}, N.SLOT_PROBA)
+            ctx.copy_rows(N.SLOT_P, row, N.SLOT_PROBA, 0, width)
+            return True
+        lin = model.linear_arrays() if hasattr(model, "linear_arrays") else None
+        if lin is not None:
+            ctx.linear_predict(lin["coef"], float(lin["intercept"]), N.SLOT_P, row)
+            return True
+        write = getattr(model, "write_rows", None)
+        return bool(write is not None and write(ctx, method, N.SLOT_P, row))
+    except N.NativeError as e:
+        if e.code == N.SE_ERR_STATE:
+            return False
+        raise
+
+
+def tree_list(members) -> list | None:
+    """The tree arrays of every member, or None when one of them is not a tree."""
+    trees = []
+    for m in members:
+        t = m.tree_arrays() if hasattr(m, "tree_arrays") else None
+        if t is None:
+            return None
+        trees.append(t)
+    return trees
+
+
+def _stacker_fit_device(ctx: Context, stacker, n: int, W: int, weighted: bool, num_classes: int | None):
+    """The stacker fitted over the meta-features in the context's SLOT_X; None for a stacker without a device fit."""
+    from .learners import DeviceLinearRegression
+    cols = np.arange(W, dtype=np.int32)
+    wslot = N.SLOT_W if weighted else -1
+    if isinstance(stacker, DeviceLinearRegression):
+        return stacker.fit_resident(ctx, N.SLOT_X, cols, N.SLOT_Y, 0, wslot, 0, False, None)
+    if not getattr(stacker, "device_learner", False):
+        return None
+    # candidates from the meta-features of the sampled rows, as stacker.fit over the downloaded matrix draws them
+    ctx.tree_fit_bins(stacker.split_candidates(ctx.download(N.SLOT_X).reshape(W, n).T))
+    ctx.alloc(N.SLOT_RAW, 1, n)
+    if num_classes is None:
+        return stacker.fit_resident(ctx, N.SLOT_Y, 0, wslot, 0, False, cols, N.SLOT_RAW, 0)
+    return stacker.fit_resident(ctx, int(num_classes), N.SLOT_Y, 0, wslot, 0, False, cols, N.SLOT_RAW, 0)
+
+
+def stacking_fit(est: Params, dataset: DataFrame, num_classes: int | None = None):
+    """(member models, stack, widths) of a Stacking fit.  Members get the weights only when every member takes them; the
+    stacker always gets them (or ones).  Host route (residentFeatures=False): the reference's data flow.  Device route:
+    one context holds X (uploaded once), the labels and weights; device learners fit in it and write their outputs into
+    their rows of SLOT_P, other members are fitted on their own and scored into their rows on the device when they have
+    a device form (on the host otherwise); the meta-features then become SLOT_X and a device stacker fits over them."""
+    X, y, w = extract_instances(est, dataset)
+    X = np.asarray(X, dtype=np.float32)
+    n, d = X.shape
+    members = list(est("baseLearners"))
+    stacker = est("stacker")
+    method = est("stackMethod").lower() if est.hasParam("stackMethod") else "class"
+    mw = w if (w is not None and all(takes_weights(m) for m in members)) else None
+    wc = mw is not None and est("weightCol")
+    sw = np.ones(n) if w is None else w
+    widths = [member_width(m, method, num_classes) for m in members]
+    if not est("residentFeatures"):
+        models = [fit_member(est, m, dataset, X, y, mw, num_classes, wc) for m in members]
+        meta = np.concatenate([model_outputs(mod, X, method, k) for mod, k in zip(models, widths)])
+        return models, _fit_stacker_host(est, stacker, meta.T, y, sw, num_classes), widths
+    from .learners import DeviceLinearRegression
+    W = sum(widths)
+    models = []
+    with resident_context(est.device, X) as ctx:
+        ctx.alloc(N.SLOT_Y, n)
+        ctx.upload(N.SLOT_Y, y)
+        if w is not None:
+            ctx.alloc(N.SLOT_W, n)
+            ctx.upload(N.SLOT_W, w)
+        ctx.alloc(N.SLOT_P, W, n)
+        all_cols = np.arange(d, dtype=np.int32)
+        mslot = N.SLOT_W if mw is not None else -1
+        row = 0
+        for m, k in zip(members, widths):
+            if isinstance(m, DeviceLinearRegression):
+                model = m.fit_resident(ctx, N.SLOT_X, all_cols, N.SLOT_Y, 0, mslot, 0, False, N.SLOT_P, row)
+            elif getattr(m, "device_learner", False):
+                ctx.tree_fit_bins(m.split_candidates(X))
+                if not is_classifier(m):
+                    model = m.fit_resident(ctx, N.SLOT_Y, 0, mslot, 0, False, all_cols, N.SLOT_P, row)
+                else:
+                    check_class_labels(y, int(num_classes), n)
+                    model = m.fit_resident(ctx, int(num_classes), N.SLOT_Y, 0, mslot, 0, False, all_cols, N.SLOT_P,
+                                           row, proba=(k > 1))
+                    if k > 1 and method == "raw" and not write_member_rows(ctx, model, method, row, k):
+                        ctx.upload(N.SLOT_P, model_outputs(model, X, method, k), offset=row * n)
+            else:
+                model = fit_member(est, m, dataset, X, y, mw, num_classes, wc)
+                if not write_member_rows(ctx, model, method, row, k):
+                    ctx.upload(N.SLOT_P, model_outputs(model, X, method, k), offset=row * n)
+            models.append(model)
+            row += k
+        ctx.alloc(N.SLOT_X, W, n)
+        ctx.copy_slot(N.SLOT_X, N.SLOT_P)
+        stack = _stacker_fit_device(ctx, stacker, n, W, w is not None, num_classes)
+        if stack is None:
+            meta = ctx.download(N.SLOT_P).reshape(W, n).T.astype(np.float64)
+    if stack is None:
+        stack = _fit_stacker_host(est, stacker, meta, y, sw, num_classes)
+    return models, stack, widths
+
+
+def _fit_stacker_host(est: Params, stacker, F, y, w, num_classes: int | None):
+    """The stacker fitted on the host over meta-features F [n, W] with weights w: an estimator mirror on a frame of
+    the label, the meta-features and the weights under the stacking estimator's column names (weightCol, or "weight"
+    when it is unset), a learner on (F, y, w)."""
+    wc = (est("weightCol") if est.isDefined("weightCol") else "") or "weight"
+    frame = DataFrame(**{est("labelCol"): y, est("featuresCol"): F, wc: w})
+    return fit_member(est, stacker, frame, F, y, w, num_classes, wc)
+
+
+def stacking_predict(model: Params, X) -> np.ndarray:
+    """stack.predict(meta-features) of every row of X.  Host route: each member's outputs on the host.  Device route
+    (residentFeatures): X is uploaded once; members with a device form write their rows of SLOT_P on the device, the
+    others are predicted on the host and uploaded; the meta-features become SLOT_X and a tree or linear stack scores
+    them there."""
+    X = np.asarray(X, dtype=np.float32)
+    n = X.shape[0]
+    method = model("stackMethod").lower() if model.hasParam("stackMethod") else "class"
+    if not model("residentFeatures"):
+        meta = np.concatenate([model_outputs(m, X, method, k) for m, k in zip(model.models, model.widths)])
+        return model_predict(model.stack, meta.T)
+    W = sum(model.widths)
+    with resident_context(model.device, X) as ctx:
+        ctx.alloc(N.SLOT_P, W, n)
+        row = 0
+        for m, k in zip(model.models, model.widths):
+            if not write_member_rows(ctx, m, method, row, k):
+                ctx.upload(N.SLOT_P, model_outputs(m, X, method, k), offset=row * n)
+            row += k
+        ctx.alloc(N.SLOT_X, W, n)
+        ctx.copy_slot(N.SLOT_X, N.SLOT_P)
+        ctx.alloc(N.SLOT_RAW, 1, n)
+        if write_stack_rows(ctx, model.stack, N.SLOT_RAW):
+            return download_raw(ctx)
+        meta = ctx.download(N.SLOT_P).reshape(W, n).T.astype(np.float64)
+    return model_predict(model.stack, meta)
+
+
+def write_stack_rows(ctx: Context, stack, out_slot: int) -> bool:
+    """The stack's prediction (a tree's value or label, or a linear model) of every row of SLOT_X into out_slot."""
+    try:
+        t = stack.tree_arrays() if hasattr(stack, "tree_arrays") else None
+        if t is not None:
+            ctx.tree_predict(t, out_slot, 0)
+            return True
+    except N.NativeError as e:
+        if e.code == N.SE_ERR_STATE:
+            return False
+        raise
+    lin = stack.linear_arrays() if hasattr(stack, "linear_arrays") else None
+    if lin is not None:
+        ctx.linear_predict(lin["coef"], float(lin["intercept"]), out_slot, 0)
+        return True
+    return False
