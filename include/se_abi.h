@@ -473,6 +473,36 @@ SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* co
 SE_API int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
                              double label_shift, int label_slot, int label_row, int weight_slot, int weight_row,
                              int use_bag, double* out);
+/* ---- logistic regression over resident columns (DESIGN.md §3 "Device logistic fit") ------------------------------- */
+/* The columns, labels and weights of the three calls below: the p = n_cols columns cols[0 .. p) of src_slot
+ * (SE_SLOT_X or SE_SLOT_P, [cols][n]; any order, repeats allowed; 0 <= p <= 254), y row label_row of label_slot and
+ * c row weight_row of weight_slot (1 when weight_slot < 0).  Every sum is fp64 and the per-CTA partials are folded in a
+ * fixed order: identical calls give identical bits.  A label, weight or column that does not exist fails with
+ * SE_ERR_ARG. */
+/* One pass of the statistics a fit needs, with s = shift (NULL: 0) and 1 <= num_classes = K <= 64: writes
+ * out[3 + 2p + K] = Σc, Σc², Σc·(x_j − s_j) for every j, Σc·(x_j − s_j)² for every j, Σc·[y = k] for every k, and the
+ * number of rows whose label is not an integer in [0, K), whose weight is negative or not finite, or one of whose p
+ * features is not finite. */
+SE_API int se_logistic_stats(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
+                             int num_classes, int label_slot, int label_row, int weight_slot, int weight_row,
+                             double* out);
+/* The loss and gradient of one optimiser evaluation.  n_sets = D is 1 (binomial: the margin of class 1) or the class
+ * count 2..64 (multinomial); coef is [D][p + 1], the intercept last.  With z_j = (x_j − shift_j)·scale_j (shift NULL:
+ * 0, scale NULL: 1), z_p = 1 and m_k = Σ_j coef[k][j]·z_j, the loss of a row is log1pExp(m) − [y = 1]·m (binomial) or
+ * logsumexp(m) − m_y (multinomial), and out[1 + D(p + 1)] = Σ c·ℓ followed by Σ c·(π_k − [y = k])·z_j at
+ * 1 + k(p + 1) + j, π the sigmoid or the softmax.  Labels are compared with class indices, never used as addresses:
+ * se_logistic_stats is where a bad label is found. */
+SE_API int se_logistic_loss_grad(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
+                                 const double* scale, int n_sets, const double* coef, int label_slot, int label_row,
+                                 int weight_slot, int weight_row, double* out);
+/* Scores a logistic model over SE_SLOT_X: coef [n_sets][n_coef] in raw space over columns subspace[j] (NULL: j),
+ * intercept [n_sets], m_k = Σ_j coef[k][j]·x_j + intercept[k] in fp64.  Writes, for each slot >= 0: raw (2 rows
+ * (−m, m) when n_sets == 1, else the n_sets margins), probability (1 − σ(m), σ(m), or the softmax; a margin of +inf
+ * gives 1 to every +inf class and 0 to the others) and label (σ(m) > threshold, or the first argmax of the margins),
+ * each from its row on. */
+SE_API int se_logistic_predict(se_ctx* ctx, int n_coef, const int32_t* subspace, int n_sets, const double* coef,
+                               const double* intercept, double threshold, int raw_slot, int raw_row, int prob_slot,
+                               int prob_row, int label_slot, int label_row);
 
 #ifdef __cplusplus
 }

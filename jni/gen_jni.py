@@ -128,6 +128,20 @@ TABLE = [
                                             ("shift", "in_f64"), ("labelShift", "f64"), ("labelSlot", "i32"), ("labelRow", "i32"),
                                             ("weightSlot", "i32"), ("weightRow", "i32"), ("useBag", "bool"), ("out", "out_f64")],
      "fp64 (nCols+2)^2 moment matrix of (x_cols - shift, 1, y - labelShift), weighted, into out"),
+    ("logisticStats", "se_logistic_stats", [("ctx", "ctx"), ("srcSlot", "i32"), ("nCols", "i32"), ("cols", "in_i32"),
+                                            ("shift", "in_f64"), ("numClasses", "i32"), ("labelSlot", "i32"), ("labelRow", "i32"),
+                                            ("weightSlot", "i32"), ("weightRow", "i32"), ("out", "out_f64")],
+     "fp64 weight totals, column sums, class histogram and invalid-row count of a logistic fit, into out"),
+    ("logisticLossGrad", "se_logistic_loss_grad", [("ctx", "ctx"), ("srcSlot", "i32"), ("nCols", "i32"), ("cols", "in_i32"),
+                                                   ("shift", "in_f64"), ("scale", "in_f64"), ("nSets", "i32"), ("coef", "in_f64"),
+                                                   ("labelSlot", "i32"), ("labelRow", "i32"), ("weightSlot", "i32"),
+                                                   ("weightRow", "i32"), ("out", "out_f64")],
+     "fp64 logistic loss and gradient at coef [nSets][nCols+1], into out"),
+    ("logisticPredict", "se_logistic_predict", [("ctx", "ctx"), ("nCoef", "i32"), ("subspace", "in_i32"), ("nSets", "i32"),
+                                                ("coef", "in_f64"), ("intercept", "in_f64"), ("threshold", "f64"),
+                                                ("rawSlot", "i32"), ("rawRow", "i32"), ("probSlot", "i32"), ("probRow", "i32"),
+                                                ("labelSlot", "i32"), ("labelRow", "i32")],
+     "LogisticRegressionModel raw / probability / prediction over the resident feature matrix"),
 ]
 
 # hand-written natives (bulk transfers, handles, byte arrays): scala signature + which ABI functions they cover

@@ -475,6 +475,62 @@ class Context:
                                              N.dptr(out)))
         return out
 
+    def logistic_stats(self, src_slot: int, cols, num_classes: int, label_slot: int, label_row: int = 0,
+                       weight_slot: int = -1, weight_row: int = 0, shift=None) -> np.ndarray:
+        """One pass over columns `cols` of src_slot: fp64 [Σc, Σc², Σc(x−shift) per column, Σc(x−shift)² per column,
+        Σc[y=k] per class, invalid rows] (se_logistic_stats)."""
+        c = np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+        s = None if shift is None else np.ascontiguousarray(shift, dtype=np.float64).reshape(-1)
+        if s is not None and s.size != c.size:
+            raise ValueError("one shift per column")
+        out = np.zeros(3 + 2 * c.size + max(int(num_classes), 0))
+        self._ck(self._lib.se_logistic_stats(self._h, int(src_slot), c.size, N.iptr(c) if c.size else None,
+                                             None if s is None else N.dptr(s), int(num_classes), int(label_slot),
+                                             int(label_row), int(weight_slot), int(weight_row), N.dptr(out)))
+        return out
+
+    def logistic_loss_grad(self, src_slot: int, cols, coef, label_slot: int, label_row: int = 0, weight_slot: int = -1,
+                           weight_row: int = 0, shift=None, scale=None):
+        """(Σ c·ℓ, gradient [D][p+1]) of the logistic loss at coef [D][p+1] (intercept last) over z = (x[cols] −
+        shift)·scale (se_logistic_loss_grad): D = 1 binomial, else multinomial over D classes."""
+        c = np.ascontiguousarray(cols, dtype=np.int32).reshape(-1)
+        p = c.size
+        th = np.ascontiguousarray(coef, dtype=np.float64)
+        D = th.size // (p + 1) if th.ndim == 1 else th.shape[0]
+        if th.size != D * (p + 1):
+            raise ValueError(f"coef must be [D][{p + 1}]")
+        th = th.reshape(-1)
+        vec = []
+        for v in (shift, scale):
+            v = None if v is None else np.ascontiguousarray(v, dtype=np.float64).reshape(-1)
+            if v is not None and v.size != p:
+                raise ValueError("one shift and one scale per column")
+            vec.append(v)
+        out = np.zeros(1 + D * (p + 1))
+        self._ck(self._lib.se_logistic_loss_grad(self._h, int(src_slot), p, N.iptr(c) if p else None,
+                                                 None if vec[0] is None else N.dptr(vec[0]),
+                                                 None if vec[1] is None else N.dptr(vec[1]), int(D), N.dptr(th),
+                                                 int(label_slot), int(label_row), int(weight_slot), int(weight_row),
+                                                 N.dptr(out)))
+        return float(out[0]), out[1:].reshape(D, p + 1)
+
+    def logistic_predict(self, coef, intercept, threshold: float = 0.5, raw=None, prob=None, label=None,
+                         subspace=None):
+        """A logistic model scored over SLOT_X (se_logistic_predict): coef [D][p] raw space, intercept [D].  raw, prob
+        and label are (slot, row) pairs or None: raw and prob take 2 rows (D = 1) or D rows, label one."""
+        th = np.ascontiguousarray(np.atleast_2d(coef), dtype=np.float64)
+        b = np.ascontiguousarray(np.atleast_1d(intercept), dtype=np.float64)
+        D, p = th.shape
+        if b.size != D:
+            raise ValueError("one intercept per coefficient set")
+        sub = None if subspace is None else np.ascontiguousarray(subspace, dtype=np.int32)
+        if sub is not None and sub.size != p:
+            raise ValueError("one column per coefficient")
+        (rs, rr), (ps, pr), (ls, lr) = (o if o is not None else (-1, 0) for o in (raw, prob, label))
+        self._ck(self._lib.se_logistic_predict(self._h, p, None if sub is None else N.iptr(sub), D,
+                                               N.dptr(th.reshape(-1)), N.dptr(b), float(threshold), int(rs), int(rr),
+                                               int(ps), int(pr), int(ls), int(lr)))
+
     # ---- regression-tree fit on the device
     def tree_fit_bins(self, candidates):
         """Split candidates of a fit, one sorted fp32 list per column of SLOT_X (se_tree_fit_bins)."""

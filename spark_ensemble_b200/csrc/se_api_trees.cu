@@ -649,3 +649,148 @@ int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols
   memcpy(out, hout, sizeof(double) * (size_t)m * m);
   return SE_OK;
 }
+
+namespace {
+// The inputs se_logistic_stats and se_logistic_loss_grad share: the columns of src_slot, the label row and the weight
+// row (none when weight_slot < 0), checked; the column list goes to d_small.
+int logistic_inputs(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, int label_slot, int label_row,
+                    int weight_slot, int weight_row, LogisticArgs* a) {
+  if (!ctx || (n_cols > 0 && !cols)) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, src_slot == SE_SLOT_X || src_slot == SE_SLOT_P, SE_ERR_ARG,
+             "source slot %d: only SE_SLOT_X or SE_SLOT_P", src_slot);
+  SE_REQUIRE(ctx, n_cols >= 0 && n_cols <= kLogisticMaxCols, SE_ERR_ARG, "%d columns (0..%d supported)", n_cols,
+             kLogisticMaxCols);
+  const SlotBuf& X = ctx->slot[src_slot];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "source slot %d not allocated", src_slot);
+  const int64_t n = X.cols;
+  for (int k = 0; k < n_cols; ++k)
+    SE_REQUIRE(ctx, cols[k] >= 0 && cols[k] < X.rows, SE_ERR_ARG, "column list entry %d: column %d outside slot %d "
+               "with %lld columns", k, cols[k], src_slot, (long long)X.rows);
+  auto row_of = [&](int slot, int row, const char* what, const float** p) -> int {
+    SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad %s slot %d", what, slot);
+    const SlotBuf& s = ctx->slot[slot];
+    SE_REQUIRE(ctx, s.d && s.cols == n && row >= 0 && row < s.rows, SE_ERR_ARG, "%s slot %d: no row %d of %lld values",
+               what, slot, row, (long long)n);
+    *p = s.d + (int64_t)row * s.ld;
+    return SE_OK;
+  };
+  SE_TRY(row_of(label_slot, label_row, "label", &a->y));
+  if (weight_slot >= 0) SE_TRY(row_of(weight_slot, weight_row, "weight", &a->w));
+  SE_TRY(begin(ctx));
+  SE_TRY(read_slot(ctx, src_slot));
+  SE_TRY(read_slot(ctx, label_slot));
+  SE_TRY(read_slot(ctx, weight_slot));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_small is reused below
+  memcpy(ctx->h_small.get(), cols, sizeof(int32_t) * (size_t)n_cols);
+  a->X = X.d; a->ld = X.ld; a->n = n; a->p = n_cols;
+  a->cols = reinterpret_cast<const int32_t*>(ctx->d_small.get());
+  return SE_OK;
+}
+
+// Launches `launch` over scratch of the sizes `scratch` asks for, after uploading `doubles` values from h_small + 1024,
+// and copies `len` results into out.
+template <class Scratch, class Launch>
+int logistic_run(se_ctx* ctx, LogisticArgs& a, size_t doubles, int len, Scratch scratch, Launch launch, double* out) {
+  size_t n_part = 0;
+  int n_cnt = 0;
+  scratch(&n_part, &n_cnt);
+  auto& L = ctx->lg;
+  SE_CUDA(ctx, L.d_part.grow(n_part));
+  SE_CUDA(ctx, L.d_cnt.grow((size_t)n_cnt));
+  SE_CUDA(ctx, L.d_out.grow((size_t)len));
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, 1024 + sizeof(double) * doubles, cudaMemcpyHostToDevice,
+                               ctx->stream));
+  SE_CUDA(ctx, cudaMemsetAsync(L.d_cnt, 0, sizeof(unsigned int) * (size_t)n_cnt, ctx->stream));
+  a.partials = L.d_part; a.counters = L.d_cnt; a.out = L.d_out;
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch());
+  double* hout = reinterpret_cast<double*>(ctx->h_small.get());
+  SE_CUDA(ctx, cudaMemcpyAsync(hout, L.d_out, sizeof(double) * (size_t)len, cudaMemcpyDeviceToHost, ctx->stream));
+  SE_TRY(end(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  memcpy(out, hout, sizeof(double) * (size_t)len);
+  return SE_OK;
+}
+}  // namespace
+
+int se_logistic_stats(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift, int num_classes,
+                      int label_slot, int label_row, int weight_slot, int weight_row, double* out) {
+  if (!ctx || !out) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, num_classes >= 1 && num_classes <= kLogisticMaxClasses, SE_ERR_ARG, "%d classes (1..%d supported)",
+             num_classes, kLogisticMaxClasses);
+  LogisticArgs a;
+  SE_TRY(logistic_inputs(ctx, src_slot, n_cols, cols, label_slot, label_row, weight_slot, weight_row, &a));
+  double* hs = reinterpret_cast<double*>(ctx->h_small.get() + 1024);
+  for (int k = 0; k < n_cols; ++k) hs[k] = shift ? shift[k] : 0.0;
+  a.shift = reinterpret_cast<const double*>(ctx->d_small.get() + 1024);
+  a.D = num_classes;
+  const int64_t n = a.n;
+  return logistic_run(
+      ctx, a, (size_t)n_cols, 3 + 2 * n_cols + num_classes,
+      [&](size_t* part, int* cnt) { logistic_stats_scratch(n_cols, num_classes, n, ctx->sms, part, cnt); },
+      [&]() { return launch_logistic_stats(a, ctx->sms, ctx->stream); }, out);
+}
+
+int se_logistic_loss_grad(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
+                          const double* scale, int n_sets, const double* coef, int label_slot, int label_row,
+                          int weight_slot, int weight_row, double* out) {
+  if (!ctx || !out || !coef) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_sets >= 1 && n_sets <= kLogisticMaxClasses, SE_ERR_ARG,
+             "%d coefficient sets (1: binomial, 2..%d: multinomial)", n_sets, kLogisticMaxClasses);
+  LogisticArgs a;
+  SE_TRY(logistic_inputs(ctx, src_slot, n_cols, cols, label_slot, label_row, weight_slot, weight_row, &a));
+  const int P1 = n_cols + 1;
+  double* hs = reinterpret_cast<double*>(ctx->h_small.get() + 1024);
+  for (int k = 0; k < n_cols; ++k) {
+    hs[k] = shift ? shift[k] : 0.0;
+    hs[n_cols + k] = scale ? scale[k] : 1.0;
+  }
+  memcpy(hs + 2 * n_cols, coef, sizeof(double) * (size_t)n_sets * P1);
+  const double* ds = reinterpret_cast<const double*>(ctx->d_small.get() + 1024);
+  a.shift = ds;
+  a.scale = ds + n_cols;
+  a.coef = ds + 2 * n_cols;
+  a.D = n_sets;
+  const int64_t n = a.n;
+  return logistic_run(
+      ctx, a, (size_t)2 * n_cols + (size_t)n_sets * P1, 1 + n_sets * P1,
+      [&](size_t* part, int* cnt) { logistic_loss_grad_scratch(n_cols, n_sets, n, ctx->sms, part, cnt); },
+      [&]() { return launch_logistic_loss_grad(a, ctx->sms, ctx->stream); }, out);
+}
+
+int se_logistic_predict(se_ctx* ctx, int n_coef, const int32_t* subspace, int n_sets, const double* coef,
+                        const double* intercept, double threshold, int raw_slot, int raw_row, int prob_slot,
+                        int prob_row, int label_slot, int label_row) {
+  if (!ctx || !intercept || (n_coef > 0 && !coef)) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_coef >= 0 && n_coef <= kLogisticMaxCols, SE_ERR_ARG, "%d coefficients per set (0..%d supported)",
+             n_coef, kLogisticMaxCols);
+  SE_REQUIRE(ctx, n_sets >= 1 && n_sets <= kLogisticMaxClasses, SE_ERR_ARG,
+             "%d coefficient sets (1: binomial, 2..%d: multinomial)", n_sets, kLogisticMaxClasses);
+  const SlotBuf& X = ctx->slot[SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
+  for (int j = 0; j < n_coef; ++j) {
+    const int32_t col = subspace ? subspace[j] : j;
+    SE_REQUIRE(ctx, col >= 0 && col < X.rows, SE_ERR_ARG, "column %d outside X", col);
+  }
+  SE_TRY(begin(ctx));
+  LogisticPredictArgs a;
+  const int width = n_sets == 1 ? 2 : n_sets;
+  if (raw_slot >= 0) SE_TRY(out_rows(ctx, raw_slot, raw_row, width, X.cols, &a.raw, &a.ld_raw));
+  if (prob_slot >= 0) SE_TRY(out_rows(ctx, prob_slot, prob_row, width, X.cols, &a.prob, &a.ld_prob));
+  if (label_slot >= 0) SE_TRY(out_rows(ctx, label_slot, label_row, 1, X.cols, &a.label, nullptr));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // h_small is reused below
+  int32_t* hcol = reinterpret_cast<int32_t*>(ctx->h_small.get());
+  for (int j = 0; j < n_coef; ++j) hcol[j] = subspace ? subspace[j] : j;
+  double* hd = reinterpret_cast<double*>(ctx->h_small.get() + 1024);
+  memcpy(hd, coef, sizeof(double) * (size_t)n_sets * n_coef);
+  memcpy(hd + (size_t)n_sets * n_coef, intercept, sizeof(double) * (size_t)n_sets);
+  SE_CUDA(ctx, cudaMemcpyAsync(ctx->d_small, ctx->h_small, 1024 + sizeof(double) * (size_t)n_sets * (n_coef + 1),
+                               cudaMemcpyHostToDevice, ctx->stream));
+  const double* dd = reinterpret_cast<const double*>(ctx->d_small.get() + 1024);
+  a.X = X.d; a.ld = X.ld; a.n = X.cols; a.p = n_coef; a.D = n_sets;
+  a.cols = reinterpret_cast<const int32_t*>(ctx->d_small.get());
+  a.coef = dd;
+  a.intercept = dd + (size_t)n_sets * n_coef;
+  a.threshold = threshold;
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_logistic_predict(a, ctx->sms, ctx->stream));
+  return end(ctx);
+}

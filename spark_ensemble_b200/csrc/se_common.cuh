@@ -347,6 +347,27 @@ __device__ __forceinline__ bool block_reduce_publish(double (&acc)[NRED], const 
   return true;
 }
 
+// The last CTA to finish (ticket on *counter) folds the `grid` partials of `len` entries that start at part, in CTA
+// order, and hands every total to emit(entry, total).  The fixed order makes identical launches give identical bits.
+template <class Emit>
+__device__ __forceinline__ void lm_fold_last(const double* part, int len, int grid, unsigned int* counter, Emit emit) {
+  __shared__ bool last;
+  __threadfence();  // every thread's partials, before the ticket
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    last = (atomicInc(counter, (unsigned int)grid - 1) == (unsigned int)grid - 1);
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  for (int e = threadIdx.x; e < len; e += blockDim.x) {
+    double s = 0.0;
+    for (int g = 0; g < grid; ++g) s += __ldcg(&part[(size_t)g * len + e]);
+    emit(e, s);
+  }
+}
+
 // Class index of a label, validated: integer-valued and inside [0, K).  Anything else (negative, >= K, fractional,
 // NaN) raises `bad` and maps to class 0, so no kernel ever forms an out-of-range shared/global address from a label.
 __device__ __forceinline__ int checked_label(float y, int K, bool& bad) {

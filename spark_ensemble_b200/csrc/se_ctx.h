@@ -305,6 +305,11 @@ struct se_ctx {
     se_host::DevBuf<unsigned int> d_cnt;
     se_host::DevBuf<double> d_out;
   } lm;
+  struct {  // se_logistic_stats / se_logistic_loss_grad: the same, kept across the evaluations of a fit
+    se_host::DevBuf<double> d_part;
+    se_host::DevBuf<unsigned int> d_cnt;
+    se_host::DevBuf<double> d_out;
+  } lg;
   std::string err;
   // stopwatch + per-kernel-family timing
   se_host::Event tm0, tm1;

@@ -467,6 +467,45 @@ struct LinearMomentsArgs {
 void linear_moments_scratch(int p, int64_t n, int sms, size_t* partials, int* counters);
 cudaError_t launch_linear_moments(const LinearMomentsArgs& a, int sms, cudaStream_t s);
 
+// ---- logistic regression over resident columns (se_logistic.cu) -------------------------------
+constexpr int kLogisticMaxCols = 254;     // as se_linear_moments
+constexpr int kLogisticMaxClasses = 64;
+struct LogisticArgs {
+  const float* X = nullptr;          // [cols][ld] source slot
+  int64_t ld = 0, n = 0;
+  int p = 0;
+  int D = 1;                         // coefficient sets: 1 binomial, else K (multinomial); the stats pass: K
+  const int32_t* cols = nullptr;     // device [p]
+  const double* shift = nullptr;     // device [p]
+  const double* scale = nullptr;     // device [p] (loss_grad)
+  const double* coef = nullptr;      // device [D][p + 1] (loss_grad), intercept last
+  const float* y = nullptr;          // label row
+  const float* w = nullptr;          // weight row or nullptr (1)
+  double* partials = nullptr;        // logistic_*_scratch's doubles
+  unsigned int* counters = nullptr;  // logistic_*_scratch's tickets, zero before the launch
+  double* out = nullptr;
+};
+// stats: out[3 + 2p + K] = Σc, Σc², Σc(x−s)[p], Σc(x−s)²[p], Σc[y=k][K], invalid rows
+void logistic_stats_scratch(int p, int K, int64_t n, int sms, size_t* partials, int* counters);
+cudaError_t launch_logistic_stats(const LogisticArgs& a, int sms, cudaStream_t s);
+// loss and gradient: out[1 + D(p+1)] = Σ c·ℓ, Σ c·(π_k − [y=k])·z_j
+void logistic_loss_grad_scratch(int p, int D, int64_t n, int sms, size_t* partials, int* counters);
+cudaError_t launch_logistic_loss_grad(const LogisticArgs& a, int sms, cudaStream_t s);
+struct LogisticPredictArgs {
+  const float* X = nullptr;
+  int64_t ld = 0, n = 0;
+  int p = 0, D = 1;
+  const int32_t* cols = nullptr;     // device [p]
+  const double* coef = nullptr;      // device [D][p] raw space
+  const double* intercept = nullptr; // device [D]
+  double threshold = 0.5;
+  float* raw = nullptr;              // [2 or D rows], ld_out apart; nullptr: skipped
+  float* prob = nullptr;
+  float* label = nullptr;
+  int64_t ld_raw = 0, ld_prob = 0;
+};
+cudaError_t launch_logistic_predict(const LogisticPredictArgs& a, int sms, cudaStream_t s);
+
 // ---- exact quantile by radix select (se_util.cu) ---------------------------------------------
 // One pass: histogram (256 bins, fp64 counts in `hist`) of byte `shift/8` of the order-preserving key of each
 // value whose higher bytes equal `prefix` (mask = bits above the byte).  value = a[i], or |a[i] - b[i]| when b.

@@ -28,27 +28,6 @@ __device__ __forceinline__ double lm_weight(const LinearMomentsArgs& a, int64_t 
   return c;
 }
 
-// The last CTA to finish (ticket on *counter) folds the `grid` partials of `len` entries that start at part, in CTA
-// order, and hands every total to emit(entry, total).
-template <class Emit>
-__device__ __forceinline__ void lm_fold_last(const double* part, int len, int grid, unsigned int* counter, Emit emit) {
-  __shared__ bool last;
-  __threadfence();  // every thread's partials, before the ticket
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    last = (atomicInc(counter, (unsigned int)grid - 1) == (unsigned int)grid - 1);
-  }
-  __syncthreads();
-  if (!last) return;
-  __threadfence();
-  for (int e = threadIdx.x; e < len; e += blockDim.x) {
-    double s = 0.0;
-    for (int g = 0; g < grid; ++g) s += __ldcg(&part[(size_t)g * len + e]);
-    emit(e, s);
-  }
-}
-
 __global__ void __launch_bounds__(kBlock) linear_moments_small_kernel(LinearMomentsArgs a) {
   __shared__ int32_t s_col[kLmSmall];
   __shared__ double s_shift[kLmSmall];

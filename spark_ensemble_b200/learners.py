@@ -530,6 +530,255 @@ class DeviceLinearRegression:
                                      shift=X.mean(axis=0, dtype=np.float64))
 
 
+class LogisticRegressionModel(_Model):
+    """org.apache.spark.ml.classification.LogisticRegressionModel: coefficientMatrix [D][p] and interceptVector [D] in
+    raw feature space, D = 1 (binomial: the margin of class 1) or numClasses (multinomial).  Host scoring is fp64;
+    write_rows scores on the device over SLOT_X (se_logistic_predict)."""
+
+    def __init__(self, coef, intercept, num_classes: int, multinomial: bool, threshold: float = 0.5,
+                 objective_history=(), num_evaluations: int = 0):
+        self.coefficientMatrix = np.atleast_2d(np.asarray(coef, dtype=np.float64))
+        self.interceptVector = np.atleast_1d(np.asarray(intercept, dtype=np.float64))
+        self.numClasses, self.isMultinomial = int(num_classes), bool(multinomial)
+        self.threshold = float(threshold)
+        self.objectiveHistory = list(objective_history)
+        self.numEvaluations = int(num_evaluations)
+
+    @property
+    def coefficients(self) -> np.ndarray:
+        if self.isMultinomial:
+            raise ValueError("a multinomial model has a coefficient matrix: use coefficientMatrix")
+        return self.coefficientMatrix[0]
+
+    @property
+    def intercept(self) -> float:
+        if self.isMultinomial:
+            raise ValueError("a multinomial model has an intercept vector: use interceptVector")
+        return float(self.interceptVector[0])
+
+    def _margins(self, X) -> np.ndarray:
+        return np.asarray(X, dtype=np.float64) @ self.coefficientMatrix.T + self.interceptVector
+
+    def predictRaw(self, X) -> np.ndarray:
+        m = self._margins(X)
+        return np.concatenate([-m, m], axis=1) if not self.isMultinomial else m
+
+    def predictProbability(self, X) -> np.ndarray:
+        m = self._margins(X)
+        if not self.isMultinomial:
+            p1 = 1.0 / (1.0 + np.exp(-m[:, 0]))
+            return np.stack([1.0 - p1, p1], axis=1)
+        mx = m.max(axis=1, keepdims=True)
+        inf = np.isposinf(mx[:, 0])
+        with np.errstate(invalid="ignore"):
+            e = np.exp(m - mx)
+            p = e / e.sum(axis=1, keepdims=True)
+        p[inf] = np.isposinf(m[inf]).astype(np.float64)  # raw2probabilityInPlace: 1 for every +inf class
+        return p
+
+    def predict(self, X) -> np.ndarray:
+        if not self.isMultinomial:
+            return (self.predictProbability(X)[:, 1] > self.threshold).astype(np.float64)
+        return np.argmax(self._margins(X), axis=1).astype(np.float64)
+
+    def write_rows(self, ctx, method: str, out_slot: int, out_row: int, subspace=None) -> bool:
+        """Every row's label ("class"), raw vector ("raw") or probabilities ("proba") over the context's SLOT_X into
+        out_slot from row out_row (se_logistic_predict); column j of the model is column subspace[j] of X (None: j)."""
+        kind = {"class": "label", "raw": "raw", "proba": "prob"}[method]
+        ctx.logistic_predict(self.coefficientMatrix, self.interceptVector, self.threshold,
+                             subspace=subspace, **{kind: (out_slot, out_row)})
+        return True
+
+
+class DeviceLogisticRegression:
+    """org.apache.spark.ml.classification.LogisticRegression fitted on the GPU, with Spark's Params, defaults and
+    objective (λ = regParam, α = elasticNetParam, t_j = σ_j with standardization, else 1):
+
+        f = (1/Σc)·Σ c·ℓ + λ·[(1−α)/2·Σ_{k,j} (t_j·β_kj)² + α·Σ_{k,j} t_j·|β_kj|], intercepts unpenalised
+
+    One pass over the resident columns gives the weighted means, Spark's unbiased weighted σ_j, the class histogram and
+    the input checks (se_logistic_stats).  The fit then runs in Spark's standardised space, θ_kj = σ_j·β_kj over
+    z_j = (x_j − μ_j)/σ_j (μ = 0 without fitIntercept; a column with σ_j = 0 keeps β_kj = 0), and every loss and
+    gradient evaluation is one pass over the columns (se_logistic_loss_grad).  Breeze's L-BFGS / OWL-QN are third
+    party: SciPy's L-BFGS-B (m = 10) stands in, with the L1 part written exactly as split variables θ = θ⁺ − θ⁻,
+    θ± >= 0.  Its iterates differ from Breeze's; the optimum is the same.  Post-processing as Spark: multinomial
+    coefficients centred across classes when regParam = 0, multinomial intercepts always centred, and with fitIntercept
+    a single present class gives zero coefficients and an infinite intercept without any evaluation.
+
+    It is not a resident learner of the GBM, Bagging or Boosting loops: they call its `fit`, which opens a context on
+    `device`."""
+
+    def __init__(self, regParam: float = 0.0, elasticNetParam: float = 0.0, maxIter: int = 100, tol: float = 1e-6,
+                 fitIntercept: bool = True, standardization: bool = True, family: str = "auto",
+                 threshold: float = 0.5, device: int = 0):
+        self.regParam, self.elasticNetParam = float(regParam), float(elasticNetParam)
+        self.maxIter, self.tol = int(maxIter), float(tol)
+        self.fitIntercept, self.standardization = bool(fitIntercept), bool(standardization)
+        self.family, self.threshold, self.device = str(family), float(threshold), int(device)
+        self._check()
+
+    def _check(self):
+        if not self.regParam >= 0:
+            raise ValueError(f"regParam must be >= 0, got {self.regParam}")
+        if not 0.0 <= self.elasticNetParam <= 1.0:
+            raise ValueError(f"elasticNetParam must be in [0, 1], got {self.elasticNetParam}")
+        if self.maxIter < 0:
+            raise ValueError(f"maxIter must be >= 0, got {self.maxIter}")
+        if not self.tol >= 0:
+            raise ValueError(f"tol must be >= 0, got {self.tol}")
+        if self.family.lower() not in ("auto", "binomial", "multinomial"):
+            raise ValueError(f"family must be auto, binomial or multinomial, got {self.family!r}")
+        if not 0.0 <= self.threshold <= 1.0:
+            raise ValueError(f"threshold must be in [0, 1], got {self.threshold}")
+
+    def copy(self, extra=None):
+        c = DeviceLogisticRegression(self.regParam, self.elasticNetParam, self.maxIter, self.tol, self.fitIntercept,
+                                     self.standardization, self.family, self.threshold, self.device)
+        for k, v in (extra or {}).items():
+            setattr(c, k, v)
+        c._check()
+        return c
+
+    def _multinomial(self, K: int) -> bool:
+        fam = self.family.lower()
+        if fam == "binomial" and K > 2:
+            raise ValueError(f"binomial family only supports 1 or 2 outcome classes but found {K}")
+        return fam == "multinomial" or (fam == "auto" and K > 2)
+
+    def optimize(self, evaluate, stats, shift, num_classes: int) -> LogisticRegressionModel:
+        """The fit from the statistics pass `stats` (se_logistic_stats's layout, over columns shifted by `shift`) and
+        evaluate(shift, scale, coef [D][p+1]) -> (Σ c·ℓ, gradient [D][p+1]) (se_logistic_loss_grad's contract)."""
+        from scipy.optimize import fmin_l_bfgs_b
+        self._check()
+        K = int(num_classes)
+        if not 1 <= K <= N.LOGISTIC_MAX_CLASSES:
+            raise ValueError(f"the device logistic fit supports 1..{N.LOGISTIC_MAX_CLASSES} classes, got {K}")
+        multi = self._multinomial(K)
+        st = np.asarray(stats, dtype=np.float64)
+        p = (st.size - 3 - K) // 2
+        if st[-1] > 0:
+            raise ValueError(f"{int(st[-1])} rows have a label outside the integers 0..{K - 1}, a negative or "
+                             f"non-finite weight, or a non-finite feature")
+        sw, sw2 = st[0], st[1]
+        if not sw > 0:
+            raise ValueError("the logistic fit needs a positive total weight")
+        s = np.zeros(p) if shift is None else np.asarray(shift, dtype=np.float64).reshape(-1)
+        d1, d2, hist = st[2:2 + p], st[2 + p:2 + 2 * p], st[2 + 2 * p:2 + 2 * p + K]
+        mean = s + d1 / sw
+        denom = sw - sw2 / sw
+        var = np.maximum(d2 - d1 * d1 / sw, 0.0) / denom if denom > 0 else np.zeros(p)
+        sigma = np.sqrt(var)
+        live = sigma > 0
+        inv = np.where(live, 1.0 / np.where(live, sigma, 1.0), 0.0)
+        D = K if multi else 1
+        hist_mask = hist != 0
+        if self.fitIntercept and hist_mask.sum() == 1:  # a single class present: Spark's constant-label model
+            c = int(np.argmax(hist_mask))
+            b = np.zeros(D)
+            if multi:
+                b[c] = np.inf
+            else:
+                b[0] = np.inf if c == 1 else -np.inf
+            return LogisticRegressionModel(np.zeros((D, p)), b, K, multi, self.threshold, [], 0)
+        kshift = mean if self.fitIntercept else np.zeros(p)
+        lam, alpha = self.regParam, self.elasticNetParam
+        q2 = np.ones(p) if self.standardization else inv * inv
+        q1 = np.ones(p) if self.standardization else inv
+        l2, l1 = lam * (1.0 - alpha), lam * alpha
+        split = l1 > 0
+        nt, nb = D * p, (D if self.fitIntercept else 0)
+        b0 = np.zeros(D)
+        if self.fitIntercept:
+            if multi:
+                r = np.log1p(hist)
+                b0 = r - r.mean()
+            elif hist[0] > 0 and hist[1] > 0:
+                b0[0] = np.log(hist[1] / hist[0])
+        evals, history, last = [0], [], [np.nan]
+
+        def unpack(x):
+            th = (x[:nt] - x[nt:2 * nt]) if split else x[:nt]
+            b = x[(2 if split else 1) * nt:] if nb else np.zeros(D)
+            return th.reshape(D, p), b
+
+        def fun(x):
+            th, b = unpack(x)
+            loss, g = evaluate(kshift, inv, np.concatenate([th, b[:, None]], axis=1))
+            evals[0] += 1
+            g = np.asarray(g, dtype=np.float64).reshape(D, p + 1) / sw
+            gt = g[:, :p] + l2 * q2 * th
+            f = loss / sw + 0.5 * l2 * float(np.sum(q2 * th * th))
+            parts = [gt.reshape(-1)]
+            if split:
+                f += l1 * float(np.sum(q1 * (x[:nt] + x[nt:2 * nt]).reshape(D, p)))
+                parts = [(gt + l1 * q1).reshape(-1), (-gt + l1 * q1).reshape(-1)]
+            if nb:
+                parts.append(g[:, p])
+            last[0] = f
+            return f, np.concatenate(parts)
+
+        x0 = np.concatenate([np.zeros(nt * (2 if split else 1)), b0[:nb]])
+        bounds = [(0.0, None)] * (2 * nt) + [(None, None)] * nb if split else None
+        history.append(fun(x0)[0])
+        x, _, _ = fmin_l_bfgs_b(fun, x0, bounds=bounds, m=10, pgtol=self.tol,
+                                factr=max(self.tol / np.finfo(float).eps, 1.0), maxiter=self.maxIter,
+                                callback=lambda xk: history.append(last[0]))
+        th, b = unpack(x)
+        th, b = th.copy(), b.copy()
+        if multi and lam == 0.0:
+            th -= th.mean(axis=0, keepdims=True)
+        if multi and self.fitIntercept:
+            b -= b.mean()
+        beta = th * inv
+        intercept = (b - beta @ kshift) if self.fitIntercept else np.zeros(D)
+        return LogisticRegressionModel(beta, intercept, K, multi, self.threshold, history, evals[0])
+
+    def fit_resident(self, ctx, src_slot: int, cols, num_classes: int, label_slot: int, label_row: int,
+                     weight_slot: int, weight_row: int, out_slot: int | None = None, out_row: int = 0,
+                     method: str = "class", shift=None) -> LogisticRegressionModel:
+        """Fit over columns `cols` of src_slot in ctx: one se_logistic_stats pass, then one se_logistic_loss_grad call
+        per evaluation.  The stats shifts default to the values of row 0 (a few downloads).  With out_slot, every row's
+        label, raw vector or probabilities (method "class", "raw", "proba") go to out_slot from row out_row (src_slot
+        must then be SLOT_X)."""
+        cols = np.asarray(cols, dtype=np.int32).reshape(-1)
+        if cols.size > N.LOGISTIC_MAX_COLS:
+            raise ValueError(f"the device logistic fit supports up to {N.LOGISTIC_MAX_COLS} columns, got {cols.size}")
+        if out_slot is not None and src_slot != N.SLOT_X:
+            raise ValueError("outputs are written from SLOT_X only")
+        n = ctx.layout(src_slot)[1]
+        if shift is None:
+            shift = np.array([ctx.download(src_slot, count=1, offset=int(c) * n)[0] for c in cols], dtype=np.float64)
+        st = ctx.logistic_stats(src_slot, cols, num_classes, label_slot, label_row, weight_slot, weight_row, shift)
+
+        def evaluate(kshift, scale, coef):
+            return ctx.logistic_loss_grad(src_slot, cols, coef, label_slot, label_row, weight_slot, weight_row,
+                                          kshift, scale)
+        model = self.optimize(evaluate, st, shift, num_classes)
+        if out_slot is not None:
+            model.write_rows(ctx, method, out_slot, out_row, subspace=cols)
+        return model
+
+    def fit(self, X, y, w=None, num_classes: int | None = None) -> LogisticRegressionModel:
+        X = np.asarray(X, dtype=np.float32)
+        n, d = X.shape
+        if n == 0:
+            raise ValueError("DeviceLogisticRegression.fit needs at least one row")
+        y = np.asarray(y, dtype=np.float64).reshape(-1)
+        K = int(num_classes) if num_classes is not None else int(np.nanmax(y)) + 1
+        with Context(self.device) as ctx:
+            ctx.alloc(N.SLOT_X, d, n)
+            ctx.upload_rowmajor(N.SLOT_X, X)
+            ctx.alloc(N.SLOT_Y, n)
+            ctx.upload(N.SLOT_Y, y.astype(np.float32))
+            if w is not None:
+                ctx.alloc(N.SLOT_W, n)
+                ctx.upload(N.SLOT_W, np.asarray(w, dtype=np.float32))
+            # row 0's values, the shifts fit_resident downloads by default: a fit over the same resident data in
+            # another context (a stacker fitted in the stacking context) follows the same path to the same bits
+            return self.fit_resident(ctx, N.SLOT_X, np.arange(d, dtype=np.int32), K, N.SLOT_Y, 0,
+                                     N.SLOT_W if w is not None else -1, 0, shift=X[0].astype(np.float64))
+
+
 class LinearRegression:
     """Stand-in for org.apache.spark.ml.regression.LinearRegression (ridge via regParam)."""
 

@@ -335,11 +335,13 @@ def tree_list(members) -> list | None:
 
 def _stacker_fit_device(ctx: Context, stacker, n: int, W: int, weighted: bool, num_classes: int | None):
     """The stacker fitted over the meta-features in the context's SLOT_X; None for a stacker without a device fit."""
-    from .learners import DeviceLinearRegression
+    from .learners import DeviceLinearRegression, DeviceLogisticRegression
     cols = np.arange(W, dtype=np.int32)
     wslot = N.SLOT_W if weighted else -1
     if isinstance(stacker, DeviceLinearRegression):
         return stacker.fit_resident(ctx, N.SLOT_X, cols, N.SLOT_Y, 0, wslot, 0, False, None)
+    if isinstance(stacker, DeviceLogisticRegression) and num_classes is not None:
+        return stacker.fit_resident(ctx, N.SLOT_X, cols, int(num_classes), N.SLOT_Y, 0, wslot, 0)
     if not getattr(stacker, "device_learner", False):
         return None
     # candidates from the meta-features of the sampled rows, as stacker.fit over the downloaded matrix draws them
@@ -370,7 +372,7 @@ def stacking_fit(est: Params, dataset: DataFrame, num_classes: int | None = None
         models = [fit_member(est, m, dataset, X, y, mw, num_classes, wc) for m in members]
         meta = np.concatenate([model_outputs(mod, X, method, k) for mod, k in zip(models, widths)])
         return models, _fit_stacker_host(est, stacker, meta.T, y, sw, num_classes), widths
-    from .learners import DeviceLinearRegression
+    from .learners import DeviceLinearRegression, DeviceLogisticRegression
     W = sum(widths)
     models = []
     with resident_context(est.device, X) as ctx:
@@ -386,6 +388,9 @@ def stacking_fit(est: Params, dataset: DataFrame, num_classes: int | None = None
         for m, k in zip(members, widths):
             if isinstance(m, DeviceLinearRegression):
                 model = m.fit_resident(ctx, N.SLOT_X, all_cols, N.SLOT_Y, 0, mslot, 0, False, N.SLOT_P, row)
+            elif isinstance(m, DeviceLogisticRegression) and num_classes is not None:
+                model = m.fit_resident(ctx, N.SLOT_X, all_cols, int(num_classes), N.SLOT_Y, 0, mslot, 0, N.SLOT_P, row,
+                                       method if k > 1 else "class")
             elif getattr(m, "device_learner", False):
                 ctx.tree_fit_bins(m.split_candidates(X))
                 if not is_classifier(m):
@@ -424,8 +429,8 @@ def _fit_stacker_host(est: Params, stacker, F, y, w, num_classes: int | None):
 def stacking_predict(model: Params, X) -> np.ndarray:
     """stack.predict(meta-features) of every row of X.  Host route: each member's outputs on the host.  Device route
     (residentFeatures): X is uploaded once; members with a device form write their rows of SLOT_P on the device, the
-    others are predicted on the host and uploaded; the meta-features become SLOT_X and a tree or linear stack scores
-    them there."""
+    others are predicted on the host and uploaded; the meta-features become SLOT_X and a tree, linear or logistic stack
+    scores them there."""
     X = np.asarray(X, dtype=np.float32)
     n = X.shape[0]
     method = model("stackMethod").lower() if model.hasParam("stackMethod") else "class"
@@ -450,7 +455,8 @@ def stacking_predict(model: Params, X) -> np.ndarray:
 
 
 def write_stack_rows(ctx: Context, stack, out_slot: int) -> bool:
-    """The stack's prediction (a tree's value or label, or a linear model) of every row of SLOT_X into out_slot."""
+    """The stack's prediction (a tree's value or label, a linear model, or a logistic regression's label) of every row
+    of SLOT_X into out_slot; False for any other stack, which is then predicted on the host."""
     try:
         t = stack.tree_arrays() if hasattr(stack, "tree_arrays") else None
         if t is not None:
@@ -464,4 +470,7 @@ def write_stack_rows(ctx: Context, stack, out_slot: int) -> bool:
     if lin is not None:
         ctx.linear_predict(lin["coef"], float(lin["intercept"]), out_slot, 0)
         return True
+    from .learners import LogisticRegressionModel
+    if isinstance(stack, LogisticRegressionModel):  # its write_rows writes only the label row of out_slot
+        return stack.write_rows(ctx, "class", out_slot, 0)
     return False
