@@ -495,6 +495,18 @@ SE_API int se_logistic_stats(se_ctx* ctx, int src_slot, int n_cols, const int32_
 SE_API int se_logistic_loss_grad(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
                                  const double* scale, int n_sets, const double* coef, int label_slot, int label_row,
                                  int weight_slot, int weight_row, double* out);
+/* se_logistic_loss_grad for B = n_members members (1..1024) over the same src_slot, labels, weights and n_sets = D, in
+ * one call: member b has p_b = n_cols[b] columns (0..254) and takes the next p_b entries of cols, shift and scale
+ * (NULL: 0 and 1) and the next D(p_b + 1) entries of coef, and gets the next 1 + D(p_b + 1) entries of out in
+ * se_logistic_loss_grad's layout.  A row of weight 0 contributes nothing to any member whatever its features (Spark's
+ * aggregator skips zero-weight instances: a bag's out-of-bag rows).  Each member runs its own kernel grid and fold, so
+ * its bits depend on its inputs, the rows and the device only: not on which members share the call or where it sits in
+ * the batch.  The members' CTAs over the same rows run together, so the L2 serves their repeated reads of the columns
+ * they share. */
+SE_API int se_logistic_loss_grad_batch(se_ctx* ctx, int src_slot, int n_members, const int32_t* n_cols,
+                                       const int32_t* cols, const double* shift, const double* scale, int n_sets,
+                                       const double* coef, int label_slot, int label_row, int weight_slot,
+                                       int weight_row, double* out);
 /* Scores a logistic model over SE_SLOT_X: coef [n_sets][n_coef] in raw space over columns subspace[j] (NULL: j),
  * intercept [n_sets], m_k = Σ_j coef[k][j]·x_j + intercept[k] in fp64.  Writes, for each slot >= 0: raw (2 rows
  * (−m, m) when n_sets == 1, else the n_sets margins), probability (1 − σ(m), σ(m), or the softmax; a margin of +inf

@@ -137,6 +137,12 @@ TABLE = [
                                                    ("labelSlot", "i32"), ("labelRow", "i32"), ("weightSlot", "i32"),
                                                    ("weightRow", "i32"), ("out", "out_f64")],
      "fp64 logistic loss and gradient at coef [nSets][nCols+1], into out"),
+    ("logisticLossGradBatch", "se_logistic_loss_grad_batch", [("ctx", "ctx"), ("srcSlot", "i32"), ("nMembers", "i32"),
+                                                              ("nCols", "in_i32"), ("cols", "in_i32"), ("shift", "in_f64"),
+                                                              ("scale", "in_f64"), ("nSets", "i32"), ("coef", "in_f64"),
+                                                              ("labelSlot", "i32"), ("labelRow", "i32"), ("weightSlot", "i32"),
+                                                              ("weightRow", "i32"), ("out", "out_f64")],
+     "fp64 logistic loss and gradient of nMembers members (their columns and coef one after another), into out"),
     ("logisticPredict", "se_logistic_predict", [("ctx", "ctx"), ("nCoef", "i32"), ("subspace", "in_i32"), ("nSets", "i32"),
                                                 ("coef", "in_f64"), ("intercept", "in_f64"), ("threshold", "f64"),
                                                 ("rawSlot", "i32"), ("rawRow", "i32"), ("probSlot", "i32"), ("probRow", "i32"),

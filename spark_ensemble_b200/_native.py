@@ -33,6 +33,7 @@ FOREST_AGG_MAX_CLASSES = 32  # SE_FOREST_AGG_MAX_CLASSES: se_forest_agg's class 
 FOREST_MEDIAN_MAX_TREES = 64  # SE_FOREST_MEDIAN_MAX_TREES: se_forest_median's tree limit
 LINEAR_MOMENTS_MAX_COLS = 254  # se_linear_moments: p + 2 <= 256
 LOGISTIC_MAX_COLS, LOGISTIC_MAX_CLASSES = 254, 64  # se_logistic_*
+LOGISTIC_MAX_BATCH = 1024  # members of one se_logistic_loss_grad_batch call
 
 # enum se_kernel_family
 KERNEL_FAMILIES = ["sq_stats", "eval", "update", "resid", "mean_loss", "boost_real", "boost_err",
@@ -124,6 +125,7 @@ PROTOTYPES = {
     "se_linear_moments": [_vp, _i32, _i32, _ip, _dp, _d, _i32, _i32, _i32, _i32, _i32, _dp],
     "se_logistic_stats": [_vp, _i32, _i32, _ip, _dp, _i32, _i32, _i32, _i32, _i32, _dp],
     "se_logistic_loss_grad": [_vp, _i32, _i32, _ip, _dp, _dp, _i32, _dp, _i32, _i32, _i32, _i32, _dp],
+    "se_logistic_loss_grad_batch": [_vp, _i32, _i32, _ip, _ip, _dp, _dp, _i32, _dp, _i32, _i32, _i32, _i32, _dp],
     "se_logistic_predict": [_vp, _i32, _ip, _i32, _dp, _dp, _d, _i32, _i32, _i32, _i32, _i32, _i32],
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,

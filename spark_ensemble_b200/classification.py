@@ -17,7 +17,8 @@ from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_classifier_params, shared_predictor_params, subbag_params)
 from .routes import (STACK_METHODS, bagging_fit, device_fit, device_trees, extract_instances, load_boosting,
-                     member_route, one_pass, split_validation, stacking_fit, stacking_predict, tree_list)
+                     member_route, one_pass, resident_linear, split_validation, stacking_fit, stacking_predict,
+                     tree_list)
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -224,6 +225,7 @@ class BoostingClassifier(Params):
         real = self("algorithm").lower() == "real"
         learner = self("baseLearner")
         fit_on_device = device_fit(self, learner, require_resident=True)
+        linear_on_device = resident_linear(self, learner)
         resident = bool(self("residentFeatures"))
         out_slot = N.SLOT_PROBA if real else N.SLOT_PRED  # the member's probabilities (SAMME.R) or labels (SAMME)
         models, est_weights, history = [], [], []
@@ -238,12 +240,16 @@ class BoostingClassifier(Params):
                     # are invariant under the common 1 / sumWeights scale of :184-187
                     model = learner.fit_resident(ctx, K, N.SLOT_Y, 0, N.SLOT_BW, 0, False, all_cols, out_slot, 0,
                                                  proba=real)
+                elif linear_on_device:  # the same: Spark's logistic objective is divided by Σ c
+                    model = learner.fit_resident(ctx, N.SLOT_X, np.arange(X.shape[1], dtype=np.int32), K, N.SLOT_Y, 0,
+                                                 N.SLOT_BW, 0, out_slot, 0, "proba" if real else "class",
+                                                 shift=np.asarray(X[0], dtype=np.float64))
                 else:
                     wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)  # weight = boostingWeight / sumWeights :184-187
                     model = learner.fit(X, y, wn, num_classes=K)    # third party :189-195
                 if real and not hasattr(model, "predictProbability"):
                     raise RuntimeError('algorithm "real" is not compatible with base learner')  # :261-263
-                if not fit_on_device:  # the member's output into out_slot: on the device when it is a tree
+                if not (fit_on_device or linear_on_device):  # the output into out_slot: on the device for a tree
                     t = model.tree_arrays() if resident else None
                     if t is not None:
                         if real:

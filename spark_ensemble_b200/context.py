@@ -514,6 +514,48 @@ class Context:
                                                  N.dptr(out)))
         return float(out[0]), out[1:].reshape(D, p + 1)
 
+    def logistic_loss_grad_batch(self, src_slot: int, members, label_slot: int, label_row: int = 0,
+                                 weight_slot: int = -1, weight_row: int = 0) -> list:
+        """logistic_loss_grad of several members in one call (se_logistic_loss_grad_batch): members is a list of
+        (cols, coef [D][p+1], shift, scale) with one D; returns one (Σ c·ℓ, gradient [D][p+1]) per member.  Rows of
+        weight 0 contribute nothing whatever their features, and a member's bits do not depend on the other members."""
+        if not members:
+            return []
+        cols, shifts, scales, coefs, ps = [], [], [], [], []
+        D = None
+        for c, th, s, sc in members:
+            c = np.ascontiguousarray(c, dtype=np.int32).reshape(-1)
+            p = c.size
+            th = np.ascontiguousarray(th, dtype=np.float64)
+            d = th.size // (p + 1) if th.ndim == 1 else th.shape[0]
+            if th.size != d * (p + 1):
+                raise ValueError(f"coef must be [D][{p + 1}]")
+            if D is not None and d != D:
+                raise ValueError("every member of a batch has the same number of coefficient sets")
+            D = d
+            for v, default, acc in ((s, 0.0, shifts), (sc, 1.0, scales)):
+                v = np.full(p, default) if v is None else np.ascontiguousarray(v, dtype=np.float64).reshape(-1)
+                if v.size != p:
+                    raise ValueError("one shift and one scale per column")
+                acc.append(v)
+            cols.append(c)
+            coefs.append(th.reshape(-1))
+            ps.append(p)
+        n_cols = np.asarray(ps, dtype=np.int32)
+        c_all, s_all, sc_all, th_all = (np.ascontiguousarray(np.concatenate(a)) for a in (cols, shifts, scales, coefs))
+        c_all = c_all.astype(np.int32, copy=False)
+        lens = [1 + D * (p + 1) for p in ps]
+        out = np.zeros(sum(lens))
+        self._ck(self._lib.se_logistic_loss_grad_batch(
+            self._h, int(src_slot), len(ps), N.iptr(n_cols), N.iptr(c_all) if c_all.size else None,
+            N.dptr(s_all) if s_all.size else None, N.dptr(sc_all) if sc_all.size else None, int(D), N.dptr(th_all),
+            int(label_slot), int(label_row), int(weight_slot), int(weight_row), N.dptr(out)))
+        res, o = [], 0
+        for p, ln in zip(ps, lens):
+            res.append((float(out[o]), out[o + 1:o + ln].reshape(D, p + 1)))
+            o += ln
+        return res
+
     def logistic_predict(self, coef, intercept, threshold: float = 0.5, raw=None, prob=None, label=None,
                          subspace=None):
         """A logistic model scored over SLOT_X (se_logistic_predict): coef [D][p] raw space, intercept [D].  raw, prob

@@ -653,13 +653,13 @@ int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols
 namespace {
 // The inputs se_logistic_stats and se_logistic_loss_grad share: the columns of src_slot, the label row and the weight
 // row (none when weight_slot < 0), checked; the column list goes to d_small.
+// (se_logistic_loss_grad_batch: cols is every member's list, one after another, max_cols their total's limit.)
 int logistic_inputs(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, int label_slot, int label_row,
-                    int weight_slot, int weight_row, LogisticArgs* a) {
+                    int weight_slot, int weight_row, LogisticArgs* a, int max_cols = kLogisticMaxCols) {
   if (!ctx || (n_cols > 0 && !cols)) return fail(ctx, SE_ERR_ARG, "null argument");
   SE_REQUIRE(ctx, src_slot == SE_SLOT_X || src_slot == SE_SLOT_P, SE_ERR_ARG,
              "source slot %d: only SE_SLOT_X or SE_SLOT_P", src_slot);
-  SE_REQUIRE(ctx, n_cols >= 0 && n_cols <= kLogisticMaxCols, SE_ERR_ARG, "%d columns (0..%d supported)", n_cols,
-             kLogisticMaxCols);
+  SE_REQUIRE(ctx, n_cols >= 0 && n_cols <= max_cols, SE_ERR_ARG, "%d columns (0..%d supported)", n_cols, max_cols);
   const SlotBuf& X = ctx->slot[src_slot];
   SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "source slot %d not allocated", src_slot);
   const int64_t n = X.cols;
@@ -755,6 +755,93 @@ int se_logistic_loss_grad(se_ctx* ctx, int src_slot, int n_cols, const int32_t* 
       ctx, a, (size_t)2 * n_cols + (size_t)n_sets * P1, 1 + n_sets * P1,
       [&](size_t* part, int* cnt) { logistic_loss_grad_scratch(n_cols, n_sets, n, ctx->sms, part, cnt); },
       [&]() { return launch_logistic_loss_grad(a, ctx->sms, ctx->stream); }, out);
+}
+
+int se_logistic_loss_grad_batch(se_ctx* ctx, int src_slot, int n_members, const int32_t* n_cols, const int32_t* cols,
+                                const double* shift, const double* scale, int n_sets, const double* coef,
+                                int label_slot, int label_row, int weight_slot, int weight_row, double* out) {
+  if (!ctx || !out || !coef || !n_cols) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_members >= 1 && n_members <= kLogisticMaxBatch, SE_ERR_ARG, "%d members (1..%d supported)",
+             n_members, kLogisticMaxBatch);
+  SE_REQUIRE(ctx, n_sets >= 1 && n_sets <= kLogisticMaxClasses, SE_ERR_ARG,
+             "%d coefficient sets (1: binomial, 2..%d: multinomial)", n_sets, kLogisticMaxClasses);
+  int64_t total = 0;
+  for (int b = 0; b < n_members; ++b) {
+    SE_REQUIRE(ctx, n_cols[b] >= 0 && n_cols[b] <= kLogisticMaxCols, SE_ERR_ARG,
+               "member %d: %d columns (0..%d supported)", b, n_cols[b], kLogisticMaxCols);
+    total += n_cols[b];
+  }
+  LogisticArgs a;  // every column of every member is checked against the slot here
+  SE_TRY(logistic_inputs(ctx, src_slot, (int)total, cols, label_slot, label_row, weight_slot, weight_row, &a,
+                         kLogisticMaxBatch * kLogisticMaxCols));
+  const int D = n_sets;
+  std::vector<LogisticArgs> mem((size_t)n_members, a);
+  size_t n_part = 0, n_in_doubles = 0, n_out = 0;
+  int n_cnt = 0;
+  for (int b = 0; b < n_members; ++b) {
+    size_t part = 0;
+    int cnt = 0;
+    logistic_loss_grad_scratch(n_cols[b], D, a.n, ctx->sms, &part, &cnt);
+    LogisticArgs& m = mem[(size_t)b];
+    m.p = n_cols[b];
+    m.D = D;
+    // offsets for now, pointers once the buffers exist
+    m.partials = reinterpret_cast<double*>(n_part);
+    m.counters = reinterpret_cast<unsigned int*>((size_t)n_cnt);
+    m.out = reinterpret_cast<double*>(n_out);
+    n_part += part;
+    n_cnt += cnt;
+    n_out += 1 + (size_t)D * (m.p + 1);
+    n_in_doubles += 2 * (size_t)m.p + (size_t)D * (m.p + 1);
+  }
+  const int count = logistic_batch_items(mem.data(), n_members, ctx->sms, nullptr);
+  const size_t items_bytes = ((sizeof(LogisticBatchItem) * (size_t)count + 15) / 16) * 16;
+  const size_t cols_bytes = ((sizeof(int32_t) * (size_t)total + 15) / 16) * 16;
+  const size_t in_bytes = items_bytes + cols_bytes + sizeof(double) * n_in_doubles;
+  auto& L = ctx->lg;
+  SE_CUDA(ctx, L.d_part.grow(n_part));
+  SE_CUDA(ctx, L.d_cnt.grow((size_t)n_cnt));
+  SE_CUDA(ctx, L.d_out.grow(n_out));
+  SE_CUDA(ctx, L.d_in.grow(in_bytes));
+  SE_CUDA(ctx, L.h_in.grow(std::max(in_bytes, sizeof(double) * n_out)));
+  unsigned char* h = L.h_in.get();
+  unsigned char* d = L.d_in.get();
+  memcpy(h + items_bytes, cols, sizeof(int32_t) * (size_t)total);
+  double* hd = reinterpret_cast<double*>(h + items_bytes + cols_bytes);
+  const double* dd = reinterpret_cast<const double*>(d + items_bytes + cols_bytes);
+  size_t col_off = 0, dbl_off = 0, coef_off = 0;
+  for (int b = 0; b < n_members; ++b) {
+    LogisticArgs& m = mem[(size_t)b];
+    const int p = m.p, P1 = p + 1;
+    for (int k = 0; k < p; ++k) {
+      hd[dbl_off + k] = shift ? shift[col_off + k] : 0.0;
+      hd[dbl_off + p + k] = scale ? scale[col_off + k] : 1.0;
+    }
+    memcpy(hd + dbl_off + 2 * p, coef + coef_off, sizeof(double) * (size_t)D * P1);
+    m.cols = reinterpret_cast<const int32_t*>(d + items_bytes) + col_off;
+    m.shift = dd + dbl_off;
+    m.scale = dd + dbl_off + p;
+    m.coef = dd + dbl_off + 2 * p;
+    m.partials = L.d_part.get() + reinterpret_cast<size_t>(m.partials);
+    m.counters = L.d_cnt.get() + reinterpret_cast<size_t>(m.counters);
+    m.out = L.d_out.get() + reinterpret_cast<size_t>(m.out);
+    col_off += (size_t)p;
+    dbl_off += 2 * (size_t)p + (size_t)D * P1;
+    coef_off += (size_t)D * P1;
+  }
+  LogisticBatchItem* items = reinterpret_cast<LogisticBatchItem*>(h);
+  logistic_batch_items(mem.data(), n_members, ctx->sms, items);
+  SE_CUDA(ctx, cudaMemcpyAsync(d, h, in_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  SE_CUDA(ctx, cudaMemsetAsync(L.d_cnt, 0, sizeof(unsigned int) * (size_t)n_cnt, ctx->stream));
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_logistic_loss_grad_batch(items, reinterpret_cast<const LogisticBatchItem*>(d),
+                                                                 count, ctx->stream));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the staged items are read by the copy above: reuse h_in after it
+  double* hout = reinterpret_cast<double*>(L.h_in.get());
+  SE_CUDA(ctx, cudaMemcpyAsync(hout, L.d_out, sizeof(double) * n_out, cudaMemcpyDeviceToHost, ctx->stream));
+  SE_TRY(end(ctx));
+  SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  memcpy(out, hout, sizeof(double) * n_out);
+  return SE_OK;
 }
 
 int se_logistic_predict(se_ctx* ctx, int n_coef, const int32_t* subspace, int n_sets, const double* coef,

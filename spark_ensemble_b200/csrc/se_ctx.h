@@ -309,6 +309,9 @@ struct se_ctx {
     se_host::DevBuf<double> d_part;
     se_host::DevBuf<unsigned int> d_cnt;
     se_host::DevBuf<double> d_out;
+    // se_logistic_loss_grad_batch: the work items and the members' columns and coefficients, staged and on the device
+    se_host::PinnedBuf<unsigned char> h_in;
+    se_host::DevBuf<unsigned char> d_in;
   } lg;
   std::string err;
   // stopwatch + per-kernel-family timing

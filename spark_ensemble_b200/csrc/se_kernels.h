@@ -470,6 +470,7 @@ cudaError_t launch_linear_moments(const LinearMomentsArgs& a, int sms, cudaStrea
 // ---- logistic regression over resident columns (se_logistic.cu) -------------------------------
 constexpr int kLogisticMaxCols = 254;     // as se_linear_moments
 constexpr int kLogisticMaxClasses = 64;
+constexpr int kLogisticMaxBatch = 1024;   // members of one se_logistic_loss_grad_batch call
 struct LogisticArgs {
   const float* X = nullptr;          // [cols][ld] source slot
   int64_t ld = 0, n = 0;
@@ -491,6 +492,23 @@ cudaError_t launch_logistic_stats(const LogisticArgs& a, int sms, cudaStream_t s
 // loss and gradient: out[1 + D(p+1)] = Σ c·ℓ, Σ c·(π_k − [y=k])·z_j
 void logistic_loss_grad_scratch(int p, int D, int64_t n, int sms, size_t* partials, int* counters);
 cudaError_t launch_logistic_loss_grad(const LogisticArgs& a, int sms, cudaStream_t s);
+// Batched loss and gradient (se_logistic_loss_grad_batch): one work item per member of the register kernels and per
+// j-tile of a member of the tiled kernel.  Each member runs the kernel, grid and partials a lone launch would give it
+// (logistic_loss_grad_scratch's sizes at its a.partials / a.counters), except that rows of weight 0 contribute nothing
+// whatever their features.
+struct LogisticBatchItem {
+  LogisticArgs a;
+  int kind = 0;              // 0, 1: the register kernel at width 16, 40; 2: the tiled kernel
+  int ctas = 0;              // the member's grid
+  int tile = 0, nk = 0, L = 0, zs = 0;  // tiled: the item's j-tile and the member's shape
+  int64_t rows_per_cta = 0;
+  size_t smem = 0;
+};
+// Fills items (when not null) from the B members' arguments, grouped by kind; returns the number of items.
+int logistic_batch_items(const LogisticArgs* members, int B, int sms, LogisticBatchItem* items);
+// items on the host and the same array at d_items on the device: one launch per kind present
+cudaError_t launch_logistic_loss_grad_batch(const LogisticBatchItem* items, const LogisticBatchItem* d_items,
+                                            int count, cudaStream_t s);
 struct LogisticPredictArgs {
   const float* X = nullptr;
   int64_t ld = 0, n = 0;

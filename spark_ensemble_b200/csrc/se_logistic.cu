@@ -11,6 +11,8 @@
 //     weights), in two widths so that a few columns do not pay the registers of 40;
 //   * otherwise a CTA stages 32 rows of z in shared memory in fp64, forms their D margins, turns them into residuals
 //     c·(π_k − [y=k]) and accumulates a (4·nk)×(4·nj) tile of the gradient, 4×4 entries per thread, with FFMA64.
+#include <algorithm>
+
 #include "se_common.cuh"
 #include "se_kernels.h"
 
@@ -140,8 +142,10 @@ __global__ void __launch_bounds__(kBlock) logistic_stats_kernel(LogisticArgs a, 
 }
 
 // ---- loss and gradient: registers (D = 1, p + 1 <= kLgSmall) ----------------------------------------------------------
-template <int kLgSmall>
-__global__ void __launch_bounds__(kBlock) logistic_small_kernel(LogisticArgs a) {
+// CTA `cta` of `ctas` over the rows of member a.  kSkipZero: rows of weight 0 are skipped before any of their values is
+// read (a batch's out-of-bag rows), so that a non-finite feature there contributes nothing.
+template <int kLgSmall, bool kSkipZero>
+__device__ __forceinline__ void lg_small_body(const LogisticArgs& a, int cta, int ctas) {
   __shared__ int32_t s_col[kLgSmall];
   __shared__ double s_shift[kLgSmall], s_scale[kLgSmall], s_coef[kLgSmall];
   const int p = a.p;
@@ -157,7 +161,9 @@ __global__ void __launch_bounds__(kBlock) logistic_small_kernel(LogisticArgs a) 
 #pragma unroll
   for (int j = 0; j < kLgSmall; ++j) acc[j] = 0.0;
   double loss = 0.0;
-  for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * kBlock) {
+  for (int64_t i = (int64_t)cta * kBlock + threadIdx.x; i < a.n; i += (int64_t)ctas * kBlock) {
+    const double c = lg_weight(a.w, i);
+    if (kSkipZero && c == 0.0) continue;
     double z[kLgSmall];
     double m = 0.0;
 #pragma unroll
@@ -168,7 +174,7 @@ __global__ void __launch_bounds__(kBlock) logistic_small_kernel(LogisticArgs a) 
       z[j] = v;
       m = fma(s_coef[j], v, m);
     }
-    const double r = lg_binomial(m, ld_stream1(a.y + i), lg_weight(a.w, i), &loss);
+    const double r = lg_binomial(m, ld_stream1(a.y + i), c, &loss);
 #pragma unroll
     for (int j = 0; j < kLgSmall; ++j) acc[j] = fma(r, z[j], acc[j]);
   }
@@ -184,18 +190,26 @@ __global__ void __launch_bounds__(kBlock) logistic_small_kernel(LogisticArgs a) 
   if (threadIdx.x < kLen) {
     double v = 0.0;
     for (int w = 0; w < kBlock / 32; ++w) v += sm[threadIdx.x][w];
-    a.partials[(size_t)blockIdx.x * kLen + threadIdx.x] = v;
+    a.partials[(size_t)cta * kLen + threadIdx.x] = v;
   }
-  lm_fold_last(a.partials, kLen, gridDim.x, a.counters, [&](int e, double s) {
+  lm_fold_last(a.partials, kLen, ctas, a.counters, [&](int e, double s) {
     if (e <= p + 1) a.out[e] = s;
   });
+}
+template <int kLgSmall>
+__global__ void __launch_bounds__(kBlock) logistic_small_kernel(LogisticArgs a) {
+  lg_small_body<kLgSmall, false>(a, blockIdx.x, gridDim.x);
 }
 
 // ---- loss and gradient: shared-memory row blocks and a register-tiled gradient ----------------------------------------
 // Thread t owns gradient entries (k, j) = (tk + nk·u, j0 + tj + nj·v), u, v < 4, with tk = t / nj, tj = t % nj and
 // j0 = blockIdx.y·4·nj.  Margins: L lanes per (row, class) pair split the p + 1 products and add them butterfly-wise.
-__global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, int64_t rows_per_cta, int nk, int L,
-                                                               int zs) {
+// CTA `cta` of `ctas` over j-tile `tile` of member a, whose partials start at a.partials + tile·ctas·kLgPart and whose
+// ticket is a.counters[tile].  kSkipZero: a row of weight 0 is staged as z = 0 (the intercept's 1 aside), so that its
+// terms are exact zeros whatever its features.
+template <bool kSkipZero>
+__device__ __forceinline__ void lg_tile_body(const LogisticArgs& a, int cta, int ctas, int tile, int64_t rows_per_cta,
+                                             int nk, int L, int zs) {
   extern __shared__ double lg_smem[];
   double* Z = lg_smem;                           // [kLgRows][zs]
   double* Rs = Z + kLgRows * zs;                 // [kLgRows][64]: margins, then residuals
@@ -206,7 +220,7 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, i
   const int lane = t & 31, warp = t >> 5;
   for (int j = t; j < p; j += kBlock) s_col[j] = a.cols[j];
   const int nj = kBlock / nk, tk = t / nj, tj = t % nj;
-  const int j0 = blockIdx.y * 4 * nj;
+  const int j0 = tile * 4 * nj;
   int nu = 0;
 #pragma unroll
   for (int u = 0; u < 4; ++u) nu += (tk + nk * u < D) ? 1 : 0;
@@ -217,7 +231,7 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, i
     for (int v = 0; v < 4; ++v) acc[u][v] = 0.0;
   double loss = 0.0;
   __syncthreads();
-  const int64_t r0 = (int64_t)blockIdx.x * rows_per_cta;
+  const int64_t r0 = (int64_t)cta * rows_per_cta;
   const int64_t r1 = min(a.n, r0 + rows_per_cta);
   for (int64_t base = r0; base < r1; base += kLgRows) {
     if (t < kLgRows) {
@@ -230,7 +244,9 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, i
       const int r = t % kLgRows;
       const int64_t i = base + r;
       double v = 0.0;
-      if (i < r1) v = (j < p) ? ((double)ld_stream1(a.X + (int64_t)s_col[j] * a.ld + i) - a.shift[j]) * a.scale[j] : 1.0;
+      const bool live = !kSkipZero || j == p || (i < r1 && (!a.w || __ldg(a.w + i) != 0.f));
+      if (i < r1 && live)
+        v = (j < p) ? ((double)ld_stream1(a.X + (int64_t)s_col[j] * a.ld + i) - a.shift[j]) * a.scale[j] : 1.0;
       Z[r * zs + j] = v;
     }
     __syncthreads();
@@ -289,7 +305,7 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, i
     }
     __syncthreads();
   }
-  double* part = a.partials + (size_t)blockIdx.y * gridDim.x * kLgPart + (size_t)blockIdx.x * kLgPart;
+  double* part = a.partials + (size_t)tile * ctas * kLgPart + (size_t)cta * kLgPart;
   const int TJ = 4 * nj;
 #pragma unroll
   for (int u = 0; u < 4; ++u)
@@ -304,15 +320,19 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, i
     for (int w = 0; w < kBlock / 32; ++w) s += sl[w];
     part[kLgTileEntries] = s;
   }
-  lm_fold_last(a.partials + (size_t)blockIdx.y * gridDim.x * kLgPart, kLgPart, gridDim.x, a.counters + blockIdx.y,
+  lm_fold_last(a.partials + (size_t)tile * ctas * kLgPart, kLgPart, ctas, a.counters + tile,
                [&](int e, double s) {
                  if (e == kLgTileEntries) {
-                   if (blockIdx.y == 0) a.out[0] = s;
+                   if (tile == 0) a.out[0] = s;
                    return;
                  }
                  const int k = e / TJ, j = j0 + e % TJ;
                  if (k < D && j < P1) a.out[1 + (size_t)k * P1 + j] = s;
                });
+}
+__global__ void __launch_bounds__(kBlock) logistic_tile_kernel(LogisticArgs a, int64_t rows_per_cta, int nk, int L,
+                                                               int zs) {
+  lg_tile_body<false>(a, blockIdx.x, gridDim.x, blockIdx.y, rows_per_cta, nk, L, zs);
 }
 
 // the tiled kernel's shape: nk thread rows (4·nk >= D), L lanes per margin, j-tiles, shared memory
@@ -337,6 +357,23 @@ LgShape lg_shape(int p, int D) {
 int lg_small(int p, int D) {
   if (D != 1 || p + 1 > kLgWide) return 0;
   return p + 1 <= kLgNarrow ? kLgNarrow : kLgWide;
+}
+
+// ---- loss and gradient of a batch of members (se_logistic_loss_grad_batch) ------------------------------------------
+// blockIdx.x is the work item, blockIdx.y the CTA of its rows: the members' CTAs over the same rows are adjacent in
+// launch order, so they run together and the L2 serves the members' repeated reads of the columns they share.  An item
+// runs its member's own kernel body, grid and partials, so a member's bits do not depend on the rest of the batch; CTAs
+// beyond an item's own grid return at once.
+template <int kLgSmall>
+__global__ void __launch_bounds__(kBlock) logistic_small_batch_kernel(const LogisticBatchItem* items) {
+  const LogisticBatchItem& it = items[blockIdx.x];
+  if ((int)blockIdx.y >= it.ctas) return;
+  lg_small_body<kLgSmall, true>(it.a, blockIdx.y, it.ctas);
+}
+__global__ void __launch_bounds__(kBlock) logistic_tile_batch_kernel(const LogisticBatchItem* items) {
+  const LogisticBatchItem& it = items[blockIdx.x];
+  if ((int)blockIdx.y >= it.ctas) return;
+  lg_tile_body<true>(it.a, blockIdx.y, it.ctas, it.tile, it.rows_per_cta, it.nk, it.L, it.zs);
 }
 
 // ---- scoring --------------------------------------------------------------------------------------------------------
@@ -442,6 +479,73 @@ cudaError_t launch_logistic_loss_grad(const LogisticArgs& a, int sms, cudaStream
   if (e != cudaSuccess) return e;
   logistic_tile_kernel<<<dim3((unsigned)g, (unsigned)s.tiles), kBlock, s.smem, st>>>(a, per, s.nk, s.L, s.zs);
   return cudaGetLastError();
+}
+
+int logistic_batch_items(const LogisticArgs* members, int B, int sms, LogisticBatchItem* items) {
+  int count = 0;
+  for (int kind = 0; kind < 3; ++kind)  // grouped by kernel: narrow registers, wide registers, tiled
+    for (int b = 0; b < B; ++b) {
+      const LogisticArgs& a = members[b];
+      const int w = lg_small(a.p, a.D);
+      if (kind != (w == kLgNarrow ? 0 : w == kLgWide ? 1 : 2)) continue;
+      if (kind < 2) {
+        if (items) {
+          LogisticBatchItem& it = items[count];
+          it = LogisticBatchItem{};
+          it.a = a;
+          it.kind = kind;
+          it.ctas = grid_rows(a.n, kBlock, 4, sms);
+        }
+        ++count;
+        continue;
+      }
+      const LgShape s = lg_shape(a.p, a.D);
+      int g;
+      int64_t per;
+      lg_row_grid(a.n, kLgRows, (2 * (int64_t)sms + s.tiles - 1) / s.tiles, &g, &per);
+      for (int t = 0; t < s.tiles; ++t, ++count) {
+        if (!items) continue;
+        LogisticBatchItem& it = items[count];
+        it = LogisticBatchItem{};
+        it.a = a;
+        it.kind = kind;
+        it.ctas = g;
+        it.rows_per_cta = per;
+        it.tile = t;
+        it.nk = s.nk; it.L = s.L; it.zs = s.zs;
+        it.smem = s.smem;
+      }
+    }
+  return count;
+}
+
+cudaError_t launch_logistic_loss_grad_batch(const LogisticBatchItem* items, const LogisticBatchItem* d_items,
+                                            int count, cudaStream_t st) {
+  for (int i0 = 0; i0 < count;) {
+    const int kind = items[i0].kind;
+    int i1 = i0, ctas = 1;
+    size_t smem = 0;
+    for (; i1 < count && items[i1].kind == kind; ++i1) {
+      const LogisticArgs& a = items[i1].a;
+      if (a.p < 0 || a.p > kLogisticMaxCols || a.D < 1 || a.D > kLogisticMaxClasses || a.n < 1) return cudaErrorInvalidValue;
+      ctas = max(ctas, items[i1].ctas);
+      smem = std::max(smem, items[i1].smem);
+    }
+    const dim3 grid((unsigned)(i1 - i0), (unsigned)ctas);
+    if (kind == 0) {
+      logistic_small_batch_kernel<kLgNarrow><<<grid, kBlock, 0, st>>>(d_items + i0);
+    } else if (kind == 1) {
+      logistic_small_batch_kernel<kLgWide><<<grid, kBlock, 0, st>>>(d_items + i0);
+    } else {
+      const cudaError_t e = allow_dynamic_smem(logistic_tile_batch_kernel, smem);
+      if (e != cudaSuccess) return e;
+      logistic_tile_batch_kernel<<<grid, kBlock, smem, st>>>(d_items + i0);
+    }
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+    i0 = i1;
+  }
+  return cudaSuccess;
 }
 
 cudaError_t launch_logistic_predict(const LogisticPredictArgs& a, int sms, cudaStream_t st) {

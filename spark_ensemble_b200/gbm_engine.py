@@ -13,7 +13,8 @@ import numpy as np
 from . import _native as N
 from .context import Context
 from .ensemble import subspace
-from .routes import bag_counts
+from .learners import DeviceLinearRegression
+from .routes import bag_counts, resident_linear
 from .sharded import make_context
 
 
@@ -56,6 +57,7 @@ class GBMEngine:
         c.upload_rowmajor(N.SLOT_X, X)  # transposed on the device, chunked + double buffered
         self._X_host = X
         self._fit_bins = None
+        self._col_mean = None
         if Xv is not None and self.nv > 0:
             Xv = np.asarray(Xv)
             c.alloc(N.SLOT_VX, Xv.shape[1], Xv.shape[0])
@@ -72,21 +74,28 @@ class GBMEngine:
         return r, wout
 
     def fit_direction(self, j: int, learner, subspace, newton: bool = False, bag: bool = False):
-        """Fit the device tree learner on R row j (weights: WOUT row j in newton mode, else W when the fit has
-        weights; the bag's multiplicities when `bag`) and write its output into H row j.  The split candidates are
-        set once per fit, on the first call.  Nothing but the fitted tree crosses PCIe."""
+        """Fit the device tree learner or DeviceLinearRegression on R row j over the round's subspace (weights: WOUT
+        row j in newton mode, else W when the fit has weights; the bag's multiplicities when `bag`) and write its
+        output into H row j.  A tree's split candidates are set once per fit, on the first call; a linear fit is
+        shifted by the column means, as its `fit` is.  Nothing but the fitted model crosses PCIe."""
         if not self._x_resident:
             raise ValueError("the device tree learner needs the features on the device (residentFeatures=True)")
         c = self.ctx
-        if self._fit_bins is None:
-            c.tree_fit_bins(learner.split_candidates(self._X_host))
-            self._fit_bins = learner
         if newton:
             wslot, wrow = N.SLOT_WOUT, j
         elif self.has_weights:
             wslot, wrow = N.SLOT_W, 0
         else:
             wslot, wrow = -1, 0
+        if isinstance(learner, DeviceLinearRegression):
+            if self._col_mean is None:
+                self._col_mean = np.asarray(self._X_host, dtype=np.float32).mean(axis=0, dtype=np.float64)
+            sub = np.asarray(subspace, dtype=np.int32)
+            return learner.fit_resident(c, N.SLOT_X, sub, N.SLOT_R, j, wslot, wrow, bag, N.SLOT_H, j,
+                                        shift=self._col_mean[sub])
+        if self._fit_bins is None:
+            c.tree_fit_bins(learner.split_candidates(self._X_host))
+            self._fit_bins = learner
         return learner.fit_resident(c, N.SLOT_R, j, wslot, wrow, bag, subspace, N.SLOT_H, j)
 
     def set_direction(self, h, validation: bool = False):
@@ -170,6 +179,7 @@ def fit_rounds(est, X, y, w, Xv, yv, dim: int, loss: str, param: float, F0, vF0,
     seed, num_learners = est("seed"), est("numBaseLearners")
     counts = bag_counts(n, est("subsampleRatio"), est("replacement"), seed)  # same bag every round (quirk 3)
     subspaces = [subspace(est("subspaceRatio"), X.shape[1], seed + i) for i in range(num_learners)]
+    linear_fit = resident_linear(est, learner)
     ctx = make_context(est.device, est("devices"))
     try:
         eng = GBMEngine(ctx, n, nv, dim, loss, param, has_weights=w is not None)
@@ -188,7 +198,7 @@ def fit_rounds(est, X, y, w, Xv, yv, dim: int, loss: str, param: float, F0, vF0,
                 ctx.gbm_set_loss_param(ctx.gbm_abs_residual_quantile(est("alpha")))
                 eng.residuals(False)
             sub = subspaces[i]
-            if device_fit:  # each dimension's tree is fitted where the residuals live: only the tree comes back
+            if device_fit or linear_fit:  # each dimension's fit is where the residuals live: only the model comes back
                 imodels = [eng.fit_direction(j, learner, sub, newton=newton, bag=counts is not None)
                            for j in range(dim)]
             else:

@@ -102,6 +102,19 @@ def continuous_split_candidates(values, max_bins: int) -> np.ndarray:
     return np.unique(out)  # sorted; clamping can only merge two candidates at the extremes
 
 
+def distinct_subspaces(subspaces):
+    """The distinct subspaces (each fitted once) and, per member, the index of its distinct subspace."""
+    keys, first, index = {}, [], []
+    for s in subspaces:
+        s = np.asarray(s, dtype=np.int32).reshape(-1)
+        key = s.tobytes()
+        if key not in keys:
+            keys[key] = len(first)
+            first.append(s)
+        index.append(keys[key])
+    return first, index
+
+
 def check_class_labels(y: np.ndarray, num_classes: int, n: int):
     """The device classification tree's labels: n of them, each an integer class index in [0, num_classes)."""
     if y.size != n or np.any(y < 0) or np.any(y != np.floor(y)) or np.any(y >= num_classes):
@@ -214,17 +227,7 @@ class _DeviceTreeLearner:
             raise ValueError(f"{type(self).__name__}.fit needs at least one row and one column")
         return X
 
-    def _forest_subspaces(self, subspaces):
-        """The distinct subspaces (each fitted once) and, per member, the index of its distinct subspace."""
-        keys, first, index = {}, [], []
-        for s in subspaces:
-            s = np.asarray(s, dtype=np.int32).reshape(-1)
-            key = s.tobytes()
-            if key not in keys:
-                keys[key] = len(first)
-                first.append(s)
-            index.append(keys[key])
-        return first, index
+    _forest_subspaces = staticmethod(distinct_subspaces)
 
 
 class DeviceDecisionTreeRegressor(_DeviceTreeLearner):
@@ -479,8 +482,10 @@ class DeviceLinearRegression:
     which, with the default regParam = 0, is Spark's default (least squares with an intercept) on full-rank data.  One
     pass over the resident columns forms the fp64 moment matrix of (x − s, 1, y − s_y) (se_linear_moments); the host
     solves its (p+1)-sized centred normal equations (solve_linear_moments).  Its model is LinearRegressionModel, scored
-    on the device by se_linear_predict.  It is not a resident learner of the GBM, Bagging or Boosting loops: they call
-    its `fit`, which opens a context on `device`."""
+    on the device by se_linear_predict.  With residentFeatures the GBM, Bagging and Boosting loops fit it where their data
+    live: GBM on the round's residuals (fit_resident), Boosting on the boosting weights (weight_scale = 1 / sumWeights),
+    Bagging every member from one moment pass over the union of their columns (fit_members_resident).  Without it
+    they call `fit`, which opens a context on `device`."""
 
     def __init__(self, regParam: float = 0.0, device: int = 0):
         self.regParam, self.device = float(regParam), int(device)
@@ -492,10 +497,12 @@ class DeviceLinearRegression:
 
     def fit_resident(self, ctx, src_slot: int, cols, label_slot: int, label_row: int, weight_slot: int,
                      weight_row: int, use_bag: bool, out_slot: int | None, out_row: int = 0,
-                     shift=None) -> LinearRegressionModel:
+                     shift=None, weight_scale: float = 1.0) -> LinearRegressionModel:
         """Fit over columns `cols` of src_slot in ctx: one se_linear_moments call, then the host solve.  The shifts
-        default to the values of row 0 (a few downloads), which keeps the centring well away from cancellation.  With
-        out_slot, every row's prediction goes to its row out_row (src_slot must then be SLOT_X)."""
+        default to the values of row 0 (a few downloads), which keeps the centring well away from cancellation.  The
+        weights are multiplied by weight_scale (the moments are linear in them): with regParam > 0 the objective
+        depends on their scale.  With out_slot, every row's prediction goes to its row out_row (src_slot must then be
+        SLOT_X)."""
         cols = np.asarray(cols, dtype=np.int32).reshape(-1)
         n = ctx.layout(src_slot)[1]
         if shift is None:
@@ -503,6 +510,8 @@ class DeviceLinearRegression:
         label_shift = float(ctx.download(label_slot, count=1, offset=int(label_row) * n)[0])
         M = ctx.linear_moments(src_slot, cols, label_slot, label_row, weight_slot, weight_row, use_bag, shift,
                                label_shift)
+        if weight_scale != 1.0:
+            M = M * float(weight_scale)
         coef, intercept = solve_linear_moments(M, shift, label_shift, self.regParam)
         model = LinearRegressionModel(coef, intercept)
         if out_slot is not None:
@@ -511,6 +520,24 @@ class DeviceLinearRegression:
             a = model.linear_arrays()
             ctx.linear_predict(a["coef"], float(a["intercept"]), out_slot, out_row, subspace=cols)
         return model
+
+    def fit_members_resident(self, ctx, subspaces, label_slot: int, label_row: int, weight_slot: int, weight_row: int,
+                             shift, label_shift: float) -> list:
+        """One model per subspace over columns of SLOT_X, the same labels and weights: one se_linear_moments pass per
+        group of subspaces whose union holds at most 254 columns, each member's matrix sliced out of it (a moment of
+        two columns does not depend on the others).  shift holds one value per column of SLOT_X."""
+        shift = np.asarray(shift, dtype=np.float64).reshape(-1)
+        subs = [np.asarray(c, dtype=np.int32).reshape(-1) for c in subspaces]
+        models = [None] * len(subs)
+        for group in column_groups(subs, N.LINEAR_MOMENTS_MAX_COLS):
+            U = np.unique(np.concatenate([subs[i] for i in group])).astype(np.int32)
+            M = ctx.linear_moments(N.SLOT_X, U, label_slot, label_row, weight_slot, weight_row, False, shift[U],
+                                   label_shift)
+            for i in group:
+                idx = np.concatenate([np.searchsorted(U, subs[i]), [U.size, U.size + 1]])
+                coef, b = solve_linear_moments(M[np.ix_(idx, idx)], shift[subs[i]], label_shift, self.regParam)
+                models[i] = LinearRegressionModel(coef, b)
+        return models
 
     def fit(self, X, y, w=None) -> LinearRegressionModel:
         X = np.asarray(X, dtype=np.float32)
@@ -605,8 +632,10 @@ class DeviceLogisticRegression:
     coefficients centred across classes when regParam = 0, multinomial intercepts always centred, and with fitIntercept
     a single present class gives zero coefficients and an infinite intercept without any evaluation.
 
-    It is not a resident learner of the GBM, Bagging or Boosting loops: they call its `fit`, which opens a context on
-    `device`."""
+    With residentFeatures, Boosting fits it on the labels and boosting weights where they live (fit_resident: the
+    objective is divided by Σc, so the 1 / sumWeights scale does not change it), and Bagging fits every member in one
+    context, their L-BFGS runs in lock step so that one se_logistic_loss_grad_batch call serves every member's
+    evaluation (fit_members_resident).  Without it they call `fit`, which opens a context on `device`."""
 
     def __init__(self, regParam: float = 0.0, elasticNetParam: float = 0.0, maxIter: int = 100, tol: float = 1e-6,
                  fitIntercept: bool = True, standardization: bool = True, family: str = "auto",
@@ -758,6 +787,32 @@ class DeviceLogisticRegression:
             model.write_rows(ctx, method, out_slot, out_row, subspace=cols)
         return model
 
+    def fit_members_resident(self, ctx, subspaces, num_classes: int, label_slot: int, label_row: int,
+                             weight_slot: int, weight_row: int, shifts) -> list:
+        """One model per subspace over columns of SLOT_X, the same labels and weights: one se_logistic_stats pass per
+        member (shifts: one array per member), then every member's optimize in lock step (lockstep), each evaluation
+        round one se_logistic_loss_grad_batch call over the live members.  A member's fit is the one fit_resident
+        gives over its columns, since its bits do not depend on the other members of a batch."""
+        self._check()
+        subs = [np.asarray(c, dtype=np.int32).reshape(-1) for c in subspaces]
+        for c in subs:
+            if c.size > N.LOGISTIC_MAX_COLS:
+                raise ValueError(f"the device logistic fit supports up to {N.LOGISTIC_MAX_COLS} columns, got {c.size}")
+        stats = [ctx.logistic_stats(N.SLOT_X, c, num_classes, label_slot, label_row, weight_slot, weight_row, s)
+                 for c, s in zip(subs, shifts)]
+
+        def evaluate_batch(requests):
+            out = []
+            for k in range(0, len(requests), N.LOGISTIC_MAX_BATCH):
+                out += ctx.logistic_loss_grad_batch(
+                    N.SLOT_X, [(subs[i], coef, kshift, scale) for i, kshift, scale, coef in
+                               requests[k:k + N.LOGISTIC_MAX_BATCH]],
+                    label_slot, label_row, weight_slot, weight_row)
+            return out
+
+        jobs = [lambda evaluate, st=st, s=s: self.optimize(evaluate, st, s, num_classes) for st, s in zip(stats, shifts)]
+        return lockstep(jobs, evaluate_batch)
+
     def fit(self, X, y, w=None, num_classes: int | None = None) -> LogisticRegressionModel:
         X = np.asarray(X, dtype=np.float32)
         n, d = X.shape
@@ -777,6 +832,107 @@ class DeviceLogisticRegression:
             # another context (a stacker fitted in the stacking context) follows the same path to the same bits
             return self.fit_resident(ctx, N.SLOT_X, np.arange(d, dtype=np.int32), K, N.SLOT_Y, 0,
                                      N.SLOT_W if w is not None else -1, 0, shift=X[0].astype(np.float64))
+
+
+def column_groups(subspaces, max_cols: int) -> list:
+    """Indices of subspaces in consecutive groups whose union of columns holds at most max_cols columns (a subspace
+    with more than max_cols distinct columns makes a group of its own)."""
+    groups, cur, union = [], [], set()
+    for i, c in enumerate(subspaces):
+        u = union | {int(v) for v in c}
+        if cur and len(u) > max_cols:
+            groups.append(cur)
+            cur, u = [], {int(v) for v in c}
+        cur.append(i)
+        union = u
+    if cur:
+        groups.append(cur)
+    return groups
+
+
+class _Stop(Exception):
+    """Raised in a lock-step job's evaluate once another job or the batch evaluation has failed."""
+
+
+def lockstep(jobs, evaluate_batch) -> list:
+    """Runs jobs (job(evaluate) -> result, e.g. a member's DeviceLogisticRegression.optimize) in lock step, one thread
+    each.  A job's evaluate(kshift, scale, coef) posts its request and waits; once every job still running has posted,
+    evaluate_batch([(job index, kshift, scale, coef), ...]) (in job order) answers all of them with one list of
+    (loss, gradient).  A job that returns leaves the batch.  An exception in a job or in evaluate_batch stops every
+    other job at its next evaluation and is raised here (the lowest job's, evaluate_batch's first) once all threads
+    have ended.  evaluate_batch runs on the calling thread, so a context is only used from the thread that owns it.
+    As long as evaluate_batch answers a request independently of the rest of its batch, each job's result is the one
+    it gets alone."""
+    import threading
+    cond = threading.Condition()
+    live = set(range(len(jobs)))
+    posted, answers, errors = {}, {}, {}
+    results = [None] * len(jobs)
+    stop = [False]
+
+    def evaluate_of(i):
+        def evaluate(kshift, scale, coef):
+            with cond:
+                if stop[0]:
+                    raise _Stop()
+                posted[i] = (kshift, scale, coef)
+                cond.notify_all()
+                while i not in answers and not stop[0]:
+                    cond.wait()
+                if i not in answers:
+                    raise _Stop()
+                return answers.pop(i)
+        return evaluate
+
+    def run(i):
+        try:
+            r = jobs[i](evaluate_of(i))
+            with cond:
+                results[i] = r
+        except _Stop:
+            pass
+        except BaseException as e:  # noqa: BLE001 - handed to the caller below
+            with cond:
+                errors[i] = e
+                stop[0] = True
+        finally:
+            with cond:
+                live.discard(i)
+                cond.notify_all()
+
+    threads = [threading.Thread(target=run, args=(i,), daemon=True) for i in range(len(jobs))]
+    for t in threads:
+        t.start()
+    try:
+        while True:
+            with cond:
+                while not stop[0] and live and len(posted) < len(live):
+                    cond.wait()
+                if stop[0] or not live:
+                    break
+                batch = sorted(posted.items())
+                posted.clear()
+            try:
+                out = evaluate_batch([(i,) + req for i, req in batch])
+            except BaseException as e:  # noqa: BLE001
+                with cond:
+                    errors[-1] = e
+                    stop[0] = True
+                    cond.notify_all()
+                break
+            with cond:
+                for (i, _), r in zip(batch, out):
+                    answers[i] = r
+                cond.notify_all()
+    finally:
+        with cond:
+            stop[0] = stop[0] or bool(live)
+            cond.notify_all()
+        for t in threads:
+            t.join()
+    if errors:
+        raise errors[min(errors)]
+    return results
 
 
 class LinearRegression:

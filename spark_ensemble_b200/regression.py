@@ -16,8 +16,8 @@ from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_predictor_params, subbag_params)
 from .routes import (bagging_fit, device_fit, device_trees, download_raw, extract_instances, forest_sum, load_boosting,
-                     member_route, one_pass, resident_context, split_validation, stack_outputs, stacking_fit,
-                     stacking_predict, tree_list)
+                     member_route, one_pass, resident_context, resident_linear, split_validation, stack_outputs,
+                     stacking_fit, stacking_predict, tree_list)
 
 _REG_LOSSES = ("squared", "absolute", "huber", "quantile")  # GBMRegressor.scala:119-120
 _REG_INIT = ("constant", "zero", "base")                     # :121-123
@@ -233,17 +233,24 @@ class BoostingRegressor(Params):
         # A device learner fits where the boosting weights live when the features are resident.  Without
         # residentFeatures it keeps the learner.fit route below (its own context per round) rather than raising.
         fit_on_device = device_fit(self, learner, require_resident=False)
+        linear_on_device = resident_linear(self, learner)
         models, est_weights, history = [], [], []
         with Context(self.device) as ctx:
             ctx.boostreg_configure(y.shape[0])
             # X only for the device fit: a host-fitted tree is not walked on the device here (BoostingClassifier does)
             all_cols, sum_w = load_boosting(ctx, X, y, w, learner, fit_on_device,  # :205-212
-                                            upload_features=fit_on_device)
+                                            upload_features=fit_on_device or linear_on_device)
+            if linear_on_device:  # the shifts learner.fit takes: the column means
+                cols = np.arange(X.shape[1], dtype=np.int32)
+                shift = np.asarray(X, dtype=np.float32).mean(axis=0, dtype=np.float64)
             i, best, done = 0, 0, False
             while i < self("numBaseLearners") and not done and sum_w > 0:  # :218
                 if fit_on_device:  # fitted on SLOT_Y / SLOT_BW where they live, straight into SLOT_PRED; the splits are
                     # invariant under the common 1 / sumWeights scale of :222-225
                     model = learner.fit_resident(ctx, N.SLOT_Y, 0, N.SLOT_BW, 0, False, all_cols, N.SLOT_PRED, 0)
+                elif linear_on_device:  # on the normalised weights of :222-225, since regParam > 0 depends on their scale
+                    model = learner.fit_resident(ctx, N.SLOT_X, cols, N.SLOT_Y, 0, N.SLOT_BW, 0, False, N.SLOT_PRED, 0,
+                                                 shift=shift, weight_scale=1.0 / sum_w)
                 else:
                     wn = ctx.download(N.SLOT_BW, scale=1.0 / sum_w)  # :222-225
                     model = learner.fit(X, y, wn)                     # third party :231-233

@@ -17,7 +17,7 @@ import numpy as np
 from . import _native as N
 from .context import Context
 from .ensemble import DataFrame, spark_bernoulli_sample, subspace
-from .learners import check_class_labels
+from .learners import check_class_labels, distinct_subspaces
 from .params import Params
 
 
@@ -82,6 +82,16 @@ def device_fit(est: Params, learner, require_resident: bool) -> bool:
     return True
 
 
+def resident_linear(est: Params, learner) -> bool:
+    """True when a DeviceLinearRegression or DeviceLogisticRegression base learner fits in the estimator's own context,
+    over the data already there: residentFeatures is set and Param `devices`, if the estimator has it, names at most
+    one GPU (sharded.ShardedContext has no linear or logistic calls).  Otherwise the learner's `fit` is used."""
+    from .learners import DeviceLinearRegression, DeviceLogisticRegression
+    if not isinstance(learner, (DeviceLinearRegression, DeviceLogisticRegression)) or not est("residentFeatures"):
+        return False
+    return not (est.hasParam("devices") and len(est("devices")) >= 2)
+
+
 # ---- Bagging: every member sees the same bag (reference quirk 3) and differs only in its subspace -----------------
 def bagging_fit(est: Params, X, y, w, num_classes: int | None = None):
     """(subspaces, models) of a Bagging fit.  The bag is drawn once with numpy.  With residentFeatures and a device tree
@@ -97,6 +107,8 @@ def bagging_fit(est: Params, X, y, w, num_classes: int | None = None):
     bw = counts if w is None else counts * w
     if device_fit(est, learner, require_resident=False):
         return subs, _bagging_forest_fit(est.device, learner, X, y, bw, subs, num_classes)
+    if resident_linear(est, learner):
+        return subs, _bagging_linear_fit(est.device, learner, X, y, bw, subs, num_classes)
     keep = bw > 0
     kw = {} if num_classes is None else {"num_classes": num_classes}
     return subs, [learner.fit(X[keep][:, subs[i]], y[keep], bw[keep], **kw) for i in range(M)]
@@ -131,6 +143,44 @@ def _bagging_forest_fit(device: int, learner, X, y, bw, subs, num_classes: int |
         if num_classes is None:
             return learner.fit_forest_resident(ctx, N.SLOT_Y, 0, N.SLOT_W, 0, True, subs)
         return learner.fit_forest_resident(ctx, int(num_classes), N.SLOT_Y, 0, N.SLOT_W, 0, True, subs)
+
+
+def _bagging_linear_fit(device: int, learner, X, y, bw, subs, num_classes: int | None) -> list:
+    """Bagging's linear or logistic members fitted in one context: X is uploaded once, the weights bw go to SLOT_W (0
+    outside the bag) and equal subspaces are fitted once.  A member sees what learner.fit(X[keep][:, sub], y[keep],
+    bw[keep]) sees: the same weighted sums, with the same shifts (the in-bag column means for a linear member, the
+    first in-bag row for a logistic one), since rows of weight 0 add exact zeros.  The out-of-bag rows' labels and
+    non-finite features, which that route never reads, are replaced by 0 in what is uploaded, so they fail nothing;
+    an in-bag one fails the fit as it does there."""
+    from .learners import DeviceLogisticRegression
+    keep = bw > 0
+    rows = np.flatnonzero(keep)
+    if rows.size == 0:
+        raise ValueError(f"{type(learner).__name__}.fit needs at least one row")
+    X = np.asarray(X, dtype=np.float32)
+    n, d = X.shape
+    finite = np.isfinite(X).all(axis=1)
+    if not finite[~keep].all():
+        X = np.where((keep | finite)[:, None], X, np.where(np.isfinite(X), X, np.float32(0)))
+    y = np.asarray(y, dtype=np.float64).reshape(-1)
+    distinct, index = distinct_subspaces(subs)
+    with Context(device) as ctx:
+        ctx.alloc(N.SLOT_X, d, n)
+        ctx.upload_rowmajor(N.SLOT_X, X)
+        ctx.alloc(N.SLOT_Y, n)
+        ctx.upload(N.SLOT_Y, np.where(keep, y, 0.0).astype(np.float32))
+        ctx.alloc(N.SLOT_W, n)
+        ctx.upload(N.SLOT_W, np.where(keep, bw, 0.0).astype(np.float32))
+        if isinstance(learner, DeviceLogisticRegression):
+            K = int(num_classes) if num_classes is not None else int(np.nanmax(y[rows])) + 1
+            first = X[rows[0]].astype(np.float64)
+            models = learner.fit_members_resident(ctx, distinct, K, N.SLOT_Y, 0, N.SLOT_W, 0,
+                                                  [first[c] for c in distinct])
+        else:
+            shift = X[rows].mean(axis=0, dtype=np.float64)
+            models = learner.fit_members_resident(ctx, distinct, N.SLOT_Y, 0, N.SLOT_W, 0, shift,
+                                                  float(np.float32(y[rows[0]])))
+    return [models[i] for i in index]
 
 
 # ---- Boosting ----------------------------------------------------------------------------------------------------------
