@@ -222,9 +222,22 @@ int fetch_scalars(se_ctx* ctx, int off, int count, double* out, int op) {
   return check_p2p(ctx);
 }
 
+// Carried fused squared rounds may leave R pending (gbm.r_pending): apply the steps before anything else touches R or
+// writes H.  The stored values are the ones the carried statistics were summed over, so they stay current.
+int settle_r(se_ctx* ctx) {
+  if (ctx->gbm.r_pending == 0) return SE_OK;
+  SE_CUDA(ctx, cudaSetDevice(ctx->device));
+  SE_LAUNCH_T(ctx, SE_KF_OTHER, launch_gbm_settle_r(ctx->slot[SE_SLOT_R].d, ctx->slot[SE_SLOT_H].d, ctx->d_rchain,
+                                                    ctx->gbm.r_pending, ctx->gbm.n, ctx->sms, ctx->stream));
+  ctx->gbm.r_pending = 0;
+  return SE_OK;
+}
+
 // The residual-mode fused squared round leaves F owed (gbm.f_owed): rebuild it as y - r before anything reads train F
-// or writes Y, F or R.  R is re-derived from the rebuilt F (y - F), as an eager update would have left it.
+// or writes Y, F or R.  R is re-derived from the rebuilt F (y - F), as an eager update would have left it.  A pending
+// R is settled first: F = y - r.
 int settle_f(se_ctx* ctx) {
+  SE_TRY(settle_r(ctx));
   if (!ctx->gbm.f_owed) return SE_OK;
   SE_CUDA(ctx, cudaSetDevice(ctx->device));
   SE_LAUNCH_T(ctx, SE_KF_OTHER, launch_gbm_settle_f(ctx->slot[SE_SLOT_Y].d, ctx->slot[SE_SLOT_R].d, ctx->slot[SE_SLOT_F].d,
@@ -245,7 +258,10 @@ int write_slot(se_ctx* ctx, int slot) {
       ctx->gbm.sq_stats_current = false;
       if (slot == SE_SLOT_Y) ctx->y_state[0] = 0;  // labels checked as class indices
       break;
-    case SE_SLOT_H: ctx->gbm.sq_stats_current = false; break;  // the squared round's carried statistics
+    case SE_SLOT_H:
+      SE_TRY(settle_r(ctx));  // the pending steps go along the old h
+      ctx->gbm.sq_stats_current = false;  // the squared round's carried statistics
+      break;
     case SE_SLOT_VY: ctx->y_state[1] = 0; break;
     case SE_SLOT_W: case SE_SLOT_BAG: ctx->gbm.wsum_valid = false; break;
     case SE_SLOT_WOUT: ctx->wout_scaled = false; break;  // se_download's 1/S factor
@@ -255,7 +271,16 @@ int write_slot(se_ctx* ctx, int slot) {
   return SE_OK;
 }
 
-int read_slot(se_ctx* ctx, int slot) { return slot == SE_SLOT_F ? settle_f(ctx) : SE_OK; }
+// Every entry point that reads a caller-chosen slot calls this first.  A caller that reads R between rounds over one
+// direction would pay a settle for every deferred round: the next carried round stores r' instead.
+int read_slot(se_ctx* ctx, int slot) {
+  if (slot == SE_SLOT_F) return settle_f(ctx);
+  if (slot == SE_SLOT_R) {
+    ctx->gbm.sq_defer_ok = false;
+    return settle_r(ctx);
+  }
+  return SE_OK;
+}
 int slot_alloc2d(se_ctx* ctx, int slot, int64_t rows, int64_t cols) {
   SE_REQUIRE(ctx, slot >= 0 && slot < SE_NUM_SLOTS, SE_ERR_ARG, "bad slot %d", slot);
   SE_REQUIRE(ctx, rows >= 1 && cols >= 0, SE_ERR_ARG, "bad slot shape %lld x %lld", (long long)rows,
@@ -340,6 +365,7 @@ int se_ctx_create(int device, se_ctx** out) {
   SE_CUDA(nullptr, cudaHostGetDevicePointer(&ctx->d_bad_label, ctx->h_bad_label, 0));
   SE_CUDA(nullptr, ctx->d_fsync.grow(1));
   SE_CUDA(nullptr, cudaMemset(ctx->d_fsync, 0, sizeof(FusedSync)));
+  SE_CUDA(nullptr, ctx->d_rchain.grow(kSqDeferMax));
   ctx->clock_khz = prop.clockRate > 0 ? prop.clockRate : 1965000;
   if (const char* s = getenv("SE_FUSED_ROUND")) ctx->fused_round = atoi(s) != 0 ? 1 : 0;
   if (const char* s = getenv("SE_FUSED_RESIDENT")) ctx->fused_resident = atoi(s) != 0;
@@ -497,6 +523,8 @@ const Option kOptions[] = {
   {"fused_ctas_per_sm", SE_GET(c->fused_ctas_per_sm), SE_SET(c->fused_ctas_per_sm = iv), SE_IN(iv >= 1 && iv <= 8),
    "fused_ctas_per_sm in [1,8]"},
   {"fused_resident", SE_GET(c->fused_resident), SE_SET(c->fused_resident = iv != 0)},
+  {"sq_defer_max", SE_GET(c->sq_defer_max), SE_SET(c->sq_defer_max = iv), SE_IN(iv >= 0 && iv <= kSqDeferMax),
+   "sq_defer_max in [0,64]"},
   {"ls_mode", SE_GET(c->ls_mode), SE_SET(c->ls_mode = iv), SE_IN(iv >= 0 && iv <= 2), "ls_mode in {0,1,2}"},
   {"ls_resident", SE_GET(c->ls_resident), SE_SET(c->ls_resident = iv != 0)},
   {"ls_ctas_per_sm", SE_GET(c->ls_ctas_per_sm), SE_SET(c->ls_ctas_per_sm = iv), SE_IN(iv >= 1 && iv <= 8),
@@ -520,6 +548,8 @@ const Option kOptions[] = {
   {"last_fused_update_us", SE_GET(c->last_fused_us[2])},
   {"last_round_fused", SE_GET(c->last_round_fused)},
   {"last_round_stats_carried", SE_GET(c->last_round_carried)},
+  {"last_round_deferred", SE_GET(c->last_round_deferred)},
+  {"r_pending", SE_GET(c->gbm.r_pending)},
   {"last_ls_workers", SE_GET(c->last_ls_workers)},
   {"last_ls_passes", SE_GET(c->last_ls_passes)},
   {"last_ls_hit_ratio", SE_GET(0.0)},  // kept for compatibility: no L2 window is ever requested

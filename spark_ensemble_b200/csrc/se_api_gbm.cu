@@ -102,6 +102,7 @@ int se_gbm_configure(se_ctx* ctx, int64_t n_train, int64_t n_valid, int dim, int
   g.use_bag = false;
   g.r_current = false;
   g.sq_stats_current = false;
+  g.sq_defer_ok = false;
   g.wsum_valid = false; g.counts_valid = false;
   ctx->y_state[0] = ctx->y_state[1] = 0;
   SE_TRY(slot_alloc2d(ctx, SE_SLOT_Y, 1, n_train));
@@ -533,8 +534,16 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   // The update then walks its tiles opposite to the previous one, so that it starts on what is still in the L2.
   const bool stats_out = write_r && !loss_reduce;
   const bool carried = stats_out && g.r_current && g.sq_stats_current;
+  // Only a carried round reads a pending R (and applies its steps in registers); every other round reads it settled.
+  if (!carried) SE_TRY(settle_r(ctx));
   a.carried = carried ? 1 : 0;
   a.forward = (carried && !g.sq_last_up) ? 1 : 0;
+  // A carried round after another one whose R nobody read stores nothing (8 B/row, not 12) while fewer than
+  // sq_defer_max steps are pending; the round that would exceed the cap stores r' with all of them applied.  The
+  // first carried round over a direction stores: a caller that reads R after it pays no settle.
+  a.r_chain = ctx->d_rchain;
+  a.r_pending = carried ? g.r_pending : 0;
+  a.r_defer = (carried && g.sq_defer_ok && g.r_pending < ctx->sq_defer_max) ? 1 : 0;
   a.ws_next.partials = ctx->d_partials + (size_t)(kMaxGridPartials / 2) * 4;  // ws_b's, unused without a row-reduced loss
   a.ws_next.counter = &ctx->d_fsync->counter_b;
   a.ws_next.out = ctx->d_scal + kScalCarry;
@@ -571,6 +580,9 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
                                                            ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots));
   ctx->last_fused_grid = grid;
   ctx->last_round_carried = carried ? 1 : 0;
+  ctx->gbm.r_pending = a.r_defer ? a.r_pending + 1 : 0;  // the kernel ran: its step joined the chain or R was stored
+  ctx->gbm.sq_defer_ok = carried;
+  ctx->last_round_deferred = a.r_defer;
   ctx->last_fused_resident_tiles = resident_slots / 4.0;  // float4 groups per thread, U_SQ = 4 to a tile
   ctx->gbm.r_current = write_r != 0;
   const bool owed_before = ctx->gbm.f_owed;
@@ -616,6 +628,7 @@ int se_gbm_round(se_ctx* ctx, double learning_rate, int optimized, double tol, i
   SE_REQUIRE(ctx, ctx->gbm.on && ctx->gbm.dim == 1, SE_ERR_STATE, "se_gbm_round needs dim == 1");
   ctx->last_round_fused = 0;
   ctx->last_round_carried = 0;
+  ctx->last_round_deferred = 0;
   const bool sq_search = optimized && ctx->gbm.loss == SE_LOSS_SQUARED && !(flags & SE_UPD_NEWTON) && max_iter >= 1;
   if (sq_search) {
     // commons-math3 BrentOptimizer constructor checks (the host path performs them in brent_impl's caller)

@@ -59,10 +59,10 @@ int se_slot_info(const se_ctx* ctx, int slot, void** device_ptr, int64_t* count)
   if (device_ptr) {
     // the caller may read or write through the raw pointer
     se_ctx* mctx = const_cast<se_ctx*>(ctx);
-    const bool owed = ctx->gbm.f_owed;
+    const int64_t launches = ctx->launches;
     SE_TRY(write_slot(mctx, slot));
-    // F was just rebuilt: the caller's own stream may touch the slot next
-    if (owed && !ctx->gbm.f_owed) SE_CUDA(mctx, cudaStreamSynchronize(ctx->stream));
+    // F was just rebuilt or R settled: the caller's own stream may touch the slot next
+    if (ctx->launches != launches) SE_CUDA(mctx, cudaStreamSynchronize(ctx->stream));
     *device_ptr = ctx->slot[slot].d;
   }
   if (count) *count = ctx->slot[slot].rows * ctx->slot[slot].cols;

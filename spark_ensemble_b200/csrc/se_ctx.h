@@ -184,6 +184,11 @@ struct se_ctx {
     // residual fused round summed them over what it wrote.  Dropped by every write of Y, F, R or H.
     bool sq_stats_current = false;
     bool sq_last_up = false;  // the last fused round's update pass walked its tiles upwards (ended on the highest)
+    // SE_SLOT_R is pending: it holds an older r0, and the residual is r0 after the r_pending fp32 steps in d_rchain
+    // along H (carried rounds that stored nothing).  settle_r applies them; nothing else may touch R, or write H,
+    // while r_pending > 0.
+    int r_pending = 0;
+    bool sq_defer_ok = false;  // the last round was carried and R has not been read since: the next may defer
     double wsum = 0.0;
     bool wsum_valid = false;
     double n_global = 0.0, nv_global = 0.0;
@@ -245,6 +250,9 @@ struct se_ctx {
   int fused_loss_reduce = 0;          // 1: reduce the train loss over the rows even when the closed form applies
   int fused_timing = 0;               // diagnostic: in-kernel %globaltimer stamps of the fused round
   int fused_resident = 1;             // residual rounds reading r carry the statistics pass's tail in shared memory
+  // carried rounds leave at most this many steps pending on R before one stores it (0: every round stores r')
+  int sq_defer_max = 16;
+  se_host::DevBuf<float> d_rchain;    // the pending steps [kSqDeferMax]
   double last_fused_resident_tiles = 0.0;  // tiles per CTA the last fused round carried in shared memory
   double last_fused_us[3] = {0, 0, 0};  // statistics phase, fold+exchange+Brent, update phase
   int ls_mode = 1;                    // non-squared line search: 0 one launch per evaluation (round-1 kernels), 1 one
@@ -255,7 +263,7 @@ struct se_ctx {
   int clock_khz = 1965000;
   double peer_timeout_ms = 120000.0;  // spin bound of the fused peer exchange (0 = wait forever)
   // diagnostics of the last call (se_ctx_get_option)
-  int last_round_fused = 0, last_round_carried = 0, last_ls_workers = 0, last_ls_resident = 0, last_ls_passes = 0, last_fused_grid = 0;
+  int last_round_fused = 0, last_round_carried = 0, last_round_deferred = 0, last_ls_workers = 0, last_ls_resident = 0, last_ls_passes = 0, last_fused_grid = 0;
   double last_round_stats[3] = {0.0, 0.0, 0.0};
   // newton updates: SE_SLOT_WOUT holds 1/2 hc w; the 1/S_j of each dimension is applied on download
   std::vector<float> wout_scale;
@@ -393,6 +401,7 @@ se::RedWs red_ws(se_ctx* ctx, int out_offset = 0, bool exchange = true);
 int allreduce_dev(se_ctx* ctx, int off, int count, int op = kNcclSum);
 int check_labels(se_ctx* ctx);
 int fetch_scalars(se_ctx* ctx, int off, int count, double* out, int op = kNcclSum);
+int settle_r(se_ctx* ctx);
 int settle_f(se_ctx* ctx);
 int write_slot(se_ctx* ctx, int slot);
 int read_slot(se_ctx* ctx, int slot);

@@ -424,6 +424,33 @@ __global__ void __launch_bounds__(kBlock) settle_f_kernel(const float* __restric
   }
 }
 
+// R pending after carried squared-loss rounds: apply their fp32 steps in place, in the order the rounds took them,
+// with the fmaf each round's update applies (se_gbm_fused.cu) -- the r the last of them would have stored
+__global__ void __launch_bounds__(kBlock) settle_r_kernel(float* __restrict__ r, const float* __restrict__ h,
+                                                         const float* __restrict__ chain, int m, int64_t n) {
+  __shared__ float s_chain[kSqDeferMax];
+  for (int j = threadIdx.x; j < m; j += kBlock) s_chain[j] = chain[j];
+  __syncthreads();
+  const int64_t n4 = n >> 2;
+  for (int64_t g = (int64_t)blockIdx.x * kBlock + threadIdx.x; g < n4; g += (int64_t)gridDim.x * kBlock) {
+    float4 vr = ld_rw4(r + 4 * g);
+    const float4 vh = ld_stream4(h + 4 * g);
+    for (int j = 0; j < m; ++j) {
+      const float c = s_chain[j];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) f4at(vr, e) = fmaf(-c, f4at(vh, e), f4at(vr, e));
+    }
+    st_stream4(r + 4 * g, vr);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const int64_t i = (n4 << 2) + threadIdx.x;
+    const float hi = h[i];
+    float v = r[i];
+    for (int j = 0; j < m; ++j) v = fmaf(-s_chain[j], hi, v);
+    r[i] = v;
+  }
+}
+
 __global__ void sq_alpha_kernel(const double* stats, double* out) {
   const double s1 = stats[1], s2 = stats[2];
   double al = (s2 > 0.0) ? s1 / s2 : 1.0;
@@ -534,6 +561,13 @@ cudaError_t launch_gbm_pack_signed(const float* y, const float* F, const float* 
 
 cudaError_t launch_gbm_settle_f(const float* y, float* r, float* F, int64_t n, int sms, cudaStream_t st) {
   settle_f_kernel<<<grid_for(n >> 2, kBlock, 4, sms), kBlock, 0, st>>>(y, r, F, n);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_gbm_settle_r(float* r, const float* h, const float* chain, int m, int64_t n, int sms,
+                                cudaStream_t st) {
+  if (m < 1 || m > kSqDeferMax) return cudaErrorInvalidValue;
+  settle_r_kernel<<<grid_for(n >> 2, kBlock, 4, sms), kBlock, 0, st>>>(r, h, chain, m, n);
   return cudaGetLastError();
 }
 

@@ -17,6 +17,11 @@
 //    r' = (y - F) - c h, 16 B/row.  Without residual mode the update is F' = F + c h (F, y, h read; F written).
 //    A residual round without a bag also sums the statistics of (r', h) in its update pass; while R and H stay as
 //    it left them, the next round takes those sums and skips the statistics pass (12 B/row).
+//    Such a carried round may also leave R pending (se_api_ctx.cu settle_r): it stores nothing (8 B/row), and the
+//    Brent thread appends its fp32 step to a chain on the device.  The next carried round reads the older r0 and
+//    applies the chain in registers, t = fmaf(-c_j, h, t), before its own step -- the fmaf a storing round applies,
+//    so every r it sums its statistics over, and the r it stores when the chain reaches the context's cap, is the one
+//    the storing rounds would have left, bit for bit.
 //
 //  * gbm_linesearch_persist_kernel — Brent's <= MaxEval evaluations of the line-search objective
 //    (boosting/GBMLoss.scala:50-74 through RDDLossFunction; GBMRegressor.scala:408-421) for the non-squared scalar
@@ -86,6 +91,9 @@ __device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
   // MaxEval exceeded: the host reports SE_ERR_OPT and F must stay what it was (r - 0*h == r, F + 0*h == F; the host
   // does not mark F as owed)
   const double step = (rc == kBrentOk) ? a.lr * x : 0.0;
+  // a deferring round's step, as phase B rounds it, joins the pending chain (a 0 step too: fmaf(-0, h, r) is what
+  // the stored round applies)
+  if (a.r_defer) a.r_chain[a.r_pending] = (float)step;
   a.sync->x = step;
   st_release_gpu_u64(&a.sync->flag, a.epoch);  // the grid starts the update NOW; the host is served next
   if (a.timing) a.out[12] = global_timer_us();  // step published
@@ -131,6 +139,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   constexpr int U = U_SQ;
   extern __shared__ float4 s_res[];  // FROM_R, CARRIED: [slot][r, h][kBlock]
   __shared__ float s_coef;
+  __shared__ float s_chain[kSqDeferMax];  // CARRIED: the steps pending on the residual slot
   __shared__ float4 s_brent_regs[2 * U];  // FROM_R, CARRIED: the Brent thread's tile registers while it runs Brent
   const int64_t n4 = a.n >> 2;
   constexpr int64_t tile = (int64_t)kBlock * U;
@@ -201,7 +210,11 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     }
   };
 
+  // CARRIED: the pending steps, read before the Brent thread appends this round's (the barrier before phase B
+  // publishes them).  The count and the store flag are read from the kernel parameters where they are used: kept in
+  // registers they would spill.
   if constexpr (CARRIED) {
+    for (int j = threadIdx.x; j < a.r_pending; j += kBlock) s_chain[j] = a.r_chain[j];
     // the first tile into registers, the S groups after it into shared memory (each thread copies, and in phase B
     // reads back, only its own slots: no barrier)
     if (cnt > 0) load_tile(0);
@@ -330,10 +343,22 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   for (int64_t k = 0; k < cnt; ++k) {
     const int64_t i = up ? k : cnt - 1 - k;
     const int64_t base = (blockIdx.x + i * G) * tile + threadIdx.x;
+    if constexpr (CARRIED) {
+      // the pending steps, in the order the rounds took them: the r each of them would have stored and the next read
+      for (int j = 0; j < a.r_pending; ++j) {
+        const float c = s_chain[j];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) f4at(vy[u], e) = fmaf(-c, f4at(vh[u], e), f4at(vy[u], e));
+        }
+      }
+    }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
-      if (!ok[u]) continue;
       const int64_t g = base + (int64_t)u * kBlock;
+      // CARRIED: the bound is tested again rather than kept from the load, which leaves the chain's registers free
+      if (CARRIED ? g >= n4 : !ok[u]) continue;
       float4 o;
       float l_acc = 0.f, s0 = 0.f, s1 = 0.f, s2 = 0.f;
 #pragma unroll
@@ -357,8 +382,12 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
           s2 = fmaf(h, h, s2);
         }
       }
-      if (WRITE_R) st_stream4_p(a.r + 4 * g, o, pol_keep);  // the next statistics pass starts where this one ends
-      else st_stream4_p(a.F + 4 * g, o, pol_stream);
+      // the next statistics pass starts where this one ends; a deferring round stores nothing
+      if (WRITE_R) {
+        if (!CARRIED || !a.r_defer) st_stream4_p(a.r + 4 * g, o, pol_keep);
+      } else {
+        st_stream4_p(a.F + 4 * g, o, pol_stream);
+      }
       if (LOSS_REDUCE) accb[0] += (double)l_acc;
       if (STATS_OUT) accn[0] += (double)s0, accn[1] += (double)s1, accn[2] += (double)s2;
     }
@@ -368,8 +397,12 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     const int64_t j = (n4 << 2) + threadIdx.x;
     float d;
     if constexpr (WRITE_R) {
-      d = fmaf(-coef, a.h[j], from_r ? a.r[j] : a.y[j] - a.F[j]);
-      a.r[j] = d;
+      const float h = a.h[j];
+      float r = from_r ? a.r[j] : a.y[j] - a.F[j];
+      if constexpr (CARRIED)
+        for (int q = 0; q < a.r_pending; ++q) r = fmaf(-s_chain[q], h, r);
+      d = fmaf(-coef, h, r);
+      if (!CARRIED || !a.r_defer) a.r[j] = d;
     } else {
       const float p = fmaf(coef, a.h[j], a.F[j]);
       d = a.y[j] - p;
@@ -725,6 +758,9 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
       gbm_round_sq_fused_kernel<true, false, false, true>};
   const bool carried = a0.carried != 0;
   if (carried && !(write_r && !loss_reduce && a0.bag == nullptr)) return cudaErrorInvalidValue;
+  // only a carried round reads pending steps or defers its own, and the chain holds at most kSqDeferMax of them
+  if ((a0.r_pending || a0.r_defer) && !(carried && a0.r_chain)) return cudaErrorInvalidValue;
+  if (a0.r_pending < 0 || a0.r_pending + (a0.r_defer ? 1 : 0) > kSqDeferMax) return cudaErrorInvalidValue;
   const bool from_r = !carried && write_r && a0.stats_from_r && a0.bag == nullptr;
   const int which = carried ? 6 : from_r ? 4 + (loss_reduce ? 1 : 0) : (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
   // function attributes and occupancy are per DEVICE (a process may drive several GPUs, as in launch_ls)

@@ -58,6 +58,12 @@ cudaError_t launch_gbm_pack_signed(const float* y, const float* F, const float* 
 // squared loss, F owed after a residual-mode fused round: F = y - r, then r = y - F (the residual an update of that F
 // would have left), 16 B/row
 cudaError_t launch_gbm_settle_f(const float* y, float* r, float* F, int64_t n, int sms, cudaStream_t stream);
+// Most fp32 steps a carried squared-loss round may leave pending on the residual slot (SqRoundArgs::r_chain).
+constexpr int kSqDeferMax = 64;
+// squared loss, R pending after carried fused rounds: r = fmaf(-c_j, h, r) for j = 0..m-1 in place, 12 B/row -- the
+// values the rounds would have stored, bit for bit
+cudaError_t launch_gbm_settle_r(float* r, const float* h, const float* chain, int m, int64_t n, int sms,
+                                cudaStream_t stream);
 // LogLoss(K) for K > kMaxDim (se_gbm_generic.cu): coefficients, per-CTA partials [grid][K+1] and the K+1 sums live in
 // device buffers sized for K; the cross-GPU sum of `out` is an NCCL all-reduce issued by the caller
 struct GenericArgs {
@@ -109,6 +115,13 @@ struct SqRoundArgs {
   RedWs ws_next{};
   int carried = 0;  // 1: ws_next.out holds the statistics of (r, h): skip the statistics pass
   int forward = 0;  // carried round: walk the update's tiles upwards (the previous update ended on the lowest ones)
+  // Carried rounds only: the residual slot holds an older r0, and the logical r is r0 after the r_pending fp32 steps
+  // r_chain[0..r_pending) along h (t = fmaf(-c_j, h, t)).  The kernel applies them in registers before its own step.
+  // r_defer: store nothing; the Brent thread appends this round's step at r_chain[r_pending] (0 when MaxEval is
+  // exceeded).  Otherwise the round stores r' and the chain is empty afterwards.
+  float* r_chain = nullptr;
+  int r_pending = 0;
+  int r_defer = 0;
   double* out = nullptr;       // [0..2] statistics, [4] alpha, [5] objective, [6] +-evaluations, [8] Σloss
   double* host_res = nullptr;  // mapped host copy of out[0..6] (nullable)
   // loss-from-statistics mode: the Brent thread also serves the host (final value + ticket) before the update phase ends
