@@ -515,6 +515,27 @@ SE_API int se_logistic_loss_grad_batch(se_ctx* ctx, int src_slot, int n_members,
 SE_API int se_logistic_predict(se_ctx* ctx, int n_coef, const int32_t* subspace, int n_sets, const double* coef,
                                const double* intercept, double threshold, int raw_slot, int raw_row, int prob_slot,
                                int prob_row, int label_slot, int label_row);
+/* An ensemble of M = n_members linear and logistic members scored in ONE pass over X (which = 0: SE_SLOT_X, 1:
+ * SE_SLOT_VX), with what se_agg_configure + se_agg_run would write over SE_SLOT_P filled by se_logistic_predict per
+ * member: RAW, PROB and LABEL for the classifier kinds, row out_row of out_slot for the regressor kinds.  SE_SLOT_P is
+ * not allocated.  kind, num_classes, dim, loss, weights and init mean what they mean for se_agg_run (se_forest_agg for
+ * the GBM classifier's member_class).  Member m reads columns cols[col_offsets[m] .. col_offsets[m+1]) of X (its
+ * subspace, already mapped; 0..254 of them, repeats allowed) and has D = n_sets[m] coefficient sets: coef holds every
+ * member's [D][p] raw-space coefficients one member after another, intercept every member's [D] intercepts, threshold
+ * [M] the binomial members' thresholds (NULL: 0.5).  Its margins are se_logistic_predict's, and what it contributes:
+ *   GBM / Bagging regressor, Boosting mean and median, GBM classifier: its value (float) m_0 (D must be 1), summed as
+ *     se_agg_run sums (the mean kinds bit for bit, in fp32 batches folded into fp64; the median bit for bit, 1..
+ *     SE_FOREST_MEDIAN_MAX_TREES members), or w · value to class member_class[m] in fp64 (GBM classifier);
+ *   Bagging hard, SAMME: its label, σ(m) > threshold for D = 1, else the first argmax (D must be 1 or num_classes);
+ *   Bagging soft, SAMME.R: its probabilities as se_logistic_predict writes them (D = num_classes, or D = 1 with two
+ *     classes), or their lg2 max(p, EPSILON).
+ * The classifier kinds add every term in fp64 in model order and finish the rows with se_forest_agg's epilogue
+ * (2..SE_FOREST_AGG_MAX_CLASSES classes).  Fails with SE_ERR_ARG, naming the member, on a member with more than 254
+ * columns, a column outside X, a D the kind does not take, or more median members than the limit. */
+SE_API int se_linear_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, int loss, int n_members,
+                         const int32_t* col_offsets, const int32_t* cols, const int32_t* n_sets, const double* coef,
+                         const double* intercept, const double* threshold, const int32_t* member_class,
+                         const double* weights, const double* init, int out_slot, int out_row);
 
 #ifdef __cplusplus
 }

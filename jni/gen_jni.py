@@ -148,6 +148,12 @@ TABLE = [
                                                 ("rawSlot", "i32"), ("rawRow", "i32"), ("probSlot", "i32"), ("probRow", "i32"),
                                                 ("labelSlot", "i32"), ("labelRow", "i32")],
      "LogisticRegressionModel raw / probability / prediction over the resident feature matrix"),
+    ("linearAgg", "se_linear_agg", [("ctx", "ctx"), ("which", "i32"), ("kind", "i32"), ("numClasses", "i32"), ("dim", "i32"),
+                                    ("loss", "i32"), ("nMembers", "i32"), ("colOffsets", "in_i32"), ("cols", "in_i32"),
+                                    ("nSets", "in_i32"), ("coef", "in_f64"), ("intercept", "in_f64"), ("threshold", "in_f64"),
+                                    ("memberClass", "in_i32"), ("weights", "in_f64"), ("init", "in_f64"), ("outSlot", "i32"),
+                                    ("outRow", "i32")],
+     "an ensemble of linear and logistic members in one pass, with the aggregation's results and no member outputs"),
 ]
 
 # hand-written natives (bulk transfers, handles, byte arrays): scala signature + which ABI functions they cover

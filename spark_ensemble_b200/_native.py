@@ -127,6 +127,8 @@ PROTOTYPES = {
     "se_logistic_loss_grad": [_vp, _i32, _i32, _ip, _dp, _dp, _i32, _dp, _i32, _i32, _i32, _i32, _dp],
     "se_logistic_loss_grad_batch": [_vp, _i32, _i32, _ip, _ip, _dp, _dp, _i32, _dp, _i32, _i32, _i32, _i32, _dp],
     "se_logistic_predict": [_vp, _i32, _ip, _i32, _dp, _dp, _d, _i32, _i32, _i32, _i32, _i32, _i32],
+    "se_linear_agg": [_vp, _i32, _i32, _i32, _i32, _i32, _i32, _ip, _ip, _ip, _dp, _dp, _dp, _ip, _dp, _dp, _i32,
+                      _i32],
     "se_tree_fit_bins": [_vp, _i32, _ip, _fp],
     "se_tree_fit": [_vp, _i32, _i32, _i32, _i32, _i32, _ip, _i32, _i32, _i32, _d, _d, _i32, _i32, _i32,
                     _ip, _fp, _ip, _ip, _fp, _dp, C.POINTER(_i32)],

@@ -18,10 +18,10 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIB = os.path.join(LIBDIR, "libse_b200.so")
 SOURCES = ["se_api_ctx.cu", "se_api_slots.cu", "se_api_gbm.cu", "se_api_boost.cu", "se_api_trees.cu", "se_api_tree_fit.cu",
-           "se_gbm.cu", "se_gbm_tiled.cu", "se_gbm_fused.cu", "se_gbm_generic.cu", "se_boost.cu", "se_agg.cu", "se_models.cu", "se_tree_fit.cu", "se_linear_fit.cu", "se_logistic.cu", "se_util.cu"]
+           "se_gbm.cu", "se_gbm_tiled.cu", "se_gbm_fused.cu", "se_gbm_generic.cu", "se_boost.cu", "se_agg.cu", "se_models.cu", "se_tree_fit.cu", "se_linear_fit.cu", "se_logistic.cu", "se_linear_agg.cu", "se_util.cu"]
 # the device Brent must round every multiply and add separately to reproduce the host line search bit for bit
 EXTRA_FLAGS = {"se_gbm_fused.cu": ["-fmad=false"]}
-HEADERS = ["se_ctx.h", "se_common.cuh", "se_kernels.h", "se_loss.cuh", "se_tma.cuh", "se_brent.h", "se_sortnet.h", os.path.join("..", "..", "include", "se_abi.h")]
+HEADERS = ["se_ctx.h", "se_common.cuh", "se_kernels.h", "se_loss.cuh", "se_tma.cuh", "se_brent.h", "se_sortnet.h", "se_row_steps.cuh", os.path.join("..", "..", "include", "se_abi.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + [
     "-lineinfo", "-O3", "-std=c++17",

@@ -16,9 +16,9 @@ from .ensemble import DataFrame, fit_dummy_classifier, java_string_hash
 from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_classifier_params, shared_predictor_params, subbag_params)
-from .routes import (STACK_METHODS, bagging_fit, device_fit, device_trees, extract_instances, load_boosting,
-                     member_route, one_pass, resident_linear, split_validation, stacking_fit, stacking_predict,
-                     tree_list)
+from .routes import (STACK_METHODS, bagging_fit, device_fit, device_linear, device_trees, extract_instances,
+                     linear_kw, linear_list, load_boosting, member_route, one_pass, resident_linear, split_validation,
+                     stacking_fit, stacking_predict, tree_list)
 
 _CLS_LOSSES = ("logloss", "exponential", "bernoulli")  # GBMClassifier.scala:102-103
 _CLS_INIT = ("uniform", "prior")                        # :104-106
@@ -80,18 +80,41 @@ class _ClassifierModelBase(Params):
         return one_pass(self.device, X, trees, lambda ctx, t: ctx.forest_agg(kind, self.numClasses, t, **kw),
                         self._fetch)
 
+    def _linear_agg_resident(self, X, kind: int, members, **kw):
+        """Scores linear and logistic members in one pass over the device-resident features (se_linear_agg), with the
+        keyword arguments of _forest_agg_resident.  None without such members (device_linear) or above
+        FOREST_AGG_MAX_CLASSES classes: the caller scores member by member."""
+        if self.numClasses > N.FOREST_AGG_MAX_CLASSES:
+            return None
+        return one_pass(self.device, X, members,
+                        lambda ctx, mb: ctx.linear_agg(kind, self.numClasses, mb, **linear_kw(kw)), self._fetch)
+
+    def _one_pass(self, X):
+        """The tree route (se_forest_agg), then the linear route (se_linear_agg); None leaves the member route."""
+        kind, members, kw = self._forest_agg_args()
+        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
+        if out is None:
+            out = self._linear_agg_resident(X, kind, device_linear(self, members), **kw)
+        return out
+
     def _forest_agg_args(self):  # -> (kind, the members in forest order, keyword arguments of forest_agg)
         raise NotImplementedError
 
     def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
-        """A stacking member's meta-features over ctx's SLOT_X, on the device, when every member is a tree: one
-        se_forest_agg pass, then its probability (proba), raw (raw) or label rows are copied into out_slot from
-        out_row on.  False when the forest is outside se_forest_agg's reach."""
+        """A stacking member's meta-features over ctx's SLOT_X, on the device, when every member is a tree (one
+        se_forest_agg pass) or a linear or logistic model (one se_linear_agg pass): its probability (proba), raw (raw)
+        or label rows are then copied into out_slot from out_row on.  False when the members are outside both."""
         kind, members, kw = self._forest_agg_args()
-        trees = tree_list(members) if members else None
-        if trees is None or self.numClasses > N.FOREST_AGG_MAX_CLASSES:
+        if not members or self.numClasses > N.FOREST_AGG_MAX_CLASSES:
             return False
-        ctx.forest_agg(kind, self.numClasses, trees, **kw)
+        trees = tree_list(members)
+        lin = linear_list(members) if trees is None else None
+        if trees is not None:
+            ctx.forest_agg(kind, self.numClasses, trees, **kw)
+        elif lin is not None:
+            ctx.linear_agg(kind, self.numClasses, lin, **linear_kw(kw))
+        else:
+            return False
         src, count = {"proba": (N.SLOT_PROB, self._out_classes), "raw": (N.SLOT_RAW, self._out_classes)}.get(
             method, (N.SLOT_LABEL, 1))
         ctx.copy_rows(out_slot, out_row, src, 0, count)
@@ -193,8 +216,7 @@ class GBMClassificationModel(_ClassifierModelBase):
 
     def _raw_prob_label(self, X):
         n, M, dim = X.shape[0], self.numModels, self.dim
-        kind, members, kw = self._forest_agg_args()
-        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
+        out = self._one_pass(X)
         if out is not None:
             return out
         P = np.zeros((max(M, 1), dim, n), dtype=np.float32)
@@ -317,10 +339,10 @@ class BoostingClassificationModel(_ClassifierModelBase):
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         real = self("algorithm").lower() == "real"
-        kind, members, kw = self._forest_agg_args()
-        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
+        out = self._one_pass(X)
         if out is not None:
             return out
+        kind = self._forest_agg_args()[0]
         if real:
             P = np.zeros((max(M, 1), K, n), dtype=np.float32)
             for i, m in enumerate(self.models):
@@ -389,10 +411,10 @@ class BaggingClassificationModel(_ClassifierModelBase):
     def _raw_prob_label(self, X):
         n, M, K = X.shape[0], self.numModels, self.numClasses
         soft = self("votingStrategy").lower() == "soft"
-        kind, members, kw = self._forest_agg_args()
-        out = self._forest_agg_resident(X, kind, device_trees(self, members), **kw)
+        out = self._one_pass(X)
         if out is not None:
             return out
+        kind = self._forest_agg_args()[0]
         P = np.zeros((M, K, n) if soft else (M, n), dtype=np.float32)
         for i, m in enumerate(self.models):
             Xs = X[:, self.subspaces[i]]

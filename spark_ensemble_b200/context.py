@@ -451,6 +451,47 @@ class Context:
                                          None if p is None else N.fptr(p), None if cls is None else N.iptr(cls),
                                          None if w is None else N.dptr(w), None if ini is None else N.dptr(ini)))
 
+    def linear_agg(self, kind: int, num_classes: int, members, out_slot: int = -1, out_row: int = 0, weights=None,
+                   init=None, member_class=None, dim: int = 1, loss=0, validation: bool = False, subspaces=None):
+        """An ensemble of linear and logistic members scored in one pass over the resident feature matrix
+        (se_linear_agg): RAW, PROB and LABEL as agg_configure + agg_run lay them out for a classifier kind, row out_row
+        of out_slot for a regressor kind, with no member-output matrix.  members are dicts {coef [D][p], intercept [D],
+        threshold} (margin_arrays()); `subspaces[m]` maps member m's columns to columns of X (None: 0..p-1)."""
+        offs = np.zeros(len(members) + 1, dtype=np.int32)
+        cols, coefs, icpts, sets, thr = [], [], [], [], []
+        for i, mb in enumerate(members):
+            th = np.atleast_2d(np.asarray(mb["coef"], dtype=np.float64))
+            D, p = th.shape
+            sub = subspaces[i] if subspaces is not None and subspaces[i] is not None else np.arange(p)
+            sub = np.asarray(sub, dtype=np.int32).reshape(-1)
+            if sub.size != p:
+                raise ValueError(f"member {i}: one column per coefficient")
+            b = np.asarray(mb["intercept"], dtype=np.float64).reshape(-1)
+            if b.size != D:
+                raise ValueError(f"member {i}: one intercept per coefficient set")
+            offs[i + 1] = offs[i] + p
+            cols.append(sub)
+            coefs.append(th.reshape(-1))
+            icpts.append(b)
+            sets.append(D)
+            thr.append(float(mb.get("threshold", 0.5)))
+        c = np.ascontiguousarray(np.concatenate(cols) if cols else np.zeros(0), dtype=np.int32)
+        th = np.ascontiguousarray(np.concatenate(coefs) if coefs else np.zeros(0), dtype=np.float64)
+        b = np.ascontiguousarray(np.concatenate(icpts) if icpts else np.zeros(0), dtype=np.float64)
+        ns, t = np.asarray(sets, dtype=np.int32), np.asarray(thr, dtype=np.float64)
+        w = None if weights is None else np.ascontiguousarray(weights, dtype=np.float64).reshape(-1)
+        if w is not None and w.size != len(members):
+            raise ValueError("one weight per member")
+        cls = None if member_class is None else np.ascontiguousarray(member_class, dtype=np.int32)
+        ini = None if init is None else np.ascontiguousarray(np.atleast_1d(init), dtype=np.float64)
+        lid = N.LOSS[loss] if isinstance(loss, str) else int(loss)
+        self._ck(self._lib.se_linear_agg(self._h, int(validation), int(kind), int(num_classes), int(dim), lid,
+                                         len(members), N.iptr(offs), N.iptr(c) if c.size else None,
+                                         N.iptr(ns) if ns.size else None, N.dptr(th) if th.size else None,
+                                         N.dptr(b) if b.size else None, N.dptr(t) if t.size else None,
+                                         None if cls is None else N.iptr(cls), None if w is None else N.dptr(w),
+                                         None if ini is None else N.dptr(ini), int(out_slot), int(out_row)))
+
     def linear_predict(self, coef, intercept: float, out_slot: int, out_row: int = 0,
                        validation: bool = False, subspace=None):
         c = np.ascontiguousarray(coef, dtype=np.float32)

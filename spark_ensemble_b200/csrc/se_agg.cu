@@ -15,19 +15,13 @@
 #include "se_loss.cuh"
 #include "se_tma.cuh"
 #include "se_sortnet.h"
+#include "se_row_steps.cuh"
 #include <type_traits>
 #include "../../include/se_abi.h"
 
 namespace se {
 
 namespace {
-
-constexpr float kSparkEps = 2.220446049250313e-16f;
-constexpr int MU = 8;  // models loaded per batch: 8 independent 16 B requests per thread
-
-// lg2 max(p, ε): the clamp is the exact constant lg2 2^-52 = -52 (NaN clamps too), so the sums of pure-leaf outputs
-// (exact 0s and 1s) are exact multiples of 52 and equal vote counts give equal totals
-__device__ __forceinline__ float lg2_clamped(float p) { return (p > kSparkEps) ? lg2_approx(p) : -52.0f; }
 
 // out[c][i] = init_c + Σ_m a[m][c] · f(P[m][c][i]),  f = identity
 // P row (m,c) lives at P + (cols ? cols[m] : m*width + c) * ld.
@@ -83,12 +77,8 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
             s.z = fmaf(wv[u], x.z, s.z); s.w = fmaf(wv[u], x.w, s.w);
           }
         }
-        if (wide) {
-          d0 += (double)(s0.x + s1.x); d1 += (double)(s0.y + s1.y);
-          d2 += (double)(s0.z + s1.z); d3 += (double)(s0.w + s1.w);
-        } else {
-          carry.x += s0.x + s1.x; carry.y += s0.y + s1.y; carry.z += s0.z + s1.z; carry.w += s0.w + s1.w;
-        }
+        agg_fold_batch(wide, s0.x + s1.x, d0, carry.x); agg_fold_batch(wide, s0.y + s1.y, d1, carry.y);
+        agg_fold_batch(wide, s0.z + s1.z, d2, carry.z); agg_fold_batch(wide, s0.w + s1.w, d3, carry.w);
       }
       if constexpr (LOGP) {
         const float4 hi = make_float4((float)d0, (float)d1, (float)d2, (float)d3);
@@ -97,11 +87,9 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
                                                             (float)(d2 - (double)hi.z), (float)(d3 - (double)hi.w)));
         continue;
       }
-      if (!wide) { d0 = (double)carry.x; d1 = (double)carry.y; d2 = (double)carry.z; d3 = (double)carry.w; }
       const double b = init ? (double)init[c] : 0.0;
-      d0 += b; d1 += b; d2 += b; d3 += b;
-      if (post_div != 0.f) { const double pd = (double)post_div; d0 /= pd; d1 /= pd; d2 /= pd; d3 /= pd; }
-      const float4 r = make_float4((float)d0, (float)d1, (float)d2, (float)d3);
+      const float4 r = make_float4(agg_fold_end(wide, d0, carry.x, b, post_div), agg_fold_end(wide, d1, carry.y, b, post_div),
+                                   agg_fold_end(wide, d2, carry.z, b, post_div), agg_fold_end(wide, d3, carry.w, b, post_div));
       st_stream4(out + c * ld_out + 4 * g, r);
     }
   }
@@ -114,7 +102,8 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
       for (int m = 0; m < M; ++m) {
         const int64_t rowi = cols ? (int64_t)cols[m] : (int64_t)m * width + c;
         const float x = P[rowi * ld + i];
-        sd += LOGP ? (double)lg2_clamped(x) : (double)((a ? a[(int64_t)m * width + c] : 1.0f) * x);
+        if (LOGP) sd += (double)lg2_clamped(x);
+        else agg_tail_add(sd, a ? a[(int64_t)m * width + c] : 1.0f, x);
       }
       if (LOGP) {
         out[c * ld_out + i] = (float)sd;
@@ -124,84 +113,6 @@ __global__ void __launch_bounds__(kBlock) agg_sum_kernel(const float* __restrict
       if (post_div != 0.f) sd /= (double)post_div;
       out[c * ld_out + i] = (float)sd;
     }
-  }
-}
-
-// Per-row epilogue on the C per-class sums t_c (from shared memory or from the RAW slot): raw, prob, label.
-struct FinArgs {
-  int kind, C, K, dim, loss, M;
-  double sum_a;  // Σ a_m (boosting discrete)
-  int64_t n, ld;
-  float* raw;
-  float* prob;
-  float* label;
-  int* bad_label;  // raised when a vote is not a class index in [0, K)
-  double inv_km1;  // 1 / (K - 1)
-};
-
-// raw value from the stage-1 sum.  Discrete: K·A_k − Σa subtracts nearly equal numbers and is formed in fp64 before
-// the single rounding to the fp32 output.  (SAMME.R has its own epilogue, finalize_real_row.)
-template <class T>
-__device__ __forceinline__ float fin_raw(const FinArgs& f, T t, float mean_t) {
-  switch (f.kind) {
-    case SE_AGG_BOOSTING_DISCRETE:  // +a on the vote, −a/(K-1) elsewhere   :371-376
-      return (float)(((double)t * (double)f.K - f.sum_a) * f.inv_km1);  // one reciprocal instead of an fp64 division per class
-    default: return (float)t;
-  }
-}
-
-// SAMME.R epilogue.  get(c) returns T_c = Σ_m lg2 max(p_mc, ε) in fp64 (exact for pure leaves).  With L = T ln 2:
-// raw_c = (K-1)(L_c − mean L) (BoostingClassifier.scala:355-360) and prob = softmax(raw/(K-1)) = 2^(T_c − T_max) / Σ
-// (:342-346), formed from the fp64 differences, not from the rounded raw (|raw| reaches (K-1)·36·M, where one fp32 ulp
-// of raw is already 1e-5 of a probability).  First-maximum argmax of T, which orders the classes as raw does.
-// Three sweeps over the classes, each reading get(c) again: the third overwrites what the stage-1 sums were read from.
-template <class Get>
-__device__ __forceinline__ void finalize_real_row(const FinArgs& f, int64_t i, Get get) {
-  const int C = f.C;
-  double s = 0.0, tmax = -INFINITY;
-  int am = 0;
-  for (int c = 0; c < C; ++c) {
-    const double t = get(c);
-    s += t;
-    if (t > tmax) tmax = t, am = c;  // Vector.argmax: first maximum
-  }
-  const double mean = s / (double)C;
-  const double rs = (double)(f.K - 1) * 0.6931471805599453;
-  float ssum = 0.f;
-  for (int c = 0; c < C; ++c) ssum += ex2_approx((float)(get(c) - tmax));
-  const float inv = 1.0f / ssum;
-  for (int c = 0; c < C; ++c) {
-    const double t = get(c);
-    f.prob[c * f.ld + i] = ex2_approx((float)(t - tmax)) * inv;
-    f.raw[c * f.ld + i] = (float)(rs * (t - mean));
-  }
-  f.label[i] = (float)am;
-}
-
-// get(c) returns the stage-1 sum of class c for this row.  Two sweeps over the classes: (1) raw values with an
-// online max / Σexp / first-argmax, (2) write raw and probability.
-template <class Get>
-__device__ __forceinline__ void finalize_row(const FinArgs& f, int64_t i, Get get) {
-  const int C = f.C;
-  const float mean_t = 0.f;
-  const bool softmax = (f.kind == SE_AGG_BOOSTING_DISCRETE || f.kind == SE_AGG_GBM_CLASSIFIER);
-  // boosting: softmax(raw/(K-1)) (BoostingClassifier.scala:342-346); GBM logloss: softmax(raw) (GBMLoss.scala:258-261)
-  const float sc = (f.kind == SE_AGG_GBM_CLASSIFIER) ? kLog2e : kLog2e / (float)(f.K - 1);
-  float best = -INFINITY, ssum = 0.f;
-  int am = 0;
-  for (int c = 0; c < C; ++c) {
-    const float r = fin_raw(f, get(c), mean_t);
-    if (r > best) am = c;  // Vector.argmax: first maximum
-    const float mn = fmaxf(best, r);
-    if (softmax) ssum = fmaf(ssum, ex2_approx((best - mn) * sc), ex2_approx((r - mn) * sc));
-    best = mn;
-  }
-  f.label[i] = (float)am;
-  const float inv = softmax ? rcp_approx(ssum) : 1.0f / (float)f.M;  // bagging: prob = raw·(1/M) (BaggingClassifier.scala:285-287)
-  for (int c = 0; c < C; ++c) {
-    const float r = fin_raw(f, get(c), mean_t);
-    f.prob[c * f.ld + i] = softmax ? ex2_approx((r - best) * sc) * inv : r * inv;
-    f.raw[c * f.ld + i] = r;
   }
 }
 
@@ -609,24 +520,6 @@ __global__ void __launch_bounds__(32) agg_class_tile_kernel(const ClassTileArgs 
   }
 }
 
-// Binary GBM classifier with dim 1 (GBMClassifier.scala:583-584 + GBMLoss.scala:284-289,311-316): raw = (−F, F) from
-// the one total F = res.
-__device__ __forceinline__ void finalize_binary_row(const FinArgs& f, int64_t i, float res) {
-  const float r0 = -res;
-  // p1 = 1/(1+e^x), p0 = 1 - p1 with x = raw(0) (bernoulli) or -2 raw(0) (exponential); both
-  // formed from t = e^-|x| so the small one keeps full relative precision
-  const float x = (f.loss == SE_LOSS_EXPONENTIAL) ? -2.0f * r0 : r0;
-  const float t = exp_neg_fast(-fabsf(x));
-  const float inv = rcp_approx(1.0f + t);
-  const float p1 = (x >= 0.f) ? t * inv : inv;
-  const float p0 = (x >= 0.f) ? inv : t * inv;
-  f.raw[i] = r0;
-  f.raw[f.ld + i] = res;
-  f.prob[i] = p0;
-  f.prob[f.ld + i] = p1;
-  f.label[i] = (res > r0) ? 1.0f : 0.0f;  // argmax, first maximum on ties
-}
-
 // Stage 2 for the sum-based kinds: per-row epilogue on tmp[C][n] (in RAW) -> raw, prob, label.
 __global__ void __launch_bounds__(kBlock) agg_finalize_kernel(const FinArgs f) {
   for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < f.n;
@@ -651,14 +544,6 @@ __global__ void __launch_bounds__(kBlock) agg_finalize_kernel(const FinArgs f) {
 // whole warp, O(M log² M) compare-exchanges instead of the O(M²) threshold scan it replaces (far from the HBM
 // roofline because per-lane pruning diverges).  Total and running sums are then accumulated in fp64 in
 // sorted order, exactly like the reference.
-__device__ __forceinline__ uint32_t wm_key(float x) {
-  const uint32_t u = __float_as_uint(x + 0.0f);  // -0 -> +0: equal values stay ties
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float wm_unkey(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 template <int T>
 __global__ void __launch_bounds__(T) agg_wmedian_kernel(const float* __restrict__ P, int64_t n, int64_t ld, int M,
                                                        int Mp, const double* __restrict__ a,
@@ -770,35 +655,6 @@ __global__ void __launch_bounds__(32 * kWmWarps) agg_wmedian_warp_kernel(const f
   }
 }
 
-// sort of the (key, model) words + the reference's sorted-order cumulative sums (ensemble/Utils.scala:31-38)
-template <int MP>
-__device__ __forceinline__ unsigned long long wm_exact_pick(unsigned long long (&w)[MP], int M, const double* s_a) {
-  sortnet_oddeven<MP>(w, [](unsigned long long& x, unsigned long long& y) {
-    const bool swap = x > y;
-    const unsigned long long lo = swap ? y : x, hi = swap ? x : y;
-    x = lo;
-    y = hi;
-  });
-  double total = 0.0;
-#pragma unroll
-  for (int m = 0; m < MP; ++m)
-    if (m < M) total += s_a[(unsigned)w[m]];
-  const double half = 0.5 * total;
-  double cum = 0.0;
-  bool found = false;
-  unsigned long long pick = 0ull;
-#pragma unroll
-  for (int m = 0; m < MP; ++m) {
-    if (m < M) {
-      cum += s_a[(unsigned)w[m]];
-      const bool hit = !found && (cum >= half);
-      pick = (hit || (!found && m == M - 1)) ? w[m] : pick;  // last element when nothing reaches half (NaN weights)
-      found = found || hit;
-    }
-  }
-  return pick;
-}
-
 // Same algorithm with the row's words in REGISTERS (Mp <= 64): the network is fully unrolled, so every
 // compare-exchange is ~6 ALU instructions and no memory traffic — the shared-memory form above moves 32 B per
 // compare-exchange and thread and is bound by shared-memory bandwidth.
@@ -845,78 +701,6 @@ __global__ void __launch_bounds__(128) agg_wmedian_reg_kernel(const __grid_const
     const unsigned long long pick = wm_exact_pick<MP>(w, M, s_a);
     if (in) out[row] = wm_unkey((uint32_t)(pick >> 32));
   }
-}
-
-// ---- weighted median, fast path (M <= 64, all weights finite and >= 0) -------------------------------------------
-// The exact kernels above carry (key, model) words through the sort because the reference accumulates the weights in
-// SORTED order (ensemble/Utils.scala:31-38) — 6 ALU-pipe instructions per compare-exchange, and the ALU pipe issues at
-// half rate.  With weights >= 0 the answer is `the smallest value v whose group-end
-// cumulative weight C(v) reaches h = total / 2` (cumulative sums are monotone in fp64 too).  C(v) and h are recursive
-// fp64 sums of the same addends as Ĉ(v) = Σ_{x_j <= v} a_j and ĥ = T̂ / 2 taken in MODEL order, so
-//     |(C(v) - h) - (Ĉ(v) - ĥ)| <= 3 (M - 1) 2^-53 T (1 + eps)
-// and whenever both neighbours of the crossing clear the margin tau = 8 M 2^-53 T̂ the model-order decision IS the
-// reference's decision.  So: sort the 32-bit keys alone (min/max, 2 instructions per compare-exchange, Batcher's
-// 191-element network), bisect the sorted keys on Ĉ (5 x 32 predicated DADDs with the weights as constant-bank
-// operands), and send the rows that do not clear the margin — none for generic weights, the exact ties for
-// small-integer weights — to the exact kernel through a compacted list (mode 2: all weights equal, where both orders
-// produce the same sums and no margin is needed).
-struct WmWeights {
-  double w[64];
-};
-
-template <int MP, int L>
-__device__ __forceinline__ uint32_t wm_candidate(const uint32_t (&s)[MP], uint32_t t) {
-  // level-L bisection probe: position step - 1 + t * 2 * step, t in [0, 2^L) — a select tree over static indices
-  constexpr int step = MP >> (L + 1);
-  uint32_t v = s[step - 1];
-#pragma unroll
-  for (int q = 1; q < (1 << L); ++q) v = (t == (uint32_t)q) ? s[step - 1 + q * 2 * step] : v;
-  return v;
-}
-
-// The fast path's pick for a row of keys key[0..MP) in model order (padding keys ~0u carry weight 0): the smallest key
-// whose model-order cumulative weight reaches half the total.  safe: the crossing clears the margin tau on both sides,
-// so the reference's sorted-order sums pick the same key.  w is a __grid_constant__ parameter: the DFMAs of the
-// bisection read the weights as constant-bank operands.
-template <int MP>
-__device__ __forceinline__ uint32_t wm_fast_pick(const uint32_t (&key)[MP], const double (&w)[64], double total,
-                                                 double tau, bool& safe) {
-  constexpr int LOG = (MP == 1) ? 0 : (MP == 2) ? 1 : (MP == 4) ? 2 : (MP == 8) ? 3 : (MP == 16) ? 4 : (MP == 32) ? 5 : 6;
-  uint32_t s[MP];
-#pragma unroll
-  for (int m = 0; m < MP; ++m) s[m] = key[m];
-  sortnet_oddeven<MP>(s, [](uint32_t& x, uint32_t& y) {
-    const uint32_t lo = min(x, y), hi = max(x, y);
-    x = lo;
-    y = hi;
-  });
-  const double half = 0.5 * total;
-  // invariant: P(lo) false, P(hi) true with P(k) := Ĉ(s[k]) >= ĥ; lo = t - 1, hi = t after LOG probes
-  uint32_t t = 0, v_hi = s[MP - 1];
-  double c_lo = 0.0, c_hi = total;
-  auto probe = [&](uint32_t v) {
-    double c = 0.0;
-#pragma unroll
-    for (int m = 0; m < MP; ++m) {
-      // model order; padding (and m >= M) weights are 0.  fma(w, 1.0 or 0.0, c) is c + w rounded once, or c: one
-      // select of the high word of the 0/1 factor instead of the two selects `if (...) c += w` compiles to
-      const double b = __hiloint2double((key[m] <= v) ? 0x3ff00000 : 0, 0);
-      c = fma(w[m], b, c);
-    }
-    const bool right = !(c >= half);
-    c_lo = right ? c : c_lo;
-    c_hi = right ? c_hi : c;
-    v_hi = right ? v_hi : v;
-    t = 2u * t + (right ? 1u : 0u);
-  };
-  if constexpr (LOG > 0) probe(wm_candidate<MP, 0>(s, t));
-  if constexpr (LOG > 1) probe(wm_candidate<MP, 1>(s, t));
-  if constexpr (LOG > 2) probe(wm_candidate<MP, 2>(s, t));
-  if constexpr (LOG > 3) probe(wm_candidate<MP, 3>(s, t));
-  if constexpr (LOG > 4) probe(wm_candidate<MP, 4>(s, t));
-  if constexpr (LOG > 5) probe(wm_candidate<MP, 5>(s, t));
-  safe = (c_hi - half > tau) && (half - c_lo > tau);
-  return v_hi;
 }
 
 template <int MP>
@@ -1190,33 +974,8 @@ __global__ void __launch_bounds__(kForestMedianTile, 1) forest_median_kernel(con
       forest_walk<TILE>(s_nodes, s_toff, ch.T, myr + ch.blob_bytes,
                         [&](int t, int leaf) { v[t * TILE] = s_val[s_toff[t] + leaf]; });
     }
-    // agg_wmedian_fast_kernel's pick (wm_fast_pick) on the row's values (modes 1 and 2)
-    uint32_t pick = 0;
-    bool exact = (g.mode == 0);
-    if constexpr (MP == 1) {  // one tree: both routes return its value (one weight is always "all equal": no margin)
-      pick = wm_key(vals[0]);
-      exact = false;
-    } else if (in && g.mode != 0) {
-      uint32_t key[MP];
-#pragma unroll
-      for (int m = 0; m < MP; ++m) {
-        key[m] = 0xFFFFFFFFu;  // padding sorts last and carries weight 0
-        if (m < M) key[m] = wm_key(vals[m * TILE]);
-      }
-      bool safe;
-      pick = wm_fast_pick<MP>(key, g.w, g.total, g.tau, safe);
-      exact = (g.mode == 1) && !safe;
-    }
-    // the exact (key, model) sort and sorted-order sums, as agg_wmedian_list_kernel / agg_wmedian_reg_kernel
-    if (in && exact) {
-      unsigned long long w[MP];
-#pragma unroll
-      for (int m = 0; m < MP; ++m) {
-        w[m] = ~0ull;
-        if (m < M) w[m] = ((unsigned long long)wm_key(vals[m * TILE]) << 32) | (unsigned long long)(unsigned)m;
-      }
-      pick = (uint32_t)(wm_exact_pick<MP>(w, M, s_a) >> 32);
-    }
+    bool exact;
+    const uint32_t pick = wm_pick_row<MP>(vals, TILE, M, g.mode, g.w, g.total, g.tau, s_a, in, exact);
     if (in) g.out[row] = wm_unkey(pick);
     if (g.mode == 1 && g.deferred != nullptr) {  // rows inside the margin, for se_ctx_get_option("last_wm_deferred")
       const unsigned mask = __ballot_sync(0xffffffffu, in && exact);

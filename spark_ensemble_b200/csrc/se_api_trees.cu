@@ -881,3 +881,130 @@ int se_logistic_predict(se_ctx* ctx, int n_coef, const int32_t* subspace, int n_
   SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_logistic_predict(a, ctx->sms, ctx->stream));
   return end(ctx);
 }
+
+// An ensemble of linear and logistic members in one pass over X with se_agg_run's results (see se_abi.h).
+int se_linear_agg(se_ctx* ctx, int which, int kind, int num_classes, int dim, int loss, int n_members,
+                  const int32_t* col_offsets, const int32_t* cols, const int32_t* n_sets, const double* coef,
+                  const double* intercept, const double* threshold, const int32_t* member_class,
+                  const double* weights, const double* init, int out_slot, int out_row) {
+  if (!ctx || !col_offsets || !n_sets || !intercept) return fail(ctx, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, kind >= SE_AGG_GBM_REGRESSOR && kind <= SE_AGG_BOOSTING_REG_MEAN, SE_ERR_ARG, "bad kind %d", kind);
+  SE_REQUIRE(ctx, n_members >= 1 && n_members <= (1 << 20), SE_ERR_ARG, "bad member count %d", n_members);
+  const bool median = (kind == SE_AGG_BOOSTING_REG_MEDIAN);
+  const bool reg = median || kind == SE_AGG_GBM_REGRESSOR || kind == SE_AGG_BAGGING_REGRESSOR ||
+                   kind == SE_AGG_BOOSTING_REG_MEAN;
+  const bool gbm = (kind == SE_AGG_GBM_CLASSIFIER);
+  const bool vec = (kind == SE_AGG_BAGGING_SOFT || kind == SE_AGG_BOOSTING_REAL);
+  const bool value = reg || gbm;  // the member's output is its value: one margin
+  SE_REQUIRE(ctx, !median || n_members <= SE_FOREST_MEDIAN_MAX_TREES, SE_ERR_ARG,
+             "the weighted median serves 1..%d members, got %d: evaluate the members with se_logistic_predict + "
+             "se_agg_run", SE_FOREST_MEDIAN_MAX_TREES, n_members);
+  if (!reg)
+    SE_REQUIRE(ctx, num_classes >= 2 && num_classes <= SE_FOREST_AGG_MAX_CLASSES, SE_ERR_ARG,
+               "se_linear_agg's classifier kinds support 2..%d classes, got %d", SE_FOREST_AGG_MAX_CLASSES, num_classes);
+  if (gbm) {
+    SE_REQUIRE(ctx, dim >= 1 && dim <= SE_FOREST_AGG_MAX_CLASSES && (dim > 1 || num_classes == 2), SE_ERR_ARG,
+               "bad dim %d for %d classes", dim, num_classes);
+    SE_REQUIRE(ctx, member_class, SE_ERR_ARG, "the GBM classifier needs member_class");
+  }
+  SE_REQUIRE(ctx, weights || !(kind == SE_AGG_GBM_REGRESSOR || gbm || kind == SE_AGG_BOOSTING_DISCRETE || median ||
+                               kind == SE_AGG_BOOSTING_REG_MEAN),
+             SE_ERR_ARG, "weights required for aggregation kind %d", kind);
+  const SlotBuf& X = ctx->slot[which ? SE_SLOT_VX : SE_SLOT_X];
+  SE_REQUIRE(ctx, X.d && X.cols > 0, SE_ERR_STATE, "feature matrix slot not allocated");
+  SE_REQUIRE(ctx, col_offsets[0] == 0, SE_ERR_ARG, "col_offsets[0] must be 0");
+  SE_REQUIRE(ctx, !reg || out_slot != (which ? SE_SLOT_VX : SE_SLOT_X), SE_ERR_ARG,
+             "the output row cannot be a row of the feature matrix the members read");
+  std::vector<LinearAggMember> mem((size_t)n_members);
+  int max_d = 1;
+  int64_t n_coef = 0, n_icpt = 0;
+  for (int m = 0; m < n_members; ++m) {
+    const int64_t p = (int64_t)col_offsets[m + 1] - col_offsets[m];
+    const int D = n_sets[m];
+    SE_REQUIRE(ctx, p >= 0 && p <= kLinearAggMaxCols, SE_ERR_ARG, "member %d: %lld columns (0..%d supported)", m,
+               (long long)p, kLinearAggMaxCols);
+    SE_REQUIRE(ctx, p == 0 || cols, SE_ERR_ARG, "null argument");
+    SE_REQUIRE(ctx, value ? D == 1 : (D == 1 || D == num_classes), SE_ERR_ARG,
+               "member %d: %d coefficient sets where %s", m, D, value ? "this kind takes the value of one" : "1 or K are");
+    SE_REQUIRE(ctx, !vec || D > 1 || num_classes == 2, SE_ERR_ARG,
+               "member %d: a binomial member gives 2 probabilities, not %d", m, num_classes);
+    for (int64_t j = col_offsets[m]; j < col_offsets[m + 1]; ++j)
+      SE_REQUIRE(ctx, cols[j] >= 0 && cols[j] < X.rows, SE_ERR_ARG, "member %d: column %d outside X with %lld columns",
+                 m, cols[j], (long long)X.rows);
+    if (gbm)
+      SE_REQUIRE(ctx, member_class[m] >= 0 && member_class[m] < dim, SE_ERR_ARG, "member %d: class %d outside [0, %d)",
+                 m, member_class[m], dim);
+    LinearAggMember& mb = mem[(size_t)m];
+    mb.col0 = col_offsets[m]; mb.p = (int)p; mb.D = D; mb.cls = gbm ? member_class[m] : 0;
+    mb.coef0 = (int)n_coef;
+    n_coef += (int64_t)D * p;
+    mb.icpt0 = (int)n_icpt;  // moved past the coefficients below
+    n_icpt += D;
+    mb.threshold = threshold ? threshold[m] : 0.5;
+    // the weights as se_agg_run takes them: fp32 for the sums and the SAMME votes, fp64 for the GBM classifier
+    const bool sum_w = (kind == SE_AGG_GBM_REGRESSOR || kind == SE_AGG_BOOSTING_REG_MEAN);
+    mb.wf = sum_w ? (float)weights[m] : 1.f;
+    mb.w = kind == SE_AGG_BOOSTING_DISCRETE ? (double)(float)weights[m] : gbm ? weights[m] : 1.0;
+    max_d = std::max(max_d, D);
+  }
+  SE_REQUIRE(ctx, n_coef == 0 || coef, SE_ERR_ARG, "null argument");
+  SE_REQUIRE(ctx, n_coef + n_icpt <= (int64_t)1 << 28, SE_ERR_ARG, "%lld coefficients: too many",
+             (long long)(n_coef + n_icpt));
+  for (LinearAggMember& mb : mem) mb.icpt0 += (int)n_coef;
+  const int64_t n = X.cols;
+  SE_TRY(begin(ctx));
+  LinearAggArgs g;
+  g.kind = kind; g.K = num_classes; g.M = n_members; g.loss = loss;
+  g.dim = gbm ? dim : 1;
+  g.C = reg ? 1 : gbm ? dim : num_classes;
+  const int out_c = (gbm && dim == 1) ? 2 : g.C;
+  if (reg) {
+    SE_TRY(out_rows(ctx, out_slot, out_row, 1, n, &g.out, nullptr));
+  } else {
+    SE_TRY(slot_alloc2d(ctx, SE_SLOT_RAW, out_c, n));
+    SE_TRY(slot_alloc2d(ctx, SE_SLOT_PROB, out_c, n));
+    SE_TRY(slot_alloc2d(ctx, SE_SLOT_LABEL, 1, n));
+    const SlotBuf& R = ctx->slot[SE_SLOT_RAW];
+    g.raw = R.d; g.prob = ctx->slot[SE_SLOT_PROB].d; g.label = ctx->slot[SE_SLOT_LABEL].d;
+    g.ld_out = R.ld;
+  }
+  // se_agg_run's scalars: (float) init of the GBM regressor, the divisor of the mean kinds (M, or Σ of the fp32
+  // weights), Σ of the SAMME vote weights
+  double sum_f = 0.0;
+  for (int m = 0; m < n_members; ++m) sum_f += (double)mem[(size_t)m].wf;
+  if (kind == SE_AGG_GBM_REGRESSOR) g.init[0] = init ? (double)(float)init[0] : 0.0;
+  if (kind == SE_AGG_BAGGING_REGRESSOR) g.post_div = (float)n_members;
+  if (kind == SE_AGG_BOOSTING_REG_MEAN) g.post_div = (float)sum_f;
+  if (gbm)
+    for (int c = 0; c < dim; ++c) g.init[c] = init ? init[c] : 0.0;
+  for (int m = 0; m < n_members; ++m) g.sum_a += mem[(size_t)m].w;
+  g.n4 = reg ? (n & ~(int64_t)3) : n;
+  if (median) {  // as se_forest_median
+    g.mode = ctx->wm_fast ? wm_weight_mode(weights, n_members) : 0;
+    for (int m = 0; m < kForestMedianMaxTrees; ++m) {
+      g.w[m] = (m < n_members) ? weights[m] : 0.0;
+      g.total += g.w[m];
+    }
+    g.tau = (g.mode == 1) ? 8.0 * (double)n_members * 1.1102230246251565e-16 * g.total : -1.0;
+    ctx->last_wm_mode = g.mode;
+  }
+  // the members, the 64-bit offsets of their columns and their coefficients, in one blob
+  const size_t total_cols = (size_t)col_offsets[n_members];
+  const size_t mem_bytes = forest_pad(sizeof(LinearAggMember) * (size_t)n_members, 16);
+  const size_t col_bytes = forest_pad(sizeof(unsigned long long) * total_cols, 16);
+  std::vector<unsigned char> blob(mem_bytes + col_bytes + sizeof(double) * (size_t)(n_coef + n_icpt));
+  memcpy(blob.data(), mem.data(), sizeof(LinearAggMember) * (size_t)n_members);
+  unsigned long long* co = reinterpret_cast<unsigned long long*>(blob.data() + mem_bytes);
+  for (size_t j = 0; j < total_cols; ++j) co[j] = (unsigned long long)cols[j] * (unsigned long long)X.ld;
+  double* cf = reinterpret_cast<double*>(blob.data() + mem_bytes + col_bytes);
+  if (n_coef) memcpy(cf, coef, sizeof(double) * (size_t)n_coef);
+  memcpy(cf + n_coef, intercept, sizeof(double) * (size_t)n_icpt);
+  SE_TRY(forest_upload(ctx, blob.data(), blob.size()));
+  const unsigned char* d = ctx->d_forest;
+  g.members = reinterpret_cast<const LinearAggMember*>(d);
+  g.coloff = reinterpret_cast<const unsigned long long*>(d + mem_bytes);
+  g.coef = reinterpret_cast<const double*>(d + mem_bytes + col_bytes);
+  g.X = X.d; g.n = n;
+  SE_LAUNCH_T(ctx, SE_KF_LINEAR, launch_linear_agg(g, max_d, ctx->sms, ctx->stream));
+  return end(ctx);
+}

@@ -382,6 +382,42 @@ struct ForestMedianArgs {
 cudaError_t launch_forest_median(const ForestMedianArgs& a, size_t smem, int sms, cudaStream_t s);
 // CTAs of the kernel for M trees one SM can hold by its registers alone (>= 1)
 cudaError_t forest_median_ctas_per_sm(int M, int* ctas);
+// An ensemble of linear and logistic members in ONE pass over X (se_linear_agg, se_linear_agg.cu): one row per thread,
+// every member's margins formed from its columns of X (read through L1, so the members' shared columns come from HBM
+// once per tile) and its output folded at once into the row's aggregate: classifier totals in fp64 in shared memory
+// ([C][kLinearAggTile]), agg_sum_kernel's fold for the sum kinds, the M values in shared memory for the median.
+constexpr int kLinearAggTile = 128;
+constexpr int kLinearAggMaxCols = 254;  // as se_logistic_predict
+struct LinearAggMember {
+  int col0 = 0, p = 0;    // its columns' offsets coloff[col0 .. col0 + p)
+  int D = 1, cls = 0;     // margins; GBM classifier: the class its value adds to
+  int coef0 = 0, icpt0 = 0;  // coef [D][p] at coef[coef0 ..], intercept [D] at coef[icpt0 ..]
+  float wf = 1.f;         // the sum kinds' weight, narrowed to fp32 as se_agg_run narrows it
+  double w = 1.0;         // the classifier kinds' fp64 term weight (hard votes 1, SAMME (float) a_m)
+  double threshold = 0.5; // D = 1 labels: σ(m) > threshold
+};
+struct LinearAggArgs {
+  const float* X = nullptr;
+  int64_t n = 0;
+  int64_t n4 = 0;          // sum kinds: rows from n4 on are agg_sum_kernel's tail rows (n & ~3)
+  const LinearAggMember* members = nullptr;
+  const unsigned long long* coloff = nullptr;  // column · ld of every member's columns
+  const double* coef = nullptr;
+  int kind = 0, K = 0, C = 1, dim = 1, loss = 0, M = 0;
+  double init[kForestAggMaxClasses] = {};  // classifier totals start here; the sum kinds' (float) init in init[0]
+  float post_div = 0.f;                    // sum kinds: se_agg_run's divisor (0: none)
+  double sum_a = 0.0;                      // Σ of the vote weights (boosting discrete epilogue)
+  float* out = nullptr;                    // regressor kinds: the output row
+  float* raw = nullptr;
+  float* prob = nullptr;
+  float* label = nullptr;
+  int64_t ld_out = 0;
+  int mode = 0;                            // median: as ForestMedianArgs
+  double total = 0.0, tau = -1.0;
+  double w[kForestMedianMaxTrees] = {};
+};
+// max_d: the largest D of the members
+cudaError_t launch_linear_agg(const LinearAggArgs& g, int max_d, int sms, cudaStream_t s);
 // ---- regression- and classification-tree fit over the uint8 rank matrix (se_tree_fit.cu) -----
 // Nodes are heap-indexed (root 1, children 2h, 2h + 1), so depth <= 8 needs 511 records.
 constexpr int kTreeFitHeap = 512;

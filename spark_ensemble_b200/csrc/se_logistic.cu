@@ -15,6 +15,7 @@
 
 #include "se_common.cuh"
 #include "se_kernels.h"
+#include "se_row_steps.cuh"
 
 namespace se {
 namespace {
@@ -377,8 +378,10 @@ __global__ void __launch_bounds__(kBlock) logistic_tile_batch_kernel(const Logis
 }
 
 // ---- scoring --------------------------------------------------------------------------------------------------------
-// The binomial case (D = 1) keeps its one margin in a register and its coefficients in shared memory; the multinomial
-// case keeps the D margins of a row in a per-thread array and reads the coefficients through the read-only cache.
+// The per-row steps are se_row_steps.cuh's (lg_row_*), which se_linear_agg's kernels share.  The binomial case (D = 1)
+// keeps its coefficients in shared memory; the multinomial case reads them through the read-only cache.  MAXD >= D
+// keeps the margins in registers.
+template <int MAXD>
 __global__ void __launch_bounds__(kBlock) logistic_predict_kernel(LogisticPredictArgs a) {
   __shared__ int32_t s_col[kLogisticMaxCols];
   __shared__ double s_coef[kLogisticMaxCols];
@@ -389,45 +392,24 @@ __global__ void __launch_bounds__(kBlock) logistic_predict_kernel(LogisticPredic
   }
   __syncthreads();
   for (int64_t i = (int64_t)blockIdx.x * kBlock + threadIdx.x; i < a.n; i += (int64_t)gridDim.x * kBlock) {
-    if (D == 1) {
-      double mm = 0.0;
-      for (int j = 0; j < p; ++j) mm = fma(s_coef[j], (double)ld_stream1(a.X + (int64_t)s_col[j] * a.ld + i), mm);
-      mm += a.intercept[0];
-      const double p1 = 1.0 / (1.0 + exp(-mm));
-      if (a.raw) {
-        a.raw[i] = (float)(-mm);
-        a.raw[a.ld_raw + i] = (float)mm;
-      }
-      if (a.prob) {
-        a.prob[i] = (float)(1.0 - p1);
-        a.prob[a.ld_prob + i] = (float)p1;
-      }
-      if (a.label) a.label[i] = p1 > a.threshold ? 1.f : 0.f;
-      continue;
-    }
-    double m[kLogisticMaxClasses];
-    for (int k = 0; k < D; ++k) m[k] = 0.0;
-    for (int j = 0; j < p; ++j) {
-      const double x = (double)ld_stream1(a.X + (int64_t)s_col[j] * a.ld + i);
-      for (int k = 0; k < D; ++k) m[k] = fma(__ldg(a.coef + (size_t)k * p + j), x, m[k]);
-    }
-    for (int k = 0; k < D; ++k) m[k] += a.intercept[k];
-    int best = 0;
-    for (int k = 1; k < D; ++k)
-      if (m[k] > m[best]) best = k;
-    const double mx = m[best];
-    if (a.raw)
-      for (int k = 0; k < D; ++k) a.raw[(int64_t)k * a.ld_raw + i] = (float)m[k];
-    if (a.prob) {
-      if (mx == INFINITY) {
-        for (int k = 0; k < D; ++k) a.prob[(int64_t)k * a.ld_prob + i] = (m[k] == INFINITY) ? 1.f : 0.f;
+    const auto x = [&](int j) { return (double)ld_stream1(a.X + (int64_t)s_col[j] * a.ld + i); };
+    double m[MAXD];
+    if (D == 1) lg_row_margins<MAXD>(p, 1, [&](int, int j) { return s_coef[j]; }, x, a.intercept, m);
+    else lg_row_margins<MAXD>(p, D, [&](int k, int j) { return __ldg(a.coef + (size_t)k * p + j); }, x, a.intercept, m);
+    double mx;
+    const int best = lg_row_argmax<MAXD>(D, m, &mx);
+    if (a.raw) {
+      if (D == 1) {
+        a.raw[i] = (float)(-m[0]);
+        a.raw[a.ld_raw + i] = (float)m[0];
       } else {
-        double S = 0.0;
-        for (int k = 0; k < D; ++k) S += exp(m[k] - mx);
-        for (int k = 0; k < D; ++k) a.prob[(int64_t)k * a.ld_prob + i] = (float)(exp(m[k] - mx) / S);
+#pragma unroll
+        for (int k = 0; k < MAXD; ++k)
+          if (k < D) a.raw[(int64_t)k * a.ld_raw + i] = (float)m[k];
       }
     }
-    if (a.label) a.label[i] = (float)best;
+    if (a.prob) lg_row_probs<MAXD>(D, m, mx, [&](int k, float v) { a.prob[(int64_t)k * a.ld_prob + i] = v; });
+    if (a.label) a.label[i] = lg_row_label(D, m[0], best, a.threshold);
   }
 }
 
@@ -550,8 +532,10 @@ cudaError_t launch_logistic_loss_grad_batch(const LogisticBatchItem* items, cons
 
 cudaError_t launch_logistic_predict(const LogisticPredictArgs& a, int sms, cudaStream_t st) {
   if (a.p < 0 || a.D < 1 || a.D > kLogisticMaxClasses || a.n < 1) return cudaErrorInvalidValue;
-  logistic_predict_kernel<<<grid_rows(a.n, kBlock, 4, sms), kBlock, 0, st>>>(a);
-  return cudaGetLastError();
+  return with_maxd(a.D, [&](auto md) {
+    logistic_predict_kernel<decltype(md)::value><<<grid_rows(a.n, kBlock, 4, sms), kBlock, 0, st>>>(a);
+    return cudaGetLastError();
+  });
 }
 
 }  // namespace se

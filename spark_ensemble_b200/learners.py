@@ -43,6 +43,11 @@ class _Model:
     def linear_arrays(self):
         return None
 
+    def margin_arrays(self):
+        """{coef [D][p], intercept [D] (fp64), threshold}: the form in which se_linear_agg scores a linear or logistic
+        member; None for other models."""
+        return None
+
 
 class DecisionTreeRegressionModel(_Model):
     def __init__(self, sk):
@@ -449,6 +454,9 @@ class LinearRegressionModel(_Model):
     def linear_arrays(self):
         return {"coef": self.coefficients.astype(np.float32), "intercept": np.float32(self.intercept)}
 
+    def margin_arrays(self):
+        return {"coef": self.coefficients.reshape(1, -1), "intercept": np.array([self.intercept]), "threshold": 0.5}
+
 
 def solve_linear_moments(M, shift, label_shift: float, reg_param: float = 0.0):
     """(coefficients, intercept) minimising Σ w·(y − xβ − b)² + α‖β‖², α = max(reg_param, 1e-12), b unpenalised, from the
@@ -607,6 +615,9 @@ class LogisticRegressionModel(_Model):
         if not self.isMultinomial:
             return (self.predictProbability(X)[:, 1] > self.threshold).astype(np.float64)
         return np.argmax(self._margins(X), axis=1).astype(np.float64)
+
+    def margin_arrays(self):
+        return {"coef": self.coefficientMatrix, "intercept": self.interceptVector, "threshold": self.threshold}
 
     def write_rows(self, ctx, method: str, out_slot: int, out_row: int, subspace=None) -> bool:
         """Every row's label ("class"), raw vector ("raw") or probabilities ("proba") over the context's SLOT_X into

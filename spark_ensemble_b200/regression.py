@@ -15,9 +15,9 @@ from .ensemble import DataFrame, exact_quantile, fit_dummy_regressor, java_strin
 from .gbm_engine import fit_rounds
 from .params import (DEVICES, LINE_SEARCH, RESIDENT_FEATURES, Param, Params, ParamValidators, boosting_params,
                      gbm_params, random_uid, shared_predictor_params, subbag_params)
-from .routes import (bagging_fit, device_fit, device_trees, download_raw, extract_instances, forest_sum, load_boosting,
-                     member_route, one_pass, resident_context, resident_linear, split_validation, stack_outputs,
-                     stacking_fit, stacking_predict, tree_list)
+from .routes import (bagging_fit, device_fit, device_linear, device_trees, download_raw, extract_instances, forest_sum,
+                     linear_list, linear_sum, load_boosting, member_route, one_pass, resident_context, resident_linear,
+                     split_validation, stack_outputs, stacking_fit, stacking_predict, tree_list)
 
 _REG_LOSSES = ("squared", "absolute", "huber", "quantile")  # GBMRegressor.scala:119-120
 _REG_INIT = ("constant", "zero", "base")                     # :121-123
@@ -122,19 +122,27 @@ class GBMRegressionModel(Params):
         return members, subs, a, init
 
     def write_rows(self, ctx: Context, method: str, out_slot: int, out_row: int) -> bool:
-        """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
-        (a stacking member's meta-feature)."""
+        """Its prediction over ctx's SLOT_X into row out_row of out_slot in one pass when every member is a tree, or a
+        linear model after a constant init (a stacking member's meta-feature)."""
         members, subs, a, init = self._forest()
         trees = tree_list(members) if members else None
-        if trees is None:
+        if trees is not None:
+            ctx.forest_predict(trees, out_slot, weights=a, init=init, out_row=out_row, subspaces=subs)
+            return True
+        lin = linear_list(self.models) if (self.models and hasattr(self.init, "prediction")) else None
+        if lin is None:
             return False
-        ctx.forest_predict(trees, out_slot, weights=a, init=init, out_row=out_row, subspaces=subs)
+        ctx.linear_agg(N.AGG_GBM_REGRESSOR, 0, lin, out_slot, out_row, weights=self.weights, init=[init],
+                       subspaces=self.subspaces)
         return True
 
     def _aggregate(self, X) -> np.ndarray:
         const_init = hasattr(self.init, "prediction")
         members, subs, a, init = self._forest()
         out = forest_sum(self.device, X, device_trees(self, members), subs, a, init)
+        if out is None and const_init:
+            out = linear_sum(self.device, X, device_linear(self, self.models), self.subspaces, N.AGG_GBM_REGRESSOR,
+                             weights=self.weights, init=[init])
         if out is not None:
             return out
         P = stack_outputs(self.models, self.subspaces, X, None if const_init else self.init.predict(X))
@@ -194,16 +202,23 @@ class BaggingRegressionModel(Params):
         """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
         (a stacking member's meta-feature): Σ_t tree_t(x) / M as weights 1/M."""
         trees = tree_list(self.models) if self.models else None
-        if trees is None:
+        if trees is not None:
+            ctx.forest_predict(trees, out_slot, weights=np.full(len(trees), 1.0 / len(trees)), out_row=out_row,
+                               subspaces=self.subspaces)
+            return True
+        lin = linear_list(self.models) if self.models else None
+        if lin is None:
             return False
-        ctx.forest_predict(trees, out_slot, weights=np.full(len(trees), 1.0 / len(trees)), out_row=out_row,
-                           subspaces=self.subspaces)
+        ctx.linear_agg(N.AGG_BAGGING_REGRESSOR, 0, lin, out_slot, out_row, subspaces=self.subspaces)
         return True
 
     def _aggregate(self, X) -> np.ndarray:
         s = forest_sum(self.device, X, device_trees(self, self.models), self.subspaces, None, 0.0)
         if s is not None:  # (Σ_t tree_t(x)) / M in one pass over the device-resident features
             return s / self.numModels
+        s = linear_sum(self.device, X, device_linear(self, self.models), self.subspaces, N.AGG_BAGGING_REGRESSOR)
+        if s is not None:
+            return s
         P = stack_outputs(self.models, self.subspaces, X)
         return member_route(self.device, N.AGG_BAGGING_REGRESSOR, P)
 
@@ -304,9 +319,15 @@ class BoostingRegressionModel(Params):
         """Its prediction over ctx's SLOT_X into row out_row of out_slot in one forest pass when every member is a tree
         (a stacking member's meta-feature): the weighted median of at most 64 trees, or the weighted mean."""
         trees = tree_list(self.models) if self.models else None
+        median = self("votingStrategy").lower() == "median"
         if trees is None:
-            return False
-        if self("votingStrategy").lower() == "median":
+            lin = linear_list(self.models) if self.models else None
+            if lin is None or (median and len(lin) > N.FOREST_MEDIAN_MAX_TREES):
+                return False
+            ctx.linear_agg(N.AGG_BOOSTING_REG_MEDIAN if median else N.AGG_BOOSTING_REG_MEAN, 0, lin, out_slot, out_row,
+                           weights=self.weights)
+            return True
+        if median:
             if len(trees) > N.FOREST_MEDIAN_MAX_TREES:
                 return False
             ctx.forest_median(trees, out_slot, self.weights, out_row=out_row)
@@ -342,6 +363,9 @@ class BoostingRegressionModel(Params):
     def _aggregate(self, X) -> np.ndarray:
         median = self("votingStrategy").lower() == "median"
         out = self._aggregate_resident(X, median)
+        if out is None and (not median or len(self.models) <= N.FOREST_MEDIAN_MAX_TREES):
+            out = linear_sum(self.device, X, device_linear(self, self.models), None,
+                             N.AGG_BOOSTING_REG_MEDIAN if median else N.AGG_BOOSTING_REG_MEAN, weights=self.weights)
         if out is not None:
             return out
         P = np.ascontiguousarray(np.stack([m.predict(X) for m in self.models]), dtype=np.float32)

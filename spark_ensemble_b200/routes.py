@@ -3,6 +3,7 @@ fit, the set-up of a Bagging or Boosting fit, and the two routes by which a mode
 
 - one pass over the device-resident features when every member is a tree (se_forest_predict / se_forest_median /
   se_forest_agg), which returns None when the forest's thresholds do not fit the rank matrix;
+- one pass over them when every member is a linear or logistic model (se_linear_agg);
 - the member route: every member's output stacked on the host, uploaded as SLOT_P and aggregated on the device
   (se_agg_run).
 
@@ -217,6 +218,31 @@ def device_trees(model: Params, members) -> list | None:
     return trees
 
 
+def linear_list(members) -> list | None:
+    """The fp64 margin arrays (margin_arrays()) of every member, or None when one of them is not a linear or logistic
+    model, or reads more columns than se_linear_agg takes."""
+    out = []
+    for m in members:
+        a = m.margin_arrays() if hasattr(m, "margin_arrays") else None
+        if a is None or np.atleast_2d(a["coef"]).shape[1] > N.LOGISTIC_MAX_COLS:
+            return None
+        out.append(a)
+    return out
+
+
+def device_linear(model: Params, members) -> list | None:
+    """The packed members when the model scores them in one se_linear_agg pass: residentFeatures is set, there is at
+    least one member, and every member is a linear or logistic model (linear_list).  None keeps the member route."""
+    if not model("residentFeatures") or not members:
+        return None
+    return linear_list(members)
+
+
+def linear_kw(kw: dict) -> dict:
+    """forest_agg's keyword arguments as linear_agg takes them: a member's GBM class is its member_class."""
+    return {("member_class" if k == "tree_class" else k): v for k, v in kw.items()}
+
+
 def resident_context(device: int, X) -> Context:
     """A context whose SLOT_X holds the rows of X column-major: the matrix the forest kernels walk."""
     X = np.asarray(X, dtype=np.float32)
@@ -256,6 +282,15 @@ def forest_sum(device: int, X, trees, subspaces, weights, init: float) -> np.nda
         ctx.alloc(N.SLOT_RAW, 1, X.shape[0])
         ctx.forest_predict(trees, N.SLOT_RAW, weights=weights, init=init, subspaces=subspaces)
     return one_pass(device, X, trees, score, download_raw)
+
+
+def linear_sum(device: int, X, members, subspaces, kind: int, weights=None, init=None) -> np.ndarray | None:
+    """A regressor kind's aggregate of linear members (device_linear) through se_linear_agg: what agg_run gives over
+    their outputs, without them; None without members."""
+    def score(ctx, members):
+        ctx.alloc(N.SLOT_RAW, 1, X.shape[0])
+        ctx.linear_agg(kind, 0, members, N.SLOT_RAW, weights=weights, init=init, subspaces=subspaces)
+    return one_pass(device, X, members, score, download_raw)
 
 
 def stack_outputs(models, subspaces, X, extra=None) -> np.ndarray:
