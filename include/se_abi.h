@@ -469,7 +469,9 @@ SE_API int se_linear_predict(se_ctx* ctx, int which, int n_coef, const float* co
  * SE_SLOT_BAG's multiplicity (1 unless use_bag).  Writes out[(p+2)·(p+2)], row-major and symmetric, = Σ_i c·z zᵀ in fp64:
  * XᵀWX, XᵀWy, the weighted column sums, Σ c and yᵀWy of the shifted values (shift NULL: 0).  Every fp32 product is exact
  * in fp64, every sum is fp64, and the per-CTA partials are folded in a fixed order: identical calls give identical bits.
- * 0 <= p <= 254; a label, weight or bag row that does not exist, or a column outside the slot, fails with SE_ERR_ARG. */
+ * Newton weights (weight_slot SE_SLOT_WOUT after se_gbm_pseudo_residuals / se_gbm_update with newton) are read as the
+ * learner's weights, 1/2 hc w x 1/S_row, as se_download returns them: the matrix does not depend on whether the
+ * weights were read on the device or downloaded first.  0 <= p <= 254; a label, weight or bag row that does not exist, or a column outside the slot, fails with SE_ERR_ARG. */
 SE_API int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols, const double* shift,
                              double label_shift, int label_slot, int label_row, int weight_slot, int weight_row,
                              int use_bag, double* out);

@@ -221,8 +221,10 @@ int gbm_fetch(se_ctx* ctx, int count, double* out) {
 static int newton_finish(se_ctx* ctx, double* sum_hess) {
   // S_j (all-reduced) -> the base-learner weights are WOUT_j * 1/S_j  (GBMRegressor.scala:373,379;
   // GBMClassifier.scala:344-355,364).  The kernel left the unnormalised 1/2 hc w in SE_SLOT_WOUT; the per-dimension
-  // factor 1/S_j is applied where the weights LEAVE the device (se_download / se_download_scaled on SE_SLOT_WOUT) —
-  // no separate 8 B/row pass over WOUT for it.
+  // factor 1/S_j is applied wherever WOUT is read as weights, and only there: where they LEAVE the device (se_download /
+  // se_download_scaled on SE_SLOT_WOUT) and where a device fit reads them (se_linear_moments scales its matrix; a tree
+  // fit needs no factor, its splits and leaves do not change when every weight is scaled) — no separate 8 B/row pass
+  // over WOUT for it.
   const int dim = ctx->gbm.dim;
   std::vector<double> s((size_t)dim + 1);
   SE_TRY(gbm_fetch(ctx, 1 + dim, s.data()));

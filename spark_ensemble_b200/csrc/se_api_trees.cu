@@ -647,6 +647,12 @@ int se_linear_moments(se_ctx* ctx, int src_slot, int n_cols, const int32_t* cols
   SE_TRY(end(ctx));
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   memcpy(out, hout, sizeof(double) * (size_t)m * m);
+  if (weight_slot == SE_SLOT_WOUT && ctx->wout_scaled && (size_t)weight_row < ctx->wout_scale.size()) {
+    // Newton weights: WOUT holds 1/2 hc w, the learner's weights are that x 1/S_row (newton_finish); the moments are
+    // linear in the weights, so the factor se_download applies per value is applied to the matrix here
+    const double s = (double)ctx->wout_scale[(size_t)weight_row];
+    for (int i = 0; i < m * m; ++i) out[i] *= s;
+  }
   return SE_OK;
 }
 

@@ -75,7 +75,8 @@ class GBMEngine:
 
     def fit_direction(self, j: int, learner, subspace, newton: bool = False, bag: bool = False):
         """Fit the device tree learner or DeviceLinearRegression on R row j over the round's subspace (weights: WOUT
-        row j in newton mode, else W when the fit has weights; the bag's multiplicities when `bag`) and write its
+        row j in newton mode, read ×1/S_j as the reference normalises them, else W when the fit has weights; the bag's
+        multiplicities when `bag`) and write its
         output into H row j.  A tree's split candidates are set once per fit, on the first call; a linear fit is
         shifted by the column means, as its `fit` is.  Nothing but the fitted model crosses PCIe."""
         if not self._x_resident:

@@ -7,7 +7,8 @@ sets: cpusmall (regression), adult8k (binary) and letter (26 classes).
   member's final objective, evaluated in fp64 by oracle/np_logistic.py on the member's own in-bag rows, to the
   optimiser's tolerance; the ensemble's labels (a near-tie may go either way).  Out-of-bag rows holding non-finite
   features must not fail the fit.  The lock-step fit equals, bit for bit, the fit of every member in a batch of its own.
-- Boosting (SAMME, SAMME.R, AdaBoost.R2) and GBM: the per-round history and the outputs at 1e-5, as the tree tests do."""
+- Boosting (SAMME, SAMME.R, AdaBoost.R2): the per-round history and the outputs at 1e-5, as the tree tests do.
+- GBM (every regressor and classifier loss, gradient and Newton updates): as `_gbm_routes` states."""
 import numpy as np
 import pytest
 
@@ -209,25 +210,99 @@ def test_boosting_regressor_linear(loss, reg):
     np.testing.assert_allclose(resident.transform(df)[col], member.transform(df)[col], rtol=1e-5, atol=1e-5)
 
 
-@pytest.mark.parametrize("loss", ["squared"])
-@pytest.mark.parametrize("bagged", [False, True])
-def test_gbm_regressor_linear(loss, bagged):
+def _gbm_routes(monkeypatch, est, df, quadratic):
+    """The member route's and the resident route's fits of a GBM.  With the squared loss, every round's α, trainLoss and
+    validationLoss agree at 1e-5.  Elsewhere α comes from Brent or L-BFGS-B over a sum of fp32 per-row losses, which
+    pins it only to the objective's resolution: the two routes' α of each round are compared through the objective
+    instead, both evaluated on the resident fit's context, which holds that round's F and h, at 1e-5.  The first round
+    starts both routes from the same F, so its losses agree at 1e-5; after it the routes' F differ by that resolution,
+    and the next residuals (signs, clipped or saturated in F) carry it into the next directions: measured up to 3e-4 of
+    the loss over five rounds on cpusmall, allowed 1e-3.  tests/test_gpu_resident_linear_gbm.py checks every round of
+    the resident route against fp64 instead."""
+    from spark_ensemble_b200.gbm_engine import GBMEngine
+    member = est.setResidentFeatures(False).fit(df)
+    alphas = [np.atleast_1d(h["alpha"]) for h in member.trainingHistory]
+    f = []
+
+    def spied(real):
+        def run(eng, tol, max_iter):
+            out = real(eng, tol, max_iter)
+            a_mem = alphas[len(f)] if len(f) < len(alphas) else np.atleast_1d(out[0])
+            f.append((eng.ctx.gbm_linesearch_eval(out[0])[0], eng.ctx.gbm_linesearch_eval(a_mem)[0]))
+            return out
+        return run
+
+    if not quadratic:
+        monkeypatch.setattr(GBMEngine, "line_search_brent", spied(GBMEngine.line_search_brent))
+        monkeypatch.setattr(GBMEngine, "line_search_lbfgsb", spied(GBMEngine.line_search_lbfgsb))
+    resident = est.setResidentFeatures(True).fit(df)
+    monkeypatch.undo()
+    ha, hb = resident.trainingHistory, member.trainingHistory
+    if quadratic:
+        _history_close(ha, hb, ("alpha", "trainLoss", "validationLoss"))
+    else:
+        assert len(ha) == len(hb)
+        for i, (a, b) in enumerate(zip(ha, hb)):
+            for k in ("trainLoss", "validationLoss"):
+                np.testing.assert_allclose(a[k], b[k], rtol=1e-5 if i == 0 else 1e-3, err_msg=f"round {i} {k}")
+    for i, (fa, fb) in enumerate(f):
+        assert abs(fa - fb) <= 1e-5 * max(1.0, abs(fa)), (i, fa, fb)
+    return resident, member
+
+
+# standardised features: the device direction is scored with fp32 coefficients (se_linear_predict, as every resident
+# linear direction is), and cpusmall's raw column scales (up to 4e5) turn their rounding into 1e-5 of α
+@pytest.mark.parametrize("bagged,weighted", [(False, False), (True, True)])
+@pytest.mark.parametrize("loss,updates,reg", [("squared", "gradient", 0.1), ("absolute", "gradient", 0.1),
+                                              ("huber", "gradient", 0.1), ("quantile", "gradient", 0.1),
+                                              ("squared", "newton", 0.5)])
+def test_gbm_regressor_linear(monkeypatch, loss, updates, reg, bagged, weighted):
     from spark_ensemble_b200.learners import DeviceLinearRegression
     from spark_ensemble_b200.regression import GBMRegressor
     X, y = _golden("cpusmall")
-    # standardised features: the device direction is scored with fp32 coefficients (se_linear_predict, as every
-    # resident linear direction is), and cpusmall's raw column scales (up to 4e5) turn their rounding into 1e-5 of α
     X = (X - X.mean(axis=0)) / X.std(axis=0)
-    df = _frame(X, y, False)
+    df = _frame(X, y, weighted, seed=6)
     val = np.zeros(y.size, dtype=bool)
     val[::5] = True
-    df = df.__class__(**{**{k: df[k] for k in ("features", "label")}, "val": val})
-    est = (GBMRegressor().setBaseLearner(DeviceLinearRegression(regParam=0.1)).setNumBaseLearners(5)
-           .setLoss(loss).setSubspaceRatio(0.7).setValidationIndicatorCol("val"))
+    df = df.__class__(**{**{k: df[k] for k in df.columns}, "val": val})
+    est = (GBMRegressor().setBaseLearner(DeviceLinearRegression(regParam=reg)).setNumBaseLearners(5)
+           .setLoss(loss).setSubspaceRatio(0.7).setValidationIndicatorCol("val").set("updates", updates))
     if bagged:
         est = est.setSubsampleRatio(0.8)
-    resident = est.setResidentFeatures(True).fit(df)
-    member = est.setResidentFeatures(False).fit(df)
-    _history_close(resident.trainingHistory, member.trainingHistory, ("alpha", "trainLoss", "validationLoss"))
+    if weighted:
+        est = est.setWeightCol("weight")
+    resident, member = _gbm_routes(monkeypatch, est, df, loss == "squared")
     col = resident("predictionCol")
-    np.testing.assert_allclose(resident.transform(df)[col], member.transform(df)[col], rtol=1e-5, atol=1e-5)
+    pa, pb = np.asarray(resident.transform(df)[col]), np.asarray(member.transform(df)[col])
+    if loss == "squared":
+        np.testing.assert_allclose(pa, pb, rtol=1e-5, atol=1e-5 * np.abs(pb).max())
+    else:  # as the losses; rows far out along a direction carry its difference further (measured 4e-3 of the scale)
+        assert np.abs(pa - pb).mean() <= 1e-3 * np.abs(pb).mean()
+        assert np.abs(pa - pb).max() <= 1e-2 * np.abs(pb).max()
+
+
+@pytest.mark.parametrize("updates", ["gradient", "newton"])
+@pytest.mark.parametrize("loss", ["bernoulli", "exponential", "logloss"])
+def test_gbm_classifier_linear(monkeypatch, loss, updates):
+    from spark_ensemble_b200.classification import GBMClassifier
+    from spark_ensemble_b200.learners import DeviceLinearRegression
+    if loss == "logloss":  # 4 classes of letter, a ragged row count
+        X, y = _golden("letter")
+        keep = np.flatnonzero(y < 4)[:2501]
+        X, y = X[keep], y[keep]
+    else:
+        X, y = _golden("adult8k")
+    X = (X - X.mean(axis=0)) / np.maximum(X.std(axis=0), 1e-12)
+    df = _frame(X, y, True, seed=8)
+    val = np.zeros(y.size, dtype=bool)
+    val[1::6] = True
+    df = df.__class__(**{**{k: df[k] for k in df.columns}, "val": val})
+    est = (GBMClassifier().setBaseLearner(DeviceLinearRegression(regParam=0.5)).setNumBaseLearners(4)
+           .setLoss(loss).set("updates", updates).setSubspaceRatio(0.7).setSubsampleRatio(0.8)
+           .setValidationIndicatorCol("val").setWeightCol("weight"))
+    resident, member = _gbm_routes(monkeypatch, est, df, False)
+    # the members' weights are L-BFGS-B's α, which the routes share only to the objective's resolution (as the losses)
+    ta, tb = resident.transform(df), member.transform(df)
+    for col in (resident("probabilityCol"), resident("rawPredictionCol")):
+        np.testing.assert_allclose(ta[col], tb[col], rtol=1e-3, atol=1e-4)
+    assert np.mean(np.asarray(ta[resident("predictionCol")]) != np.asarray(tb[resident("predictionCol")])) <= 2e-3
