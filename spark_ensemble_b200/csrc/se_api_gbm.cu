@@ -247,7 +247,7 @@ int se_gbm_pseudo_residuals(se_ctx* ctx, int newton, double* sum_hess) {
   ctx->gbm.sq_stats_current = false;  // R is rewritten
   if (newton) SE_TRY(slot_alloc2d(ctx, SE_SLOT_WOUT, ctx->gbm.dim, ctx->gbm.n));
   GbmArgs a = gbm_args(ctx, false);
-  ctx->wout_scaled = false;
+  if (newton) ctx->wout_scaled = false;  // a gradient-mode call leaves WOUT, and the 1/S of its download, as they were
   if (newton) a.ws = red_ws(ctx);  // Σ max(H,1e-2): reducing launch
   SE_TRY(gbm_launch(ctx, SE_KF_RESID, newton ? GBM_RESID_NEWTON : GBM_RESID, a, nullptr));
   if (newton) SE_TRY(newton_finish(ctx, sum_hess));
@@ -586,6 +586,7 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   ctx->gbm.sq_defer_ok = carried;
   ctx->last_round_deferred = a.r_defer;
   ctx->last_fused_resident_tiles = resident_slots / 4.0;  // float4 groups per thread, U_SQ = 4 to a tile
+  const bool r_current_before = ctx->gbm.r_current;
   ctx->gbm.r_current = write_r != 0;
   const bool owed_before = ctx->gbm.f_owed;
   if (write_r) ctx->gbm.f_owed = true;  // F = y - r from here on (unless the step turns out to be 0, below)
@@ -611,9 +612,10 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   if (n_eval) *n_eval = (int)fabs(res[6]);
   if (loss_sum) *loss_sum = ls;
   if (res[6] < 0.0) {
-    // the step was 0: F was not moved, so it is exactly as current as before the round (r = y - F when the round read
-    // y and F), and a download returns it bit for bit
+    // the step was 0: F was not moved, so it is exactly as current as before the round, and a download returns it bit
+    // for bit.  R too: a round that read r stored r - 0*h, one that read y and F (R not current) stored nothing.
     ctx->gbm.f_owed = owed_before;
+    ctx->gbm.r_current = r_current_before;
     return fail(ctx, SE_ERR_OPT, "Brent exceeded MaxEval(%d)", max_iter);
   }
   if (stats_out) {

@@ -139,6 +139,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   constexpr int U = U_SQ;
   extern __shared__ float4 s_res[];  // FROM_R, CARRIED: [slot][r, h][kBlock]
   __shared__ float s_coef;
+  __shared__ bool s_store_r;
   __shared__ float s_chain[kSqDeferMax];  // CARRIED: the steps pending on the residual slot
   __shared__ float4 s_brent_regs[2 * U];  // FROM_R, CARRIED: the Brent thread's tile registers while it runs Brent
   const int64_t n4 = a.n >> 2;
@@ -334,10 +335,14 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     }
     while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {}
     s_coef = (float)a.sync->x;  // same rounding as the host path: (float)(lr * alpha)
+    // MaxEval exceeded on a round that read y and F: its residual slot was not current, and the failed round must
+    // leave it as it was rather than store y - F (the Brent thread wrote the count before it released the step)
+    s_store_r = !(WRITE_R && !from_r && a.out[6] < 0.0);
   }
   if constexpr (CARRIED) asm volatile("cp.async.wait_all;" ::: "memory");  // this thread's slots have landed
   __syncthreads();
   const float coef = s_coef;
+  const bool store_r = s_store_r;
   double accb[1] = {0.0};
   double accn[3] = {0.0, 0.0, 0.0};  // STATS_OUT: Σr'², Σhr', Σh² over what this pass writes, as phase A sums them
   for (int64_t k = 0; k < cnt; ++k) {
@@ -384,7 +389,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       }
       // the next statistics pass starts where this one ends; a deferring round stores nothing
       if (WRITE_R) {
-        if (!CARRIED || !a.r_defer) st_stream4_p(a.r + 4 * g, o, pol_keep);
+        if ((!CARRIED || !a.r_defer) && store_r) st_stream4_p(a.r + 4 * g, o, pol_keep);
       } else {
         st_stream4_p(a.F + 4 * g, o, pol_stream);
       }
@@ -402,7 +407,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
       if constexpr (CARRIED)
         for (int q = 0; q < a.r_pending; ++q) r = fmaf(-s_chain[q], h, r);
       d = fmaf(-coef, h, r);
-      if (!CARRIED || !a.r_defer) a.r[j] = d;
+      if ((!CARRIED || !a.r_defer) && store_r) a.r[j] = d;
     } else {
       const float p = fmaf(coef, a.h[j], a.F[j]);
       d = a.y[j] - p;
