@@ -7,9 +7,14 @@ in registers and, with `fused_resident`, the groups before it in shared memory (
 `phase_b_offchip_read_bytes` is what the update phase then still reads from the L2 or HBM.
 
 Consecutive rounds over one direction are carried (`last_round_stats_carried`): the previous update phase summed their
-statistics, so the statistics phase is only the cross-GPU exchange and the "statistics" stamp measures the time to
-it.  `carry: 0` drops the carried statistics before every round (handing out H's device pointer, which launches
-nothing), so that every round runs its statistics pass."""
+statistics, so the statistics phase is only the fold of the previous update's per-CTA partials (and the cross-GPU
+exchange) and the "statistics" stamp measures the time to it.  On one GPU every CTA of a carried round folds and
+runs Brent itself, and the stamps are CTA 0's.  Such a round is launched as a programmatic dependent of the kernel
+before it: its `kernel_event_us` is not an event pair (events between two such rounds order them in full) but the
+kernel's own stamps, CTA 0's entry to the last CTA's exit, which overlap the previous round's tail.
+
+`carry: 0` drops the carried statistics before every round (handing out H's device pointer, which launches nothing),
+so that every round runs its statistics pass."""
 import json
 import math
 import os

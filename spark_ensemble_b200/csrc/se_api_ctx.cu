@@ -74,13 +74,33 @@ int fail(se_ctx* ctx, int code, const char* fmt, ...) {
 int drain_kernel_events(se_ctx* ctx) {
   if (ctx->kpending == 0) return SE_OK;
   SE_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  unsigned long long st[2 * se_ctx::kRing];
+  if (ctx->d_kstamp)
+    SE_CUDA(ctx, cudaMemcpy(st, ctx->d_kstamp, sizeof(unsigned long long) * 2 * ctx->kpending, cudaMemcpyDeviceToHost));
   for (int i = 0; i < ctx->kpending; ++i) {
     float ms = 0.f;
-    SE_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->kev[i][0], ctx->kev[i][1]));
+    if (ctx->kstamped[i]) ms = (float)(1e-6 * (double)(st[2 * i + 1] - st[2 * i]));
+    else SE_CUDA(ctx, cudaEventElapsedTime(&ms, ctx->kev[i][0], ctx->kev[i][1]));
     ctx->kms[ctx->kfam[i]] += (double)ms;
     ctx->kcount[ctx->kfam[i]] += 1;
   }
   ctx->kpending = 0;
+  return SE_OK;
+}
+
+int kernel_stamp_slot(se_ctx* ctx, int family, unsigned long long** stamps) {
+  *stamps = nullptr;
+  if (!ctx->ktiming) return SE_OK;
+  if (ctx->kpending == se_ctx::kRing) SE_TRY(drain_kernel_events(ctx));
+  if (!ctx->d_kstamp) {
+    // zeroed once: a slot's exit stamp is an atomicMax, and what an earlier launch left there is older
+    SE_CUDA(ctx, ctx->d_kstamp.grow(2 * se_ctx::kRing));
+    SE_CUDA(ctx, cudaMemsetAsync(ctx->d_kstamp, 0, sizeof(unsigned long long) * 2 * se_ctx::kRing, ctx->stream));
+  }
+  const int slot = ctx->kpending++;
+  ctx->kfam[slot] = family;
+  ctx->kstamped[slot] = true;
+  *stamps = ctx->d_kstamp + 2 * slot;
   return SE_OK;
 }
 
@@ -366,6 +386,7 @@ int se_ctx_create(int device, se_ctx** out) {
   SE_CUDA(nullptr, ctx->d_fsync.grow(1));
   SE_CUDA(nullptr, cudaMemset(ctx->d_fsync, 0, sizeof(FusedSync)));
   SE_CUDA(nullptr, ctx->d_rchain.grow(kSqDeferMax));
+  SE_CUDA(nullptr, ctx->d_sq_carry.grow((size_t)2 * (kMaxGridPartials / 2) * 3));
   ctx->clock_khz = prop.clockRate > 0 ? prop.clockRate : 1965000;
   if (const char* s = getenv("SE_FUSED_ROUND")) ctx->fused_round = atoi(s) != 0 ? 1 : 0;
   if (const char* s = getenv("SE_FUSED_RESIDENT")) ctx->fused_resident = atoi(s) != 0;

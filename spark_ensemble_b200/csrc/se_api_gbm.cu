@@ -531,8 +531,9 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   // second cross-GPU exchange, and the host is served before the update phase ends.  With a bag the statistics run
   // over the bag while the loss runs over all rows: then the loss is reduced over the rows as in the two-launch path.
   const bool loss_reduce = g.use_bag || ctx->fused_loss_reduce;
-  // Such a residual round's update pass also sums the statistics of what it writes, (r', h), into d_scal[kScalCarry]:
-  // the next round over the same direction takes them from there and skips its statistics pass (12 B/row, not 20).
+  // Such a residual round's update pass also sums the statistics of what it writes, (r', h), one partial per CTA into
+  // a parity of d_sq_carry: the next round over the same direction folds them and skips its statistics pass (12 B/row,
+  // not 20).
   // The update then walks its tiles opposite to the previous one, so that it starts on what is still in the L2.
   const bool stats_out = write_r && !loss_reduce;
   const bool carried = stats_out && g.r_current && g.sq_stats_current;
@@ -546,11 +547,17 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   a.r_chain = ctx->d_rchain;
   a.r_pending = carried ? g.r_pending : 0;
   a.r_defer = (carried && g.sq_defer_ok && g.r_pending < ctx->sq_defer_max) ? 1 : 0;
-  a.ws_next.partials = ctx->d_partials + (size_t)(kMaxGridPartials / 2) * 4;  // ws_b's, unused without a row-reduced loss
-  a.ws_next.counter = &ctx->d_fsync->counter_b;
-  a.ws_next.out = ctx->d_scal + kScalCarry;
+  // the carried partials: read from the parity the last such round stored, stored into the other one
+  constexpr size_t kCarryParity = (size_t)(kMaxGridPartials / 2) * 3;
+  const int carry_parity = g.sq_carry_parity ^ 1;
+  a.carry_in = ctx->d_sq_carry + (size_t)g.sq_carry_parity * kCarryParity;
+  a.carry_grid = g.sq_carry_grid;
+  a.carry_out = stats_out ? ctx->d_sq_carry + (size_t)carry_parity * kCarryParity : nullptr;
   ctx->gbm.sq_stats_current = false;           // until the round has succeeded
   a.ws_a = red_ws(ctx, kScalRound);            // sequence number s (statistics)
+  // on one GPU a carried round may start before the kernel before it ends: it loads r that early only when no
+  // kernel since the last deferring round has written R (every write of R settles the pending steps first)
+  a.r_early = (carried && (a.ws_a.nranks <= 1 || a.ws_a.mbox == nullptr) && a.r_pending > 0) ? 1 : 0;
   a.ws_a.host_out = nullptr;                   // the mirror ticket is written after Brent / the second reduction
   a.ws_a.host_flag = nullptr;
   if (ctx->mirror_valid) --ctx->mirror_ticket; // red_ws armed the mirror for ws_a: re-armed below
@@ -578,8 +585,23 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   a.epoch = ++ctx->fused_epoch;
   a.timing = ctx->fused_timing;
   int grid = 0, resident_slots = 0;
-  SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->fused_resident, ctx->sms,
-                                                           ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots));
+  auto launch = [&]() {
+    return launch_gbm_round_sq_fused(a, write_r, loss_reduce ? 1 : 0, ctx->fused_resident, ctx->sms,
+                                     ctx->fused_ctas_per_sm, ctx->stream, &grid, &resident_slots);
+  };
+  if (carried && (a.ws_a.nranks <= 1 || a.ws_a.mbox == nullptr)) {
+    // a programmatic dependent launch: kernel timing takes the kernel's own stamps, not events around it
+    SE_TRY(kernel_stamp_slot(ctx, SE_KF_UPDATE, &a.kstamp));
+    const cudaError_t e = launch();
+    ctx->launches++;
+    if (e != cudaSuccess) {
+      if (a.kstamp) --ctx->kpending;  // give back the slot claimed above: nothing will stamp it
+      return fail(ctx, SE_ERR_CUDA, "%s:%d launch launch_gbm_round_sq_fused -> %s", __FILE__, __LINE__,
+                  cudaGetErrorString(e));
+    }
+  } else {
+    SE_LAUNCH_T(ctx, SE_KF_UPDATE, launch());
+  }
   ctx->last_fused_grid = grid;
   ctx->last_round_carried = carried ? 1 : 0;
   ctx->gbm.r_pending = a.r_defer ? a.r_pending + 1 : 0;  // the kernel ran: its step joined the chain or R was stored
@@ -621,6 +643,8 @@ int round_squared_fused(se_ctx* ctx, double learning_rate, double tol, int max_i
   if (stats_out) {
     ctx->gbm.sq_stats_current = true;
     ctx->gbm.sq_last_up = a.forward != 0;
+    ctx->gbm.sq_carry_parity = carry_parity;
+    ctx->gbm.sq_carry_grid = grid;
   }
   return SE_OK;
 }

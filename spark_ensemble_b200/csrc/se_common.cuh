@@ -292,15 +292,11 @@ __device__ __forceinline__ void peer_exchange(const double* tot, int nred, const
   }
 }
 
-// Block-reduce NRED per-thread fp64 accumulators, publish the block partial, and let the last CTA
-// to arrive reduce all partials in a fixed order (deterministic for a fixed launch configuration).
-// Returns true in every thread of the CTA that performed the final reduction (its ws.out writes are then complete
-// after a __syncthreads()).
+// The two halves of block_reduce_publish.  block_reduce_store: block-reduce NRED per-thread fp64 accumulators and
+// store the CTA's partial at partials[blockIdx.x * NRED + k] (written by lane 0 of warp 0; every thread calls it).
 template <int NRED, int BLOCK = kBlock>
-__device__ __forceinline__ bool block_reduce_publish(double (&acc)[NRED], const RedWs& ws) {
+__device__ __forceinline__ void block_reduce_store(double (&acc)[NRED], double* partials) {
   __shared__ double sm[NRED][BLOCK / 32];
-  __shared__ double tot[NRED];
-  __shared__ bool is_last;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int k = 0; k < NRED; ++k) {
@@ -313,23 +309,22 @@ __device__ __forceinline__ bool block_reduce_publish(double (&acc)[NRED], const 
     for (int k = 0; k < NRED; ++k) {
       double v = (lane < BLOCK / 32) ? sm[k][lane] : 0.0;
       v = warp_sum(v);
-      if (lane == 0) ws.partials[(size_t)blockIdx.x * NRED + k] = v;
+      if (lane == 0) partials[(size_t)blockIdx.x * NRED + k] = v;
     }
   }
-  if (threadIdx.x == 0) {
-    __threadfence();
-    const unsigned int ticket = atomicInc(ws.counter, gridDim.x - 1);  // wraps to 0: self-resetting
-    is_last = (ticket == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (!is_last) return false;
-  __threadfence();
-  // fixed-order accumulation over blocks: thread t takes blocks t, t+BLOCK, ...
+}
+
+// fold_partials: the `grid` partials of NRED entries in a fixed order -- thread t takes blocks t, t+BLOCK, ..., then
+// the warps and the CTA sum what they hold -- into tot (shared memory, complete in every thread on return).  The same
+// partials give the same bits whichever CTA, or however many CTAs, fold them.
+template <int NRED, int BLOCK = kBlock>
+__device__ __forceinline__ void fold_partials(const double* partials, unsigned int grid, double* tot) {
+  __shared__ double sm[NRED][BLOCK / 32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int k = 0; k < NRED; ++k) {
     double v = 0.0;
-    for (unsigned int b = threadIdx.x; b < gridDim.x; b += BLOCK)
-      v += __ldcg(&ws.partials[(size_t)b * NRED + k]);
+    for (unsigned int b = threadIdx.x; b < grid; b += BLOCK) v += __ldcg(&partials[(size_t)b * NRED + k]);
     v = warp_sum(v);
     if (lane == 0) sm[k][warp] = v;
   }
@@ -343,6 +338,26 @@ __device__ __forceinline__ bool block_reduce_publish(double (&acc)[NRED], const 
     }
   }
   __syncthreads();
+}
+
+// Block-reduce NRED per-thread fp64 accumulators, publish the block partial, and let the last CTA
+// to arrive reduce all partials in a fixed order (deterministic for a fixed launch configuration).
+// Returns true in every thread of the CTA that performed the final reduction (its ws.out writes are then complete
+// after a __syncthreads()).
+template <int NRED, int BLOCK = kBlock>
+__device__ __forceinline__ bool block_reduce_publish(double (&acc)[NRED], const RedWs& ws) {
+  __shared__ double tot[NRED];
+  __shared__ bool is_last;
+  block_reduce_store<NRED, BLOCK>(acc, ws.partials);
+  if (threadIdx.x == 0) {
+    __threadfence();
+    const unsigned int ticket = atomicInc(ws.counter, gridDim.x - 1);  // wraps to 0: self-resetting
+    is_last = (ticket == gridDim.x - 1);
+  }
+  __syncthreads();
+  if (!is_last) return false;
+  __threadfence();
+  fold_partials<NRED, BLOCK>(ws.partials, gridDim.x, tot);
   peer_exchange(tot, NRED, ws);  // per-GPU totals -> ws.out (summed across GPUs when a peer communicator is attached)
   return true;
 }

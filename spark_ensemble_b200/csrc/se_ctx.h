@@ -42,7 +42,6 @@ extern thread_local std::string g_last_error;
 constexpr int kScal = 1024;         // doubles in the device/host scalar blocks ([0, 160): generic reductions)
 constexpr int kScalHist = 704;      // 256-bin radix-select histogram
 constexpr int kScalRound = 160;     // offset of the squared-round results (statistics, alpha, loss)
-constexpr int kScalCarry = 184;     // the squared round's carried statistics (3 values, gbm.sq_stats_current)
 constexpr int kScalHost = 192;      // offset used by se_comm_allreduce_host (up to kScalHist - kScalHost values)
 constexpr int kSmallBytes = 1 << 20;  // small device scratch: weights, init, tree arrays, factors
 
@@ -180,9 +179,12 @@ struct se_ctx {
     bool r_current = false;  // SE_SLOT_R holds -g(y, F) of the CURRENT F (squared loss: y - F)
     bool f_owed = false;     // SE_SLOT_F is stale: its value is y - r (residual-mode fused squared round); settle_f
                              // rebuilds it.  Implies r_current.
-    // d_scal[kScalCarry..+2] holds this GPU's Σr², Σhr, Σh² over the current R and H: the update pass of the last
-    // residual fused round summed them over what it wrote.  Dropped by every write of Y, F, R or H.
+    // d_sq_carry's parity sq_carry_parity holds this GPU's Σr², Σhr, Σh² over the current R and H as the
+    // sq_carry_grid partials of the CTAs of the last residual fused round's update pass, which summed them over what it
+    // wrote.  Dropped by every write of Y, F, R or H.
     bool sq_stats_current = false;
+    int sq_carry_parity = 0;
+    int sq_carry_grid = 0;
     bool sq_last_up = false;  // the last fused round's update pass walked its tiles upwards (ended on the highest)
     // SE_SLOT_R is pending: it holds an older r0, and the residual is r0 after the r_pending fp32 steps in d_rchain
     // along H (carried rounds that stored nothing).  settle_r applies them; nothing else may touch R, or write H,
@@ -253,6 +255,10 @@ struct se_ctx {
   // carried rounds leave at most this many steps pending on R before one stores it (0: every round stores r')
   int sq_defer_max = 16;
   se_host::DevBuf<float> d_rchain;    // the pending steps [kSqDeferMax]
+  // the squared round's carried statistics: two parities of [kMaxGridPartials / 2][3] CTA partials.  A round stores
+  // into the parity its predecessor did not, so its first CTAs to finish never overwrite what its last ones fold.  Not
+  // the shared reduction workspace: the partials must outlive the calls between two rounds, a read of R among them.
+  se_host::DevBuf<double> d_sq_carry;
   double last_fused_resident_tiles = 0.0;  // tiles per CTA the last fused round carried in shared memory
   double last_fused_us[3] = {0, 0, 0};  // statistics phase, fold+exchange+Brent, update phase
   int ls_mode = 1;                    // non-squared line search: 0 one launch per evaluation (round-1 kernels), 1 one
@@ -328,6 +334,10 @@ struct se_ctx {
   static constexpr int kRing = 128;
   se_host::Event kev[kRing][2];
   int kfam[kRing] = {};
+  // a launch timed by its own %globaltimer stamps instead of events: d_kstamp[2 * slot] is CTA 0's entry and
+  // [2 * slot + 1] the latest exit of any CTA, in ns (kernel_stamp_slot)
+  bool kstamped[kRing] = {};
+  se_host::DevBuf<unsigned long long> d_kstamp;
   int kpending = 0;
   double kms[SE_KF_COUNT] = {};
   int64_t kcount[SE_KF_COUNT] = {};
@@ -355,6 +365,10 @@ int fail(se_ctx* ctx, int code, const char* fmt, ...);
   } while (0)
 
 int drain_kernel_events(se_ctx* ctx);
+// With kernel timing on: a slot of the timing ring for a launch that stamps its own start and end (*stamps, nullptr
+// with kernel timing off).  CUDA events recorded around a programmatic dependent launch would order it after the
+// kernel before it in full, so such a launch is timed from inside instead.
+int kernel_stamp_slot(se_ctx* ctx, int family, unsigned long long** stamps);
 
 // launch bracketed by CUDA events on the context stream when kernel timing is on
 #define SE_LAUNCH_T(ctx, family, call)                                                        \
@@ -376,6 +390,7 @@ int drain_kernel_events(se_ctx* ctx);
     if (slot__ >= 0) {                                                                        \
       SE_CUDA(ctx, cudaEventRecord((ctx)->kev[slot__][1], (ctx)->stream));                    \
       (ctx)->kfam[slot__] = (family);                                                         \
+      (ctx)->kstamped[slot__] = false;                                                        \
       (ctx)->kpending = slot__ + 1;                                                           \
     }                                                                                         \
   } while (0)

@@ -15,8 +15,10 @@
 //    F = y - r.  The host marks F as owed and rebuilds it from y and r when F is next accessed (se_api_ctx.cu settle_f).
 //    A round whose residual slot is not current (Y, F or R were just written) reads (y, F, h) instead of (r, h):
 //    r' = (y - F) - c h, 16 B/row.  Without residual mode the update is F' = F + c h (F, y, h read; F written).
-//    A residual round without a bag also sums the statistics of (r', h) in its update pass; while R and H stay as
-//    it left them, the next round takes those sums and skips the statistics pass (12 B/row).
+//    A residual round without a bag also sums the statistics of (r', h) in its update pass, one partial per CTA;
+//    while R and H stay as it left them, the next round folds those partials and skips the statistics pass
+//    (12 B/row).  On one GPU every CTA of that carried round folds them and runs Brent itself: no CTA waits for
+//    another, and the round is launched as a programmatic dependent that starts while the round before it drains.
 //    Such a carried round may also leave R pending (se_api_ctx.cu settle_r): it stores nothing (8 B/row), and the
 //    Brent thread appends its fp32 step to a chain on the device.  The next carried round reads the older r0 and
 //    applies the chain in registers, t = fmaf(-c_j, h, t), before its own step -- the fmaf a storing round applies,
@@ -59,12 +61,13 @@ __device__ __forceinline__ void red_release_gpu_add_u32(unsigned int* p, unsigne
   asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// bulk L2 prefetch of a contiguous global range (bytes: multiple of 16, address 16 B aligned)
-__device__ __forceinline__ double global_timer_us() {
+__device__ __forceinline__ unsigned long long global_timer_ns() {
   unsigned long long t;
   asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return (double)t * 1e-3;
+  return t;
 }
+__device__ __forceinline__ double global_timer_us() { return (double)global_timer_ns() * 1e-3; }
+// bulk L2 prefetch of a contiguous global range (bytes: multiple of 16, address 16 B aligned)
 __device__ __forceinline__ void prefetch_l2_bulk(const void* p, unsigned int bytes) {
   asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p), "r"(bytes) : "memory");
 }
@@ -76,26 +79,32 @@ constexpr int U_SQ = 4;  // float4 groups per thread per tile (as the two-launch
 // that a slot, not a whole 32 KB tile, is the unit the SM's shared memory is split into.
 constexpr int kSqSlotBytes = 2 * kBlock * 16;
 
-// The line search of the fused round, executed by ONE thread of the last CTA once the statistics are folded (and
-// summed across GPUs) while every other CTA waits for the step with its first update tile's loads in flight.
+// The line search of the fused round, executed by ONE thread once the statistics s0, s1, s2 are folded (and summed
+// across GPUs): by the last CTA while every other CTA waits for the step with its first update tile's loads in flight,
+// or, in a carried round on one GPU, by every CTA for itself.  Returns the step.  `serve`: this thread also writes the
+// round's results (out[4..8], the host mirror and its ticket) and appends a deferring round's step to the chain;
+// `release`: it hands the step to the grid through a.sync.
 template <bool LOSS_REDUCE>
-__device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
-  if (a.timing) a.out[11] = global_timer_us();  // statistics folded (and summed across GPUs)
-  const double s0 = a.out[0], s1 = a.out[1], s2 = a.out[2];
+__device__ __forceinline__ double fused_round_brent(const SqRoundArgs& a, double s0, double s1, double s2, bool serve,
+                                                    bool release) {
+  if (a.timing && serve) a.out[11] = global_timer_us();  // statistics folded (and summed across GPUs)
   const BrentParabola f{s0, s1, s2, a.wsum};
   double x = 1.0, fx = 0.0;
   int evals = 0;
   const int rc = brent_core(f, a.lo, a.hi, a.start, a.rel, a.abs_tol, a.max_eval, &x, &fx, &evals);
-  const double ne = (rc == kBrentOk) ? (double)evals : -(double)evals;  // negative: MaxEval exceeded
-  a.out[4] = x, a.out[5] = fx, a.out[6] = ne;
   // MaxEval exceeded: the host reports SE_ERR_OPT and F must stay what it was (r - 0*h == r, F + 0*h == F; the host
   // does not mark F as owed)
   const double step = (rc == kBrentOk) ? a.lr * x : 0.0;
+  if (!serve) return step;
+  const double ne = (rc == kBrentOk) ? (double)evals : -(double)evals;  // negative: MaxEval exceeded
+  a.out[4] = x, a.out[5] = fx, a.out[6] = ne;
   // a deferring round's step, as phase B rounds it, joins the pending chain (a 0 step too: fmaf(-0, h, r) is what
   // the stored round applies)
   if (a.r_defer) a.r_chain[a.r_pending] = (float)step;
-  a.sync->x = step;
-  st_release_gpu_u64(&a.sync->flag, a.epoch);  // the grid starts the update NOW; the host is served next
+  if (release) {
+    a.sync->x = step;
+    st_release_gpu_u64(&a.sync->flag, a.epoch);  // the grid starts the update NOW; the host is served next
+  }
   if (a.timing) a.out[12] = global_timer_us();  // step published
   if (a.host_res) {  // mapped host memory, above what a reducing kernel writes before its ticket
     a.host_res[0] = s0, a.host_res[1] = s1, a.host_res[2] = s2;
@@ -118,6 +127,7 @@ __device__ __forceinline__ void fused_round_brent(const SqRoundArgs& a) {
   } else if (a.host_res) {
     __threadfence_system();
   }
+  return step;
 }
 
 __device__ __forceinline__ void cp_async16(float4* smem, const float* gmem) {
@@ -128,9 +138,14 @@ __device__ __forceinline__ void cp_async16(float4* smem, const float* gmem) {
 // FROM_R (a fit's round after a new direction: residual mode, the residual slot current, no bag) is a compile-time
 // specialisation: it carries phase A's tail into phase B on chip (kSqSlotBytes) and has no y / F / bag arrays live.
 // CARRIED (the rounds after it over the same direction) has no phase A at all: the previous round's update pass left
-// the statistics of (r, h) in a.ws_next.out.  One CTA sums them across GPUs and runs Brent while every CTA has its
-// first update tile in registers and, with resident slots, the groups after it in flight to shared memory.
-// Residual rounds whose loss comes from the statistics (STATS_OUT) sum the next round's statistics in phase B.
+// each CTA's partial statistics of (r, h) in a.carry_in.  They are folded and Brent runs while every CTA has its first
+// update tile in registers and, with resident slots, the groups after it in flight to shared memory.  Across GPUs
+// CTA 0 folds, sums across GPUs, runs Brent and publishes the step to the others (a cooperative launch).  On one GPU
+// every CTA folds the same partials in the same order and runs Brent itself, so no CTA waits for another: the launch
+// is an ordinary one, a programmatic dependent of the kernel before it (griddepcontrol), and CTA 0 alone serves the
+// host and the chain.
+// Residual rounds whose loss comes from the statistics (STATS_OUT) store the next round's partial statistics in
+// phase B.
 template <bool WRITE_R, bool LOSS_REDUCE, bool FROM_R, bool CARRIED>
 __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqRoundArgs a) {
   static_assert(WRITE_R || !FROM_R, "FROM_R is a residual-mode round");
@@ -140,6 +155,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   extern __shared__ float4 s_res[];  // FROM_R, CARRIED: [slot][r, h][kBlock]
   __shared__ float s_coef;
   __shared__ bool s_store_r;
+  __shared__ double s_stats[3];  // CARRIED: the folded statistics
   __shared__ float s_chain[kSqDeferMax];  // CARRIED: the steps pending on the residual slot
   __shared__ float4 s_brent_regs[2 * U];  // FROM_R, CARRIED: the Brent thread's tile registers while it runs Brent
   const int64_t n4 = a.n >> 2;
@@ -168,18 +184,19 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   const uint64_t pol_carried = l2_policy(true);
 
   if (a.timing && blockIdx.x == 0 && threadIdx.x == 0) a.out[10] = global_timer_us();
+  if (a.kstamp && blockIdx.x == 0 && threadIdx.x == 0) a.kstamp[0] = global_timer_ns();
   // phase B's tile registers.  FROM_R: phase A loads into them, so that its last tile is where phase B starts; the
   // other rounds keep phase A's tiles local, so that nothing is live across the wait but what phase B loads.
   float4 vy[U], vF[U], vh[U];  // from_r: vy holds r and vF is unused
   bool ok[U];
   // the Brent thread parks the tile registers in shared memory meanwhile: Brent needs more registers than are left
   // beside them, and local memory would be the alternative
-  auto run_brent = [&]() {
+  auto run_brent = [&](const double* s, bool serve, bool release) {
     if constexpr (FROM_R || CARRIED) {
 #pragma unroll
       for (int u = 0; u < U; ++u) s_brent_regs[u] = vy[u], s_brent_regs[U + u] = vh[u];
     }
-    fused_round_brent<LOSS_REDUCE>(a);
+    s_coef = (float)fused_round_brent<LOSS_REDUCE>(a, s[0], s[1], s[2], serve, release);
     if constexpr (FROM_R || CARRIED) {
 #pragma unroll
       for (int u = 0; u < U; ++u) vy[u] = s_brent_regs[u], vh[u] = s_brent_regs[U + u];
@@ -214,23 +231,43 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   // CARRIED: the pending steps, read before the Brent thread appends this round's (the barrier before phase B
   // publishes them).  The count and the store flag are read from the kernel parameters where they are used: kept in
   // registers they would spill.
+  const bool solo = CARRIED && (a.ws_a.nranks <= 1 || a.ws_a.mbox == nullptr);
   if constexpr (CARRIED) {
-    for (int j = threadIdx.x; j < a.r_pending; j += kBlock) s_chain[j] = a.r_chain[j];
     // the first tile into registers, the S groups after it into shared memory (each thread copies, and in phase B
     // reads back, only its own slots: no barrier)
-    if (cnt > 0) load_tile(0);
-    for (int64_t s = 0; s < S; ++s) {
-      const int64_t k = 1 + s / U, i = up ? k : cnt - 1 - k;
-      const int64_t g = (blockIdx.x + i * G) * tile + threadIdx.x + (s % U) * (int64_t)kBlock;
-      if (g < n4) {
-        cp_async16(&s_res[(2 * s) * kBlock + threadIdx.x], a.r + 4 * g);
-        cp_async16(&s_res[(2 * s + 1) * kBlock + threadIdx.x], a.h + 4 * g);
+    auto prologue = [&]() {
+      if (cnt > 0) load_tile(0);
+      for (int64_t s = 0; s < S; ++s) {
+        const int64_t k = 1 + s / U, i = up ? k : cnt - 1 - k;
+        const int64_t g = (blockIdx.x + i * G) * tile + threadIdx.x + (s % U) * (int64_t)kBlock;
+        if (g < n4) {
+          cp_async16(&s_res[(2 * s) * kBlock + threadIdx.x], a.r + 4 * g);
+          cp_async16(&s_res[(2 * s + 1) * kBlock + threadIdx.x], a.h + 4 * g);
+        }
       }
+    };
+    // On one GPU this kernel may start while the one before it still runs (programmatic dependent launch): until
+    // griddepcontrol.wait returns, it reads nothing but h, which nothing between two carried rounds writes, and r
+    // when the host says R has not been written since the last deferring round.  Everything the kernel before it
+    // writes (r', the chain, the partials, the results) is read after the wait.  A CTA lets the next kernel start only
+    // once its own wait has returned, so that kernel cannot begin before this one's predecessor has completed.
+    if (a.r_early) prologue();
+    if (solo) {
+      asm volatile("griddepcontrol.wait;" ::: "memory");
+      asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     }
-    if (blockIdx.x == 0) {
-      peer_exchange(a.ws_next.out, 3, a.ws_a);  // this GPU's statistics -> a.out[0..2], summed across GPUs
+    if (!a.r_early) prologue();
+    for (int j = threadIdx.x; j < a.r_pending; j += kBlock) s_chain[j] = a.r_chain[j];
+    if (solo) {
+      // the statistics, bit for bit as CTA 0 would fold them, and the step, in every CTA
+      fold_partials<3>(a.carry_in, (unsigned)a.carry_grid, s_stats);
+      if (blockIdx.x == 0 && threadIdx.x < 3) a.out[threadIdx.x] = s_stats[threadIdx.x];
+      if (threadIdx.x == 0) run_brent(s_stats, blockIdx.x == 0, false);
+    } else if (blockIdx.x == 0) {
+      fold_partials<3>(a.carry_in, (unsigned)a.carry_grid, s_stats);
+      peer_exchange(s_stats, 3, a.ws_a);  // this GPU's statistics -> a.out[0..2], summed across GPUs
       __syncthreads();
-      if (threadIdx.x == 0) run_brent();
+      if (threadIdx.x == 0) run_brent(a.out, true, true);
     }
   } else {
   // ---- phase A: Σ(y-F)², Σh(y-F), Σh² (from the current residual slot when it is valid: 8 B/row)
@@ -308,7 +345,7 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
   const bool last = block_reduce_publish<3>(acc, a.ws_a);  // the last CTA also sums across GPUs (peer_exchange)
   if (last) {
     __syncthreads();  // a.out[0..2] were written by other threads of this CTA
-    if (threadIdx.x == 0) run_brent();
+    if (threadIdx.x == 0) run_brent(a.out, true, true);
   }
   // in flight while the last CTA reduces, exchanges and runs Brent (FROM_R: still in registers from phase A)
   if (!FROM_R && cnt > 0) load_tile(0);
@@ -333,8 +370,10 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
         }
       }
     }
-    while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {}
-    s_coef = (float)a.sync->x;  // same rounding as the host path: (float)(lr * alpha)
+    if (!solo) {  // on one GPU a carried round's thread 0 computed the step itself
+      while (ld_acquire_gpu_u64(&a.sync->flag) != a.epoch) {}
+      s_coef = (float)a.sync->x;  // same rounding as the host path: (float)(lr * alpha)
+    }
     // MaxEval exceeded on a round that read y and F: its residual slot was not current, and the failed round must
     // leave it as it was rather than store y - F (the Brent thread wrote the count before it released the step)
     s_store_r = !(WRITE_R && !from_r && a.out[6] < 0.0);
@@ -423,12 +462,17 @@ __global__ void __launch_bounds__(kBlock, 3) gbm_round_sq_fused_kernel(const SqR
     const bool last_b = block_reduce_publish<1>(accb, a.ws_b);  // Σloss -> a.ws_b.out (+ cross-GPU sum, host mirror + ticket)
     if (a.timing && last_b && threadIdx.x == 0) a.out[13] = global_timer_us();
   } else {
-    // the next round's statistics, this GPU's: a carried round reads them before any CTA of it arrives here
-    if constexpr (STATS_OUT) block_reduce_publish<3>(accn, a.ws_next);
+    // the next round's statistics, this GPU's, as one partial per CTA.  A carried round stores them into the other of
+    // the context's two buffers than the one it folded, which its slower CTAs may still be reading.
+    if constexpr (STATS_OUT) block_reduce_store<3>(accn, a.carry_out);
     if (a.timing) {
       // the loss came from the statistics: the latest stamp of any CTA marks the end of the update
       __syncthreads();
       if (threadIdx.x == 0) atomicMax(reinterpret_cast<unsigned long long*>(&a.out[13]), (unsigned long long)__double_as_longlong(global_timer_us()));
+    }
+    if (a.kstamp) {
+      __syncthreads();
+      if (threadIdx.x == 0) atomicMax(a.kstamp + 1, global_timer_ns());
     }
   }
 }
@@ -766,6 +810,15 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
   // only a carried round reads pending steps or defers its own, and the chain holds at most kSqDeferMax of them
   if ((a0.r_pending || a0.r_defer) && !(carried && a0.r_chain)) return cudaErrorInvalidValue;
   if (a0.r_pending < 0 || a0.r_pending + (a0.r_defer ? 1 : 0) > kSqDeferMax) return cudaErrorInvalidValue;
+  // a carried round folds the partials of a grid that fit the buffer; a residual round without a bag stores its own
+  if (carried && !(a0.carry_in && a0.carry_grid >= 1 && a0.carry_grid <= kMaxGridPartials / 2))
+    return cudaErrorInvalidValue;
+  if (write_r && !loss_reduce && !a0.carry_out) return cudaErrorInvalidValue;
+  // the same test as the kernel's (and peer_exchange's): one GPU, or no peer communicator attached
+  const bool solo = a0.ws_a.nranks <= 1 || a0.ws_a.mbox == nullptr;
+  // r is read before the kernel before this one is waited for only when that kernel cannot have written it
+  if (a0.r_early && !(carried && solo && a0.r_pending > 0)) return cudaErrorInvalidValue;
+  if (a0.kstamp && !(carried && solo)) return cudaErrorInvalidValue;
   const bool from_r = !carried && write_r && a0.stats_from_r && a0.bag == nullptr;
   const int which = carried ? 6 : from_r ? 4 + (loss_reduce ? 1 : 0) : (write_r ? 2 : 0) + (loss_reduce ? 1 : 0);
   // function attributes and occupancy are per DEVICE (a process may drive several GPUs, as in launch_ls)
@@ -838,8 +891,14 @@ cudaError_t launch_gbm_round_sq_fused(const SqRoundArgs& a0, int write_r, int lo
   lc.dynamicSmemBytes = dyn;
   lc.stream = st;
   cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeCooperative;
-  attr.val.cooperative = 1;  // co-residency of all CTAs is what makes the in-kernel flag wait deadlock-free
+  if (carried && solo) {
+    // no CTA waits for another: the round may start while the kernel before it drains (griddepcontrol in the kernel)
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+  } else {
+    attr.id = cudaLaunchAttributeCooperative;
+    attr.val.cooperative = 1;  // co-residency of all CTAs is what makes the in-kernel flag wait deadlock-free
+  }
   lc.attrs = &attr;
   lc.numAttrs = 1;
   if (grid_out) *grid_out = (int)grid;

@@ -111,10 +111,20 @@ struct SqRoundArgs {
   RedWs ws_a{};  // statistics: out = `out`, no host mirror
   RedWs ws_b{};  // loss (only when it is reduced over the rows: bags): out = out + 8, host mirror + ticket
   // Residual rounds without a bag and with the loss from the statistics: the update pass also sums Σr'², Σhr', Σh²
-  // over what it writes, i.e. the next round's statistics, into ws_next.out (this GPU's sums: no exchange, no mirror).
-  RedWs ws_next{};
-  int carried = 0;  // 1: ws_next.out holds the statistics of (r, h): skip the statistics pass
+  // over what it writes, i.e. the next round's statistics, and each CTA stores its partial at carry_out[3 * CTA + k]
+  // (this GPU's; no CTA folds them).  A carried round folds the carry_grid partials at carry_in in CTA order.
+  double* carry_out = nullptr;
+  const double* carry_in = nullptr;
+  int carry_grid = 0;
+  int carried = 0;  // 1: carry_in holds the statistics of (r, h): skip the statistics pass
   int forward = 0;  // carried round: walk the update's tiles upwards (the previous update ended on the lowest ones)
+  // Carried round on one GPU (ws_a without peers): every CTA folds carry_in and runs Brent itself, and the round is
+  // launched as a programmatic dependent of the kernel before it.  r_early: R has not been written since the round
+  // that deferred last (r_pending > 0), so the first tile and the shared-memory slots of r may be loaded before the
+  // kernel before this one is waited for; otherwise only after it.
+  int r_early = 0;
+  // nullable: kernel timing of such a launch, in ns: [0] = CTA 0's entry, [1] = atomicMax of every CTA's exit
+  unsigned long long* kstamp = nullptr;
   // Carried rounds only: the residual slot holds an older r0, and the logical r is r0 after the r_pending fp32 steps
   // r_chain[0..r_pending) along h (t = fmaf(-c_j, h, t)).  The kernel applies them in registers before its own step.
   // r_defer: store nothing; the Brent thread appends this round's step at r_chain[r_pending] (0 when MaxEval is
